@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — kNN queries/sec of the knowledge-base search path on B200.
+"""bench.py — kNN queries/sec of the knowledge-base search path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl ours|reference] [--no-extras]
+                    [--dump-outputs DIR]
     python bench.py --gpus N --single-process      (no torchrun: ONE process, one rbk_group handle over N GPUs)
 
 A "step" is one pass of the hot path (batched cosine scan + exact top-k) over one batch of
@@ -20,6 +21,10 @@ hypothesis-branch batch (cfg5, every N) and the 50M x 1024 corpus (cfg4, N = 8).
 `--impl reference` times the reference's CPU algorithm (oracle/, strict fp64 restatement;
 Node is absent so the TypeScript itself cannot run) on the box's host cores on a bounded
 sample of the same workload.
+`--dump-outputs DIR` writes what the last timed step of the main workload returned (the slots,
+fp64 scores and counts of the whole batch; rank 0's with torchrun, the group's with
+--single-process) as DIR/<name>.npy, float64: corpus and queries are generated from fixed seeds,
+so two builds can be compared output for output.  The reference arm refuses it.
 """
 from __future__ import annotations
 
@@ -49,6 +54,7 @@ WORKLOADS = {
 SEED = 0x5EED0003
 GEN_CHUNK = 65536
 PARITY_QUERIES = 64
+L2_BYTES = 50e6   # H100
 
 
 def load_synth():
@@ -60,15 +66,13 @@ def load_synth():
 
 
 def peaks():
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        j = json.loads(p.read_text())
-        return dict(hbm=j["hbm_gbs"], tf=j["bf16_tflops"], tf_sus=j.get("bf16_tflops_sustained"), src="measured")
-    return dict(hbm=6650.0, tf=1590.0, tf_sus=1400.0, src="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s.  A card with a lower power limit
+    # lowers its clocks under sustained load, so the tensor figure is an upper bound there.
+    return dict(hbm=3350.0, tf=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -115,6 +119,16 @@ class ClockSampler:
                 reasons.append(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "power_w": float(np.median(pw)) if pw else None, "reasons": reasons, "samples": len(sm)}
+
+
+def dump_outputs(out_dir: str, **arrays):
+    """Each array (device tensor or host array) as out_dir/<name>.npy in float64 (slot ids and counts are exact in
+    float64)."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy() if hasattr(t, "detach") else np.asarray(t)
+        np.save(d / f"{name}.npy", a.astype(np.float64))
 
 
 def gen_shard(ix, lo: int, hi: int, d: int, device):
@@ -318,9 +332,9 @@ def run_workload(ctx, args, name, wl, main: bool, steps: int):
     t_region0 = time.monotonic()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     # timing rule: inputs larger than L2, or L2 flushed between timed iterations.  A shard that could stay
-    # (partly) resident in the 126 MB L2 is timed step by step with a 256 MB memset between steps (outside
+    # (partly) resident in the 50 MB L2 is timed step by step with a 256 MB memset between steps (outside
     # the events); the large workloads stream far more than L2 per step and are timed as one region.
-    l2_flush = 2.0 * (hi - lo) * d < 4 * 126e6
+    l2_flush = 2.0 * (hi - lo) * d < 4 * L2_BYTES
     flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=device) if l2_flush else None
     if l2_flush:
         ms = 0.0
@@ -328,7 +342,7 @@ def run_workload(ctx, args, name, wl, main: bool, steps: int):
             with torch.cuda.stream(stream):
                 flush_buf.zero_()
                 ev0.record(stream)
-                flags = searcher.search_device_async(q_dev, k_fetch, args.min_score)[3]
+                last = searcher.search_device_async(q_dev, k_fetch, args.min_score)
                 ev1.record(stream)
             stream.synchronize()
             ms += ev0.elapsed_time(ev1)
@@ -338,10 +352,14 @@ def run_workload(ctx, args, name, wl, main: bool, steps: int):
         # are accumulated on the device by the merge kernel and checked once after the region
         ev0.record(stream)
         for _ in range(steps):
-            flags = searcher.search_device_async(q_dev, k_fetch, args.min_score)[3]
+            last = searcher.search_device_async(q_dev, k_fetch, args.min_score)
         ev1.record(stream)
         barrier()
         ms = ev0.elapsed_time(ev1)
+    flags = last[3]
+    if main and rank == 0 and args.dump_outputs:
+        # the searcher reuses its output buffers: copy the last timed step's results before anything else runs
+        dump_outputs(args.dump_outputs, slots=last[0], scores=last[1], counts=last[2])
     dirty = int(flags[-1].item()) - searcher._dirty_seen     # running count of unproven queries (merge kernel)
     searcher._dirty_seen += dirty
     st1 = ix.stats()
@@ -406,20 +424,15 @@ def run_workload(ctx, args, name, wl, main: bool, steps: int):
         tensor_bound = B > pk["tf"] * 1e12 / (pk["hbm"] * 1e9)   # arithmetic intensity ~ B flop/byte vs ridge
         tf = flops / (scan_avg_ms * 1e-3) / 1e12
         gbs = bytes_ / (scan_avg_ms * 1e-3) / 1e9
-        # ONE peak kind at every N: the burst figures of MEASURED_PEAKS.json (the sustained tensor peak alongside)
+        # ONE peak kind at every N: the data-sheet figures of peaks()
         if tensor_bound:
             roof = {"bound": "tensor", "achieved": tf, "peak": pk["tf"], "unit": "TFLOP/s", "frac": tf / pk["tf"],
-                    "peak_kind": "burst", "frac_of_sustained": tf / pk["tf_sus"] if pk["tf_sus"] else None,
-                    "hbm_gbs": gbs}
+                    "peak_kind": "data sheet", "hbm_gbs": gbs}
         else:
             roof = {"bound": "hbm", "achieved": gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": gbs / pk["hbm"],
-                    "peak_kind": "burst", "tflops": tf, "frac_of_tensor_burst": tf / pk["tf"]}
-        roof.update({"kernel": ("scan2_kernel: CTA-pair tcgen05 cta_group::2 QxC^T + fused top-k'" if B > 128
-                                else "scan_kernel: tcgen05 QxC^T + fused top-k'"), "kernel_ms": scan_avg_ms,
-                     "algorithmic_bytes": bytes_, "algorithmic_flops": flops, "peak_source": pk["src"],
-                     # dram bytes per launch of the committed ncu --set full capture of this workload on ONE GPU;
-                     # not measured by this run, and not meaningful for a 1/N shard
-                     "traffic": _profiled_traffic(name) if world == 1 else None})
+                    "peak_kind": "data sheet", "tflops": tf, "frac_of_tensor_peak": tf / pk["tf"]}
+        roof.update({"kernel": "scan_kernel: wgmma QxC^T + fused top-k'", "kernel_ms": scan_avg_ms,
+                     "algorithmic_bytes": bytes_, "algorithmic_flops": flops, "peak_source": pk["src"]})
         res = {
             "value": B * steps / (ms * 1e-3), "unit": "queries/s", "steps": steps, "ms_per_step": ms / steps,
             "config": {"workload": desc + (" [REDUCED rows: debug run]" if ctx.reduced else ""), "n_docs": n, "dim": d,
@@ -429,9 +442,9 @@ def run_workload(ctx, args, name, wl, main: bool, steps: int):
                        "pipelining": ("steps timed one by one (L2 flush between them)" if l2_flush else
                                       "value: steps enqueued back to back, exactness flags checked after the "
                                       "region; e2e: one host synchronisation per step"),
-                       "l2": (f"corpus {2.0 * n_local * d / 1e6:.0f} MB per GPU could stay in the 126 MB L2: L2 flushed "
+                       "l2": (f"corpus {2.0 * n_local * d / 1e6:.0f} MB per GPU could stay in the 50 MB L2: L2 flushed "
                               "(256 MB memset) before every timed step" if l2_flush else
-                              f"corpus {2.0 * n_local * d / 1e9:.1f} GB per GPU >> 126 MB L2, no flush needed"),
+                              f"corpus {2.0 * n_local * d / 1e9:.1f} GB per GPU >> 50 MB L2, no flush needed"),
                        "unproven_queries_in_timed_region": int(dirty),
                        "fallback_queries": int(st2["fallback_queries"]), "retry_batches": int(st2["retry_batches"])},
             "e2e": {"value": B * steps / e2e_s, "unit": "queries/s", "h2d_bytes_per_step": B * d * 4,
@@ -494,6 +507,8 @@ def run_group(args, name, wl, pk, synth, reduced):
     dt = time.perf_counter() - t0
     t_r1 = time.monotonic()
     st1 = grp.stats()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, slots=got[0], scores=got[1], counts=got[2])
     time.sleep(0.05)
     sampler.window(t_r0, t_r1)
     clocks = sampler.stop()
@@ -534,7 +549,7 @@ def run_group(args, name, wl, pk, synth, reduced):
                    "device_ms_per_step": dev_ms / args.steps},
            "gpu_launches": int(st1["kernel_launches"] - st0["kernel_launches"] + args.steps * (1 + G)),
            "roofline": {"bound": "tensor" if B > pk["tf"] * 1e12 / (pk["hbm"] * 1e9) else "hbm",
-                        "kernel_ms_per_device": scan_ms, "unit": "TFLOP/s", "peak": pk["tf"], "peak_kind": "burst",
+                        "kernel_ms_per_device": scan_ms, "unit": "TFLOP/s", "peak": pk["tf"], "peak_kind": "data sheet",
                         "achieved": flops / (max(scan_ms) * 1e-3) / 1e12,
                         "frac": flops / (max(scan_ms) * 1e-3) / 1e12 / pk["tf"], "traffic": None},
            "parity": {"queries": nq, "rows_checked": n, "k_fetch": k_fetch, "id_mismatch": id_mis,
@@ -550,7 +565,7 @@ def cublas_same_box(ix, searcher, q_dev, k_fetch, min_score, n_local, d, B, step
     fp32 accumulate, bf16 out) of the B x d query block against n_local x d rows, in 1M-row pieces, interleaved with
     the scan in two rounds of `steps` passes each.  It only computes the score matrix (and writes it: 2*B bytes per
     row, which the scan never does) - no threshold, no top-k, no exact re-rank - so it is the roof a power-capped
-    scan of this shape can be held against when boxes differ by 18 % on the identical kernel.  Measurement only:
+    scan of this shape can be held against on the same card in the same power state.  Measurement only:
     nothing the product runs goes through it."""
     import torch
     device, stream = q_dev.device, searcher.stream
@@ -568,7 +583,7 @@ def cublas_same_box(ix, searcher, q_dev, k_fetch, min_score, n_local, d, B, step
                 torch.matmul(qb, c[:rest].t(), out=out[:, :rest])
         gemm_pass()
         # the same flops as ONE GEMM with a `full` times deeper K: 1/full of the output bytes, cuBLAS at its best on
-        # this box (what MEASURED_PEAKS.json's sustained figure measures elsewhere)
+        # this card
         deep = full >= 2 and rest == 0 and 2.0 * piece * d * full < 40e9
         if deep:
             c2 = torch.randn(piece, d * full, device=device, dtype=torch.bfloat16)
@@ -654,6 +669,9 @@ def main():
                     help="only the main workload (default: also cfg5 at every N and cfg4 at N=8, in `extra_workloads`)")
     ap.add_argument("--min-score", type=float, default=None,
                     help="cosine threshold (the reference's default is 0.5); default: none (-inf), the headline runs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results of the main workload as DIR/<name>.npy (float64); "
+                         "not with --impl reference")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     wl = list(WORKLOADS[args.workload])
@@ -661,6 +679,8 @@ def main():
     if args.rows:
         wl[0] = args.rows
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs: the reference arm times a CPU sample of the workload, not the engine")
         run_reference(args, wl)
         return
 
@@ -713,14 +733,6 @@ def main():
     if ctx.world > 1:
         dist.barrier()
         dist.destroy_process_group()
-
-
-def _profiled_traffic(workload: str):
-    """dram bytes per scan launch from the committed ncu --set full capture, if any."""
-    p = ROOT / "profiles" / "traffic.json"
-    if p.exists():
-        return json.loads(p.read_text()).get(workload)
-    return None
 
 
 if __name__ == "__main__":

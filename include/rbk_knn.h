@@ -1,5 +1,5 @@
 /*
- * rbk_knn.h — C ABI of the B200-native kNN engine behind RunbookAI's VectorStore.
+ * rbk_knn.h — C ABI of the H100-native kNN engine behind RunbookAI's VectorStore.
  *
  * The reference has no FFI for this path; the seam is the TypeScript class
  * `VectorStore` (src/knowledge/store/vector-store.ts:24-333), whose hot loop is
@@ -216,7 +216,7 @@ typedef struct {
   float last_total_ms;      /* device time of the whole last search */
   int32_t last_kprime;      /* candidates kept per query by the last scan */
   int32_t sm_count;
-  int32_t last_ring_stages; /* smem ring depth of the last scan kernel (pair kernel: 7, or 6 if the smem base is unaligned) */
+  int32_t last_ring_stages; /* smem ring depth of the last scan kernel */
   int32_t retry_batches;    /* batches scanned a second time with the widest candidate margin after a failed proof */
   double scan_ms_total;     /* device time of all scan kernels that have FINISHED so far (CUDA events around every launch) */
   int64_t scans_timed;      /* number of scan launches folded into scan_ms_total */

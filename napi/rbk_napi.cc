@@ -4,7 +4,7 @@
 // next to better-sqlite3.  It has never met real Node; it IS compiled (-Wall -Wextra -Werror), linked
 // against librbk_knn.so and run in the test suite against a mock of the N-API subset it uses
 // (napi/mock/, tests/test_napi_addon.py: every method, the promise / async-work path, every error
-// path, results bit-identical to the oracle on a B200).  Logic-free by design: every method
+// path, results bit-identical to the oracle on an H100).  Logic-free by design: every method
 // maps 1:1 onto a C-ABI call; errors become `new Error(rbk_last_error())` (sync methods
 // throw, `search` rejects its Promise), the convention the reference already follows
 // (vector-store.ts:197-199, embedder.ts:169-171).

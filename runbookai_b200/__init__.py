@@ -1,4 +1,4 @@
-"""runbookai_b200 — B200-native kNN engine behind RunbookAI's knowledge-base vector search.
+"""runbookai_b200 — H100-native kNN engine behind RunbookAI's knowledge-base vector search.
 
 Host-side mirror of the reference interface for this path (the reference is TypeScript;
 Node is absent from the build image, so the mirror is Python over the same C ABI the

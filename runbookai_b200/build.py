@@ -1,7 +1,7 @@
-"""Builds runbookai_b200/lib/librbk_knn.so (hand-written sm_100a CUDA + the C ABI) in-tree.
+"""Builds runbookai_b200/lib/librbk_knn.so (hand-written sm_90a CUDA + the C ABI) in-tree.
 
-nvcc cross-compiles without a GPU, so this runs in the build container; the resulting
-.so travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU, so the library can be built on a machine without one and
+used wherever the tree is copied.
 """
 from __future__ import annotations
 
@@ -13,12 +13,10 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "lib" / "librbk_knn.so"
-SOURCES = ["rbk_capi.cu", "rbk_group.cu", "rbk_scan.cu", "rbk_scan2.cu", "rbk_scan4.cu", "rbk_scan3.cu", "rbk_ingest.cu", "rbk_finalize.cu"]
-# RBK_EXPERIMENTAL=1 in the environment of the BUILD adds -DRBK_EXPERIMENTAL: the measured-and-rejected kernel
-# variants of DESIGN.md §7 and their A/B switches (rbk_scan3.cu is empty without it).  Never set for a release.
+SOURCES = ["rbk_capi.cu", "rbk_group.cu", "rbk_scan.cu", "rbk_ingest.cu", "rbk_finalize.cu"]
 HEADERS = ["rbk_internal.h", "rbk_index_impl.h", "rbk_ptx.cuh", "rbk_epilogue.cuh", "../../include/rbk_knn.h"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-fmad=false",            # fp64 re-rank must never contract a*b+c (parity contract)
     "--extended-lambda",
@@ -46,8 +44,6 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         return LIB
     LIB.parent.mkdir(parents=True, exist_ok=True)
     cmd = [_nvcc(), *NVCC_FLAGS, *[str(CSRC / s) for s in SOURCES], "-o", str(LIB)]
-    if os.environ.get("RBK_EXPERIMENTAL") == "1":
-        cmd.insert(1, "-DRBK_EXPERIMENTAL")
     for flag in os.environ.get("RBK_EXTRA_NVCC_FLAGS", "").split():   # development probes, e.g. -DRBK_FIN_PROFILE
         cmd.insert(1, flag)
     if verbose:

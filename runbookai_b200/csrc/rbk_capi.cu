@@ -251,18 +251,6 @@ rbk_status refresh_corpus_tmap(rbk_index* ix) {
   if (ix->tmap_c_base == ix->rows && ix->tmap_c_rows == map_rows) return RBK_OK;
   rbk_status st = encode_rows_tmap(&ix->tmap_c, ix->rows, map_rows, ix->dpad, kBlockN);
   if (st != RBK_OK) return st;
-  st = encode_rows_tmap(&ix->tmap_c_half, ix->rows, map_rows, ix->dpad, kBlockN / 2);
-  if (st != RBK_OK) return st;
-  st = encode_rows_tmap(&ix->tmap_c_quarter, ix->rows, map_rows, ix->dpad, kBlockN / 4);
-  if (st != RBK_OK) return st;
-#ifdef RBK_EXPERIMENTAL
-  st = encode_rows_tmap(&ix->tmap_c_half32, ix->rows, map_rows, ix->dpad, kBlockN / 2, 32);
-  if (st != RBK_OK) return st;
-  st = encode_rows_tmap(&ix->tmap_c_pf, ix->rows, map_rows, ix->dpad, kBlockN / 2, 256);
-  if (st != RBK_OK) return st;
-  st = encode_rows_tmap(&ix->tmap_c_r32, ix->rows, map_rows, ix->dpad, scan3_box_rows());
-  if (st != RBK_OK) return st;
-#endif
   ix->tmap_c_base = ix->rows;
   ix->tmap_c_rows = map_rows;
   return RBK_OK;
@@ -277,11 +265,10 @@ namespace impl {
 rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem) {
   CK(ix->q_raw.ensure(static_cast<size_t>(B) * ix->dim * elem));
   // rows padded to whole query blocks: the scan's TMA boxes are 128 query rows, and a box that hangs over the end of
-  // the tensor is zero-FILLED by the TMA unit row by row - measured: a B = 1 scan over 1M rows took 0.295 ms against
-  // 0.239 ms at B = 128 for the same bytes.  With the map covering whole blocks the pad rows are ordinary (zeroed
-  // once here) memory; they only ever feed accumulator rows of queries that do not exist.
+  // the tensor is zero-FILLED by the TMA unit row by row, which is slow.  With the map covering whole blocks the pad
+  // rows are ordinary (zeroed once here) memory; they only ever feed accumulator rows of queries that do not exist.
   {
-    const size_t want = static_cast<size_t>(round_up(B, 2 * kBlockM)) * ix->dpad;
+    const size_t want = static_cast<size_t>(round_up(B, kBlockM)) * ix->dpad;
     if (want > ix->q_bf16.n) {
       CK(ix->q_bf16.ensure(want));
       CK(cudaMemsetAsync(ix->q_bf16.p, 0, ix->q_bf16.n * sizeof(uint16_t), ix->stream));
@@ -293,8 +280,8 @@ rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem) {
   CK(ix->q_inv_norm.ensure(B));
   CK(ix->thr_init.ensure(B));
   CK(ix->flags.ensure(B));
-  CK(ix->cand.ensure(static_cast<size_t>(ix->sm_count) * kBlockM * kListCap * kMaxHalves));
-  CK(ix->cand_cnt.ensure(static_cast<size_t>(ix->sm_count) * kBlockM * kMaxHalves));
+  CK(ix->cand.ensure(static_cast<size_t>(ix->sm_count) * kBlockM * kListCap));
+  CK(ix->cand_cnt.ensure(static_cast<size_t>(ix->sm_count) * kBlockM));
   // hist [kMaxSubBatch][kHistBins] | maxbin [kMaxSubBatch] | gthr [kMaxSubBatch] | progress [sm_count + 8]:
   // one buffer, one memset
   CK(ix->hist.ensure(static_cast<size_t>(kMaxSubBatch) * kHistBins + 2 * kMaxSubBatch + ix->sm_count + 8));
@@ -353,52 +340,12 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
   const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
   for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
     const int Bs = std::min(kMaxSubBatch, B - q0);
-    // more than one 128-query block: CTA pairs (256 queries per pair) halve the corpus bytes per query
-    const bool pairs = Bs > kBlockM && !ix->force_1cta;
-    const int block_m = pairs ? 2 * kBlockM : kBlockM;
-    const int QB = (Bs + block_m - 1) / block_m;
-    const int units = pairs ? ix->sm_count / 2 : ix->sm_count;
-    int R = std::max(1, std::min(units / QB, n_tiles));
-    // EXPERIMENTAL builds only (RBK_KNN_CLUSTER4=1): clusters of two pairs, one operand of every k-block multicast
-    // (rbk_scan4.cu) - the kernel whose tensor pipe runs at 97 % - on every SM that can host a 4-CTA cluster (33
-    // clusters = 132 of the 148 SMs of a B200), and CONCURRENTLY the pair kernel (rbk_scan2.cu) on the SMs that
-    // cannot, over its own slice of the corpus.  Measured within 2 % of the pair kernel alone (power-bound), so the
-    // default build launches the pair kernel on all SMs.  An even number of query blocks: the pairs of a cluster
-    // take different blocks and share the corpus tile; odd: same block, alternate tiles, shared query slab.
-#ifdef RBK_EXPERIMENTAL
-    const bool aligned = pairs ? scan_smem_base_is_aligned() : false;
-    const int max_cl = (pairs && ix->cluster4) ? scan4_max_clusters(aligned) : 0;
-#else
-    const int max_cl = 0;
-#endif
-    const bool use4 = max_cl > 0 && n_tiles >= 2;
-    const bool share_c = use4 && (QB % 2) == 0;
-    int RC = 0, R4 = 0, R2 = 0, T2 = 0;   // cluster ranges; list units per query block of each kernel; tiles of the tail
-    if (use4) {
-      const int n_cols = share_c ? QB / 2 : QB;
-      RC = std::max(1, std::min(max_cl / n_cols, share_c ? n_tiles : n_tiles / 2));
-      R4 = share_c ? RC : 2 * RC;
-      // the tail: pairs on the SMs left over, if the scan is long enough to be worth a second launch
-      const int spare_pairs = (ix->sm_count - 4 * RC * n_cols) / 2;
-      R2 = ix->tail_pairs >= 0 ? std::min(ix->tail_pairs, spare_pairs / QB) : spare_pairs / QB;
-      if (n_tiles < 16 * (R4 + R2)) R2 = 0;
-      if (R2 > 0) {
-        // a pair of the tail needs tail_rho x the time of a cluster pair per tile (no multicast: 82 % vs 97 % tensor
-        // duty): tiles in proportion to capacity, so that both launches finish together
-        const double cap4 = R4, cap2 = R2 / ix->tail_rho;
-        T2 = static_cast<int>(n_tiles * cap2 / (cap4 + cap2) + 0.5);
-        if (T2 < R2) R2 = T2 = 0;
-      }
-      R = R4 + R2;
-    }
-    CUtensorMap tmap_q, tmap_q64;
-    const int q_rows = static_cast<int>(round_up(Bs, block_m));   // whole query blocks: no out-of-bounds box rows
+    const int QB = (Bs + kBlockM - 1) / kBlockM;
+    const int R = std::max(1, std::min(ix->sm_count / QB, n_tiles));
+    CUtensorMap tmap_q;
+    const int q_rows = static_cast<int>(round_up(Bs, kBlockM));   // whole query blocks: no out-of-bounds box rows
     st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM);
     if (st != RBK_OK) return st;
-    if (use4) {   // (never in the default build)
-      st = encode_rows_tmap(&tmap_q64, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM / 2);
-      if (st != RBK_OK) return st;
-    }
     ScanParams sp;
     sp.inv_norm_c = ix->inv_norm;
     sp.thr_init = ix->thr_init.p + q0;
@@ -421,77 +368,15 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
     sp.n_rows = static_cast<int>(ix->n_rows);
     sp.B = Bs;
     sp.kprime = kprime;
-    sp.num_kb = (ix->dpad + kBlockK - 1) / kBlockK;
     sp.dpad = ix->dpad;
+    sp.max_lead_tiles = ix->max_lead_tiles;
     sp.QB = QB;
     sp.R = R;
-    sp.RC = RC;
     sp.n_tiles = n_tiles;
-    sp.tile_begin = 0;
-    sp.tile_count = n_tiles - T2;
-    sp.R_local = R;
-    sp.unit_base = 0;
-    sp.prog_base = 0;
     cudaEvent_t* tev = ix->capturing ? nullptr : next_scan_events(ix);
     if (tev) CK(cudaEventRecord(tev[0], ix->stream));
-    sp.prefetch_tiles = ix->prefetch_tiles;
-    sp.perf_probe = ix->perf_probe;
-    sp.max_lead_tiles = ix->max_lead_tiles;
-#ifdef RBK_EXPERIMENTAL
-    const bool resident = pairs && !ix->force_streamed && scan2_resident_fits(ix->dpad);
-    const bool ts = pairs && ix->use_ts && scan3_fits(ix->dpad);
-#else
-    const bool resident = false, ts = false;
-#endif
-    // lists per (unit, query): the default pair kernel splits every tile between two sets of epilogue warps
-    // Eight epilogue warps (two lists per unit and query): measured in one box against four, +7-10 % at
-    // B=256 up to 1M rows and +10-17 % at B=1024 up to 0.5M rows (where the filter is busy: thresholds still
-    // rising, appends frequent), +-1 % on long scans (cfg3).  RBK_KNN_HALVES=1 forces the narrow epilogue.
-    int halves = 1;
-    if (pairs && !ts && ix->hybrid_res_kb < 0) {
-      halves = ix->epi_halves > 0 ? std::min(ix->epi_halves, kMaxHalves) : kMaxHalves;
-    }
-    // Start-up seeds (rbk_epilogue.cuh): two per thread and tile when many units feed one query's histogram
-    // (>= 4 k' seeds in total) - pair kernel only: measured in one box, B=256 scans 2 % (1M rows) to 9 % (65k
-    // rows) faster than with two seeds per 32-column chunk, but the 1-CTA kernel at B=1 became bimodal (0.03 /
-    // 0.07 ms at 65k rows): with one or two tiles per unit and only two seeds from each, a unit that reads the
-    // histogram before ~k'/2 peers have seeded finds no threshold and floods its lists.
-    sp.seed_tile = ix->seed_tile >= 0 ? ix->seed_tile : ((pairs && R * 2 * halves >= 4 * kprime) ? 1 : 0);
-#ifdef RBK_EXPERIMENTAL
-    if (use4) {
-      if (R2 > 0) CK(cudaEventRecord(ix->ev_fork, ix->stream));   // scratch zeroed, queries prepared
-      CK(launch_scan4(tmap_q, tmap_q64, ix->tmap_c_half, ix->tmap_c_quarter, sp, share_c, aligned, ix->stream,
-                      &ix->stats.last_ring_stages));
-      if (R2 > 0) {
-        // launched SECOND, on its own stream: the cluster kernel's CTAs are placed first, the tail's pairs land on
-        // the SMs no 4-CTA cluster fits on.  (Were they ever placed the other way round the result would still be
-        // right - the kernels only exchange lower bounds - just slower.)
-        ScanParams st2 = sp;
-        st2.tile_begin = n_tiles - T2;
-        st2.tile_count = T2;
-        st2.R_local = R2;
-        st2.unit_base = R4;
-        st2.prog_base = RC * (share_c ? QB / 2 : QB);
-        CK(cudaStreamWaitEvent(ix->side_stream, ix->ev_fork, 0));
-        CK(launch_scan2(tmap_q, ix->tmap_c_half, ix->tmap_c_half, st2, false, halves, ix->side_stream, nullptr));
-        CK(cudaEventRecord(ix->ev_join, ix->side_stream));
-        CK(cudaStreamWaitEvent(ix->stream, ix->ev_join, 0));
-        ix->stats.kernel_launches++;
-      }
-    } else if (pairs && !ts && ix->hybrid_res_kb >= 0)
-      CK(launch_scan2h(tmap_q, ix->tmap_c_half, sp, ix->hybrid_res_kb, ix->hybrid_slots, ix->stream));
-    else if (ts)
-      CK(launch_scan3(ix->tmap_c_r32, sp, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, ix->stream));
-    else if (pairs)
-      CK(launch_scan2(tmap_q, (resident && scan2_resident_k() == 32) ? ix->tmap_c_half32 : ix->tmap_c_half,
-                      ix->tmap_c_pf, sp, resident, halves, ix->stream, &ix->stats.last_ring_stages));
-    else CK(launch_scan(tmap_q, ix->tmap_c, sp, ix->stream));
-#else
-    if (pairs)
-      CK(launch_scan2(tmap_q, ix->tmap_c_half, ix->tmap_c_half, sp, false, halves, ix->stream,
-                      &ix->stats.last_ring_stages));
-    else CK(launch_scan(tmap_q, ix->tmap_c, sp, ix->stream));
-#endif
+    CK(launch_scan(tmap_q, ix->tmap_c, sp, ix->stream));
+    ix->stats.last_ring_stages = kStages;
     if (tev) CK(cudaEventRecord(tev[1], ix->stream));
     ix->stats.scan_launches++;
     ix->stats.kernel_launches++;
@@ -500,14 +385,14 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
       fp.cand = ix->cand.p;
       fp.cand_cnt = ix->cand_cnt.p;
       fp.QB = QB;
-      fp.R = R * halves;   // finalize sees every list as a unit of its own
+      fp.R = R;
       fp.kprime = kprime;
       fp.k_fetch = k_fetch;
       fp.B = Bs;
       fp.d = ix->dim;
       fp.dpad = ix->dpad;
       fp.q0 = q0;
-      fp.block_m = block_m;
+      fp.block_m = kBlockM;
       fp.min_score = min_score;
       fp.rows = ix->rows;
       fp.rows_f64 = ix->rows_f64;
@@ -737,7 +622,7 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
   std::vector<int> fails;
   for (int b = 0; b < B; ++b)
     if (h_flags[b]) fails.push_back(b);
-  if (!fails.empty() && ix->retry_wide && ix->stats.last_kprime < kMaxKPrime) {
+  if (!fails.empty() && ix->stats.last_kprime < kMaxKPrime) {
     // A proof fails when more rows tie with the k_fetch-th hit (within the scan's error bound) than the
     // candidate margin holds - duplicated chunks, typically.  Before paying an exhaustive fp64 pass per failing
     // query, scan the batch once more at scan speed with the widest margin (k' = 128): groups of up to ~100
@@ -803,50 +688,25 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
   if (device < 0 || device >= ndev) return fail(RBK_EINVAL, "device ordinal out of range");
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(RBK_ECUDA, std::string("this build targets sm_100a (Blackwell B200); device is ") + prop.name);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(RBK_ECUDA, std::string("this build targets sm_90a (Hopper H100); device is ") + prop.name);
   DeviceGuard dg(device);
   rbk_index* ix = new (std::nothrow) rbk_index();
   if (!ix) return fail(RBK_ENOMEM, "out of host memory");
   ix->dim = dim;
-  // row pitch = whole 64-element k-blocks (128 bytes): no TMA box hangs over the end of a row either
-  ix->dpad = static_cast<int>(round_up(dim, kBlockK));
+  // row pitch = whole 128-byte lines (pairs of 32-element k-blocks): no TMA box hangs over the end of a row either
+  ix->dpad = static_cast<int>(round_up(dim, 2 * kBlockK));
   ix->device = device;
   ix->keep_f64 = (flags & RBK_INDEX_KEEP_F64) != 0;
   ix->sm_count = prop.multiProcessorCount;
   memset(&ix->stats, 0, sizeof ix->stats);
   ix->stats.sm_count = ix->sm_count;
-#ifdef RBK_EXPERIMENTAL   // A/B switches of development builds; the shipped library reads no environment
-  if (const char* m = getenv("RBK_KNN_CLUSTER4")) ix->cluster4 = atoi(m);
-  if (const char* m = getenv("RBK_KNN_GRAPH")) ix->use_graph = atoi(m) != 0;
-  if (const char* m = getenv("RBK_KNN_TAIL_PAIRS")) ix->tail_pairs = atoi(m);
-  if (const char* m = getenv("RBK_KNN_TAIL_RHO")) ix->tail_rho = std::max(0.5, std::min(3.0, atof(m)));
-  if (const char* m = getenv("RBK_KNN_MARGIN")) ix->margin = std::max(0, std::min(96, atoi(m)));
-  if (const char* m = getenv("RBK_KNN_FORCE_1CTA")) ix->force_1cta = atoi(m) != 0;
-  if (const char* m = getenv("RBK_KNN_RESIDENT")) ix->force_streamed = atoi(m) == 0;
-  if (const char* m = getenv("RBK_KNN_TS")) ix->use_ts = atoi(m) != 0;
-  if (const char* m = getenv("RBK_KNN_MAX_LEAD")) ix->max_lead_tiles = std::max(1, atoi(m));
-  if (const char* m = getenv("RBK_KNN_SEED_TILE")) ix->seed_tile = atoi(m);
-  if (const char* m = getenv("RBK_KNN_RETRY_WIDE")) ix->retry_wide = atoi(m) != 0;
-  if (const char* m = getenv("RBK_KNN_HALVES")) ix->epi_halves = std::max(0, atoi(m));
-  if (const char* m = getenv("RBK_KNN_PERF_PROBE")) ix->perf_probe = atoi(m);   // breaks results; timing only
-  if (const char* m = getenv("RBK_KNN_HYBRID_KB")) ix->hybrid_res_kb = atoi(m);
-  if (const char* m = getenv("RBK_KNN_HYBRID_SLOTS")) ix->hybrid_slots = atoi(m);
-  if (const char* m = getenv("RBK_KNN_PREFETCH_TILES")) ix->prefetch_tiles = std::max(0, std::min(64, atoi(m)));
-#endif
   e = cudaStreamCreateWithFlags(&ix->own_stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) {
     delete ix;
     return cuda_fail(e, "cudaStreamCreate");
   }
   ix->stream = ix->own_stream;
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ix->side_stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ix->ev_fork, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ix->ev_join, cudaEventDisableTiming);
-  if (e != cudaSuccess) {
-    rbk_index_destroy(ix);
-    return cuda_fail(e, "cudaStreamCreate");
-  }
   e = cudaMalloc(reinterpret_cast<void**>(&ix->d_counter), 2 * sizeof(int));
   if (e == cudaSuccess) e = cudaMemset(ix->d_counter, 0, 2 * sizeof(int));
   if (e != cudaSuccess) {
@@ -909,12 +769,6 @@ void rbk_index_destroy(rbk_index* ix) {
     for (auto& pr : ix->tev)
       for (cudaEvent_t e : pr)
         if (e) cudaEventDestroy(e);
-    if (ix->side_stream) {
-      cudaStreamSynchronize(ix->side_stream);
-      cudaStreamDestroy(ix->side_stream);
-    }
-    if (ix->ev_fork) cudaEventDestroy(ix->ev_fork);
-    if (ix->ev_join) cudaEventDestroy(ix->ev_join);
     if (ix->own_stream) cudaStreamDestroy(ix->own_stream);
   }
   delete ix;

@@ -14,9 +14,6 @@
 #include "rbk_internal.h"
 #include "rbk_ptx.cuh"
 
-#ifdef RBK_EPI_PROFILE
-#include <cstdio>
-#endif
 namespace rbk {
 
 struct FilterState {
@@ -27,7 +24,6 @@ struct FilterState {
   int mb_cache;    // highest bin this thread already published to maxbin
   int cnt;         // entries in the list
   bool valid;
-  int probe;       // timing experiments only (ScanParams::perf_probe)
   bool nohist;     // appends are not counted in the histogram (second pass over a seeded tile)
   unsigned long long* list;
   unsigned int* hist_q;  // [kHistBins]
@@ -53,7 +49,6 @@ __device__ __forceinline__ void filter_init(FilterState& s, bool valid, float th
   s.qn = s.valid ? 1.0f / inv_q : 0.f;
   s.tb = (s.valid && thr_init > -INFINITY) ? score_bin(thr_init * inv_q) : -1;
   s.mb_cache = -1;
-  s.probe = 0;
   s.nohist = false;
   s.cnt = 0;
   s.list = list;
@@ -62,11 +57,10 @@ __device__ __forceinline__ void filter_init(FilterState& s, bool valid, float th
 }
 
 // Raise thr from the global histogram (source 3).  Per-thread, no warp collectives.
-// Bins are fetched 16 at a time (four independent 16-byte L2 loads in flight): a dependent chain
-// of single loads cost ~0.7 us per 4 bins and made this function 23 % of the epilogue's time.
-// The walk is out of line (it is long and rare) and takes / returns SCALARS: handing it the FilterState by
-// reference forced the whole struct into local memory, and the hot loop then paid a local store per tile
-// (8.5 % of the warp samples of profiles/r01_scan_cfg3_final2.txt sat on `STL [R1+0x8]`).
+// Bins are fetched 16 at a time (four independent 16-byte L2 loads in flight) rather than as a dependent chain
+// of single loads.  The walk is out of line (it is long and rare) and takes / returns SCALARS: handing it the
+// FilterState by reference would force the whole struct into local memory and cost the hot loop a local store
+// per tile.
 // Returns 0 if no bin edge with >= k' rows at or above it exists above bin `tb`; else (bin << 32) | raw-threshold bits.
 static __device__ __noinline__ unsigned long long histogram_walk(const unsigned int* hist_q, int mb, int tb, float qn,
                                                                   int kprime) {
@@ -95,7 +89,7 @@ static __device__ __noinline__ unsigned long long histogram_walk(const unsigned 
   return 0ull;
 }
 __device__ __forceinline__ bool filter_refresh(FilterState& s, int kprime) {
-  if (!s.valid || (kExperimental && s.probe == 3)) return false;
+  if (!s.valid) return false;
   const int mb = __ldcg(s.maxbin_q);
   if (mb <= s.tb) return false;
   const unsigned long long r = histogram_walk(s.hist_q, mb, s.tb, s.qn, kprime);
@@ -157,14 +151,14 @@ __device__ __forceinline__ void hist_add(FilterState& s, float t) {
 __device__ __forceinline__ void filter_append(FilterState& s, float t, uint32_t row) {
   s.list[s.cnt] = pack_key(t, row);
   ++s.cnt;
-  if (s.nohist || (kExperimental && s.probe == 3)) return;
+  if (s.nohist) return;
   hist_add(s, t);
 }
 
 // Seeding pass over a unit's FIRST tile.  With no threshold yet, the plain filter appends (and counts) every
-// row it sees until the histogram holds k' rows: measured on B200, those few hundred appends per thread cost
-// 50-100 k cycles per unit (scattered 8-byte stores plus ~5 k atomics per query landing on the same three or
-// four histogram lines from every SM at once) - 80 us of fixed cost per search.  Instead the first tile is
+// row it sees until the histogram holds k' rows: a few hundred appends per thread (scattered 8-byte stores plus
+// thousands of atomics per query landing on the same few histogram lines from every SM at once), a fixed cost
+// of every search.  Instead the first tile is
 // read twice: this pass only counts the two best group maxima of every 32-column chunk (two distinct rows,
 // 16 per unit and tile, which is where the query's best rows so far are with overwhelming probability), all
 // units' seeds then give the threshold, and the regular pass over the same accumulators appends the handful
@@ -214,10 +208,6 @@ __device__ __forceinline__ void filter_chunk(FilterState& s, const uint32_t (&v)
     const float a3 = __uint_as_float(v[4 * j + 3]) * w.w;
     g[j] = fmaxf(fmaxf(a0, a1), fmaxf(a2, a3));   // fmaxf drops NaN (dead / out-of-range rows)
     m = fmaxf(m, g[j]);
-  }
-  if (kExperimental && s.probe == 2) {   // probe: fast path only
-    if (m == 12345.678f) s.cnt = 1;
-    return;
   }
   if (m > s.thr) {
     // Rare per LANE but not per WARP while thresholds are still converging (1024 (query,row) pairs per warp
@@ -322,151 +312,88 @@ __device__ __forceinline__ void filter_compact_if_needed(FilterState& s, int kpr
 }
 
 
-// The whole epilogue role (thread <-> query) shared by the scan kernels.  kPair: CTA-pair kernels (256-query
-// blocks, remote arrive on the leader's tmem_empty barrier).  invc: per-accumulator-stage staging of the
-// tile's 1/||c||.
-// kHalves = 1: 4 warps, each thread filters all 256 columns of a tile for its query.
-// kHalves = 2: 8 warps (warps 2-5 take columns 0-127, warps 6-9 columns 128-255; a warp may only read the
-// TMEM lane quadrant warp%4, which both sets cover), every thread with its own candidate list - to the
-// finalize kernel a unit simply looks like two.  One epilogue warp per SM sub-partition is latency-bound
-// (~0.15 IPC: dependent TMEM-load / multiply / max chains and divergent append blocks with nothing to
-// overlap them); two per sub-partition hide each other's latencies and halve the per-tile work of each.
-// Tile sequence of a unit: tile(it) = t0 + it * t_step for it in [0, n_iter); a tile index >= t1 is a PHANTOM
-// (the cluster kernel keeps its two pairs in step when a range has an odd number of tiles): it is redirected to
-// tile p.n_tiles, whose rows lie beyond n_rows - TMA zero-fills them, their 1/||c|| is the NaN padding of the norm
-// array, so nothing is ever appended from it.
-template <bool kPair, int kHalves = 1>
+// Floats per row of the CTA's score buffer: 4 more than a tile row so that the 8 threads of a quarter warp, which
+// read 16 bytes of 8 consecutive rows, hit 8 different groups of 4 banks.
+constexpr int kScorePitch = kBlockN + 4;
+
+// 32 consecutive scores of one row of the score buffer.
+__device__ __forceinline__ void load_chunk(const float* src, uint32_t (&v)[32]) {
+  const float4* s4 = reinterpret_cast<const float4*>(src);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 w = s4[j];
+    v[4 * j + 0] = __float_as_uint(w.x);
+    v[4 * j + 1] = __float_as_uint(w.y);
+    v[4 * j + 2] = __float_as_uint(w.z);
+    v[4 * j + 3] = __float_as_uint(w.w);
+  }
+}
+
+// The whole epilogue role (thread <-> query) of the scan kernel: 128 threads (four warps), thread et filters the
+// kBlockN scores of query row et of every tile of its unit [t0, t1).  scores: the CTA's score buffer (kBlockM rows of
+// kScorePitch floats), filled by the wgmma warpgroups; sc_full / sc_empty hand it back and forth.  invc_stage: per-tile
+// staging of the tile's 1/||c||, double-buffered by tile parity.
 __device__ __forceinline__ void run_epilogue(const ScanParams& p, float (*invc_stage)[kBlockN],
-                                             unsigned long long* tmem_full, unsigned long long* tmem_empty,
-                                             uint32_t tmem_base, int qb, int r, uint32_t rank, int t0, int t1,
-                                             int warp, int lane, int t_step = 1, int n_iter = -1) {
-  if (n_iter < 0) n_iter = t1 - t0;
-  auto tile_of = [&](int it) {
-    const int t = t0 + it * t_step;
-    return t < t1 ? t : p.n_tiles;
-  };
-  constexpr int kEpi = 128 * kHalves;
-  constexpr int kBlockQ = kPair ? 2 * kBlockM : kBlockM;
-  constexpr int kCols = kBlockN / kHalves;          // columns of a tile this thread filters
-  const int half = kHalves == 2 ? ((warp - 2) >> 2) : 0;
-  const int col0 = half * kCols;
-  const int quad = warp & 3;            // TMEM lane quadrant this warp may read
-  const int qrow = quad * 32 + lane;    // TMEM lane
-  const int qin = (kPair ? static_cast<int>(rank) * kBlockM : 0) + qrow;   // row inside the query block
-  const int q = qb * kBlockQ + qin;
+                                             unsigned long long* sc_full, unsigned long long* sc_empty,
+                                             const float* scores, int qb, int r, int t0, int t1, int et, int lane) {
+  constexpr int kEpi = kBlockM;
+  const int q = qb * kBlockM + et;
   const bool q_valid = q < p.B;
-  const int et = threadIdx.x - 64;      // 0..kEpi-1
-  const size_t list_id = static_cast<size_t>((qb * p.R + r) * kHalves + half) * kBlockQ + qin;
+  const size_t list_id = static_cast<size_t>(qb * p.R + r) * kBlockM + et;
   FilterState fs;
   filter_init(fs, q_valid, q_valid ? p.thr_init[q] : INFINITY, q_valid ? p.inv_norm_q[q] : 0.f,
               p.cand + list_id * static_cast<size_t>(kListCap),
               p.hist + static_cast<size_t>(q_valid ? q : 0) * kHistBins, p.maxbin + (q_valid ? q : 0));
-  fs.probe = kExperimental ? p.perf_probe : 0;
-#ifdef RBK_EPI_PROFILE   // cycle breakdown of one epilogue thread per CTA (development builds only)
-  long long c_wait = 0, c_chunk = 0, c_compact = 0, c_pub = 0, c_bar = 0, c_seed = 0;
-  long long c_tile[4] = {0, 0, 0, 0}, c_sub[4] = {0, 0, 0, 0};
-  int n_tile[4] = {0, 0, 0, 0};
-  const long long c_begin = clock64();
-#define RBK_PROF(var, ...) { const long long t_ = clock64(); __VA_ARGS__; var += clock64() - t_; }
-#else
-#define RBK_PROF(var, ...) { __VA_ARGS__; }
-#endif
-  int as = 0;
-  uint32_t aph = 0;
+  const int n_iter = t1 - t0;
   // 1/||c|| of a tile's 256 rows are staged in shared memory behind one barrier of all epilogue threads per
   // tile (the warps wait there for the slowest of the previous tile); the NEXT tile's values travel in registers
-  // while this one is processed, which hides their L2/HBM latency.  -DRBK_NORMS_L1 builds the alternative that
-  // was tried to get rid of the barrier - every warp reads the norms straight from the array through L1 with
-  // uniform 16-byte loads, next tile prefetched - and measured 15-25 % SLOWER on B200 (cfg2 scan 0.34 -> 0.42 ms,
-  // B=1024 x 4M rows 4.87 -> 5.43 ms): the L1 round trip of 8 loads per chunk costs more than the barrier wait.
-#ifndef RBK_NORMS_L1
-  constexpr bool kGN = false;
+  // while this one is processed, which hides their L2/HBM latency.
   float nx0 = 0.f, nx1 = 0.f;
-#else
-  constexpr bool kGN = true;
-  (void)invc_stage;
-#endif
   unsigned int* gthr_q = p.gthr + (q_valid ? q : 0);
   unsigned int ngt = 0u;   // published threshold, fetched one tile ahead
   if (n_iter > 0) {
-#ifndef RBK_NORMS_L1
-    nx0 = __ldg(p.inv_norm_c + tile_of(0) * kBlockN + et);
-    if (kHalves == 1) nx1 = __ldg(p.inv_norm_c + tile_of(0) * kBlockN + kEpi + et);
-#else
-    if (lane < kBlockN / 32) prefetch_l1(p.inv_norm_c + static_cast<size_t>(tile_of(0)) * kBlockN + lane * 32);
-#endif
+    nx0 = __ldg(p.inv_norm_c + t0 * kBlockN + et);
+    nx1 = __ldg(p.inv_norm_c + t0 * kBlockN + kEpi + et);
   }
+  const float* srow = scores + et * kScorePitch;
   for (int it = 0; it < n_iter; ++it) {
-    const int tile = tile_of(it);
+    const int tile = t0 + it;
     const int row0 = tile * kBlockN;
-#ifndef RBK_NORMS_L1
-    float* invc = invc_stage[as];
+    float* invc = invc_stage[it & 1];
     invc[et] = nx0;
-    if (kHalves == 1) invc[kEpi + et] = nx1;
+    invc[kEpi + et] = nx1;
     if (it + 1 < n_iter) {
-      nx0 = __ldg(p.inv_norm_c + tile_of(it + 1) * kBlockN + et);
-      if (kHalves == 1) nx1 = __ldg(p.inv_norm_c + tile_of(it + 1) * kBlockN + kEpi + et);
+      nx0 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + et);
+      nx1 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + kEpi + et);
     }
-#else
-    const float* invc = p.inv_norm_c + static_cast<size_t>(row0);
-    if (it + 1 < n_iter && lane < kBlockN / 32)
-      prefetch_l1(p.inv_norm_c + static_cast<size_t>(tile_of(it + 1)) * kBlockN + lane * 32);
-#endif
     adopt_threshold(fs, ngt);
     ngt = __ldcg(gthr_q);
-#ifndef RBK_NORMS_L1
-    RBK_PROF(c_bar, named_bar_sync(1, kEpi));
-#endif
-    RBK_PROF(c_pub, if (publish_due(it) && r == it % p.R && half == 0) publish_threshold(fs, gthr_q, p.kprime));   // overlaps this tile's MMAs
-    RBK_PROF(c_wait, mbar_wait(smem_u32(&tmem_full[as]), aph));
-    tc_fence_after();
-    // Two chunks in flight: the TMEM load of the next 32 columns is issued before the current 32 are
-    // filtered, so its latency overlaps the arithmetic (one epilogue warp per SM sub-partition is
-    // latency-bound: ~1000 cycles per chunk measured with load -> wait -> compute in sequence).
-    const uint32_t tcol =
-        tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + static_cast<uint32_t>(as * kBlockN + col0);
+    named_bar_sync(1, kEpi);
+    if (publish_due(it) && r == it % p.R) publish_threshold(fs, gthr_q, p.kprime);   // overlaps this tile's wgmma
+    mbar_wait(smem_u32(sc_full), static_cast<uint32_t>(it & 1));
     auto process = [&](uint32_t (&v)[32], int chunk) {
-      if (kExperimental && p.perf_probe == 1) {   // timing probe: keep the TMEM traffic, drop the arithmetic
-        if (v[0] == 0x7FC12345u) fs.cnt = 1;
-        return;
-      }
-      filter_chunk<kGN>(fs, v, invc + col0 + chunk * 32, static_cast<uint32_t>(row0 + col0 + chunk * 32));
+      filter_chunk(fs, v, invc + chunk * 32, static_cast<uint32_t>(row0 + chunk * 32));
       if (p.dbg_scores != nullptr && q_valid) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-          const int row = row0 + col0 + chunk * 32 + j;
+          const int row = row0 + chunk * 32 + j;
           if (row < p.n_rows)
-            p.dbg_scores[static_cast<size_t>(q) * p.n_rows + row] =
-                __uint_as_float(v[j]) * invc[col0 + chunk * 32 + j];
+            p.dbg_scores[static_cast<size_t>(q) * p.n_rows + row] = __uint_as_float(v[j]) * invc[chunk * 32 + j];
         }
       }
     };
     uint32_t va[32], vb[32];
-    if (it == 0 && (!kExperimental || p.perf_probe == 0)) {
+    if (it == 0) {
       // seeding pass (see seed_chunk): count the best rows of this tile, then take the threshold they give
-#ifdef RBK_EPI_PROFILE
-      const long long t_seed = clock64();
-#endif
-      const bool seed_tile = p.seed_tile != 0;
       float sa1 = -INFINITY, sa2 = -INFINITY;
-      tmem_ld_32x32b_x32(tcol, va);
 #pragma unroll 1
-      for (int c2 = 0; c2 < kCols / 64; ++c2) {
-        tmem_wait_ld_dep(va);
-        tmem_ld_32x32b_x32(tcol + static_cast<uint32_t>((2 * c2 + 1) * 32), vb);
-        seed_chunk<kGN>(fs, va, invc + col0 + (2 * c2) * 32, seed_tile, sa1, sa2);
-        tmem_wait_ld_dep(vb);
-        if (c2 + 1 < kCols / 64) tmem_ld_32x32b_x32(tcol + static_cast<uint32_t>((2 * c2 + 2) * 32), va);
-        seed_chunk<kGN>(fs, vb, invc + col0 + (2 * c2 + 1) * 32, seed_tile, sa1, sa2);
-      }
-      if (seed_tile) {
-        if (sa1 > fs.thr) hist_add(fs, sa1);
-        if (sa2 > fs.thr) hist_add(fs, sa2);
+      for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
+        load_chunk(srow + chunk * 32, va);
+        seed_chunk(fs, va, invc + chunk * 32, false, sa1, sa2);
       }
       // the other units' seeds land within a microsecond or so of ours: a few short retries when the
       // histogram cannot hold k' rows yet but soon will
-      const int seeds_per_unit = seed_tile ? 2 * kHalves : 16;
-      const int tries = (p.R * seeds_per_unit >= 2 * p.kprime) ? 6 : 1;
+      const int tries = (p.R * 16 >= 2 * p.kprime) ? 6 : 1;
       for (int t = 0; t < tries; ++t) {
         const bool found = filter_refresh(fs, p.kprime);
         if (__all_sync(0xFFFFFFFFu, found || !fs.valid)) break;
@@ -474,53 +401,21 @@ __device__ __forceinline__ void run_epilogue(const ScanParams& p, float (*invc_s
       }
       if (fs.valid && fs.thr > -INFINITY) atomicMax(gthr_q, f32_ordered(fs.thr));
       fs.nohist = true;
-#ifdef RBK_EPI_PROFILE
-      c_seed += clock64() - t_seed;
-#endif
     }
-    tmem_ld_32x32b_x32(tcol, va);
 #pragma unroll 1
-    for (int c2 = 0; c2 < kCols / 64; ++c2) {
-#ifdef RBK_EPI_PROFILE
-      const long long c_before = c_chunk;
-#endif
-      RBK_PROF(c_chunk,
-        tmem_wait_ld_dep(va);
-        tmem_ld_32x32b_x32(tcol + static_cast<uint32_t>((2 * c2 + 1) * 32), vb);
-        process(va, 2 * c2);
-        tmem_wait_ld_dep(vb);
-        if (c2 + 1 < kCols / 64) tmem_ld_32x32b_x32(tcol + static_cast<uint32_t>((2 * c2 + 2) * 32), va);
-        process(vb, 2 * c2 + 1));
-#ifdef RBK_EPI_PROFILE
-      c_tile[it < 3 ? it : 3] += c_chunk - c_before;
-      if (it == 0) c_sub[c2] = c_chunk - c_before;
-      n_tile[it < 3 ? it : 3] = fs.cnt;
-#endif
-      RBK_PROF(c_compact, filter_compact_if_needed(fs, p.kprime, lane, 64));
+    for (int c2 = 0; c2 < kBlockN / 64; ++c2) {
+      load_chunk(srow + (2 * c2) * 32, va);
+      load_chunk(srow + (2 * c2 + 1) * 32, vb);
+      process(va, 2 * c2);
+      process(vb, 2 * c2 + 1);
+      filter_compact_if_needed(fs, p.kprime, lane, 64);
       // seeding found nothing (too few units, or their seeds were late): keep looking while the tile is filtered
       if (it == 0 && fs.valid && fs.thr == -INFINITY) adopt_threshold(fs, __ldcg(gthr_q));
     }
     fs.nohist = false;
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) {
-      if (kPair) mbar_arrive_leader(smem_u32(&tmem_empty[as]));
-      else mbar_arrive(smem_u32(&tmem_empty[as]));
-    }
-    as ^= 1;
-    if (as == 0) aph ^= 1u;
+    mbar_arrive(smem_u32(sc_empty));
   }
   p.cand_cnt[list_id] = fs.cnt;
-#ifdef RBK_EPI_PROFILE
-  if (et == 0 && (r == 0 || r == 1 || r == p.R - 1) && qb == 0 && rank == 0)
-    printf("[epi r=%d tiles=%d] total %lld  bar %lld  publish %lld  wait_full %lld  chunks %lld  compact %lld  seed %lld  cnt %d\n", r,
-           t1 - t0, clock64() - c_begin, c_bar, c_pub, c_wait, c_chunk, c_compact, c_seed, fs.cnt);
-  if (et == 0 && (r == 0 || r == 1 || r == p.R - 1) && qb == 0 && rank == 0)
-    printf("[epi r=%d] tile0 %lld (%lld %lld %lld %lld) cnt %d | tile1 %lld cnt %d | tile2 %lld cnt %d | rest %lld cnt %d\n", r,
-           c_tile[0], c_sub[0], c_sub[1], c_sub[2], c_sub[3], n_tile[0], c_tile[1], n_tile[1], c_tile[2], n_tile[2],
-           c_tile[3], n_tile[3]);
-#endif
-#undef RBK_PROF
 }
 
 // Bounded-lag lockstep of the QB producers that stream the same corpus range: nobody runs

@@ -106,22 +106,9 @@ struct rbk_index {
   rbk::impl::PinBuf<long long> h_slots;
   rbk::impl::PinBuf<double> h_scores;
   rbk::impl::PinBuf<float> h_f32;
-  CUtensorMap tmap_c, tmap_c_half, tmap_c_quarter, tmap_c_half32, tmap_c_pf, tmap_c_r32;
-  int cluster4 = 0;          // EXPERIMENTAL builds: clusters of two CTA pairs with one operand multicast (rbk_scan4.cu)
-  int tail_pairs = -1;       // pairs per query block of the concurrent pair-kernel tail (-1 = every spare SM pair)
-  double tail_rho = 1.15;    // per-tile time of a tail pair relative to a cluster pair (split of the corpus)
-  cudaStream_t side_stream = nullptr;   // the tail's stream, forked from / joined to `stream` with events
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  int perf_probe = 0;
+  CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
-  int seed_tile = -1;        // -1 = by unit count; RBK_KNN_SEED_TILE=0|1 forces
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
-  bool retry_wide = true;    // RBK_KNN_RETRY_WIDE=0: failed proofs go straight to the exhaustive kernel
-  int epi_halves = 0;        // 0 = default (2); RBK_KNN_HALVES=1|2 forces
-  int hybrid_res_kb = -1, hybrid_slots = 8;   // -1: hybrid pair kernel off
-  bool use_ts = false;  // pair kernel with queries in TMEM (dim <= 768): correct but not yet faster (DESIGN.md §7)
-  bool force_1cta = false, force_streamed = true;   // query-resident pair kernel: measured slower (DESIGN.md §7)
-  int prefetch_tiles = 0;
   const void* tmap_c_base = nullptr;
   int64_t tmap_c_rows = -1;
   std::vector<cudaEvent_t> ev;

@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(256) convert_rows_kernel(const SrcT* __restric
     }
     uint16_t o[8];
     if (c0 >= d) {
-      // pad columns (the row pitch is a whole number of 64-element k-blocks): zeros, and nothing to read
+      // pad columns (the row pitch is a whole number of 128-byte lines): zeros, and nothing to read
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = 0;
     } else if (aligned) {
@@ -156,11 +156,8 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
   const int n16 = dpad >> 3;                         // 16-byte pieces per row
   constexpr int kPieces = kNormChunk / 8;            // 16-byte pieces per row and chunk; = pieces per thread and chunk
   // piece index i of a chunk -> (row i / len16, unit i % len16): consecutive lanes = consecutive units of a row;
-  // all of a thread's 16 loads are in flight before the first is stored.  (Tried and measured on B200, 4M x 768:
-  // keeping the NEXT chunk's pieces in registers while this one is walked - no change, the kernel is not waiting on
-  // memory; forming x*x with one fp32 multiply and widening it to binary64 with integer shifts instead of two F2F
-  // conversions and a DMUL - 50 % SLOWER, the per-element range check costs more issue slots than the fp64 pipe
-  // saves.  The sequential fp64 chain per row, which the parity contract imposes, is what bounds this kernel.)
+  // all of a thread's 16 loads are in flight before the first is stored.  The sequential fp64 chain per row, which
+  // the parity contract imposes, is what bounds this kernel.
   uint4 v[kPieces];
   auto load_chunk = [&](int c0) {
     const int len16 = n16 - c0 < kPieces ? n16 - c0 : kPieces;
@@ -307,7 +304,11 @@ cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, i
                                 const unsigned int* dead_bits, int* n_dead) {
   if (n_rows <= 0) return cudaSuccess;
   const int64_t total = n_rows * (dpad >> 3);
-  const int grid = grid_for(total, 256, 148 * 16);
+  int dev = 0, sms = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) return e;
+  const int grid = grid_for(total, 256, sms * 16);   // grid-stride loop: 16 blocks per SM
   // vector loads need d % 8 == 0 (every 8-group starts 16-byte aligned) and an aligned base
   const bool aligned = (d & 7) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
   if (src_type == 0)

@@ -7,28 +7,16 @@
 namespace rbk {
 
 // ---- tiling of the fused scan (rbk_scan.cu) ----
-constexpr int kBlockM = 128;      // queries per CTA (UMMA M, TMEM lanes)
-constexpr int kBlockN = 256;      // corpus rows per tile (UMMA N, TMEM columns)
-constexpr int kBlockK = 64;       // bf16 elements per pipeline stage (one 128-byte swizzle row)
-constexpr int kStages = 4;        // smem ring depth
+constexpr int kBlockM = 128;      // queries per CTA (two wgmma warpgroups of M = 64)
+constexpr int kBlockN = 256;      // corpus rows per tile (wgmma N)
+constexpr int kBlockK = 32;       // bf16 elements per pipeline stage (one 64-byte swizzle row)
+constexpr int kStages = 3;        // smem ring depth
 constexpr int kListCap = 256;     // entries per (CTA, query) candidate list
 constexpr int kMaxKPrime = 128;   // candidates kept per query (k_fetch + margin)
-constexpr int kScanThreads = 192; // warp0 TMA, warp1 MMA/TMEM, warps2-5 epilogue
-// the CTA-pair kernel (rbk_scan2.cu) can run 8 epilogue warps: two column halves per tile, two lists per (unit, query)
-constexpr int kMaxHalves = 2;
+constexpr int kScanThreads = 384; // warpgroup 0 epilogue, warpgroups 1-2 wgmma (+ TMA issue)
 constexpr int kMaxSubBatch = 1024;  // queries per scan launch (8 query blocks)
-constexpr int kMaxLeadTiles = 4;    // lockstep: max tiles a CTA may lead the slowest peer of its range (A/B on cfg3
-                                    // under the power cap: 8 -> 74.2 k, 4 -> 76.4 k, 2 -> 77.4 k q/s; short kernels: 8 best by 2 %)
+constexpr int kMaxLeadTiles = 4;    // lockstep: max tiles a CTA may lead the slowest peer of its range
 constexpr int kHistBins = 1024;     // per-query score histogram, cosine in [-1,1] -> bin width 1/512
-
-// The default build ships ONE scan path per batch size (scan_kernel for B <= 128, the streamed CTA-pair kernel
-// above).  -DRBK_EXPERIMENTAL additionally compiles the measured-and-rejected variants of DESIGN.md §7 (query-
-// resident / hybrid / TMEM-query pair kernels, the timing probes) and the environment switches that select them.
-#ifdef RBK_EXPERIMENTAL
-constexpr bool kExperimental = true;
-#else
-constexpr bool kExperimental = false;
-#endif
 
 struct ScanParams {
   const float* inv_norm_c;  // [rows padded to kBlockN], NaN = dead / out of range
@@ -44,51 +32,15 @@ struct ScanParams {
   int n_rows;
   int B;        // queries in this launch
   int kprime;
-  int num_kb;   // k-blocks per tile = ceil(dpad / kBlockK)
-  int dpad;     // padded row length (elements)
-  int prefetch_tiles;  // query-resident pair kernel: L2 prefetch distance in tiles (0 = off)
+  int dpad;     // padded row length (elements, a multiple of kBlockK)
   int max_lead_tiles;  // lockstep: tiles a producer may lead the slowest peer of its range
-  int seed_tile;       // start-up seeding: 1 = count each thread's two best rows of its first tile, 0 = two per chunk
-  int perf_probe;      // 0 = normal.  TIMING EXPERIMENTS ONLY (results are wrong): 1 = epilogue drains TMEM but does not filter
   int QB;       // query blocks
-  int R;        // list units per query block (CTAs / CTA pairs that scan different tiles for the same queries)
-  int RC;       // cluster kernel: corpus ranges = clusters per column (R = RC when the pairs of a cluster share the
-                // corpus tile, 2 * RC when they share the query slab and alternate tiles)
+  int R;        // corpus ranges (CTAs that scan different tiles for the same queries) per query block
   int n_tiles;  // ceil(n_rows / kBlockN)
-  // A scan may be split over two concurrent launches (the cluster kernel on the SMs that can host 4-CTA clusters, the
-  // pair kernel on the rest): each launch covers tiles [tile_begin, tile_begin + tile_count) with R_local ranges,
-  // its units are numbered unit_base.. inside the query block's R lists, its pacing slots start at prog_base.
-  int tile_begin, tile_count;
-  int R_local;   // corpus ranges of THIS launch (1-CTA / pair kernels; the cluster kernel uses RC)
-  int unit_base;
-  int prog_base;
 };
 
 cudaError_t launch_scan(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const ScanParams& p,
                         cudaStream_t stream);
-size_t scan_smem_bytes();
-// CTA-pair variants (B > 128): QB counts 256-query blocks, R pairs per block.  tmap_c has 128-row boxes:
-// 64 columns / SWIZZLE_128B for the streamed kernel, 32 columns / SWIZZLE_64B for the query-resident one.
-// tmap_pf: un-swizzled 128-row x 256-col boxes, used only for L2 prefetch.
-cudaError_t launch_scan2(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const CUtensorMap& tmap_pf,
-                         const ScanParams& p, bool resident, int halves, cudaStream_t stream,
-                         int* ring_stages_out = nullptr);
-// Cluster-of-two-pairs kernel with one operand multicast (rbk_scan4.cu).  tmap_q128 / tmap_c128: 128-row boxes,
-// tmap_q64 / tmap_c64: 64-row boxes (the multicast halves), all 64 columns / SWIZZLE_128B.
-cudaError_t launch_scan4(const CUtensorMap& tmap_q128, const CUtensorMap& tmap_q64, const CUtensorMap& tmap_c128,
-                         const CUtensorMap& tmap_c64, const ScanParams& p, bool share_c, bool smem_aligned,
-                         cudaStream_t stream, int* ring_stages_out = nullptr);
-int scan4_max_clusters(bool smem_aligned);   // resident 4-CTA clusters of that kernel on the current device
-bool scan_smem_base_is_aligned();            // is the dynamic smem window 1024-byte aligned (7-stage ring possible)?
-// CTA-pair kernel with the query operand in TMEM (rbk_scan3.cu): dpad <= 768.  tmap_c: 32-row x 64-col boxes.
-cudaError_t launch_scan3(const CUtensorMap& tmap_c, const ScanParams& p, const uint16_t* q_bf16, cudaStream_t stream);
-bool scan3_fits(int dpad);
-int scan3_box_rows();   // corpus rows per CTA per TMA box of the TMEM-query kernel
-bool scan2_resident_fits(int dpad);
-// Hybrid pair kernel: res_kb resident query panels, the rest + the corpus through n_slots 16-KB ring slots.
-cudaError_t launch_scan2h(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c_half, const ScanParams& p, int res_kb,
-                          int n_slots, cudaStream_t stream);
-int scan2_resident_k();   // corpus columns per stage of the resident kernel (64 or 32)
 
 // ---- ingest (rbk_ingest.cu) ----
 // src element type: 0 = f64, 1 = f32, 2 = bf16 bits.  src is device memory, row pitch = d.
@@ -143,7 +95,7 @@ struct FinalizeParams {
   const unsigned long long* cand;
   const int* cand_cnt;
   int QB, R, kprime, k_fetch, B, d, dpad;
-  int block_m;  // queries per list block: 128 (1-CTA scan) or 256 (CTA-pair scan)
+  int block_m;  // queries per list block (kBlockM)
   int key_cap;  // keys staged in smem per query (set by launch_finalize)
   int q0;  // global index of the first query of this launch (sub-batch offset)
   double min_score;

@@ -1,7 +1,7 @@
-// rbk_ptx.cuh — thin inline-PTX wrappers for the sm_100a features the scan kernel uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the
+// rbk_ptx.cuh — thin inline-PTX wrappers for the sm_90a features the scan kernel uses:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait) and the
 // shared-memory matrix descriptor.  Hand-written for this engine; bit layouts follow the
-// PTX ISA tables for tcgen05 descriptors (see DESIGN.md §5).
+// PTX ISA tables for wgmma descriptors (see DESIGN.md §5).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -49,10 +49,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 
 // ---------------------------------------------------------------- TMA
-// Pull one 128-byte line into L1 (no register result, no scoreboard wait).
-__device__ __forceinline__ void prefetch_l1(const void* gptr) {
-  asm volatile("prefetch.global.L1 [%0];" ::"l"(reinterpret_cast<uint64_t>(gptr)) : "memory");
-}
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }
@@ -67,185 +63,71 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap,
       : "memory");
 }
 
-// Pull a box into L2 only (no smem, no barrier): hides HBM latency when the smem ring is shallow.
-__device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int32_t crd0, int32_t crd1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
-               "r"(crd0), "r"(crd1)
-               : "memory");
+// ---------------------------------------------------------------- wgmma
+// Orders earlier register / shared-memory writes before the wgmma that follow (required before the first
+// wgmma of a batch that accumulates into registers).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// Wait until at most N committed groups of this warpgroup are pending.  The accumulator registers are in/out
+// operands so that no read of them is scheduled before the wait.
+template <int N>
+__device__ __forceinline__ void wgmma_wait(float (&d)[128]) {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_result_addr, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_result_addr),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 x bf16 -> fp32.  Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread are done
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// Warp-collective: lane t reads TMEM lane (taddr.lane + t), 32 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// Same wait, with the loaded registers as in/out operands: a data dependency that keeps every use of
-// v[] after the wait even when the load was issued several statements earlier (software pipelining).
-__device__ __forceinline__ void tmem_wait_ld_dep(uint32_t (&v)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                 "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]),
-                 "+r"(v[15]), "+r"(v[16]), "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]),
-                 "+r"(v[22]), "+r"(v[23]), "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]),
-                 "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-               :
-               : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 bf16
-// (128 B) packed densely: 8-row groups are 1024 B apart (SBO); LBO is unused for
-// swizzled K-major layouts (encoded 1); version field = 1 (sm_100); layout = SWIZZLE_128B.
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
+// Shared-memory matrix descriptor, K-major operand, 64-byte swizzle, rows of 32 bf16 (64 B) packed
+// densely: 8-row groups are 512 B apart (SBO); LBO is unused for swizzled K-major layouts (encoded 1);
+// layout type [62,64) = 2 (SWIZZLE_64B).  Advancing K by 16 elements = +32 B = +2 in the address field.
+__device__ __forceinline__ uint64_t make_sw64_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // [0,14)  start address >> 4
   d |= static_cast<uint64_t>(1) << 16;                      // [16,30) leading byte offset >> 4
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;              // [32,46) stride byte offset >> 4
-  d |= static_cast<uint64_t>(1) << 46;                      // [46,48) descriptor version
-  d |= static_cast<uint64_t>(2) << 61;                      // [61,64) SWIZZLE_128B
+  d |= static_cast<uint64_t>(512 >> 4) << 32;               // [32,46) stride byte offset >> 4
+  d |= static_cast<uint64_t>(2) << 62;                      // [62,64) SWIZZLE_64B
   return d;
 }
-// Instruction descriptor, kind::f16: D=f32, A=B=bf16, both K-major, dense, M x N.
-__host__ __device__ constexpr uint32_t make_idesc_bf16_f32(int M, int N) {
-  return (1u << 4)                              // [4,6)   D format  = F32
-         | (1u << 7)                            // [7,10)  A format  = BF16
-         | (1u << 10)                           // [10,13) B format  = BF16
-         | (static_cast<uint32_t>(N >> 3) << 17)  // [17,23) N >> 3
-         | (static_cast<uint32_t>(M >> 4) << 24); // [24,29) M >> 4
-}
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// In the shared::cluster window the CTA rank sits above bit 24; clearing bit 24 of a local
-// address names the same offset in the even (leader) CTA of the pair.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Arrive on the barrier at the same offset in the leader CTA (works from either CTA).
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t local_bar) {
-  // default semantics (release at CTA scope): a cluster-scope release would drag in a
-  // MEMBAR.GPU + ERRBAR per arrive (seen in the ncu source view) for no benefit here
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(local_bar & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t smem_result_addr, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_result_addr),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load issued by either CTA of a pair into ITS OWN smem; the bytes are accounted on the
-// LEADER's mbarrier (the MMA issuer waits there for both halves).
-__device__ __forceinline__ void tma_load_2d_2cta(uint32_t smem_dst, const void* tmap, uint32_t local_bar,
-                                                 int32_t crd0, int32_t crd1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      :
-      : "r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(local_bar & kPeerBitMask), "r"(crd0), "r"(crd1)
-      : "memory");
-}
-// The same load, MULTICAST: the box is written at the same smem offset of every CTA in cta_mask (bit i = cluster
-// rank i) with ONE read of L2, and each destination's bytes are accounted on the barrier at this offset in the
-// leader (even rank) of THAT destination's pair.
-__device__ __forceinline__ void tma_load_2d_2cta_mc(uint32_t smem_dst, const void* tmap, uint32_t local_bar,
-                                                    int32_t crd0, int32_t crd1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5}], [%2], %3;"
-      :
-      : "r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(local_bar & kPeerBitMask), "h"(cta_mask),
-        "r"(crd0), "r"(crd1)
-      : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem, 128 rows per CTA] * B[smem, N/2 rows per CTA]^T; M = 256.
-__device__ __forceinline__ void umma_bf16_ss_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                                  uint32_t idesc, uint32_t accumulate) {
+// D[64 x 256] (+)= A[smem, 64 x 16] * B[smem, 256 x 16]^T, bf16 x bf16 -> fp32 in registers; warpgroup-collective
+// and asynchronous (wgmma_commit / wgmma_wait).  Thread t of the warpgroup holds d[4j + 2h + e] = D[16 * (t / 32) +
+// (t % 32) / 4 + 8h][8j + 2 * (t % 4) + e].
+__device__ __forceinline__ void wgmma_m64n256k16_bf16(float (&d)[128], uint64_t desc_a, uint64_t desc_b,
+                                                      uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once the pair's MMAs retire) on the barrier at this offset in BOTH CTAs.
-__device__ __forceinline__ void umma_commit_2cta(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      :
-      : "r"(bar), "h"(static_cast<uint16_t>(3))
-      : "memory");
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
-// Same, to the CTAs named by cta_mask (bit i = cluster rank i): clusters of more than one pair.
-__device__ __forceinline__ void umma_commit_2cta_mask(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      :
-      : "r"(bar), "h"(cta_mask)
-      : "memory");
-}
-
-// One lane of a converged warp.  The producer and MMA roles run their loops with the WHOLE warp
-// (uniform control flow, operands in uniform registers) and elect a lane only around the
-// asynchronous instruction itself: a loop that lives inside `if (lane == 0)` makes every operand
-// a per-thread value and costs an ELECT + R2UR round trip per descriptor (~16 instructions per
-// tcgen05.mma, seen in the ncu source view), which made 32-cycle N=64 MMAs issue-bound.
+// One lane of a converged warp: the TMA issue runs with the WHOLE warp (uniform control flow, operands in
+// uniform registers) and elects a lane only around the asynchronous instruction itself.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(

@@ -1,6 +1,6 @@
 """K3 ingest throughput: convert_rows_kernel (f64 -> bf16, bf16 copy) and row_norms_kernel at BASELINE scale,
 device-resident sources (the PCIe hop is not the kernel).  Prints one JSON line per case with CUDA-event times;
-run it under `ncu --metrics gpu__time_duration.sum` for the per-kernel launch list (scripts/gpu_r2_b.sh).
+use torch.profiler for the per-kernel launch list.
 
     python scripts/ingest_bench.py [rows] [dim]
 """
@@ -14,7 +14,7 @@ ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 from runbookai_b200 import Index  # noqa: E402
 
-PEAK = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 6650.0
+PEAK = 3350.0   # GB/s, HBM3 bandwidth in NVIDIA's H100 SXM data sheet
 
 
 def timed(fn):

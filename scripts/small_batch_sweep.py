@@ -1,5 +1,5 @@
-"""Scan-kernel time of the 1-CTA kernel (B <= 128) over 1M x 768 rows: how close do the HBM-bound small batches get to
-the copy peak (MEASURED_PEAKS.json) and to the TMA read roof (scripts/probes/tma_stream_probe.cu)?"""
+"""Scan-kernel time for one query block (B <= 128) over 1M x 768 rows: how close do the HBM-bound small batches get to
+the HBM bandwidth (3350 GB/s, NVIDIA's H100 SXM data sheet)?"""
 import json
 import sys
 from pathlib import Path
@@ -31,5 +31,5 @@ for b in (1, 8, 64, 128):
         res.append(ix.stats()["last_scan_ms"])
     best = min(res[2:])
     print(json.dumps({"B": b, "rows": n, "scan_ms_min": round(best, 4), "scan_ms_med": round(float(np.median(res[2:])), 4),
-                      "gbs": round(2.0 * n * d / best / 1e6), "frac_of_copy_peak": round(2.0 * n * d / best / 1e6 / 6566.1, 3)}), flush=True)
+                      "gbs": round(2.0 * n * d / best / 1e6), "frac_of_hbm_peak": round(2.0 * n * d / best / 1e6 / 3350.0, 3)}), flush=True)
 ix.close()

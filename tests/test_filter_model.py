@@ -81,7 +81,7 @@ def run_filter(scores, n_units, kprime, rng, seed_first_tile=True, publish=True,
             gthr = max(gthr, u.thr)
         nohist = False
         if it == 0 and seed_first_tile:                            # seeding pass: two best rows of every chunk
-            step = len(rows) if seed_whole_tile else CHUNK         # pair kernel with many units: two per tile
+            step = len(rows) if seed_whole_tile else CHUNK         # whole-tile seeding: two per tile
             for c0 in range(0, len(rows), step):
                 ch = rows[c0:c0 + step]
                 for r in ch[np.argsort(-scores[ch], kind="stable")[:2]]:

@@ -5,7 +5,7 @@ SURVEY.md §8(d): for N > 1M the check is a fixed 64-query subsample of the batc
 oracle.  The corpus never exists on the host as a whole: it is generated on the device, read back from
 the index chunk by chunk and handed to `oracle.search_chunked` (identical per-pair arithmetic to the
 literal loop, see rbk_oracle.c "verify" variant and tests/test_oracle.py).  Nothing here reads
-/root/reference."""
+the reference checkout."""
 import os
 import subprocess
 import sys
@@ -139,7 +139,7 @@ def test_two_rank_nccl_sharded_parity(rb):
     (scripts/dist_check.py).  Needs two GPUs."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     env = dict(os.environ, PYTHONPATH=str(ROOT))
     res = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
                           "--master-addr", "127.0.0.1", "--master-port", "29533", str(ROOT / "scripts" / "dist_check.py")],

@@ -1,7 +1,7 @@
 """GPU suite (-m gpu): the CUDA path, called through the C ABI, against the oracle on the
 same seeded inputs.  Bar: returned ids identical, fp64 scores bit-identical (the engine
 re-ranks in the reference's exact operation order), approximate scan scores within the
-engine's own error bound.  Nothing here reads /root/reference."""
+engine's own error bound.  Nothing here reads the reference checkout."""
 import json
 import math
 import os
@@ -79,9 +79,9 @@ def test_scan_scores_within_error_bound(rb):
     (40_000, 1024, 256, 32, 0, None),   # config-4 width, k_fetch 64
     (20_000, 1536, 5, 56, 0, None),     # the reference's default d, max k_fetch
     (150_000, 768, 64, 16, 0, None),    # many tiles per CTA: running thresholds + compaction
-    (4000, 100, 200, 8, 12, 0.5),       # CTA-pair kernel with a padded, non-multiple-of-64 dim
+    (4000, 100, 200, 8, 12, 0.5),       # two query blocks with a padded, non-multiple-of-64 dim
     (60_000, 384, 1100, 16, 0, None),   # > 1024 queries: two sub-batches (1024 + 76) in one call
-    (3000, 2048, 140, 5, 4, 0.5),       # wide rows (32 k-blocks), pair kernel
+    (3000, 2048, 140, 5, 4, 0.5),       # wide rows (64 k-blocks of 32), two query blocks
 ])
 def test_parity_shapes(rb, oracle_mod, n, d, b, k, planted, min_score):
     from runbookai_b200 import synth
@@ -416,7 +416,7 @@ def test_async_search_reports_unproven_queries_instead_of_fixing_them(rb, oracle
 
 def test_randomized_differential_against_oracle(rb, oracle_mod):
     """A few hundred random operations - appends of random sizes, bulk overwrites, tombstones, searches with random
-    batch size / k_fetch / threshold (1-CTA and pair kernels, sub-batching, thresholds that pass nothing or
+    batch size / k_fetch / threshold (one or several query blocks, sub-batching, thresholds that pass nothing or
     everything) - on one index, every search compared with the oracle on the mirrored host state."""
     from runbookai_b200 import synth
     rng = np.random.default_rng(2024)
