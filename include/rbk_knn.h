@@ -41,6 +41,9 @@ extern "C" {
 #define RBK_ABI_VERSION 2
 /* Largest k_fetch a single search accepts (the scan keeps k_fetch + margin <= 128). */
 #define RBK_MAX_K_FETCH 112
+/* Largest k_fetch of the large-k search (rbk_index_search_large_f64): 4 * limit for the reference's largest
+ * limit (1000, knowledge-context.ts:150). */
+#define RBK_MAX_K_FETCH_LARGE 4096
 
 typedef struct rbk_index rbk_index;
 
@@ -134,10 +137,20 @@ rbk_status rbk_index_search_device(rbk_index* idx, const void* dev_queries_f32, 
                                    double min_score, void* dev_out_slots_i64, void* dev_out_scores_f64,
                                    void* dev_out_counts_i32);
 
-/* More hits than RBK_MAX_K_FETCH (callers of the reference pass limit: 1000, knowledge-context.ts:150): the exact
- * fp64 cosine of EVERY row, out_scores[b * size() + slot], NaN for tombstoned / zero rows (which the reference's
- * `>= minScore` drops too, S3).  The host applies the threshold, the stable sort and the cut literally
- * (vector-store.ts:212-221).  One fp64 pass over the corpus per query: the large-k path, not the hot path. */
+/* Up to RBK_MAX_K_FETCH_LARGE hits per query (callers of the reference pass limit: 1000, knowledge-context.ts:150,
+ * which becomes k_fetch = 4000 through the hybrid retriever): exactly the contract of rbk_index_search_f64 - same
+ * order, threshold, NaN / tombstone rules and bit-identical fp64 scores - for 1 <= k_fetch <= 4096.  k_fetch <= 112
+ * is accepted too and gives the same answer as rbk_index_search_f64.  Two scans of the corpus (count, then emit the
+ * rows the count proved may belong to the answer) and an exact fp64 re-rank of those rows; one extra host round trip
+ * between the scans.  Host queries and outputs, synchronous; batches over 1024 queries are split.  Fails with
+ * RBK_ECUDA, never with a wrong answer, if the emit scan finds more rows than the count scan bounded (a bug). */
+rbk_status rbk_index_search_large_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
+                                      int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* kernel_ms_out);
+
+/* More hits than RBK_MAX_K_FETCH_LARGE: the exact fp64 cosine of EVERY row, out_scores[b * size() + slot], NaN for
+ * tombstoned / zero rows (which the reference's `>= minScore` drops too, S3).  The host applies the threshold, the
+ * stable sort and the cut literally (vector-store.ts:212-221).  One fp64 pass over the corpus per query. */
 rbk_status rbk_index_exact_scores_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
                                       double* out_scores);
 
@@ -204,6 +217,11 @@ rbk_status rbk_group_search_f32(rbk_group* grp, const float* queries, int32_t B,
 rbk_status rbk_group_search_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
                                 double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts,
                                 float* device_ms_out);
+/* rbk_index_search_large_f64 over the group: the count scan on every GPU, one wait for all of them, the emit scan and
+ * re-rank on every GPU, then the same all-gather and merge as rbk_group_search_f64. */
+rbk_status rbk_group_search_large_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
+                                      int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* device_ms_out);
 
 /* ---- introspection ---- */
 typedef struct {

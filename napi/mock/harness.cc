@@ -49,9 +49,9 @@ struct Result {
 
 // await ix.search(queries, B, k, minScore): fulfilled -> true + result, rejected -> false + message
 bool search(napi_env env, napi_value ix, const std::vector<double>& q, int B, int k, double min_score, Result* r,
-            std::string* error) {
+            std::string* error, const char* method = "search") {
   napi_value promise = nullptr;
-  if (!mock::call_method(env, ix, "search",
+  if (!mock::call_method(env, ix, method,
                          {mock::typed_array(env, napi_float64_array, q.data(), q.size()), mock::number(env, B),
                           mock::number(env, k), mock::number(env, min_score)},
                          &promise, error))
@@ -175,6 +175,29 @@ int main(int argc, char** argv) {
   write_bin("slots.i64", res.slots.data(), res.slots.size() * 8);
   write_bin("scores.f64", res.scores.data(), res.scores.size() * 8);
   write_bin("counts.i32", res.counts.data(), res.counts.size() * 4);
+
+  // searchLarge(): optional large.txt lists k_fetch values (up to 4096); results land in large<i>_*.  One more call
+  // with k_fetch 4097 must reject with the library's message.
+  {
+    std::ifstream lf(g_dir + "/large.txt");
+    int kl, i = 0;
+    bool any = false;
+    while (lf >> kl) {
+      any = true;
+      Result lr;
+      if (!search(env, ix, queries, n_q, kl, min_score, &lr, &err, "searchLarge")) die("searchLarge rejected: " + err);
+      const std::string p = "large" + std::to_string(i++) + "_";
+      write_bin((p + "slots.i64").c_str(), lr.slots.data(), lr.slots.size() * 8);
+      write_bin((p + "scores.f64").c_str(), lr.scores.data(), lr.scores.size() * 8);
+      write_bin((p + "counts.i32").c_str(), lr.counts.data(), lr.counts.size() * 4);
+    }
+    if (any) {
+      Result none;
+      if (search(env, ix, queries, n_q, 4097, min_score, &none, &err, "searchLarge"))
+        die("searchLarge with k_fetch 4097 did not reject");
+      log << "err_large " << err << "\n";
+    }
+  }
 
   // ---- error paths: each must surface as a JS exception / rejection with the reference's wording
   {

@@ -18,6 +18,7 @@
 //   ix.tombstone(BigInt64Array slots); ix.clear()
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
+//   await ix.searchLarge(Float64Array queries, B, kFetch, minScore)   // kFetch up to 4096, same result object
 //
 // Build (where Node headers exist):  node-gyp with  libraries: ["-lrbk_knn"], include_dirs: ["../include"].
 #include <node_api.h>
@@ -29,6 +30,12 @@
 #include <vector>
 
 #include "../include/rbk_knn.h"
+
+// The large-k entry points came after ABI version 2 was fixed, so a librbk_knn.so of the same version may lack them.
+// Weak references keep the addon loadable against such a library; `searchLarge` then throws instead of the module
+// failing to load.
+#pragma weak rbk_index_search_large_f64
+#pragma weak rbk_group_search_large_f64
 
 namespace {
 
@@ -63,6 +70,14 @@ struct Handle {
   rbk_status search(const double* q, int32_t B, int32_t qdim, int32_t k, double ms, int64_t* s, double* v, int32_t* c) {
     return grp ? rbk_group_search_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
                : rbk_index_search_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
+  }
+  bool has_search_large() const {
+    return grp ? rbk_group_search_large_f64 != nullptr : rbk_index_search_large_f64 != nullptr;
+  }
+  rbk_status search_large(const double* q, int32_t B, int32_t qdim, int32_t k, double ms, int64_t* s, double* v,
+                          int32_t* c) {
+    return grp ? rbk_group_search_large_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
+               : rbk_index_search_large_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
   }
 };
 
@@ -238,6 +253,7 @@ struct SearchJob {
   Handle* ix;
   std::vector<double> queries;
   int32_t B, dim, k;
+  bool large;   // searchLarge: rbk_*_search_large_f64
   double min_score;
   std::vector<int64_t> slots;
   std::vector<double> scores;
@@ -250,8 +266,10 @@ struct SearchJob {
 
 void search_execute(napi_env, void* data) {
   SearchJob* j = static_cast<SearchJob*>(data);
-  j->st = j->ix->search(j->queries.data(), j->B, j->dim, j->k, j->min_score, j->slots.data(), j->scores.data(),
-                        j->counts.data());
+  j->st = j->large ? j->ix->search_large(j->queries.data(), j->B, j->dim, j->k, j->min_score, j->slots.data(),
+                                        j->scores.data(), j->counts.data())
+                   : j->ix->search(j->queries.data(), j->B, j->dim, j->k, j->min_score, j->slots.data(),
+                                   j->scores.data(), j->counts.data());
   if (j->st != RBK_OK) j->err = rbk_last_error();   // thread-local: read it on the worker thread
 }
 
@@ -284,16 +302,21 @@ void search_complete(napi_env env, napi_status, void* data) {
   delete j;
 }
 
-napi_value Search(napi_env env, napi_callback_info info) {
+napi_value QueueSearch(napi_env env, napi_callback_info info, bool large) {
   size_t argc = 4;
   napi_value argv[4];
   Handle* ix = unwrap(env, info, &argc, argv);
+  if (large && !ix->has_search_large()) {
+    napi_throw_error(env, nullptr, "searchLarge: this librbk_knn.so has no large-k search (rbk_*_search_large_f64)");
+    return nullptr;
+  }
   napi_typedarray_type t;
   size_t len;
   void* data;
   NAPI_OK(napi_get_typedarray_info(env, argv[0], &t, &len, &data, nullptr, nullptr));
   auto* j = new SearchJob();
   j->ix = ix;
+  j->large = large;
   napi_get_value_int32(env, argv[1], &j->B);
   napi_get_value_int32(env, argv[2], &j->k);
   napi_get_value_double(env, argv[3], &j->min_score);   // pass -Infinity for "no threshold"
@@ -310,6 +333,9 @@ napi_value Search(napi_env env, napi_callback_info info) {
   return promise;
 }
 
+napi_value Search(napi_env env, napi_callback_info info) { return QueueSearch(env, info, false); }
+napi_value SearchLarge(napi_env env, napi_callback_info info) { return QueueSearch(env, info, true); }
+
 napi_value Init(napi_env env, napi_value exports) {
   napi_property_descriptor props[] = {
       {"appendF64", nullptr, AppendF64, nullptr, nullptr, nullptr, napi_default, nullptr},
@@ -320,6 +346,7 @@ napi_value Init(napi_env env, napi_value exports) {
       {"clear", nullptr, Clear, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"count", nullptr, Count, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"search", nullptr, Search, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"searchLarge", nullptr, SearchLarge, nullptr, nullptr, nullptr, napi_default, nullptr},
   };
   napi_value cls;
   NAPI_OK(napi_define_class(env, "RbkIndex", NAPI_AUTO_LENGTH, New, nullptr, sizeof props / sizeof props[0], props, &cls));

@@ -14,6 +14,7 @@ LIB_PATH = Path(__file__).resolve().parent / "lib" / "librbk_knn.so"
 
 RBK_OK, RBK_EINVAL, RBK_ENOMEM, RBK_ECUDA, RBK_ENCCL, RBK_EDIM = range(6)
 RBK_MAX_K_FETCH = 112
+RBK_MAX_K_FETCH_LARGE = 4096
 
 # every symbol include/rbk_knn.h declares (tests check the .so exports all of them)
 SYMBOLS = [
@@ -21,13 +22,14 @@ SYMBOLS = [
     "rbk_index_set_slot_base", "rbk_index_append_f64", "rbk_index_append_f32", "rbk_index_append_bf16",
     "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_clear",
     "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_read_rows_bf16", "rbk_index_search_f64",
-    "rbk_index_search_f32", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
+    "rbk_index_search_f32", "rbk_index_search_large_f64", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
     "rbk_packed_block_bytes", "rbk_packed_flags_offset",
     "rbk_merge_topk_packed_device", "rbk_index_stats",
     "rbk_index_debug_scores_f32",
     "rbk_group_create", "rbk_group_destroy", "rbk_group_append_f64", "rbk_group_append_f32", "rbk_group_append_bf16",
     "rbk_group_overwrite_f64_batch", "rbk_group_tombstone", "rbk_group_clear", "rbk_group_count", "rbk_group_size",
     "rbk_group_devices", "rbk_group_member", "rbk_group_redone_batches", "rbk_group_search_f32", "rbk_group_search_f64",
+    "rbk_group_search_large_f64",
 ]
 
 
@@ -79,7 +81,7 @@ def _load() -> C.CDLL:
     lib.rbk_index_dim.argtypes = [vp]
     lib.rbk_index_dim.restype = i32
     lib.rbk_index_read_rows_bf16.argtypes = [vp, i64, i64, vp]
-    for n in ("rbk_index_search_f64", "rbk_index_search_f32"):
+    for n in ("rbk_index_search_f64", "rbk_index_search_f32", "rbk_index_search_large_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_search_device.argtypes = [vp, vp, i32, i32, f64, vp, vp, vp]
     lib.rbk_index_exact_scores_f64.argtypes = [vp, vp, i32, i32, vp]
@@ -106,7 +108,7 @@ def _load() -> C.CDLL:
     lib.rbk_group_devices.restype = i32
     lib.rbk_group_member.argtypes = [vp, i32]
     lib.rbk_group_member.restype = vp
-    for n in ("rbk_group_search_f32", "rbk_group_search_f64"):
+    for n in ("rbk_group_search_f32", "rbk_group_search_f64", "rbk_group_search_large_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_debug_scores_f32.argtypes = [vp, vp, i32, vp]
     return lib
@@ -128,11 +130,26 @@ def ptr(a: np.ndarray | None):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _search_large(fn, h, queries, k_fetch: int, min_score):
+    q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
+    B = q.shape[0]
+    slots = np.empty((B, k_fetch), dtype=np.int64)
+    scores = np.empty((B, k_fetch), dtype=np.float64)
+    counts = np.empty((B,), dtype=np.int32)
+    ms = C.c_float(0)
+    ms_arg = -np.inf if min_score is None else float(min_score)
+    check(fn(h, ptr(q), B, q.shape[1], k_fetch, ms_arg, ptr(slots), ptr(scores), ptr(counts), C.byref(ms)))
+    return slots, scores, counts, ms.value
+
+
 def _search_any_k(ix, queries, k_fetch: int, min_score):
-    """Shared by Index and Group: the scan path up to RBK_MAX_K_FETCH hits per query, beyond it the exact scores of
-    every row from the device and the reference's threshold / stable sort / slice on the host."""
+    """Shared by Index and Group: the scan path up to RBK_MAX_K_FETCH hits per query, the two-pass large-k search up
+    to RBK_MAX_K_FETCH_LARGE, beyond it the exact scores of every row from the device and the reference's threshold /
+    stable sort / slice on the host."""
     if k_fetch <= RBK_MAX_K_FETCH:
         return ix.search(queries, k_fetch, min_score)
+    if k_fetch <= RBK_MAX_K_FETCH_LARGE:
+        return ix.search_large(queries, k_fetch, min_score)
     sc = ix.exact_scores(queries)
     B = sc.shape[0]
     slots = np.full((B, k_fetch), -1, dtype=np.int64)
@@ -260,16 +277,22 @@ class Index:
         check(fn(self._h, ptr(q), B, q.shape[1], k_fetch, ms_arg, ptr(slots), ptr(scores), ptr(counts), C.byref(ms)))
         return slots, scores, counts, ms.value
 
+    def search_large(self, queries, k_fetch: int, min_score: float | None = 0.5):
+        """search() for 1 <= k_fetch <= RBK_MAX_K_FETCH_LARGE (f64 queries): count scan, emit scan, exact re-rank."""
+        return _search_large(lib.rbk_index_search_large_f64, self._h, queries, k_fetch, min_score)
+
     def exact_scores(self, queries) -> np.ndarray:
-        """float64 [B, size()]: the reference's cosine of every row, NaN for tombstoned / zero rows (large-k path)."""
+        """float64 [B, size()]: the reference's cosine of every row, NaN for tombstoned / zero rows (k_fetch beyond
+        RBK_MAX_K_FETCH_LARGE)."""
         q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
         out = np.empty((q.shape[0], self.size()), dtype=np.float64)
         check(lib.rbk_index_exact_scores_f64(self._h, ptr(q), q.shape[0], q.shape[1], ptr(out)))
         return out
 
     def search_any_k(self, queries, k_fetch: int, min_score: float | None = 0.5):
-        """search() for any k_fetch: above RBK_MAX_K_FETCH the answer is cut on the host from exact_scores() with the
-        reference's own steps - `>= minScore`, stable descending sort over slot order, slice (vector-store.ts:212-221)."""
+        """search() for any k_fetch: search_large() above RBK_MAX_K_FETCH; above RBK_MAX_K_FETCH_LARGE the answer is cut
+        on the host from exact_scores() with the reference's own steps - `>= minScore`, stable descending sort over slot
+        order, slice (vector-store.ts:212-221)."""
         return _search_any_k(self, queries, k_fetch, min_score)
 
     def search_device(self, q_ptr: int, B: int, k_fetch: int, min_score: float | None, slots_ptr: int,
@@ -382,6 +405,9 @@ class Group:
         ms_arg = -np.inf if min_score is None else float(min_score)
         check(fn(self._h, ptr(q), B, q.shape[1], k_fetch, ms_arg, ptr(slots), ptr(scores), ptr(counts), C.byref(ms)))
         return slots, scores, counts, ms.value
+
+    def search_large(self, queries, k_fetch: int, min_score: float | None = 0.5):
+        return _search_large(lib.rbk_group_search_large_f64, self._h, queries, k_fetch, min_score)
 
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: every device's exact scores, put back in global slot order (4096-row blocks dealt

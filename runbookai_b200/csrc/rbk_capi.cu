@@ -288,10 +288,11 @@ rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem) {
   return RBK_OK;
 }
 
-rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, int k_fetch, double min_score) {
+rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, int k_fetch, double min_score,
+                             int max_k) {
   if (!ix) return fail(RBK_EINVAL, "null index");
   if (B < 0 || (B > 0 && !have_q)) return fail(RBK_EINVAL, "bad queries argument");
-  if (k_fetch < 1 || k_fetch > RBK_MAX_K_FETCH) return fail(RBK_EINVAL, "k_fetch must be in [1, 112]");
+  if (k_fetch < 1 || k_fetch > max_k) return fail(RBK_EINVAL, "k_fetch must be in [1, " + std::to_string(max_k) + "]");
   if (query_dim != ix->dim) return fail(RBK_EDIM, "Vectors must have the same length");  // embedder.ts:170
   if (min_score != min_score) return fail(RBK_EINVAL, "min_score is NaN");
   return RBK_OK;
@@ -461,6 +462,164 @@ rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, i
   ix->stats.queries += B;
   return run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr);
 }
+}  // namespace impl
+}  // namespace rbk
+
+namespace {
+
+// Scan parameters of one sub-batch of the large-k search; the per-launch scratch (hist | maxbin | gthr | progress)
+// is laid out as in run_scan.
+LargeScanParams large_scan_params(rbk_index* ix, int q0, int Bs, int k_fetch, int n_tiles) {
+  LargeScanParams sp{};
+  const int QB = (Bs + kBlockM - 1) / kBlockM;
+  sp.inv_norm_c = ix->inv_norm;
+  sp.thr_init = ix->thr_init.p + q0;
+  sp.inv_norm_q = ix->q_inv_norm.p + q0;
+  sp.hist = ix->hist.p;
+  sp.maxbin = reinterpret_cast<int*>(ix->hist.p + static_cast<size_t>(Bs) * kHistBins);
+  sp.gthr = reinterpret_cast<unsigned int*>(sp.maxbin + Bs);
+  sp.progress = sp.maxbin + 2 * Bs;
+  sp.n_rows = static_cast<int>(ix->n_rows);
+  sp.B = Bs;
+  sp.kprime = k_fetch;
+  sp.dpad = ix->dpad;
+  sp.max_lead_tiles = ix->max_lead_tiles;
+  sp.QB = QB;
+  sp.R = std::max(1, std::min(ix->sm_count / QB, n_tiles));
+  sp.n_tiles = n_tiles;
+  sp.q_eps = ix->q_eps.p + q0;
+  return sp;
+}
+
+rbk_status launch_large_scan(rbk_index* ix, int q0, const LargeScanParams& sp, LargeScanMode mode) {
+  CUtensorMap tmap_q;
+  const int q_rows = static_cast<int>(round_up(sp.B, kBlockM));
+  rbk_status st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM);
+  if (st != RBK_OK) return st;
+  cudaEvent_t* tev = next_scan_events(ix);
+  CK(cudaEventRecord(tev[0], ix->stream));
+  CK(launch_scan_large(tmap_q, ix->tmap_c, sp, mode, ix->stream));
+  CK(cudaEventRecord(tev[1], ix->stream));
+  ix->stats.last_ring_stages = kStages;
+  ix->stats.scan_launches++;
+  ix->stats.kernel_launches++;
+  return RBK_OK;
+}
+
+}  // namespace
+
+namespace rbk {
+namespace impl {
+
+rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, double min_score) {
+  ix->stats.searches++;
+  ix->stats.queries += B;
+  ix->stats.last_kprime = k_fetch;
+  CK(ix->lg_theta.ensure(B));
+  CK(ix->lg_cap.ensure(B));
+  CK(ix->lg_cnt.ensure(B));
+  CK(ix->lg_off.ensure(B));
+  CK(ix->lg_err.ensure(1));
+  CK(ix->h_lcap.ensure(B));
+  CK(ix->h_loff.ensure(B));
+  CK(ix->h_lerr.ensure(1));
+  // normA is computed here: the re-rank has no spare thread to walk the chain beside its candidates
+  const int Bs0 = std::min(kMaxSubBatch, B);
+  CK(launch_prep_queries(d_q, 0, B, ix->dim, ix->dpad, min_score,
+                         ix->keep_f64 ? reinterpret_cast<const float*>(ix->d_counter + 1) : nullptr,
+                         query_buffers(ix, 0), ix->stream, /*with_norm2=*/true, ix->hist.p, Bs0, ix->sm_count + 8));
+  ix->stats.kernel_launches++;
+  if (ix->n_rows == 0) {
+    memset(ix->h_lcap.p, 0, sizeof(int) * B);
+    return RBK_OK;
+  }
+  rbk_status st = refresh_corpus_tmap(ix);
+  if (st != RBK_OK) return st;
+  const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
+  for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
+    const int Bs = std::min(kMaxSubBatch, B - q0);
+    if (q0 > 0)   // the first sub-batch's scratch was zeroed by the prep kernel
+      CK(cudaMemsetAsync(ix->hist.p, 0,
+                         sizeof(unsigned int) * (static_cast<size_t>(Bs) * kHistBins + 2 * Bs + ix->sm_count + 8),
+                         ix->stream));
+    const LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch, n_tiles);
+    st = launch_large_scan(ix, q0, sp, kScanCount);
+    if (st != RBK_OK) return st;
+    CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Bs, k_fetch, ix->lg_theta.p + q0,
+                           ix->lg_cap.p + q0, ix->stream));
+    ix->stats.kernel_launches++;
+  }
+  CK(cudaMemcpyAsync(ix->h_lcap.p, ix->lg_cap.p, sizeof(int) * B, cudaMemcpyDeviceToHost, ix->stream));
+  return RBK_OK;
+}
+
+rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long long* d_slots, double* d_scores,
+                      int* d_counts) {
+  CK(cudaMemsetAsync(ix->lg_err.p, 0, sizeof(int), ix->stream));
+  CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+  if (ix->n_rows == 0) {
+    CK(cudaMemsetAsync(d_counts, 0, sizeof(int) * B, ix->stream));
+    CK(cudaMemsetAsync(d_slots, 0xFF, sizeof(long long) * B * k_fetch, ix->stream));   // -1
+    CK(cudaMemsetAsync(d_scores, 0xFF, sizeof(double) * B * k_fetch, ix->stream));     // NaN
+    return RBK_OK;
+  }
+  // segment offsets: exclusive prefix sum of C_q
+  long long total = 0;
+  for (int b = 0; b < B; ++b) {
+    ix->h_loff.p[b] = total;
+    total += ix->h_lcap.p[b];
+  }
+  CK(ix->lg_rows.ensure(static_cast<size_t>(std::max<long long>(total, 1))));
+  CK(ix->lg_scores.ensure(static_cast<size_t>(std::max<long long>(total, 1))));
+  CK(cudaMemcpyAsync(ix->lg_off.p, ix->h_loff.p, sizeof(long long) * B, cudaMemcpyHostToDevice, ix->stream));
+  CK(cudaMemsetAsync(ix->lg_cnt.p, 0, sizeof(int) * B, ix->stream));
+  const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
+  for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
+    const int Bs = std::min(kMaxSubBatch, B - q0);
+    LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch, n_tiles);
+    sp.thr_init = ix->lg_theta.p + q0;   // theta_q
+    sp.emit_off = ix->lg_off.p + q0;
+    sp.emit_cap = ix->lg_cap.p + q0;
+    sp.emit_cnt = ix->lg_cnt.p + q0;
+    sp.emit_rows = ix->lg_rows.p;
+    CK(cudaMemsetAsync(sp.progress, 0, sizeof(int) * (ix->sm_count + 8), ix->stream));
+    rbk_status st = launch_large_scan(ix, q0, sp, kScanEmit);
+    if (st != RBK_OK) return st;
+    LargeRerankParams rp;
+    rp.B = Bs;
+    rp.d = ix->dim;
+    rp.dpad = ix->dpad;
+    rp.k_fetch = k_fetch;
+    rp.min_score = min_score;
+    rp.rows = ix->rows;
+    rp.rows_f64 = ix->rows_f64;
+    rp.row_norm2 = ix->norm2;
+    rp.slot = ix->slot;
+    rp.q_f64 = ix->q_f64.p + static_cast<size_t>(q0) * ix->dim;
+    rp.q_norm2 = ix->q_norm2.p + q0;
+    rp.emit_off = sp.emit_off;
+    rp.emit_cap = sp.emit_cap;
+    rp.emit_cnt = sp.emit_cnt;
+    rp.emit_rows = ix->lg_rows.p;
+    rp.cand_scores = ix->lg_scores.p;
+    rp.out_slots = d_slots + static_cast<size_t>(q0) * k_fetch;
+    rp.out_scores = d_scores + static_cast<size_t>(q0) * k_fetch;
+    rp.out_counts = d_counts + q0;
+    rp.overflow = ix->lg_err.p;
+    const int max_cap = *std::max_element(ix->h_lcap.p + q0, ix->h_lcap.p + q0 + Bs);
+    CK(launch_large_rerank(rp, max_cap, ix->stream));
+    ix->stats.kernel_launches += max_cap > 0 ? 2 : 1;
+  }
+  CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+  return RBK_OK;
+}
+
+rbk_status large_check(rbk_index* ix) {
+  if (ix->h_lerr.p[0] == 0) return RBK_OK;
+  return fail(RBK_ECUDA, "large-k search: the emit scan found more rows than the count scan bounded for " +
+                             std::to_string(ix->h_lerr.p[0]) + " queries (the answer is not proven exact)");
+}
+
 }  // namespace impl
 }  // namespace rbk
 
@@ -756,6 +915,16 @@ void rbk_index_destroy(rbk_index* ix) {
     ix->o_scores.release();
     ix->part_scores.release();
     ix->dbg.release();
+    ix->lg_theta.release();
+    ix->lg_cap.release();
+    ix->lg_cnt.release();
+    ix->lg_rows.release();
+    ix->lg_err.release();
+    ix->lg_off.release();
+    ix->lg_scores.release();
+    ix->h_lcap.release();
+    ix->h_lerr.release();
+    ix->h_loff.release();
     ix->o_block.release();
     ix->h_block.release();
     ix->h_flags.release();
@@ -944,6 +1113,53 @@ rbk_status rbk_index_search_device(rbk_index* ix, const void* dev_queries_f32, i
   return search_core(ix, nullptr, dev_queries_f32, 4, B, ix ? ix->dim : 0, k_fetch, min_score,
                      static_cast<long long*>(dev_out_slots), static_cast<double*>(dev_out_scores),
                      static_cast<int*>(dev_out_counts), nullptr, nullptr, nullptr, nullptr);
+}
+
+rbk_status rbk_index_search_large_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
+                                      int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* kernel_ms_out) {
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, RBK_MAX_K_FETCH_LARGE);
+  if (st != RBK_OK) return st;
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  if (kernel_ms_out) *kernel_ms_out = 0.f;
+  if (B == 0) {
+    ix->stats.searches++;
+    return RBK_OK;
+  }
+  st = ensure_query_scratch(ix, B, 8);
+  if (st != RBK_OK) return st;
+  const size_t nout = static_cast<size_t>(B) * k_fetch;
+  const size_t blk = nout * 16 + static_cast<size_t>(B) * 4;   // slots | scores | counts
+  CK(ix->o_block.ensure(blk));
+  CK(ix->h_block.ensure(blk));
+  unsigned char* base = ix->o_block.p;
+  resolve_scan_events(ix, false);
+  const double scan_ms0 = ix->stats.scan_ms_total;
+  CK(cudaEventRecord(get_event(ix, 0), ix->stream));
+  CK(cudaMemcpyAsync(ix->q_raw.p, queries, static_cast<size_t>(B) * ix->dim * 8, cudaMemcpyHostToDevice, ix->stream));
+  st = large_count(ix, ix->q_raw.p, B, k_fetch, min_score);
+  if (st != RBK_OK) return st;
+  CK(cudaStreamSynchronize(ix->stream));   // C_q sizes the candidate buffer
+  st = large_emit(ix, B, k_fetch, min_score, reinterpret_cast<long long*>(base),
+                  reinterpret_cast<double*>(base + nout * 8), reinterpret_cast<int*>(base + nout * 16));
+  if (st != RBK_OK) return st;
+  CK(cudaMemcpyAsync(ix->h_block.p, base, blk, cudaMemcpyDeviceToHost, ix->stream));
+  CK(cudaEventRecord(get_event(ix, 1), ix->stream));
+  CK(cudaStreamSynchronize(ix->stream));
+  st = large_check(ix);
+  if (st != RBK_OK) return st;
+  float total = 0.f;
+  cudaEventElapsedTime(&total, get_event(ix, 0), get_event(ix, 1));
+  resolve_scan_events(ix, true);
+  ix->stats.last_total_ms = total;
+  ix->stats.last_scan_ms = static_cast<float>(ix->stats.scan_ms_total - scan_ms0);
+  if (kernel_ms_out) *kernel_ms_out = total;
+  memcpy(out_slots, ix->h_block.p, sizeof(int64_t) * nout);
+  memcpy(out_scores, ix->h_block.p + nout * 8, sizeof(double) * nout);
+  memcpy(out_counts, ix->h_block.p + nout * 16, sizeof(int32_t) * B);
+  return RBK_OK;
 }
 
 rbk_status rbk_index_exact_scores_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,

@@ -418,6 +418,159 @@ __device__ __forceinline__ void run_epilogue(const ScanParams& p, float (*invc_s
   p.cand_cnt[list_id] = fs.cnt;
 }
 
+// ---- large-k search (k_fetch up to RBK_MAX_K_FETCH_LARGE): two scans with the same tiling, no candidate lists ----
+// Both modes compute a row's approximate score with the SAME expression as filter_chunk (accumulator * 1/||c||, one
+// fp32 multiply), so a row has the same `a` in the count pass and in the emit pass.  See DESIGN.md §6.
+
+// Raw count-pass threshold for histogram bin b: the bin's lower edge lowered by `delta` (cosine domain), nudged down.
+// Monotonic in b.  The select kernel's theta_q (edge - 2 eps) stays above it by delta - 2 eps = one bin width, far more
+// than any rounding here, so every row at or above theta_q has been counted.
+__device__ __forceinline__ float count_floor_raw(int b, float qn, float delta) {
+  const float edge = static_cast<float>(b) * (2.0f / kHistBins) - 1.0f - delta;
+  const float r = edge * qn;
+  return r - fabsf(r) * 1e-6f;
+}
+
+// Count mode (pass A): every live row with a >= thr is counted in the query's global histogram, exactly once.  thr
+// starts at thr_init (min_score - eps) and rises to count_floor_raw of the highest bin with >= k_fetch counted rows
+// at or above it.  No seeding pass: the first tile's rows are all counted, so the histogram is complete down to thr.
+__device__ __forceinline__ void run_count_epilogue(const LargeScanParams& p, float (*invc_stage)[kBlockN],
+                                                   unsigned long long* sc_full, unsigned long long* sc_empty,
+                                                   const float* scores, int qb, int t0, int t1, int et) {
+  constexpr int kEpi = kBlockM;
+  const int q = qb * kBlockM + et;
+  const bool q_valid = q < p.B;
+  FilterState fs;
+  filter_init(fs, q_valid, q_valid ? p.thr_init[q] : INFINITY, q_valid ? p.inv_norm_q[q] : 0.f, nullptr,
+              p.hist + static_cast<size_t>(q_valid ? q : 0) * kHistBins, p.maxbin + (q_valid ? q : 0));
+  const float delta = q_valid ? static_cast<float>(2.0 * p.q_eps[q]) + 2.0f / kHistBins : 0.f;
+  const int n_iter = t1 - t0;
+  float nx0 = 0.f, nx1 = 0.f;
+  if (n_iter > 0) {
+    nx0 = __ldg(p.inv_norm_c + t0 * kBlockN + et);
+    nx1 = __ldg(p.inv_norm_c + t0 * kBlockN + kEpi + et);
+  }
+  const float* srow = scores + et * kScorePitch;
+  for (int it = 0; it < n_iter; ++it) {
+    const int tile = t0 + it;
+    float* invc = invc_stage[it & 1];
+    invc[et] = nx0;
+    invc[kEpi + et] = nx1;
+    if (it + 1 < n_iter) {
+      nx0 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + et);
+      nx1 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + kEpi + et);
+    }
+    named_bar_sync(1, kEpi);
+    if (fs.valid && refresh_due(it)) {
+      const int mb = __ldcg(fs.maxbin_q);
+      if (mb > fs.tb) {
+        const unsigned long long w = histogram_walk(fs.hist_q, mb, fs.tb, fs.qn, p.kprime);
+        if (w != 0ull) {
+          fs.tb = static_cast<int>(w >> 32) - 1;
+          fs.thr = fmaxf(fs.thr, count_floor_raw(fs.tb, fs.qn, delta));
+        }
+      }
+    }
+    mbar_wait(smem_u32(sc_full), static_cast<uint32_t>(it & 1));
+#pragma unroll 1
+    for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
+      uint32_t v[32];
+      load_chunk(srow + chunk * 32, v);
+      const float4* ic4 = reinterpret_cast<const float4*>(invc + chunk * 32);
+      float g[8];
+      float m = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 w = ic4[j];
+        const float a0 = __uint_as_float(v[4 * j + 0]) * w.x;
+        const float a1 = __uint_as_float(v[4 * j + 1]) * w.y;
+        const float a2 = __uint_as_float(v[4 * j + 2]) * w.z;
+        const float a3 = __uint_as_float(v[4 * j + 3]) * w.w;
+        g[j] = fmaxf(fmaxf(a0, a1), fmaxf(a2, a3));
+        m = fmaxf(m, g[j]);
+      }
+      if (m >= fs.thr) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (g[j] >= fs.thr) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float a = __uint_as_float(v[4 * j + e]) * invc[chunk * 32 + 4 * j + e];
+              if (a >= fs.thr) hist_add(fs, a);
+            }
+          }
+        }
+      }
+    }
+    mbar_arrive(smem_u32(sc_empty));
+  }
+}
+
+// Emit mode (pass B): every row with a >= theta_q (p.thr_init holds theta_q) takes a slot in query q's segment of
+// p.emit_rows.  One atomicAdd per thread and chunk for all of the chunk's survivors.  The counter keeps counting past
+// the segment's capacity C_q, so an overflow - a broken count - is visible to the re-rank kernel.
+__device__ __forceinline__ void run_emit_epilogue(const LargeScanParams& p, float (*invc_stage)[kBlockN],
+                                                  unsigned long long* sc_full, unsigned long long* sc_empty,
+                                                  const float* scores, int qb, int t0, int t1, int et) {
+  constexpr int kEpi = kBlockM;
+  const int q = qb * kBlockM + et;
+  const bool q_valid = q < p.B;
+  const float theta = q_valid ? p.thr_init[q] : INFINITY;
+  const bool live = q_valid && theta < INFINITY;
+  const long long seg = live ? p.emit_off[q] : 0;
+  const int cap = live ? p.emit_cap[q] : 0;
+  const int n_iter = t1 - t0;
+  float nx0 = 0.f, nx1 = 0.f;
+  if (n_iter > 0) {
+    nx0 = __ldg(p.inv_norm_c + t0 * kBlockN + et);
+    nx1 = __ldg(p.inv_norm_c + t0 * kBlockN + kEpi + et);
+  }
+  const float* srow = scores + et * kScorePitch;
+  for (int it = 0; it < n_iter; ++it) {
+    const int tile = t0 + it;
+    const int row0 = tile * kBlockN;
+    float* invc = invc_stage[it & 1];
+    invc[et] = nx0;
+    invc[kEpi + et] = nx1;
+    if (it + 1 < n_iter) {
+      nx0 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + et);
+      nx1 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + kEpi + et);
+    }
+    named_bar_sync(1, kEpi);
+    mbar_wait(smem_u32(sc_full), static_cast<uint32_t>(it & 1));
+#pragma unroll 1
+    for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
+      uint32_t v[32];
+      load_chunk(srow + chunk * 32, v);
+      const float4* ic4 = reinterpret_cast<const float4*>(invc + chunk * 32);
+      uint32_t hits = 0u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 w = ic4[j];
+        const float a0 = __uint_as_float(v[4 * j + 0]) * w.x;
+        const float a1 = __uint_as_float(v[4 * j + 1]) * w.y;
+        const float a2 = __uint_as_float(v[4 * j + 2]) * w.z;
+        const float a3 = __uint_as_float(v[4 * j + 3]) * w.w;
+        hits |= (a0 >= theta ? 1u : 0u) << (4 * j + 0);
+        hits |= (a1 >= theta ? 1u : 0u) << (4 * j + 1);
+        hits |= (a2 >= theta ? 1u : 0u) << (4 * j + 2);
+        hits |= (a3 >= theta ? 1u : 0u) << (4 * j + 3);
+      }
+      if (hits != 0u && live) {
+        int pos = atomicAdd(p.emit_cnt + q, __popc(hits));
+        const int row_base = row0 + chunk * 32;
+        while (hits != 0u) {
+          const int j = __ffs(hits) - 1;
+          hits &= hits - 1u;
+          if (pos < cap) p.emit_rows[seg + pos] = row_base + j;
+          ++pos;
+        }
+      }
+    }
+    mbar_arrive(smem_u32(sc_empty));
+  }
+}
+
 // Bounded-lag lockstep of the QB producers that stream the same corpus range: nobody runs
 // more than kMaxLeadTiles ahead of the slowest, so a tile pulled from HBM by the first
 // reader is still in L2 for the others (keeps DRAM traffic close to 1x the corpus).

@@ -653,11 +653,176 @@ __global__ void __launch_bounds__(kExThreads) exact_merge_kernel(ExactParams p) 
   if (tid == 0) p.out_counts[q] = n;
 }
 
-// --------------------------------------------------------------------------- all exact scores (large-k path)
+// --------------------------------------------------------------------------- large-k search (DESIGN.md §6)
+// select: one block per query, between the count pass and the emit pass.  T_q = lower edge of the highest bin j with
+// >= k_fetch counted rows in bins >= j; theta_q = max(T_q - 2 eps_q, thr_init) (raw domain, nudged down);
+// C_q = counted rows in bins >= bin(theta_q), an upper bound on the rows the emit pass finds at or above theta_q.
+__global__ void __launch_bounds__(256) large_select_kernel(const unsigned int* __restrict__ hist,
+                                                           const float* __restrict__ thr_init,
+                                                           const float* __restrict__ inv_norm_q,
+                                                           const double* __restrict__ q_eps, int k_fetch,
+                                                           float* __restrict__ theta, int* __restrict__ cap) {
+  const int q = blockIdx.x;
+  const int tid = threadIdx.x;
+  __shared__ unsigned int s_grp[256];          // suffix sums over groups of 4 bins
+  __shared__ unsigned int s_suf[kHistBins];    // rows counted in bins >= b
+  __shared__ int s_top;
+  const uint4 h = reinterpret_cast<const uint4*>(hist + static_cast<size_t>(q) * kHistBins)[tid];
+  s_grp[tid] = h.x + h.y + h.z + h.w;
+  if (tid == 0) s_top = -1;
+  __syncthreads();
+  for (int o = 1; o < 256; o <<= 1) {
+    const unsigned int v = tid + o < 256 ? s_grp[tid + o] : 0u;
+    __syncthreads();
+    s_grp[tid] += v;
+    __syncthreads();
+  }
+  const unsigned int c[4] = {h.x, h.y, h.z, h.w};
+  unsigned int suf = s_grp[tid];
+  int best = -1;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    s_suf[4 * tid + j] = suf;
+    if (suf >= static_cast<unsigned int>(k_fetch)) best = 4 * tid + j;
+    suf -= c[j];
+  }
+  if (best >= 0) atomicMax(&s_top, best);
+  __syncthreads();
+  if (tid != 0) return;
+  const float ti = thr_init[q];
+  if (!(ti < INFINITY)) {   // zero / non-finite query: nothing matches
+    theta[q] = INFINITY;
+    cap[q] = 0;
+    return;
+  }
+  float th = ti;
+  const float inv = inv_norm_q[q];
+  if (s_top >= 0) {
+    const double edge = static_cast<double>(s_top) * (2.0 / kHistBins) - 1.0;
+    const double raw = (edge - 2.0 * q_eps[q] - 1e-6) / static_cast<double>(inv);
+    float t = static_cast<float>(raw);
+    t = nextafterf(nextafterf(t, -INFINITY), -INFINITY);
+    th = fmaxf(th, t);
+  }
+  theta[q] = th;
+  // the bin of a row with a >= th is >= this one: same float expression as hist_add
+  const int b = static_cast<int>((th * inv + 1.0f) * (kHistBins * 0.5f));
+  cap[q] = static_cast<int>(s_suf[min(max(b, 0), kHistBins - 1)]);
+}
+
+// re-rank, part 1: the reference's fp64 cosine of every emitted row (one thread per candidate).
+__global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
+  const int q = blockIdx.y;
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  const int n = min(p.emit_cnt[q], p.emit_cap[q]);
+  if (i >= n) return;
+  const size_t o = static_cast<size_t>(p.emit_off[q]) + i;
+  const int row = p.emit_rows[o];
+  const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
+  const double dot = p.rows_f64 != nullptr ? exact_dot_f64(qv, p.rows_f64 + static_cast<size_t>(row) * p.d, p.d)
+                                           : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
+  p.cand_scores[o] = exact_cosine(dot, p.q_norm2[q], p.row_norm2[row]);
+}
+
+// re-rank, part 2: one block per query keeps the best k_fetch of its candidates by (score desc, row asc) in a
+// shared-memory buffer of S >= k_fetch + blockDim entries, compacted (bitonic sort, cut at k_fetch) whenever the next
+// round of pushes might not fit - so any number of candidates (every duplicate of the k-th row is one) streams through.
+constexpr int kTopThreads = 512;
+
+__device__ void large_compact(double* sc, int* rw, int S, int* s_n, int K, int* s_have, double* s_ts, int* s_tr) {
+  const int tid = threadIdx.x;
+  __syncthreads();
+  const int n = *s_n;
+  for (int i = n + tid; i < S; i += kTopThreads) {
+    sc[i] = -INFINITY;
+    rw[i] = INT_MAX;
+  }
+  __syncthreads();
+  for (int k2 = 2; k2 <= S; k2 <<= 1) {
+    for (int s = k2 >> 1; s > 0; s >>= 1) {
+      for (int i = tid; i < S; i += kTopThreads) {
+        const int j = i ^ s;
+        if (j > i) {
+          const bool desc = (i & k2) == 0;
+          const bool j_first = hit_before(sc[j], rw[j], sc[i], rw[i]);
+          if (desc ? j_first : !j_first) {
+            const double ts = sc[i];
+            sc[i] = sc[j];
+            sc[j] = ts;
+            const int tr = rw[i];
+            rw[i] = rw[j];
+            rw[j] = tr;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  if (tid == 0) {
+    const int keep = n < K ? n : K;
+    *s_n = keep;
+    if (keep == K) {
+      *s_have = 1;
+      *s_ts = sc[K - 1];
+      *s_tr = rw[K - 1];
+    }
+  }
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(kTopThreads) large_topk_kernel(LargeRerankParams p, int S) {
+  extern __shared__ __align__(16) double s_sc[];
+  int* s_rw = reinterpret_cast<int*>(s_sc + S);
+  __shared__ int s_n, s_have, s_tr;
+  __shared__ double s_ts;
+  const int q = blockIdx.x;
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    s_n = 0;
+    s_have = 0;
+  }
+  __syncthreads();
+  const int emitted = p.emit_cnt[q];
+  const int n_cand = min(emitted, p.emit_cap[q]);
+  const size_t off = static_cast<size_t>(p.emit_off[q]);
+  for (int base = 0; base < n_cand; base += kTopThreads) {
+    if (s_n > S - kTopThreads) large_compact(s_sc, s_rw, S, &s_n, p.k_fetch, &s_have, &s_ts, &s_tr);  // uniform
+    const int i = base + tid;
+    if (i < n_cand) {
+      const double sc = p.cand_scores[off + i];
+      const int row = p.emit_rows[off + i];
+      // vector-store.ts:212 (NaN fails; -inf = no threshold), then only what can still make the cut
+      if (sc >= p.min_score && (!s_have || hit_before(sc, row, s_ts, s_tr))) {
+        const int pos = atomicAdd(&s_n, 1);
+        s_sc[pos] = sc;
+        s_rw[pos] = row;
+      }
+    }
+    __syncthreads();
+  }
+  large_compact(s_sc, s_rw, S, &s_n, p.k_fetch, &s_have, &s_ts, &s_tr);
+  const int n = s_n;
+  for (int i = tid; i < p.k_fetch; i += kTopThreads) {
+    const size_t o = static_cast<size_t>(q) * p.k_fetch + i;
+    if (i < n) {
+      p.out_slots[o] = p.slot.global(s_rw[i]);
+      p.out_scores[o] = s_sc[i];
+    } else {
+      p.out_slots[o] = -1;
+      p.out_scores[o] = __longlong_as_double(0x7FF8000000000000ll);
+    }
+  }
+  if (tid == 0) {
+    p.out_counts[q] = n;
+    if (emitted > p.emit_cap[q]) atomicAdd(p.overflow, 1);   // the count pass missed rows: the answer is not proven
+  }
+}
+
+// --------------------------------------------------------------------------- all exact scores (k_fetch > 4096)
 // One thread per (row, query): the reference's fp64 cosine of EVERY row, NaN for tombstoned / zero rows.  Serves
-// requests for more hits than the scan's candidate lists hold (k_fetch > RBK_MAX_K_FETCH): the host then applies
-// `>= minScore`, the stable sort and the cut literally (vector-store.ts:212-221).  Rare and small (RunbookAI's
-// corpora are 10^4-10^5 chunks when somebody asks for 1000 results), so simplicity wins over bandwidth here.
+// requests for more hits than the large-k search keeps (k_fetch > RBK_MAX_K_FETCH_LARGE): the host then applies
+// `>= minScore`, the stable sort and the cut literally (vector-store.ts:212-221).  Beyond 4096 hits per query the
+// host-side cut dominates anyway, so simplicity wins over bandwidth here.
 __global__ void __launch_bounds__(256) exact_scores_kernel(const uint16_t* __restrict__ rows,
                                                            const double* __restrict__ rows_f64,
                                                            const double* __restrict__ row_norm2,
@@ -793,6 +958,30 @@ cudaError_t launch_exact_scores(const uint16_t* rows, const double* rows_f64, co
   dim3 grid(static_cast<unsigned>((n_rows + 255) / 256), static_cast<unsigned>(B));
   exact_scores_kernel<<<grid, 256, 0, stream>>>(rows, rows_f64, row_norm2, dead_bits, n_rows, d, dpad, q_f64, q_norm2,
                                                 out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init, const float* inv_norm_q,
+                                const double* q_eps, int B, int k_fetch, float* theta, int* cap, cudaStream_t stream) {
+  if (B <= 0) return cudaSuccess;
+  large_select_kernel<<<B, 256, 0, stream>>>(hist, thr_init, inv_norm_q, q_eps, k_fetch, theta, cap);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, cudaStream_t stream) {
+  if (p.B <= 0) return cudaSuccess;
+  if (max_cap > 0) {
+    dim3 grid(static_cast<unsigned>((max_cap + 255) / 256), static_cast<unsigned>(p.B));
+    large_score_kernel<<<grid, 256, 0, stream>>>(p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  int S = 2048;
+  while (S < p.k_fetch + kTopThreads) S <<= 1;
+  const size_t smem = static_cast<size_t>(S) * (sizeof(double) + sizeof(int));
+  cudaError_t e = cudaFuncSetAttribute(large_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  large_topk_kernel<<<p.B, kTopThreads, smem, stream>>>(p, S);
   return cudaGetLastError();
 }
 

@@ -245,6 +245,81 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
   return RBK_OK;
 }
 
+// Large-k search over the group: count scan + select on every device, ONE wait for all of them (C_q sizes each
+// device's candidate buffer), emit scan + exact re-rank on every device into its packed block (flags zero: the
+// answers are exact by construction), then the all-gather and merge of group_search.
+rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
+                              double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts,
+                              float* ms_out) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score,
+                                    RBK_MAX_K_FETCH_LARGE);
+  if (st != RBK_OK) return st;
+  if (ms_out) *ms_out = 0.f;
+  if (B == 0) return RBK_OK;
+  std::lock_guard<std::mutex> lk(g->mu);
+  const size_t q_bytes = static_cast<size_t>(B) * g->dim * 8;
+  const size_t blk = static_cast<size_t>(rbk_packed_block_bytes(B, k_fetch));
+  const size_t off_f = static_cast<size_t>(rbk_packed_flags_offset(B, k_fetch));
+  const size_t nk = static_cast<size_t>(B) * k_fetch;
+  const size_t out_bytes = nk * 16 + (2 * static_cast<size_t>(B) + 1) * 4;
+  {
+    DeviceGuard dg(g->devices[0]);
+    CK(g->h_q.ensure(q_bytes));
+    CK(g->h_out.ensure(out_bytes));
+    CK(g->out.ensure(out_bytes));
+  }
+  memcpy(g->h_q.p, queries, q_bytes);
+  for (int d = 0; d < g->G; ++d) {
+    rbk_index* ix = g->parts[d];
+    std::lock_guard<std::mutex> il(ix->mu);
+    DeviceGuard dg(ix->device);
+    CK(g->dev[d].q.ensure(q_bytes));
+    CK(g->dev[d].local.ensure(blk));
+    if (g->G > 1) CK(g->dev[d].all.ensure(blk * g->G));
+    if (d == 0) CK(cudaEventRecord(g->ev0, ix->stream));
+    CK(cudaMemcpyAsync(g->dev[d].q.p, g->h_q.p, q_bytes, cudaMemcpyHostToDevice, ix->stream));
+    st = ensure_query_scratch(ix, B, 8);
+    if (st != RBK_OK) return st;
+    st = large_count(ix, g->dev[d].q.p, B, k_fetch, min_score);
+    if (st != RBK_OK) return st;
+  }
+  for (int d = 0; d < g->G; ++d) {
+    DeviceGuard dg(g->parts[d]->device);
+    CK(cudaStreamSynchronize(g->parts[d]->stream));
+  }
+  for (int d = 0; d < g->G; ++d) {
+    rbk_index* ix = g->parts[d];
+    std::lock_guard<std::mutex> il(ix->mu);
+    DeviceGuard dg(ix->device);
+    unsigned char* l = g->dev[d].local.p;
+    st = large_emit(ix, B, k_fetch, min_score, reinterpret_cast<long long*>(l), reinterpret_cast<double*>(l + nk * 8),
+                    reinterpret_cast<int*>(l + nk * 16));
+    if (st != RBK_OK) return st;
+    CK(cudaMemsetAsync(l + off_f, 0, static_cast<size_t>(B) * 4, ix->stream));
+  }
+  st = exchange_and_merge(g, B, k_fetch, blk);
+  if (st != RBK_OK) return st;
+  {
+    rbk_index* i0 = g->parts[0];
+    DeviceGuard dg(i0->device);
+    CK(cudaMemcpyAsync(g->h_out.p, g->out.p, out_bytes, cudaMemcpyDeviceToHost, i0->stream));
+    CK(cudaEventRecord(g->ev1, i0->stream));
+  }
+  for (int d = 0; d < g->G; ++d) {   // every device's overflow counter has landed on the host
+    DeviceGuard dg(g->parts[d]->device);
+    CK(cudaStreamSynchronize(g->parts[d]->stream));
+    st = large_check(g->parts[d]);
+    if (st != RBK_OK) return st;
+  }
+  if (ms_out) cudaEventElapsedTime(ms_out, g->ev0, g->ev1);
+  memcpy(out_slots, g->h_out.p, nk * 8);
+  memcpy(out_scores, g->h_out.p + nk * 8, nk * 8);
+  memcpy(out_counts, g->h_out.p + nk * 16, static_cast<size_t>(B) * 4);
+  return RBK_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -412,6 +487,12 @@ rbk_status rbk_group_search_f64(rbk_group* g, const double* queries, int32_t B, 
                                 double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts,
                                 float* device_ms_out) {
   return group_search(g, queries, 8, B, query_dim, k_fetch, min_score, out_slots, out_scores, out_counts, device_ms_out);
+}
+rbk_status rbk_group_search_large_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,
+                                      int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* device_ms_out) {
+  return group_search_large(g, queries, B, query_dim, k_fetch, min_score, out_slots, out_scores, out_counts,
+                            device_ms_out);
 }
 
 }  // extern "C"

@@ -100,6 +100,13 @@ struct rbk_index {
   rbk::impl::DevBuf<long long> o_slots;
   rbk::impl::DevBuf<double> o_scores, part_scores;
   rbk::impl::DevBuf<float> dbg;
+  // large-k search scratch (grow-only): theta_q, C_q, emit counters, segment offsets, flat candidate rows + scores
+  rbk::impl::DevBuf<float> lg_theta;
+  rbk::impl::DevBuf<int> lg_cap, lg_cnt, lg_rows, lg_err;
+  rbk::impl::DevBuf<long long> lg_off;
+  rbk::impl::DevBuf<double> lg_scores;
+  rbk::impl::PinBuf<int> h_lcap, h_lerr;
+  rbk::impl::PinBuf<long long> h_loff;
   rbk::impl::DevBuf<unsigned char> o_block;
   rbk::impl::PinBuf<unsigned char> h_block;
   rbk::impl::PinBuf<int> h_flags, h_counts;
@@ -143,10 +150,22 @@ namespace impl {
 
 // caller holds ix->mu and has the index's device current
 rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem);
-rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, int k_fetch, double min_score);
+// max_k: RBK_MAX_K_FETCH (the search) or RBK_MAX_K_FETCH_LARGE (the large-k search)
+rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, int k_fetch, double min_score,
+                             int max_k = RBK_MAX_K_FETCH);
 // Enqueue-only search of device-resident queries: no host synchronisation, exactness flags land in d_flags.
 rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, int k_fetch, double min_score,
                           long long* d_slots, double* d_scores, int* d_counts, int* d_flags);
+// Large-k search of B device-resident f64 queries (caller holds the lock, scratch for B queries is allocated), in
+// two halves around one host synchronisation of the index stream:
+//   large_count: prep, count pass and select per sub-batch, then the D2H of C_q (enqueue only);
+//   large_emit : (after the stream has been synchronised) segment offsets on the host, emit pass and exact re-rank
+//                per sub-batch into d_slots / d_scores / d_counts, then the D2H of the overflow counter (enqueue only);
+//   large_check: (after the next synchronisation) RBK_ECUDA if any query emitted more rows than its bound.
+rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, double min_score);
+rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long long* d_slots, double* d_scores,
+                      int* d_counts);
+rbk_status large_check(rbk_index* ix);
 const char* last_error();
 
 }  // namespace impl

@@ -42,6 +42,21 @@ struct ScanParams {
 cudaError_t launch_scan(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const ScanParams& p,
                         cudaStream_t stream);
 
+// The two passes of the large-k search (k_fetch up to RBK_MAX_K_FETCH_LARGE) run the same scan with another epilogue:
+// count every row above a running threshold into the histogram, or emit every row above a fixed threshold.  Their
+// extra fields live in a derived struct so that the top-k' kernel's parameter block stays as it is.
+// kprime is k_fetch; in emit mode thr_init holds theta_q; cand / cand_cnt / dbg_scores are unused.
+struct LargeScanParams : ScanParams {
+  const double* q_eps;       // count: [B] error bound of the approximate cosine
+  const long long* emit_off; // emit: [B] start of query q's segment of emit_rows
+  const int* emit_cap;       // emit: [B] segment length C_q
+  int* emit_cnt;             // emit: [B] rows emitted (zeroed per launch; exceeds emit_cap only through a bug)
+  int* emit_rows;            // emit: flat local-row buffer
+};
+enum LargeScanMode { kScanCount = 1, kScanEmit = 2 };
+cudaError_t launch_scan_large(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const LargeScanParams& p,
+                              LargeScanMode mode, cudaStream_t stream);
+
 // ---- ingest (rbk_ingest.cu) ----
 // src element type: 0 = f64, 1 = f32, 2 = bf16 bits.  src is device memory, row pitch = d.
 // dst_f64 (nullable): exact-source sidecar rows, pitch d.
@@ -134,6 +149,32 @@ struct ExactParams {
   int* out_counts;
 };
 cudaError_t launch_exact_fallback(const ExactParams& p, cudaStream_t stream);
+
+// ---- large-k search (rbk_finalize.cu): select between the two scan passes, exact re-rank after them ----
+// theta [B] (raw domain) and cap [B] (C_q) from the count pass's histograms hist [B][kHistBins].
+cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init, const float* inv_norm_q,
+                                const double* q_eps, int B, int k_fetch, float* theta, int* cap, cudaStream_t stream);
+struct LargeRerankParams {
+  int B, d, dpad, k_fetch;
+  double min_score;
+  const uint16_t* rows;
+  const double* rows_f64;   // nullable: exact-source sidecar
+  const double* row_norm2;
+  SlotLayout slot;
+  const double* q_f64;      // offset to the sub-batch, like every per-query array below
+  const double* q_norm2;
+  const long long* emit_off;
+  const int* emit_cap;
+  const int* emit_cnt;
+  const int* emit_rows;
+  double* cand_scores;      // parallel to emit_rows
+  long long* out_slots;     // [B][k_fetch]
+  double* out_scores;       // [B][k_fetch]
+  int* out_counts;          // [B]
+  int* overflow;            // += queries whose emit pass found more rows than C_q (a broken count)
+};
+// max_cap: largest emit_cap of the launch (sizes the scoring grid)
+cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, cudaStream_t stream);
 
 // Exact fp64 cosine of every row for B prepared queries: out [B][n_rows], NaN = tombstoned / zero row.
 cudaError_t launch_exact_scores(const uint16_t* rows, const double* rows_f64, const double* row_norm2,

@@ -55,9 +55,11 @@ __device__ __forceinline__ void store_accumulators(float* scores, const float (&
   }
 }
 
+// kMode 0: top-k' candidate lists (P = ScanParams); kScanCount / kScanEmit: the large-k passes (P = LargeScanParams)
+template <int kMode, typename P>
 __global__ void __launch_bounds__(kScanThreads, 1)
 scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
-            const ScanParams p) {
+            const P p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);  // swizzled TMA boxes want 1024-B alignment
@@ -89,7 +91,12 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
 
   if (wgroup == 0) {
     // ===================== epilogue: thread <-> query =====================
-    run_epilogue(p, tail->invc, &tail->sc_full, &tail->sc_empty, scores, qb, r, t0, t1, threadIdx.x, lane);
+    if constexpr (kMode == 0)
+      run_epilogue(p, tail->invc, &tail->sc_full, &tail->sc_empty, scores, qb, r, t0, t1, threadIdx.x, lane);
+    else if constexpr (kMode == kScanCount)
+      run_count_epilogue(p, tail->invc, &tail->sc_full, &tail->sc_empty, scores, qb, t0, t1, threadIdx.x);
+    else
+      run_emit_epilogue(p, tail->invc, &tail->sc_full, &tail->sc_empty, scores, qb, t0, t1, threadIdx.x);
     return;
   }
 
@@ -153,16 +160,27 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
   if (producer && lane == 0 && p.QB > 1) prog[qb] = 0x7FFFFFFF;  // done: never hold a peer back
 }
 
+template <int kMode, typename P>
+cudaError_t launch_scan_mode(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const P& p, cudaStream_t stream) {
+  const size_t smem = static_cast<size_t>(kStages) * kStageBytes + kScoreBytes + sizeof(SmemTail) + 1024;
+  // per-device attribute; cheap enough to set on every launch
+  cudaError_t e = cudaFuncSetAttribute(scan_kernel<kMode, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  scan_kernel<kMode, P><<<p.QB * p.R, kScanThreads, smem, stream>>>(tmap_q, tmap_c, p);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 cudaError_t launch_scan(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const ScanParams& p,
                         cudaStream_t stream) {
-  const size_t smem = static_cast<size_t>(kStages) * kStageBytes + kScoreBytes + sizeof(SmemTail) + 1024;
-  // per-device attribute; cheap enough to set on every launch
-  cudaError_t e = cudaFuncSetAttribute(scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  scan_kernel<<<p.QB * p.R, kScanThreads, smem, stream>>>(tmap_q, tmap_c, p);
-  return cudaGetLastError();
+  return launch_scan_mode<0>(tmap_q, tmap_c, p, stream);
+}
+
+cudaError_t launch_scan_large(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const LargeScanParams& p,
+                              LargeScanMode mode, cudaStream_t stream) {
+  if (mode == kScanCount) return launch_scan_mode<kScanCount>(tmap_q, tmap_c, p, stream);
+  return launch_scan_mode<kScanEmit>(tmap_q, tmap_c, p, stream);
 }
 
 }  // namespace rbk

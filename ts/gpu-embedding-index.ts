@@ -149,7 +149,8 @@ export class GpuEmbeddingIndex {
   /**
    * The same for B queries in ONE device pass (what B sequential search() calls cost the reference): the entry point
    * of the micro-batcher that coalesces concurrent searches of several investigations (SURVEY 8f-3;
-   * runbookai_b200/batcher.py is the tested mirror).  limit <= 112 per pass (RBK_MAX_K_FETCH).
+   * runbookai_b200/batcher.py is the tested mirror).  limit <= 112 takes one scan (RBK_MAX_K_FETCH); up to 4096
+   * (RBK_MAX_K_FETCH_LARGE) the large-k search (two scans and an exact re-rank).
    */
   async bestBatch(queries: number[][], limit: number, minScore: number): Promise<ScoredId[][]> {
     if (!this.index || this.slotOfId.size === 0) return queries.map(() => []);
@@ -159,7 +160,10 @@ export class GpuEmbeddingIndex {
     const B = queries.length;
     const packed = new Float64Array(B * this.dim);
     queries.forEach((q, b) => packed.set(q, b * this.dim));
-    const { slots, scores, counts } = await this.index.search(packed, B, limit, minScore);
+    const { slots, scores, counts } =
+      limit > 112
+        ? await this.index.searchLarge(packed, B, limit, minScore)
+        : await this.index.search(packed, B, limit, minScore);
     return queries.map((_, b) => {
       const out: ScoredId[] = [];
       for (let i = 0; i < counts[b]; i++) {
@@ -180,7 +184,7 @@ export class GpuEmbeddingIndex {
  * (`bestBatch`), and every caller gets exactly what its own `best()` would have returned - the pass fetches for the
  * most demanding caller (largest limit, lowest minScore) and each caller's own `>= minScore` and cut are re-applied.
  * runbookai_b200/batcher.py is the tested mirror of this class (same coalescing, same per-caller cut, same
- * behaviour on close).  Callers whose limit exceeds one pass (112) go through on their own.
+ * behaviour on close).  Callers whose limit exceeds one scan (112) go through on their own, to the large-k search.
  */
 export class SearchBatcher {
   private queue: Array<{
