@@ -853,8 +853,8 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
   rbk_index* ix = new (std::nothrow) rbk_index();
   if (!ix) return fail(RBK_ENOMEM, "out of host memory");
   ix->dim = dim;
-  // row pitch = whole 128-byte lines (pairs of 32-element k-blocks): no TMA box hangs over the end of a row either
-  ix->dpad = static_cast<int>(round_up(dim, 2 * kBlockK));
+  // row pitch = whole 128-byte lines (64-element k-blocks): no TMA box hangs over the end of a row
+  ix->dpad = static_cast<int>(round_up(dim, kBlockK));
   ix->device = device;
   ix->keep_f64 = (flags & RBK_INDEX_KEEP_F64) != 0;
   ix->sm_count = prop.multiProcessorCount;

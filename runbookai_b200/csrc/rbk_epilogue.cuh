@@ -123,19 +123,6 @@ __device__ __forceinline__ void adopt_threshold(FilterState& s, unsigned int ord
   s.thr = fmaxf(s.thr, f32_from_ordered(ordered));   // 0 (nothing published) decodes to NaN, which fmaxf drops
 }
 
-// 1/||c|| of a chunk's rows: from shared memory (staged per tile) or, kGlobal, straight from the corpus-norm
-// array through L1 (every lane reads the same address: one broadcast transaction).
-template <bool kGlobal>
-__device__ __forceinline__ float4 norm4(const float4* p) {
-  if constexpr (kGlobal) return __ldg(p);
-  else return *p;
-}
-template <bool kGlobal>
-__device__ __forceinline__ float norm1(const float* p) {
-  if constexpr (kGlobal) return __ldg(p);
-  else return *p;
-}
-
 // Count one row of raw score t in the query's global histogram.  Every row must be counted AT MOST once:
 // the counts are lower bounds on "rows of the corpus with a score in this bin", which is what makes a
 // threshold read off the histogram safe.
@@ -166,18 +153,16 @@ __device__ __forceinline__ void filter_append(FilterState& s, float t, uint32_t 
 // acc1 >= acc2: with whole_tile the two best rows seen so far in this thread's part of the tile (counted by the
 // caller after the last chunk: 2 atomics per thread instead of 2 per chunk - enough when many units feed the
 // same histogram, and an order of magnitude fewer same-line atomics in the first microseconds of a scan).
-template <bool kGlobal = false>
-__device__ __forceinline__ void seed_chunk(FilterState& s, const uint32_t (&v)[32], const float* invc32,
-                                           bool whole_tile, float& acc1, float& acc2) {
-  const float4* ic4 = reinterpret_cast<const float4*>(invc32);
+// v: 32 scores (accumulator * 1/||c||, NaN for dead rows) of this thread's query.
+__device__ __forceinline__ void seed_chunk(FilterState& s, const uint32_t (&v)[32], bool whole_tile, float& acc1,
+                                           float& acc2) {
   float m1 = -INFINITY, m2 = -INFINITY;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
-    const float4 w = norm4<kGlobal>(ic4 + j);
-    const float a0 = __uint_as_float(v[4 * j + 0]) * w.x;
-    const float a1 = __uint_as_float(v[4 * j + 1]) * w.y;
-    const float a2 = __uint_as_float(v[4 * j + 2]) * w.z;
-    const float a3 = __uint_as_float(v[4 * j + 3]) * w.w;
+    const float a0 = __uint_as_float(v[4 * j + 0]);
+    const float a1 = __uint_as_float(v[4 * j + 1]);
+    const float a2 = __uint_as_float(v[4 * j + 2]);
+    const float a3 = __uint_as_float(v[4 * j + 3]);
     const float x = fmaxf(fmaxf(fmaxf(a0, a1), fmaxf(a2, a3)), -INFINITY);   // a group of dead rows: NaN -> -inf
     m2 = fmaxf(m2, fminf(m1, x));
     m1 = fmaxf(m1, x);
@@ -192,20 +177,16 @@ __device__ __forceinline__ void seed_chunk(FilterState& s, const uint32_t (&v)[3
   if (m2 > s.thr) hist_add(s, m2);
 }
 
-// 32 accumulator columns of this thread's query; invc32 = the 32 matching 1/||c||.
-template <bool kGlobal = false>
-__device__ __forceinline__ void filter_chunk(FilterState& s, const uint32_t (&v)[32], const float* invc32,
-                                             uint32_t row_base) {
-  const float4* ic4 = reinterpret_cast<const float4*>(invc32);
+// 32 scores (accumulator * 1/||c||) of this thread's query, rows row_base .. row_base + 31.
+__device__ __forceinline__ void filter_chunk(FilterState& s, const uint32_t (&v)[32], uint32_t row_base) {
   float g[8];   // maxima of the 8 groups of 4 columns (intermediates of the chunk maximum, kept for the slow path)
   float m = -INFINITY;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
-    const float4 w = norm4<kGlobal>(ic4 + j);
-    const float a0 = __uint_as_float(v[4 * j + 0]) * w.x;
-    const float a1 = __uint_as_float(v[4 * j + 1]) * w.y;
-    const float a2 = __uint_as_float(v[4 * j + 2]) * w.z;
-    const float a3 = __uint_as_float(v[4 * j + 3]) * w.w;
+    const float a0 = __uint_as_float(v[4 * j + 0]);
+    const float a1 = __uint_as_float(v[4 * j + 1]);
+    const float a2 = __uint_as_float(v[4 * j + 2]);
+    const float a3 = __uint_as_float(v[4 * j + 3]);
     g[j] = fmaxf(fmaxf(a0, a1), fmaxf(a2, a3));   // fmaxf drops NaN (dead / out-of-range rows)
     m = fmaxf(m, g[j]);
   }
@@ -218,7 +199,7 @@ __device__ __forceinline__ void filter_chunk(FilterState& s, const uint32_t (&v)
       if (g[j] > s.thr) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const float t = __uint_as_float(v[4 * j + e]) * norm1<kGlobal>(invc32 + 4 * j + e);
+          const float t = __uint_as_float(v[4 * j + e]);
           if (t > s.thr) filter_append(s, t, row_base + 4 * j + e);
         }
       }
@@ -312,11 +293,11 @@ __device__ __forceinline__ void filter_compact_if_needed(FilterState& s, int kpr
 }
 
 
-// Floats per row of the CTA's score buffer: 4 more than a tile row so that the 8 threads of a quarter warp, which
-// read 16 bytes of 8 consecutive rows, hit 8 different groups of 4 banks.
+// Floats per row of the staging buffer: 4 more than a tile row so that the 8 threads of a quarter warp, which read
+// 16 bytes of 8 different rows, hit 8 different groups of 4 banks.
 constexpr int kScorePitch = kBlockN + 4;
 
-// 32 consecutive scores of one row of the score buffer.
+// 32 consecutive scores of one staged row.
 __device__ __forceinline__ void load_chunk(const float* src, uint32_t (&v)[32]) {
   const float4* s4 = reinterpret_cast<const float4*>(src);
 #pragma unroll
@@ -329,14 +310,35 @@ __device__ __forceinline__ void load_chunk(const float* src, uint32_t (&v)[32]) 
   }
 }
 
+// One round of the hand-off from a wgmma warpgroup to the epilogue threads of its 64 queries (rbk_scan.cu): the
+// scores (accumulator * 1/||c||) of the queries in `mask` (bit i = query 64 w + i of the block) sit in `rows`, query
+// by query in bit order, kScorePitch floats apart.  Every tile has at least one round; `last` marks its final one.
+struct StageHeader {
+  unsigned long long mask;
+  int last;
+};
+struct StageLink {
+  const float* rows;           // [kStageRows][kScorePitch]
+  const StageHeader* hdr;
+  unsigned long long* full;    // arrive: the warpgroup's 128 threads
+  unsigned long long* empty;   // arrive: the 64 epilogue threads of its queries
+  volatile float* thr_pub;     // this thread's slot of the per-query thresholds the warpgroup filters with
+};
+// Waits for the next round; returns this thread's staged row, nullptr when its query is not in the round.
+__device__ __forceinline__ const float* stage_round(const StageLink& l, uint32_t phase, int qw, bool& last) {
+  mbar_wait(smem_u32(l.full), phase);
+  const unsigned long long mask = l.hdr->mask;
+  last = l.hdr->last != 0;
+  if (((mask >> qw) & 1ull) == 0ull) return nullptr;
+  return l.rows + __popcll(mask & ((1ull << qw) - 1ull)) * kScorePitch;
+}
+
 // The whole epilogue role (thread <-> query) of the scan kernel: 128 threads (four warps), thread et filters the
-// kBlockN scores of query row et of every tile of its unit [t0, t1).  scores: the CTA's score buffer (kBlockM rows of
-// kScorePitch floats), filled by the wgmma warpgroups; sc_full / sc_empty hand it back and forth.  invc_stage: per-tile
-// staging of the tile's 1/||c||, double-buffered by tile parity.
-__device__ __forceinline__ void run_epilogue(const ScanParams& p, float (*invc_stage)[kBlockN],
-                                             unsigned long long* sc_full, unsigned long long* sc_empty,
-                                             const float* scores, int qb, int r, int t0, int t1, int et, int lane) {
-  constexpr int kEpi = kBlockM;
+// kBlockN scores of query row et of every tile of its unit [t0, t1) that the wgmma warpgroup hands over (see
+// StageLink).  A tile whose rows are all at or below the threshold this thread last published is not handed over:
+// filter_chunk would append none of it.
+__device__ __forceinline__ void run_epilogue(const ScanParams& p, const StageLink& sl, int qb, int r, int t0, int t1,
+                                             int et, int lane) {
   const int q = qb * kBlockM + et;
   const bool q_valid = q < p.B;
   const size_t list_id = static_cast<size_t>(qb * p.R + r) * kBlockM + et;
@@ -345,82 +347,80 @@ __device__ __forceinline__ void run_epilogue(const ScanParams& p, float (*invc_s
               p.cand + list_id * static_cast<size_t>(kListCap),
               p.hist + static_cast<size_t>(q_valid ? q : 0) * kHistBins, p.maxbin + (q_valid ? q : 0));
   const int n_iter = t1 - t0;
-  // 1/||c|| of a tile's 256 rows are staged in shared memory behind one barrier of all epilogue threads per
-  // tile (the warps wait there for the slowest of the previous tile); the NEXT tile's values travel in registers
-  // while this one is processed, which hides their L2/HBM latency.
-  float nx0 = 0.f, nx1 = 0.f;
+  const int qw = et & 63;
+  uint32_t phase = 0;
+  float pub = -INFINITY;   // last value written to sl.thr_pub (thresholds only rise)
   unsigned int* gthr_q = p.gthr + (q_valid ? q : 0);
   unsigned int ngt = 0u;   // published threshold, fetched one tile ahead
-  if (n_iter > 0) {
-    nx0 = __ldg(p.inv_norm_c + t0 * kBlockN + et);
-    nx1 = __ldg(p.inv_norm_c + t0 * kBlockN + kEpi + et);
-  }
-  const float* srow = scores + et * kScorePitch;
   for (int it = 0; it < n_iter; ++it) {
     const int tile = t0 + it;
     const int row0 = tile * kBlockN;
-    float* invc = invc_stage[it & 1];
-    invc[et] = nx0;
-    invc[kEpi + et] = nx1;
-    if (it + 1 < n_iter) {
-      nx0 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + et);
-      nx1 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + kEpi + et);
-    }
     adopt_threshold(fs, ngt);
     ngt = __ldcg(gthr_q);
-    named_bar_sync(1, kEpi);
     if (publish_due(it) && r == it % p.R) publish_threshold(fs, gthr_q, p.kprime);   // overlaps this tile's wgmma
-    mbar_wait(smem_u32(sc_full), static_cast<uint32_t>(it & 1));
-    auto process = [&](uint32_t (&v)[32], int chunk) {
-      filter_chunk(fs, v, invc + chunk * 32, static_cast<uint32_t>(row0 + chunk * 32));
-      if (p.dbg_scores != nullptr && q_valid) {
+    if (fs.thr > pub) *sl.thr_pub = pub = fs.thr;
+    for (bool last = false; !last; phase ^= 1u) {
+      const float* srow = stage_round(sl, phase, qw, last);
+      const bool staged = srow != nullptr;
+      if (__any_sync(0xFFFFFFFFu, staged)) {
+        auto process = [&](uint32_t (&v)[32], int chunk) {
+          filter_chunk(fs, v, static_cast<uint32_t>(row0 + chunk * 32));
+          if (p.dbg_scores != nullptr && q_valid) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int row = row0 + chunk * 32 + j;
-          if (row < p.n_rows)
-            p.dbg_scores[static_cast<size_t>(q) * p.n_rows + row] = __uint_as_float(v[j]) * invc[chunk * 32 + j];
+            for (int j = 0; j < 32; ++j) {
+              const int row = row0 + chunk * 32 + j;
+              if (row < p.n_rows) p.dbg_scores[static_cast<size_t>(q) * p.n_rows + row] = __uint_as_float(v[j]);
+            }
+          }
+        };
+        uint32_t va[32], vb[32];
+        if (it == 0) {
+          // seeding pass (see seed_chunk): count the best rows of this tile, then take the threshold they give.
+          // Every query of the block is staged in some round of a unit's first tile.
+          float sa1 = -INFINITY, sa2 = -INFINITY;
+          if (staged) {
+#pragma unroll 1
+            for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
+              load_chunk(srow + chunk * 32, va);
+              seed_chunk(fs, va, false, sa1, sa2);
+            }
+          }
+          // the other units' seeds land within a microsecond or so of ours: a few short retries when the
+          // histogram cannot hold k' rows yet but soon will
+          const int tries = (p.R * 16 >= 2 * p.kprime) ? 6 : 1;
+          for (int t = 0; t < tries; ++t) {
+            const bool found = staged && filter_refresh(fs, p.kprime);
+            if (__all_sync(0xFFFFFFFFu, found || !fs.valid || !staged)) break;
+            if (t + 1 < tries) __nanosleep(400);
+          }
+          if (staged && fs.valid && fs.thr > -INFINITY) atomicMax(gthr_q, f32_ordered(fs.thr));
+          fs.nohist = staged;
         }
-      }
-    };
-    uint32_t va[32], vb[32];
-    if (it == 0) {
-      // seeding pass (see seed_chunk): count the best rows of this tile, then take the threshold they give
-      float sa1 = -INFINITY, sa2 = -INFINITY;
 #pragma unroll 1
-      for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
-        load_chunk(srow + chunk * 32, va);
-        seed_chunk(fs, va, invc + chunk * 32, false, sa1, sa2);
+        for (int c2 = 0; c2 < kBlockN / 64; ++c2) {
+          if (staged) {
+            load_chunk(srow + (2 * c2) * 32, va);
+            load_chunk(srow + (2 * c2 + 1) * 32, vb);
+            process(va, 2 * c2);
+            process(vb, 2 * c2 + 1);
+          }
+          filter_compact_if_needed(fs, p.kprime, lane, 64);
+          // seeding found nothing (too few units, or their seeds were late): keep looking while the tile is filtered
+          if (it == 0 && staged && fs.valid && fs.thr == -INFINITY) adopt_threshold(fs, __ldcg(gthr_q));
+        }
+        fs.nohist = false;
       }
-      // the other units' seeds land within a microsecond or so of ours: a few short retries when the
-      // histogram cannot hold k' rows yet but soon will
-      const int tries = (p.R * 16 >= 2 * p.kprime) ? 6 : 1;
-      for (int t = 0; t < tries; ++t) {
-        const bool found = filter_refresh(fs, p.kprime);
-        if (__all_sync(0xFFFFFFFFu, found || !fs.valid)) break;
-        if (t + 1 < tries) __nanosleep(400);
-      }
-      if (fs.valid && fs.thr > -INFINITY) atomicMax(gthr_q, f32_ordered(fs.thr));
-      fs.nohist = true;
+      mbar_arrive(smem_u32(sl.empty));
     }
-#pragma unroll 1
-    for (int c2 = 0; c2 < kBlockN / 64; ++c2) {
-      load_chunk(srow + (2 * c2) * 32, va);
-      load_chunk(srow + (2 * c2 + 1) * 32, vb);
-      process(va, 2 * c2);
-      process(vb, 2 * c2 + 1);
-      filter_compact_if_needed(fs, p.kprime, lane, 64);
-      // seeding found nothing (too few units, or their seeds were late): keep looking while the tile is filtered
-      if (it == 0 && fs.valid && fs.thr == -INFINITY) adopt_threshold(fs, __ldcg(gthr_q));
-    }
-    fs.nohist = false;
-    mbar_arrive(smem_u32(sc_empty));
+    if (fs.thr > pub) *sl.thr_pub = pub = fs.thr;
   }
   p.cand_cnt[list_id] = fs.cnt;
 }
 
 // ---- large-k search (k_fetch up to RBK_MAX_K_FETCH_LARGE): two scans with the same tiling, no candidate lists ----
-// Both modes compute a row's approximate score with the SAME expression as filter_chunk (accumulator * 1/||c||, one
-// fp32 multiply), so a row has the same `a` in the count pass and in the emit pass.  See DESIGN.md §6.
+// Both modes take a row's approximate score from the same staged value as filter_chunk (accumulator * 1/||c||, one
+// fp32 multiply in the wgmma warpgroup), so a row has the same `a` in the count pass and in the emit pass.  See
+// DESIGN.md §6.
 
 // Raw count-pass threshold for histogram bin b: the bin's lower edge lowered by `delta` (cosine domain), nudged down.
 // Monotonic in b.  The select kernel's theta_q (edge - 2 eps) stays above it by delta - 2 eps = one bin width, far more
@@ -434,10 +434,9 @@ __device__ __forceinline__ float count_floor_raw(int b, float qn, float delta) {
 // Count mode (pass A): every live row with a >= thr is counted in the query's global histogram, exactly once.  thr
 // starts at thr_init (min_score - eps) and rises to count_floor_raw of the highest bin with >= k_fetch counted rows
 // at or above it.  No seeding pass: the first tile's rows are all counted, so the histogram is complete down to thr.
-__device__ __forceinline__ void run_count_epilogue(const LargeScanParams& p, float (*invc_stage)[kBlockN],
-                                                   unsigned long long* sc_full, unsigned long long* sc_empty,
-                                                   const float* scores, int qb, int t0, int t1, int et) {
-  constexpr int kEpi = kBlockM;
+// A tile whose rows are all below the threshold this thread last published is not handed over.
+__device__ __forceinline__ void run_count_epilogue(const LargeScanParams& p, const StageLink& sl, int qb, int t0,
+                                                   int t1, int et) {
   const int q = qb * kBlockM + et;
   const bool q_valid = q < p.B;
   FilterState fs;
@@ -445,22 +444,10 @@ __device__ __forceinline__ void run_count_epilogue(const LargeScanParams& p, flo
               p.hist + static_cast<size_t>(q_valid ? q : 0) * kHistBins, p.maxbin + (q_valid ? q : 0));
   const float delta = q_valid ? static_cast<float>(2.0 * p.q_eps[q]) + 2.0f / kHistBins : 0.f;
   const int n_iter = t1 - t0;
-  float nx0 = 0.f, nx1 = 0.f;
-  if (n_iter > 0) {
-    nx0 = __ldg(p.inv_norm_c + t0 * kBlockN + et);
-    nx1 = __ldg(p.inv_norm_c + t0 * kBlockN + kEpi + et);
-  }
-  const float* srow = scores + et * kScorePitch;
+  const int qw = et & 63;
+  uint32_t phase = 0;
+  float pub = -INFINITY;
   for (int it = 0; it < n_iter; ++it) {
-    const int tile = t0 + it;
-    float* invc = invc_stage[it & 1];
-    invc[et] = nx0;
-    invc[kEpi + et] = nx1;
-    if (it + 1 < n_iter) {
-      nx0 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + et);
-      nx1 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + kEpi + et);
-    }
-    named_bar_sync(1, kEpi);
     if (fs.valid && refresh_due(it)) {
       const int mb = __ldcg(fs.maxbin_q);
       if (mb > fs.tb) {
@@ -471,48 +458,50 @@ __device__ __forceinline__ void run_count_epilogue(const LargeScanParams& p, flo
         }
       }
     }
-    mbar_wait(smem_u32(sc_full), static_cast<uint32_t>(it & 1));
+    if (fs.thr > pub) *sl.thr_pub = pub = fs.thr;
+    for (bool last = false; !last; phase ^= 1u) {
+      const float* srow = stage_round(sl, phase, qw, last);
+      if (srow != nullptr) {
 #pragma unroll 1
-    for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
-      uint32_t v[32];
-      load_chunk(srow + chunk * 32, v);
-      const float4* ic4 = reinterpret_cast<const float4*>(invc + chunk * 32);
-      float g[8];
-      float m = -INFINITY;
+        for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
+          uint32_t v[32];
+          load_chunk(srow + chunk * 32, v);
+          float g[8];
+          float m = -INFINITY;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 w = ic4[j];
-        const float a0 = __uint_as_float(v[4 * j + 0]) * w.x;
-        const float a1 = __uint_as_float(v[4 * j + 1]) * w.y;
-        const float a2 = __uint_as_float(v[4 * j + 2]) * w.z;
-        const float a3 = __uint_as_float(v[4 * j + 3]) * w.w;
-        g[j] = fmaxf(fmaxf(a0, a1), fmaxf(a2, a3));
-        m = fmaxf(m, g[j]);
-      }
-      if (m >= fs.thr) {
+          for (int j = 0; j < 8; ++j) {
+            const float a0 = __uint_as_float(v[4 * j + 0]);
+            const float a1 = __uint_as_float(v[4 * j + 1]);
+            const float a2 = __uint_as_float(v[4 * j + 2]);
+            const float a3 = __uint_as_float(v[4 * j + 3]);
+            g[j] = fmaxf(fmaxf(a0, a1), fmaxf(a2, a3));
+            m = fmaxf(m, g[j]);
+          }
+          if (m >= fs.thr) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (g[j] >= fs.thr) {
+            for (int j = 0; j < 8; ++j) {
+              if (g[j] >= fs.thr) {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float a = __uint_as_float(v[4 * j + e]) * invc[chunk * 32 + 4 * j + e];
-              if (a >= fs.thr) hist_add(fs, a);
+                for (int e = 0; e < 4; ++e) {
+                  const float a = __uint_as_float(v[4 * j + e]);
+                  if (a >= fs.thr) hist_add(fs, a);
+                }
+              }
             }
           }
         }
       }
+      mbar_arrive(smem_u32(sl.empty));
     }
-    mbar_arrive(smem_u32(sc_empty));
   }
 }
 
 // Emit mode (pass B): every row with a >= theta_q (p.thr_init holds theta_q) takes a slot in query q's segment of
 // p.emit_rows.  One atomicAdd per thread and chunk for all of the chunk's survivors.  The counter keeps counting past
-// the segment's capacity C_q, so an overflow - a broken count - is visible to the re-rank kernel.
-__device__ __forceinline__ void run_emit_epilogue(const LargeScanParams& p, float (*invc_stage)[kBlockN],
-                                                  unsigned long long* sc_full, unsigned long long* sc_empty,
-                                                  const float* scores, int qb, int t0, int t1, int et) {
-  constexpr int kEpi = kBlockM;
+// the segment's capacity C_q, so an overflow - a broken count - is visible to the re-rank kernel.  Only tiles with a
+// row at or above theta_q are handed over.
+__device__ __forceinline__ void run_emit_epilogue(const LargeScanParams& p, const StageLink& sl, int qb, int t0,
+                                                  int t1, int et) {
   const int q = qb * kBlockM + et;
   const bool q_valid = q < p.B;
   const float theta = q_valid ? p.thr_init[q] : INFINITY;
@@ -520,54 +509,35 @@ __device__ __forceinline__ void run_emit_epilogue(const LargeScanParams& p, floa
   const long long seg = live ? p.emit_off[q] : 0;
   const int cap = live ? p.emit_cap[q] : 0;
   const int n_iter = t1 - t0;
-  float nx0 = 0.f, nx1 = 0.f;
-  if (n_iter > 0) {
-    nx0 = __ldg(p.inv_norm_c + t0 * kBlockN + et);
-    nx1 = __ldg(p.inv_norm_c + t0 * kBlockN + kEpi + et);
-  }
-  const float* srow = scores + et * kScorePitch;
+  const int qw = et & 63;
+  uint32_t phase = 0;
+  *sl.thr_pub = theta;
   for (int it = 0; it < n_iter; ++it) {
-    const int tile = t0 + it;
-    const int row0 = tile * kBlockN;
-    float* invc = invc_stage[it & 1];
-    invc[et] = nx0;
-    invc[kEpi + et] = nx1;
-    if (it + 1 < n_iter) {
-      nx0 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + et);
-      nx1 = __ldg(p.inv_norm_c + (tile + 1) * kBlockN + kEpi + et);
-    }
-    named_bar_sync(1, kEpi);
-    mbar_wait(smem_u32(sc_full), static_cast<uint32_t>(it & 1));
+    const int row0 = (t0 + it) * kBlockN;
+    for (bool last = false; !last; phase ^= 1u) {
+      const float* srow = stage_round(sl, phase, qw, last);
+      if (srow != nullptr) {
 #pragma unroll 1
-    for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
-      uint32_t v[32];
-      load_chunk(srow + chunk * 32, v);
-      const float4* ic4 = reinterpret_cast<const float4*>(invc + chunk * 32);
-      uint32_t hits = 0u;
+        for (int chunk = 0; chunk < kBlockN / 32; ++chunk) {
+          uint32_t v[32];
+          load_chunk(srow + chunk * 32, v);
+          uint32_t hits = 0u;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 w = ic4[j];
-        const float a0 = __uint_as_float(v[4 * j + 0]) * w.x;
-        const float a1 = __uint_as_float(v[4 * j + 1]) * w.y;
-        const float a2 = __uint_as_float(v[4 * j + 2]) * w.z;
-        const float a3 = __uint_as_float(v[4 * j + 3]) * w.w;
-        hits |= (a0 >= theta ? 1u : 0u) << (4 * j + 0);
-        hits |= (a1 >= theta ? 1u : 0u) << (4 * j + 1);
-        hits |= (a2 >= theta ? 1u : 0u) << (4 * j + 2);
-        hits |= (a3 >= theta ? 1u : 0u) << (4 * j + 3);
-      }
-      if (hits != 0u && live) {
-        int pos = atomicAdd(p.emit_cnt + q, __popc(hits));
-        const int row_base = row0 + chunk * 32;
-        while (hits != 0u) {
-          const int j = __ffs(hits) - 1;
-          hits &= hits - 1u;
-          if (pos < cap) p.emit_rows[seg + pos] = row_base + j;
-          ++pos;
+          for (int j = 0; j < 32; ++j) hits |= (__uint_as_float(v[j]) >= theta ? 1u : 0u) << j;
+          if (hits != 0u && live) {
+            int pos = atomicAdd(p.emit_cnt + q, __popc(hits));
+            const int row_base = row0 + chunk * 32;
+            while (hits != 0u) {
+              const int j = __ffs(hits) - 1;
+              hits &= hits - 1u;
+              if (pos < cap) p.emit_rows[seg + pos] = row_base + j;
+              ++pos;
+            }
+          }
         }
       }
+      mbar_arrive(smem_u32(sl.empty));
     }
-    mbar_arrive(smem_u32(sc_empty));
   }
 }
 

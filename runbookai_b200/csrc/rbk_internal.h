@@ -9,8 +9,9 @@ namespace rbk {
 // ---- tiling of the fused scan (rbk_scan.cu) ----
 constexpr int kBlockM = 128;      // queries per CTA (two wgmma warpgroups of M = 64)
 constexpr int kBlockN = 256;      // corpus rows per tile (wgmma N)
-constexpr int kBlockK = 32;       // bf16 elements per pipeline stage (one 64-byte swizzle row)
-constexpr int kStages = 3;        // smem ring depth
+constexpr int kBlockK = 64;       // bf16 elements per pipeline stage (one 128-byte swizzle row)
+constexpr int kStages = 4;        // smem ring depth
+constexpr int kStageRows = 8;     // score rows a wgmma warpgroup hands to the epilogue per round
 constexpr int kListCap = 256;     // entries per (CTA, query) candidate list
 constexpr int kMaxKPrime = 128;   // candidates kept per query (k_fetch + margin)
 constexpr int kScanThreads = 384; // warpgroup 0 epilogue, warpgroups 1-2 wgmma (+ TMA issue)

@@ -63,6 +63,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap,
       : "memory");
 }
 
+// 1D bulk copy global -> shared (bytes and both addresses multiples of 16), completion on an mbarrier.
+__device__ __forceinline__ void bulk_load(uint32_t smem_dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               :
+               : "r"(smem_dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
+               : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma
 // Orders earlier register / shared-memory writes before the wgmma that follow (required before the first
 // wgmma of a batch that accumulates into registers).
@@ -77,15 +85,15 @@ __device__ __forceinline__ void wgmma_wait(float (&d)[128]) {
   for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Shared-memory matrix descriptor, K-major operand, 64-byte swizzle, rows of 32 bf16 (64 B) packed
-// densely: 8-row groups are 512 B apart (SBO); LBO is unused for swizzled K-major layouts (encoded 1);
-// layout type [62,64) = 2 (SWIZZLE_64B).  Advancing K by 16 elements = +32 B = +2 in the address field.
-__device__ __forceinline__ uint64_t make_sw64_kmajor_desc(uint32_t smem_addr) {
+// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 bf16 (128 B) packed
+// densely: 8-row groups are 1024 B apart (SBO); LBO is unused for swizzled K-major layouts (encoded 1);
+// layout type [62,64) = 1 (SWIZZLE_128B).  Advancing K by 16 elements = +32 B = +2 in the address field.
+__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // [0,14)  start address >> 4
   d |= static_cast<uint64_t>(1) << 16;                      // [16,30) leading byte offset >> 4
-  d |= static_cast<uint64_t>(512 >> 4) << 32;               // [32,46) stride byte offset >> 4
-  d |= static_cast<uint64_t>(2) << 62;                      // [62,64) SWIZZLE_64B
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;              // [32,46) stride byte offset >> 4
+  d |= static_cast<uint64_t>(1) << 62;                      // [62,64) SWIZZLE_128B
   return d;
 }
 
@@ -139,6 +147,16 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 // ---------------------------------------------------------------- misc
+// Per-warp register budget of the executing warpgroup (warpgroup-collective; N a multiple of 8 in [24, 256]).  What
+// one warpgroup gives back (dec) another can take (inc) as long as the CTA's total stays what it was launched with.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
