@@ -104,8 +104,20 @@ rbk_status rbk_index_overwrite_f64(rbk_index* idx, int64_t local_slot, const dou
  * written (the host mirror never overwrites a deleted id, so this is a caller bug, not a data path).  A slot named
  * more than once takes its LAST row, as Map.set twice would. */
 rbk_status rbk_index_overwrite_f64_batch(rbk_index* idx, const int64_t* local_slots, int64_t n, const double* rows);
-/* `this.embeddings.delete(id)`: the rows stop matching; slots are not reused. */
+/* `this.embeddings.delete(id)`: the rows stop matching.  Their slots stay allocated (size() does not shrink) until
+ * rbk_index_compact reclaims them. */
 rbk_status rbk_index_tombstone(rbk_index* idx, const int64_t* local_slots, int64_t n);
+/* Reclaim the slots of tombstoned rows.  The live rows move down to local slots 0 .. count()-1 in their current
+ * order (the Map's iteration order survives, so tie order and every search answer are unchanged up to the
+ * renumbering); afterwards size() == count().  old_to_new (nullable) receives, for every local slot s < size()
+ * before the call, its new local slot, or -1 if s was tombstoned; old_to_new_len must then be >= that size()
+ * (RBK_EINVAL otherwise, index untouched).  Liveness is the tombstone bits alone: a zero row stays, in its place.
+ * slot_base is kept, so global slots stay slot_base + local.  Capacity is kept: later appends reuse the reclaimed
+ * slots.  Without tombstones nothing moves and the identity map is returned.  Staging is one 64 MB buffer, allocated
+ * before the first row moves (RBK_ENOMEM leaves the index untouched).  Not available for the member indexes of a
+ * group (RBK_EINVAL).  Synchronous.  Searches enqueued before the call (rbk_index_search_device_async) run first,
+ * because the index's work is stream-ordered; their results carry the OLD slots. */
+rbk_status rbk_index_compact(rbk_index* idx, int64_t* old_to_new, int64_t old_to_new_len);
 rbk_status rbk_index_clear(rbk_index* idx);
 int64_t rbk_index_count(const rbk_index* idx); /* live rows  */
 int64_t rbk_index_size(const rbk_index* idx);  /* slots used, tombstones included */

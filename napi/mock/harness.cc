@@ -1,7 +1,8 @@
 // harness.cc - plays the JavaScript side of ts/gpu-embedding-index.ts against napi/rbk_napi.cc through the mock
 // N-API runtime (mock_napi.cc): loads the module, constructs RbkIndex (one device or a device list), loads rows as
 // SQLite-style BLOBs and as a Float64Array, overwrites, tombstones, counts, searches through the Promise/async-work
-// path, provokes every error path, clears, and lets the finalizer run.  Inputs and outputs are flat binary files in
+// path, provokes every error path, optionally (compact.txt) tombstones more, compacts and searches again, clears,
+// and lets the finalizer run.  Inputs and outputs are flat binary files in
 // the directory given as argv[1]; tests/test_napi_addon.py writes the inputs and checks the outputs against the
 // oracle.  Links against librbk_knn.so (GPU test) or against tests/napi_shim (CPU test).
 //
@@ -232,6 +233,37 @@ int main(int argc, char** argv) {
         << (again.slots == res.slots && again.counts == res.counts &&
             memcmp(again.scores.data(), res.scores.data(), res.scores.size() * 8) == 0)
         << "\n";
+  }
+
+  // compact(): optional compact.txt lists more slots to tombstone first; then compact() and the same search again,
+  // results in compact_*.  On a device-group handle compact() must throw (logged as err_compact).
+  {
+    std::ifstream cf(g_dir + "/compact.txt");
+    std::vector<int64_t> more;
+    int64_t s;
+    while (cf >> s) more.push_back(s);
+    if (!more.empty()) {
+      if (!mock::call_method(env, ix, "tombstone",
+                             {mock::typed_array(env, napi_bigint64_array, more.data(), more.size())}, &r, &err))
+        die("tombstone before compact threw: " + err);
+      if (!mock::call_method(env, ix, "compact", {}, &r, &err)) {
+        if (n_dev == 0) die("compact threw: " + err);
+        log << "err_compact " << err << "\n";
+      } else {
+        napi_typedarray_type t;
+        size_t n;
+        const void* p = mock::typed_data(r, &t, &n);
+        if (!p || t != napi_bigint64_array || n != static_cast<size_t>(n_rows)) die("compact() is not a BigInt64Array[n_rows]");
+        write_bin("compact_map.i64", p, n * 8);
+        if (!mock::call_method(env, ix, "count", {}, &r, &err)) die("count threw: " + err);
+        log << "count_after_compact " << mock::as_number(r) << "\n";
+        Result cr;
+        if (!search(env, ix, queries, n_q, k, min_score, &cr, &err)) die("search after compact rejected: " + err);
+        write_bin("compact_slots.i64", cr.slots.data(), cr.slots.size() * 8);
+        write_bin("compact_scores.f64", cr.scores.data(), cr.scores.size() * 8);
+        write_bin("compact_counts.i32", cr.counts.data(), cr.counts.size() * 4);
+      }
+    }
   }
 
   // clear(): Map.clear

@@ -16,6 +16,7 @@
 //   ix.appendBlobs(Buffer[] blobs)             -> firstSlot     // SQLite f64-LE BLOBs, packed in C++: no JS copies
 //   ix.overwriteF64(slot, Float64Array row); ix.overwriteF64Batch(BigInt64Array slots, Float64Array rows)
 //   ix.tombstone(BigInt64Array slots); ix.clear()
+//   ix.compact()                               -> BigInt64Array oldToNew   // reclaim tombstoned slots (one GPU only)
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
 //   await ix.searchLarge(Float64Array queries, B, kFetch, minScore)   // kFetch up to 4096, same result object
@@ -36,6 +37,10 @@
 // failing to load.
 #pragma weak rbk_index_search_large_f64
 #pragma weak rbk_group_search_large_f64
+// The same for compaction; `compact` throws where it is missing.  rbk_index_size, which sizes the map, is weak with it
+// so that the method as a whole needs nothing a library without compaction may lack.
+#pragma weak rbk_index_compact
+#pragma weak rbk_index_size
 
 namespace {
 
@@ -240,6 +245,28 @@ napi_value Clear(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+// compact() -> BigInt64Array old_to_new: reclaim the slots of tombstoned rows; old slot s now lives at
+// old_to_new[s] (-1 = it was deleted).  Synchronous.  Single-device handles only.
+napi_value Compact(napi_env env, napi_callback_info info) {
+  size_t argc = 0;
+  Handle* h = unwrap(env, info, &argc, nullptr);
+  if (h->grp) {
+    napi_throw_error(env, nullptr, "compaction is not available for a device group");
+    return nullptr;
+  }
+  if (rbk_index_compact == nullptr || rbk_index_size == nullptr) {
+    napi_throw_error(env, nullptr, "compact: this librbk_knn.so has no compaction (rbk_index_compact)");
+    return nullptr;
+  }
+  const int64_t n = rbk_index_size(h->ix);
+  napi_value ab, out;
+  void* p = nullptr;
+  NAPI_OK(napi_create_arraybuffer(env, (size_t)n * 8, &p, &ab));
+  if (rbk_index_compact(h->ix, static_cast<int64_t*>(p), n) != RBK_OK) return throw_rbk(env);
+  NAPI_OK(napi_create_typedarray(env, napi_bigint64_array, (size_t)n, ab, 0, &out));
+  return out;
+}
+
 napi_value Count(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
@@ -344,6 +371,7 @@ napi_value Init(napi_env env, napi_value exports) {
       {"overwriteF64Batch", nullptr, OverwriteF64Batch, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"tombstone", nullptr, Tombstone, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"clear", nullptr, Clear, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"compact", nullptr, Compact, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"count", nullptr, Count, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"search", nullptr, Search, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"searchLarge", nullptr, SearchLarge, nullptr, nullptr, nullptr, napi_default, nullptr},

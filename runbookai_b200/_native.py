@@ -20,7 +20,7 @@ RBK_MAX_K_FETCH_LARGE = 4096
 SYMBOLS = [
     "rbk_abi_version", "rbk_last_error", "rbk_index_create", "rbk_index_create_ex", "rbk_index_destroy", "rbk_index_set_stream",
     "rbk_index_set_slot_base", "rbk_index_append_f64", "rbk_index_append_f32", "rbk_index_append_bf16",
-    "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_clear",
+    "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_compact", "rbk_index_clear",
     "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_read_rows_bf16", "rbk_index_search_f64",
     "rbk_index_search_f32", "rbk_index_search_large_f64", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
     "rbk_packed_block_bytes", "rbk_packed_flags_offset",
@@ -74,6 +74,7 @@ def _load() -> C.CDLL:
     lib.rbk_index_overwrite_f64.argtypes = [vp, i64, vp]
     lib.rbk_index_overwrite_f64_batch.argtypes = [vp, vp, i64, vp]
     lib.rbk_index_tombstone.argtypes = [vp, vp, i64]
+    lib.rbk_index_compact.argtypes = [vp, vp, i64]
     lib.rbk_index_clear.argtypes = [vp]
     for n in ("rbk_index_count", "rbk_index_size"):
         getattr(lib, n).argtypes = [vp]
@@ -241,6 +242,14 @@ class Index:
     def tombstone(self, slots) -> None:
         s = np.ascontiguousarray(slots, dtype=np.int64)
         check(lib.rbk_index_tombstone(self._h, ptr(s), s.shape[0]))
+
+    def compact(self) -> np.ndarray:
+        """Reclaim the slots of tombstoned rows: the live rows move down to slots 0 .. count()-1 in their current
+        order.  Returns old_to_new, int64 [size() before the call]: each old local slot's new one, -1 if it was
+        tombstoned."""
+        out = np.empty(self.size(), dtype=np.int64)
+        check(lib.rbk_index_compact(self._h, ptr(out), out.shape[0]))
+        return out
 
     def clear(self) -> None:
         check(lib.rbk_index_clear(self._h))

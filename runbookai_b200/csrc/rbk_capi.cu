@@ -894,6 +894,8 @@ void rbk_index_destroy(rbk_index* ix) {
     cudaFree(ix->d_counter);
     ix->stage.release();
     ix->d_slots.release();
+    ix->cp_map.release();
+    ix->cp_scan.release();
     ix->q_raw.release();
     ix->q_bf16.release();
     ix->q_f64.release();
@@ -1071,6 +1073,79 @@ rbk_status rbk_index_clear(rbk_index* ix) {
   CK(cudaStreamSynchronize(ix->stream));
   ix->n_rows = 0;
   ix->n_live = 0;
+  return RBK_OK;
+}
+
+rbk_status rbk_index_compact(rbk_index* ix, int64_t* old_to_new, int64_t old_to_new_len) {
+  if (!ix) return fail(RBK_EINVAL, "null index");
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  const int64_t n = ix->n_rows, n_live = ix->n_live;
+  if (old_to_new && old_to_new_len < n) return fail(RBK_EINVAL, "old_to_new_len is shorter than size()");
+  if (ix->slot.block != 0)   // block-cyclic rows: moving them would break the group's slot layout
+    return fail(RBK_EINVAL, "compaction is not available for a member of a device group");
+  if (n_live == n) {         // no tombstones (or an empty index): nothing moves, every cache stays valid
+    for (int64_t s = 0; old_to_new && s < n; ++s) old_to_new[s] = s;
+    return RBK_OK;
+  }
+  // Staging chunk: whole 32-row words, 64 MB (the append path's staging size) of packed rows.
+  //   stage = bf16 rows [C][dpad] | f64 rows [C][dim] (KEEP_F64) | norm2 [C] | inv_norm [C]
+  const int64_t row_bytes = static_cast<int64_t>(ix->dpad) * 2 + (ix->keep_f64 ? static_cast<int64_t>(ix->dim) * 8 : 0) + 12;
+  const int64_t C = std::min(round_up(n, 32), std::max<int64_t>(32, (64ll << 20) / row_bytes / 32 * 32));
+  const int64_t n_chunks = (n + C - 1) / C;
+  const int64_t n_words = (n + 31) / 32, n_blocks = (n_words + 1023) / 1024;
+  // every allocation before the first row moves: RBK_ENOMEM leaves the index untouched
+  CK(ix->stage.ensure(static_cast<size_t>(C * row_bytes)));
+  CK(ix->cp_map.ensure(static_cast<size_t>(n)));
+  CK(ix->cp_scan.ensure(static_cast<size_t>(n_words + n_blocks + n_chunks + 1)));
+  int* word_pref = ix->cp_scan.p;
+  int* block_sum = word_pref + n_words;
+  int* chunk_pref_d = block_sum + n_blocks;
+  std::vector<int> chunk_pref(static_cast<size_t>(n_chunks + 1));
+  CK(launch_compact_map(ix->dead_bits, n, C, word_pref, block_sum, ix->cp_map.p, chunk_pref_d, ix->stream));
+  ix->stats.kernel_launches += 3;
+  CK(cudaMemcpyAsync(chunk_pref.data(), chunk_pref_d, sizeof(int) * (n_chunks + 1), cudaMemcpyDeviceToHost, ix->stream));
+  if (old_to_new)
+    CK(cudaMemcpyAsync(old_to_new, ix->cp_map.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, ix->stream));
+  CK(cudaStreamSynchronize(ix->stream));
+  if (chunk_pref[n_chunks] != n_live)
+    return fail(RBK_ECUDA, "compaction: the tombstone bits count " + std::to_string(chunk_pref[n_chunks]) +
+                               " live rows, the index " + std::to_string(n_live) + " (the index was not changed)");
+  unsigned char* st = ix->stage.p;
+  uint16_t* st_rows = reinterpret_cast<uint16_t*>(st);
+  double* st_f64 = reinterpret_cast<double*>(st + C * ix->dpad * 2);
+  double* st_norm2 = reinterpret_cast<double*>(st + C * (row_bytes - 12));
+  float* st_inv = reinterpret_cast<float*>(st + C * (row_bytes - 4));
+  // In place, stable, one chunk of sources at a time.  Chunk [s0, s1) holds L live rows that land at [d0, d0 + L) with
+  // d0 + L <= s1: the copies overwrite only rows of this chunk and of earlier ones, all already staged, never a
+  // source of a later chunk.  Chunks before the first tombstone (d0 == s0, L == s1 - s0) do not move.
+  for (int64_t c = 0; c < n_chunks; ++c) {
+    const int64_t s0 = c * C, s1 = std::min(n, s0 + C);
+    const int64_t d0 = chunk_pref[c], L = chunk_pref[c + 1] - d0;
+    if ((d0 == s0 && L == s1 - s0) || L == 0) continue;
+    CK(launch_compact_gather(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, ix->norm2, ix->inv_norm, ix->cp_map.p,
+                             s0, s1 - s0, d0, ix->dim, ix->dpad, st_rows, st_f64, st_norm2, st_inv, ix->sm_count,
+                             ix->stream));
+    ix->stats.kernel_launches++;
+    CK(cudaMemcpyAsync(ix->rows + d0 * ix->dpad, st_rows, static_cast<size_t>(L) * ix->dpad * 2,
+                       cudaMemcpyDeviceToDevice, ix->stream));
+    if (ix->keep_f64)
+      CK(cudaMemcpyAsync(ix->rows_f64 + d0 * ix->dim, st_f64, static_cast<size_t>(L) * ix->dim * 8,
+                         cudaMemcpyDeviceToDevice, ix->stream));
+    CK(cudaMemcpyAsync(ix->norm2 + d0, st_norm2, static_cast<size_t>(L) * 8, cudaMemcpyDeviceToDevice, ix->stream));
+    CK(cudaMemcpyAsync(ix->inv_norm + d0, st_inv, static_cast<size_t>(L) * 4, cudaMemcpyDeviceToDevice, ix->stream));
+  }
+  // the tail looks like never-appended rows: zero bf16 rows (read by the scan's last tile), NaN 1/||c||, no tombstones
+  CK(cudaMemsetAsync(ix->rows + n_live * ix->dpad, 0, static_cast<size_t>(n - n_live) * ix->dpad * 2, ix->stream));
+  CK(cudaMemsetAsync(ix->inv_norm + n_live, 0xFF, static_cast<size_t>(n - n_live) * 4, ix->stream));
+  CK(cudaMemsetAsync(ix->dead_bits, 0, static_cast<size_t>(n_words) * 4, ix->stream));
+  CK(cudaStreamSynchronize(ix->stream));
+  ix->n_rows = n_live;
+  // caches keyed on the corpus: the captured search graph (GraphKey.n_rows) and the corpus tensor map (map_rows) are
+  // dropped here so that the next search rebuilds them; the large-k scratch is sized per call from C_q, not from the
+  // corpus, and the fallback / exact-scores / debug buffers from n_rows at each call.
+  drop_graph(ix);
+  ix->tmap_c_rows = -1;
   return RBK_OK;
 }
 

@@ -89,6 +89,9 @@ struct rbk_index {
   // ingest staging
   rbk::impl::DevBuf<unsigned char> stage;
   rbk::impl::DevBuf<int64_t> d_slots;
+  // compaction scratch: old_to_new, and word prefixes | block sums | chunk prefixes of the liveness scan
+  rbk::impl::DevBuf<long long> cp_map;
+  rbk::impl::DevBuf<int> cp_scan;
   // search scratch
   rbk::impl::DevBuf<unsigned char> q_raw;
   rbk::impl::DevBuf<uint16_t> q_bf16;

@@ -77,6 +77,19 @@ cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_b
 cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows, float* inv_norm,
                              unsigned int* dead_bits, int* n_killed, cudaStream_t stream);
 
+// ---- compaction (rbk_compact.cu) ----
+// old_to_new [n_rows] (new local slot, -1 = tombstoned) from dead_bits by a two-level exclusive scan over the 32-row
+// words.  Scratch: word_pref [ceil(n_rows / 32)], block_sum [ceil(n_rows / 32768)].  chunk_pref [n_chunks + 1]:
+// [c] = live rows before row c * chunk_rows (a multiple of 32), [n_chunks] = all live rows.
+cudaError_t launch_compact_map(const unsigned int* dead_bits, int64_t n_rows, int64_t chunk_rows, int* word_pref,
+                               int* block_sum, long long* old_to_new, int* chunk_pref, cudaStream_t stream);
+// Packs the live rows among source rows [s0, s0 + n) into staging row old_to_new[s] - d0: bf16 row (pitch dpad),
+// f64 row (pitch d; skipped when rows_f64 is null), norm2, inv_norm.
+cudaError_t launch_compact_gather(const uint16_t* rows, const double* rows_f64, const double* norm2,
+                                  const float* inv_norm, const long long* old_to_new, int64_t s0, int64_t n,
+                                  long long d0, int d, int dpad, uint16_t* st_rows, double* st_f64, double* st_norm2,
+                                  float* st_inv, int sm_count, cudaStream_t stream);
+
 // ---- query preparation + finalize + exhaustive fallback + shard merge (rbk_finalize.cu) ----
 struct QueryBuffers {
   uint16_t* q_bf16;    // [B][dpad]

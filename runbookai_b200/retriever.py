@@ -8,7 +8,8 @@ store stays empty unless something else fills it.  This variant keeps the refere
   * searches through `HybridRetriever` (FTS5 + the device index + RRF) when an embedder is configured,
     through the FTS store alone otherwise (the reference behaviour);
   * in `sync()` mirrors every upserted document into the vector store: its old vectors are tombstoned
-    (`deleteDocument`) and its chunks embedded and appended in one `addChunks` call.
+    (`deleteDocument`) and its chunks embedded and appended in one `addChunks` call; once enough slots are dead
+    the vector store is compacted (`VectorStore.compact`), so repeated syncs do not grow the device index.
 Loading documents from disk / Confluence / ... (src/knowledge/sources) is out of scope: `sources` are
 callables returning document dicts in the reference's KnowledgeDocument shape.
 """
@@ -21,6 +22,7 @@ from . import embedder as _emb
 from .fts_store import KnowledgeStore
 from .hybrid_search import HybridRetriever
 
+_COMPACT_MIN_DEAD = 4096   # sync() compacts the vector store from this many tombstoned slots (and >= size() / 4)
 _BUCKET = {"runbook": "runbooks", "postmortem": "postmortems", "architecture": "architecture",
            "known_issue": "knownIssues"}
 
@@ -72,8 +74,22 @@ class KnowledgeRetriever:
                     added += 1
                 self.store.upsert_document(doc)
                 self._mirror(doc)
+        self._reclaim()
         self.initialized = True
         return {"added": added, "updated": updated}
+
+    def _reclaim(self) -> None:
+        """Every mirrored update tombstones the document's old chunks, so a long-running process would otherwise
+        keep their device memory and scan time for good.  Once the dead slots reach a quarter of all slots (and at
+        least _COMPACT_MIN_DEAD - below that they cost less than the call) the vector store is compacted."""
+        vs = self.vector_store
+        ix = vs._index if vs is not None else None
+        if ix is None or getattr(ix, "compact", None) is None:
+            return
+        size = ix.size()
+        dead = size - ix.count()
+        if dead >= _COMPACT_MIN_DEAD and 4 * dead >= size:
+            vs.compact()
 
     def _mirror(self, doc: dict) -> None:
         vs = self.vector_store

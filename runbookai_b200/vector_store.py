@@ -463,6 +463,31 @@ class VectorStore:
             self.db.execute("DELETE FROM vector_embeddings WHERE document_id = ?", (document_id,))
             self._bump_generation()
 
+    def compact(self) -> int:
+        """Give the slots of deleted rows back (the reference's `Map.delete` frees its entry; a tombstone does not):
+        the device index moves its live rows down in Map order and the slot <-> id table follows its old_to_new map.
+        Returns the number of slots reclaimed.  An index without `compact` (a device group) is left as it is.  The
+        SQLite table, the reload sidecar (which describes the table, not slots) and `bad_ids` do not change.  Holds
+        the state lock, like every search, so no search maps its slots through a half-updated table."""
+        with self._st.lock:
+            ix = self._index
+            fn = getattr(ix, "compact", None)
+            if fn is None:
+                return 0
+            before = ix.size()
+            old_to_new = fn()
+            ids: list[str | None] = [None] * ix.size()
+            for s, vid in enumerate(self._ids):
+                if vid is None:
+                    continue
+                new = int(old_to_new[s])
+                if new < 0:
+                    raise RuntimeError(f"compaction dropped the live slot {s} ({vid})")
+                ids[new] = vid
+                self._slot_of[vid] = new
+            self._ids[:] = ids
+            return before - ix.size()
+
     def get_count(self) -> int:
         """vector-store.ts:302-307."""
         return self.db.execute("SELECT COUNT(*) as count FROM vector_embeddings").fetchone()["count"]

@@ -4,10 +4,11 @@
  * reference performs on it in its hot loop (:207-221): "all ids whose cosine with the query is
  * >= minScore, best first, stable, first 2*topK".
  *
- * NOT COMPILED in the build image (no Node/tsc).  It is deliberately tiny: the Map's ordered-key
- * semantics (insertion slot, re-set keeps the slot, delete frees the key but never the slot) on top
- * of the N-API addon (napi/rbk_napi.cc -> include/rbk_knn.h).  The tested mirror of the same
- * bookkeeping is runbookai_b200/vector_store.py (`_set`, `delete_document`, `_load_embeddings`).
+ * NOT COMPILED in the build image (no Node/tsc); `compact()` below is no exception.  It is deliberately
+ * tiny: the Map's ordered-key semantics (insertion slot, re-set keeps the slot, delete frees the key and
+ * `compact()` later its slot) on top of the N-API addon (napi/rbk_napi.cc -> include/rbk_knn.h).  The
+ * tested mirror of the same bookkeeping is runbookai_b200/vector_store.py (`_set`, `delete_document`,
+ * `_load_embeddings`, `compact`).
  * INTEGRATION.md shows the few lines of vector-store.ts that change to use it.
  */
 // eslint-disable-next-line @typescript-eslint/no-var-requires
@@ -32,6 +33,11 @@ export class GpuEmbeddingIndex {
   private dim = 0;
   /** ids whose stored vector has another length: while one is in the Map the reference's search throws (S2) */
   private badIds = new Set<string>();
+  /** bestBatch calls between their device call and the slot -> id lookup; compact() waits for them */
+  private inFlight = 0;
+  private drained: Array<() => void> = [];
+  /** set while compact() runs: new bestBatch calls wait for it */
+  private compacting: Promise<void> | null = null;
 
   /**
    * One device index per resolved db path in the process, reference-counted: the reference builds and closes a
@@ -153,6 +159,7 @@ export class GpuEmbeddingIndex {
    * (RBK_MAX_K_FETCH_LARGE) the large-k search (two scans and an exact re-rank).
    */
   async bestBatch(queries: number[][], limit: number, minScore: number): Promise<ScoredId[][]> {
+    while (this.compacting) await this.compacting; // never search against a table that is being renumbered
     if (!this.index || this.slotOfId.size === 0) return queries.map(() => []);
     if (this.badIds.size > 0 || queries.some((q) => q.length !== this.dim)) {
       throw new Error('Vectors must have the same length');
@@ -160,17 +167,51 @@ export class GpuEmbeddingIndex {
     const B = queries.length;
     const packed = new Float64Array(B * this.dim);
     queries.forEach((q, b) => packed.set(q, b * this.dim));
-    const { slots, scores, counts } =
-      limit > 112
-        ? await this.index.searchLarge(packed, B, limit, minScore)
-        : await this.index.search(packed, B, limit, minScore);
-    return queries.map((_, b) => {
-      const out: ScoredId[] = [];
-      for (let i = 0; i < counts[b]; i++) {
-        out.push({ id: this.idOfSlot[Number(slots[b * limit + i])]!, score: scores[b * limit + i] });
-      }
-      return out;
-    });
+    this.inFlight++;
+    try {
+      const { slots, scores, counts } =
+        limit > 112
+          ? await this.index.searchLarge(packed, B, limit, minScore)
+          : await this.index.search(packed, B, limit, minScore);
+      return queries.map((_, b) => {
+        const out: ScoredId[] = [];
+        for (let i = 0; i < counts[b]; i++) {
+          out.push({ id: this.idOfSlot[Number(slots[b * limit + i])]!, score: scores[b * limit + i] });
+        }
+        return out;
+      });
+    } finally {
+      if (--this.inFlight === 0) this.drained.splice(0).forEach((wake) => wake());
+    }
+  }
+
+  /**
+   * Give the slots of deleted ids back (the reference's Map.delete frees its entry; a tombstone alone does not): the
+   * device index moves its live rows down in Map order and returns oldToNew, through which slotOfId and idOfSlot are
+   * renumbered.  Holds back new bestBatch calls and waits for those in flight first, so no search result is ever mapped
+   * through the other table.  Returns the number of slots reclaimed.  Throws for a device group (RUNBOOK_KNN_DEVICES).
+   */
+  async compact(): Promise<number> {
+    while (this.compacting) await this.compacting;
+    let done!: () => void;
+    this.compacting = new Promise<void>((resolve) => (done = resolve));
+    try {
+      if (this.inFlight > 0) await new Promise<void>((resolve) => this.drained.push(resolve));
+      if (!this.index) return 0;
+      const oldToNew: BigInt64Array = this.index.compact();
+      const ids: (string | null)[] = [];
+      this.idOfSlot.forEach((id, slot) => {
+        if (id === null || id === undefined) return;
+        const to = Number(oldToNew[slot]);
+        ids[to] = id;
+        this.slotOfId.set(id, to);
+      });
+      this.idOfSlot = ids;
+      return oldToNew.length - ids.length;
+    } finally {
+      this.compacting = null;
+      done();
+    }
   }
 
   private remember(id: string, slot: number): void {
