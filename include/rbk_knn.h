@@ -70,6 +70,19 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * vector-store.ts:71-88), not only for bf16-representable ones.  The scan's error bound grows by the largest
  * angle between a row and its bf16 rounding, so more queries may take the exhaustive path on near-tied data. */
 #define RBK_INDEX_KEEP_F64 1u
+/* RBK_INDEX_F64_ON_HOST (only together with RBK_INDEX_KEEP_F64, else RBK_EINVAL): the [capacity][dim] float64 rows
+ * live in pinned, mapped host memory (cudaHostAlloc Mapped | Portable) instead of on the GPU; every other buffer stays
+ * where it is.  Answers are bit-identical to a KEEP_F64 index on the device fed the same calls - slots, scores, counts,
+ * exactness flags, fallback and retry decisions, compaction maps: the same values go through the same operations in
+ * the same order, only the bytes come over PCIe.  Device memory per row at d = 1536 drops from 15,372 to 3,084 bytes
+ * (about 5x the rows per GPU); host RAM pays 8*dim bytes per row (12 KB at d = 1536), and growing the capacity holds
+ * the old and the new buffer at once (peak old + new).  The scan is unchanged.  Cost: each search reads k'*8*dim
+ * bytes of host rows per query (k' = candidates re-ranked, <= 128; about 590 KB at k_fetch 20, d = 1536), the large-k
+ * search 8*dim bytes per emitted candidate, and the rare exhaustive fallback / rbk_index_exact_scores_f64 the whole
+ * corpus, all at PCIe speed; appends write the rows over PCIe.  Every write to the host rows is stream-ordered (a kernel
+ * or copy on the index stream, or the host after a synchronisation), so searches enqueued earlier never see a
+ * half-written row.  The placement is fixed for the index's life. */
+#define RBK_INDEX_F64_ON_HOST 2u
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out);
 void rbk_index_destroy(rbk_index* idx); /* NULL is a no-op */
 
@@ -122,6 +135,10 @@ rbk_status rbk_index_clear(rbk_index* idx);
 int64_t rbk_index_count(const rbk_index* idx); /* live rows  */
 int64_t rbk_index_size(const rbk_index* idx);  /* slots used, tombstones included */
 int32_t rbk_index_dim(const rbk_index* idx);
+/* Persistent corpus storage at the current capacity, in bytes: bf16 rows, inv_norm, norm2, tombstone bits and the
+ * float64 rows (KEEP_F64), split by where they live.  Search and compaction scratch are not counted.  Either output
+ * may be NULL. */
+rbk_status rbk_index_storage_bytes(const rbk_index* idx, int64_t* device_bytes, int64_t* pinned_host_bytes);
 /* Copy stored rows back (bf16 bits), for tests and for reload sidecars. */
 rbk_status rbk_index_read_rows_bf16(rbk_index* idx, int64_t first_local_slot, int64_t n_rows, uint16_t* out);
 
@@ -210,7 +227,8 @@ rbk_status rbk_merge_topk_packed_device(int32_t device, void* cuda_stream, int32
  * and error conventions are those of the rbk_index_* call of the same name. */
 typedef struct rbk_group rbk_group;
 rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_devices, int64_t capacity_hint,
-                            uint32_t flags /* RBK_INDEX_KEEP_F64 */, rbk_group** out);
+                            uint32_t flags /* RBK_INDEX_KEEP_F64 [| RBK_INDEX_F64_ON_HOST]: every member */,
+                            rbk_group** out);
 void rbk_group_destroy(rbk_group* grp); /* NULL is a no-op */
 rbk_status rbk_group_append_f64(rbk_group* grp, const double* rows, int64_t n_rows, int64_t* first_slot_out);
 rbk_status rbk_group_append_f32(rbk_group* grp, const float* rows, int64_t n_rows, int64_t* first_slot_out);

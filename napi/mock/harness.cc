@@ -1,5 +1,6 @@
 // harness.cc - plays the JavaScript side of ts/gpu-embedding-index.ts against napi/rbk_napi.cc through the mock
-// N-API runtime (mock_napi.cc): loads the module, constructs RbkIndex (one device or a device list), loads rows as
+// N-API runtime (mock_napi.cc): loads the module, constructs RbkIndex (one device or a device list, optionally with
+// hostRows), loads rows as
 // SQLite-style BLOBs and as a Float64Array, overwrites, tombstones, counts, searches through the Promise/async-work
 // path, provokes every error path, optionally (compact.txt) tombstones more, compacts and searches again, clears,
 // and lets the finalizer run.  Inputs and outputs are flat binary files in
@@ -120,15 +121,22 @@ int main(int argc, char** argv) {
   napi_value cls = mock::get_property(env, exports, "RbkIndex");
   if (!cls) die("exports.RbkIndex is missing");
 
-  // new RbkIndex(dim, device | [devices], capacityHint)
+  // new RbkIndex(dim, device | [devices], capacityHint [, hostRows])
   napi_value dev_arg = mock::number(env, 0);
   if (n_dev > 0) {
     std::vector<napi_value> e;
     for (int d : devs) e.push_back(mock::number(env, d));
     dev_arg = mock::array(env, e);
   }
+  // optional host_rows.txt: the constructor's 4th argument (hostRows: float64 rows in pinned host memory)
+  std::vector<napi_value> ctor_args = {mock::number(env, dim), dev_arg, mock::number(env, n_rows)};
+  {
+    std::ifstream hf(g_dir + "/host_rows.txt");
+    int host_rows = 0;
+    if (hf >> host_rows) ctor_args.push_back(mock::number(env, host_rows));
+  }
   napi_value ix = nullptr;
-  if (!mock::construct(env, cls, {mock::number(env, dim), dev_arg, mock::number(env, n_rows)}, &ix, &err)) {
+  if (!mock::construct(env, cls, ctor_args, &ix, &err)) {
     write_text("error.txt", err);
     mock::delete_env(env);
     return 3;   // e.g. no CUDA device: the constructor throws, nothing falls back

@@ -12,6 +12,7 @@
 //   const { RbkIndex } = require('./build/Release/rbk_knn.node')
 //   const ix = new RbkIndex(dim, device, capacityHint)          // one GPU  (rbk_index_*)
 //   const ix = new RbkIndex(dim, [0, 1, 2, 3], capacityHint)    // several GPUs behind one handle (rbk_group_*)
+//   const ix = new RbkIndex(dim, device, capacityHint, hostRows) // hostRows != 0: float64 rows in pinned host RAM
 //   ix.appendF64(Float64Array rows)            -> firstSlot
 //   ix.appendBlobs(Buffer[] blobs)             -> firstSlot     // SQLite f64-LE BLOBs, packed in C++: no JS copies
 //   ix.overwriteF64(slot, Float64Array row); ix.overwriteF64Batch(BigInt64Array slots, Float64Array rows)
@@ -102,18 +103,21 @@ void finalize_index(napi_env, void* data, void*) {
 }
 
 napi_value New(napi_env env, napi_callback_info info) {
-  size_t argc = 3;
-  napi_value argv[3], self;
+  size_t argc = 4;
+  napi_value argv[4], self;
   NAPI_OK(napi_get_cb_info(env, info, &argc, argv, &self, nullptr));
-  int32_t dim = 0, device = 0;
+  int32_t dim = 0, device = 0, host_rows = 0;
   int64_t hint = 0;
   NAPI_OK(napi_get_value_int32(env, argv[0], &dim));
   if (argc > 2) napi_get_value_int64(env, argv[2], &hint);
+  if (argc > 3) napi_get_value_int32(env, argv[3], &host_rows);
   Handle* h = new Handle();
   h->dim = dim;
   bool is_array = false;
   if (argc > 1) napi_is_array(env, argv[1], &is_array);
-  // KEEP_F64: the reference stores float64 embeddings; keep them so results are exact for any input
+  // KEEP_F64: the reference stores float64 embeddings; keep them so results are exact for any input.  hostRows
+  // (RUNBOOK_KNN_F64_ON_HOST in ts/gpu-embedding-index.ts): keep them in pinned host memory instead of on the GPU.
+  const uint32_t flags = RBK_INDEX_KEEP_F64 | (host_rows != 0 ? RBK_INDEX_F64_ON_HOST : 0u);
   rbk_status st;
   if (is_array) {   // [0, 1, ...]: the corpus sharded over these GPUs, one call per search (rbk_group_*)
     uint32_t n = 0;
@@ -124,10 +128,10 @@ napi_value New(napi_env env, napi_callback_info info) {
       napi_get_element(env, argv[1], i, &e);
       napi_get_value_int32(env, e, &devs[i]);
     }
-    st = rbk_group_create(dim, devs.data(), (int32_t)n, hint, RBK_INDEX_KEEP_F64, &h->grp);
+    st = rbk_group_create(dim, devs.data(), (int32_t)n, hint, flags, &h->grp);
   } else {
     if (argc > 1) napi_get_value_int32(env, argv[1], &device);
-    st = rbk_index_create_ex(dim, device, hint, RBK_INDEX_KEEP_F64, &h->ix);
+    st = rbk_index_create_ex(dim, device, hint, flags, &h->ix);
   }
   if (st != RBK_OK) {
     delete h;

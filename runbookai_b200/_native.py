@@ -15,13 +15,15 @@ LIB_PATH = Path(__file__).resolve().parent / "lib" / "librbk_knn.so"
 RBK_OK, RBK_EINVAL, RBK_ENOMEM, RBK_ECUDA, RBK_ENCCL, RBK_EDIM = range(6)
 RBK_MAX_K_FETCH = 112
 RBK_MAX_K_FETCH_LARGE = 4096
+RBK_INDEX_KEEP_F64 = 1
+RBK_INDEX_F64_ON_HOST = 2
 
 # every symbol include/rbk_knn.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "rbk_abi_version", "rbk_last_error", "rbk_index_create", "rbk_index_create_ex", "rbk_index_destroy", "rbk_index_set_stream",
     "rbk_index_set_slot_base", "rbk_index_append_f64", "rbk_index_append_f32", "rbk_index_append_bf16",
     "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_compact", "rbk_index_clear",
-    "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_read_rows_bf16", "rbk_index_search_f64",
+    "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_storage_bytes", "rbk_index_read_rows_bf16", "rbk_index_search_f64",
     "rbk_index_search_f32", "rbk_index_search_large_f64", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
     "rbk_packed_block_bytes", "rbk_packed_flags_offset",
     "rbk_merge_topk_packed_device", "rbk_index_stats",
@@ -81,6 +83,7 @@ def _load() -> C.CDLL:
         getattr(lib, n).restype = i64
     lib.rbk_index_dim.argtypes = [vp]
     lib.rbk_index_dim.restype = i32
+    lib.rbk_index_storage_bytes.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     lib.rbk_index_read_rows_bf16.argtypes = [vp, i64, i64, vp]
     for n in ("rbk_index_search_f64", "rbk_index_search_f32", "rbk_index_search_large_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
@@ -131,6 +134,11 @@ def ptr(a: np.ndarray | None):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _index_flags(keep_f64: bool, f64_on_host: bool) -> int:
+    """f64_on_host without keep_f64 is passed through: the library rejects it with its own message."""
+    return (RBK_INDEX_KEEP_F64 if keep_f64 else 0) | (RBK_INDEX_F64_ON_HOST if f64_on_host else 0)
+
+
 def _search_large(fn, h, queries, k_fetch: int, min_score):
     q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
     B = q.shape[0]
@@ -169,11 +177,14 @@ def _search_any_k(ix, queries, k_fetch: int, min_score):
 class Index:
     """Thin object wrapper over rbk_index* (one GPU shard)."""
 
-    def __init__(self, dim: int, device: int = 0, capacity_hint: int = 0, keep_f64: bool = False):
-        """keep_f64: RBK_INDEX_KEEP_F64 — exact for arbitrary float64 rows at 8*dim extra bytes per row."""
+    def __init__(self, dim: int, device: int = 0, capacity_hint: int = 0, keep_f64: bool = False,
+                 f64_on_host: bool = False):
+        """keep_f64: RBK_INDEX_KEEP_F64 — exact for arbitrary float64 rows at 8*dim extra bytes per row.
+        f64_on_host: RBK_INDEX_F64_ON_HOST — those float64 rows live in pinned host memory instead of on the GPU (same
+        answers; the re-rank reads them over PCIe).  Requires keep_f64."""
         self._h = None
         h = C.c_void_p()
-        check(lib.rbk_index_create_ex(dim, device, capacity_hint, 1 if keep_f64 else 0, C.byref(h)))
+        check(lib.rbk_index_create_ex(dim, device, capacity_hint, _index_flags(keep_f64, f64_on_host), C.byref(h)))
         self._h = h
         self.dim = dim
         self.device = device
@@ -260,6 +271,12 @@ class Index:
     def size(self) -> int:
         return lib.rbk_index_size(self._h)
 
+    def storage_bytes(self) -> tuple[int, int]:
+        """(device bytes, pinned host bytes) of the corpus storage at the current capacity; scratch not counted."""
+        dev, host = C.c_int64(0), C.c_int64(0)
+        check(lib.rbk_index_storage_bytes(self._h, C.byref(dev), C.byref(host)))
+        return dev.value, host.value
+
     def read_rows_bf16(self, first: int, n: int) -> np.ndarray:
         out = np.empty((n, self.dim), dtype=np.uint16)
         check(lib.rbk_index_read_rows_bf16(self._h, first, n, ptr(out)))
@@ -334,11 +351,13 @@ class Group:
     """rbk_group*: one corpus sharded over several GPUs behind one handle; the Index surface with GLOBAL slots.
     Every search is one C call: per-GPU scans, one NCCL all-gather, merge on devices[0], one synchronisation."""
 
-    def __init__(self, dim: int, devices, capacity_hint: int = 0, keep_f64: bool = False):
+    def __init__(self, dim: int, devices, capacity_hint: int = 0, keep_f64: bool = False, f64_on_host: bool = False):
+        """f64_on_host: every member keeps its float64 rows in its own pinned host buffer (see Index)."""
         self._h = None
         devs = np.ascontiguousarray(list(devices), dtype=np.int32)
         h = C.c_void_p()
-        check(lib.rbk_group_create(dim, ptr(devs), devs.shape[0], capacity_hint, 1 if keep_f64 else 0, C.byref(h)))
+        check(lib.rbk_group_create(dim, ptr(devs), devs.shape[0], capacity_hint, _index_flags(keep_f64, f64_on_host),
+                                   C.byref(h)))
         self._h = h
         self.dim = dim
         self.devices = [int(d) for d in devs]

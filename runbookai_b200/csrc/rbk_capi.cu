@@ -147,9 +147,27 @@ rbk_status ensure_capacity(rbk_index* ix, int64_t need) {
   double* r64 = nullptr;
   const size_t dead_words = static_cast<size_t>((ncap + 31) / 32);
   cudaError_t e;
-  if (ix->keep_f64 &&
-      (e = cudaMalloc(reinterpret_cast<void**>(&r64), static_cast<size_t>(ncap) * ix->dim * 8)) != cudaSuccess)
-    return cuda_fail(e, "cudaMalloc(f64 sidecar)");
+  if (ix->keep_f64) {
+    const size_t bytes = static_cast<size_t>(ncap) * ix->dim * 8;
+    if (ix->f64_on_host) {
+      // not write-combined: the host reads these rows when the index grows
+      if ((e = cudaHostAlloc(reinterpret_cast<void**>(&r64), bytes, cudaHostAllocMapped | cudaHostAllocPortable)) !=
+          cudaSuccess)
+        return cuda_fail(e, "cudaHostAlloc(f64 rows on the host)");
+      void* dp = nullptr;
+      if ((e = cudaHostGetDevicePointer(&dp, r64, 0)) != cudaSuccess || dp != r64) {
+        cudaFreeHost(r64);
+        if (e != cudaSuccess) return cuda_fail(e, "cudaHostGetDevicePointer(f64 rows on the host)");
+        return fail(RBK_ECUDA, "pinned host rows are mapped at another device address (no unified addressing)");
+      }
+    } else if ((e = cudaMalloc(reinterpret_cast<void**>(&r64), bytes)) != cudaSuccess) {
+      return cuda_fail(e, "cudaMalloc(f64 sidecar)");
+    }
+  }
+  auto free_r64 = [&](double* p) {
+    if (ix->f64_on_host) cudaFreeHost(p);
+    else cudaFree(p);
+  };
   if ((e = cudaMalloc(reinterpret_cast<void**>(&rows), static_cast<size_t>(ncap) * ix->dpad * 2)) != cudaSuccess ||
       (e = cudaMalloc(reinterpret_cast<void**>(&inv), static_cast<size_t>(inv_norm_len(ncap)) * 4)) != cudaSuccess ||
       (e = cudaMalloc(reinterpret_cast<void**>(&n2), static_cast<size_t>(ncap) * 8)) != cudaSuccess ||
@@ -158,7 +176,7 @@ rbk_status ensure_capacity(rbk_index* ix, int64_t need) {
     cudaFree(inv);
     cudaFree(n2);
     cudaFree(dead);
-    cudaFree(r64);
+    free_r64(r64);
     return cuda_fail(e, "cudaMalloc(index storage)");
   }
   cudaStream_t st = ix->stream;
@@ -173,16 +191,19 @@ rbk_status ensure_capacity(rbk_index* ix, int64_t need) {
     CK(cudaMemcpyAsync(n2, ix->norm2, static_cast<size_t>(ix->n_rows) * 8, cudaMemcpyDeviceToDevice, st));
     CK(cudaMemcpyAsync(dead, ix->dead_bits, static_cast<size_t>((ix->n_rows + 31) / 32) * 4,
                        cudaMemcpyDeviceToDevice, st));
-    if (r64)
+    if (r64 && !ix->f64_on_host)
       CK(cudaMemcpyAsync(r64, ix->rows_f64, static_cast<size_t>(ix->n_rows) * ix->dim * 8, cudaMemcpyDeviceToDevice,
                          st));
   }
   CK(cudaStreamSynchronize(st));
+  // host rows: copied by the host, now that every kernel that wrote or read the old rows has finished
+  if (r64 && ix->f64_on_host && ix->n_rows > 0)
+    memcpy(r64, ix->rows_f64, static_cast<size_t>(ix->n_rows) * ix->dim * 8);
   cudaFree(ix->rows);
   cudaFree(ix->inv_norm);
   cudaFree(ix->norm2);
   cudaFree(ix->dead_bits);
-  cudaFree(ix->rows_f64);
+  free_r64(ix->rows_f64);
   ix->rows_f64 = r64;
   ix->rows = rows;
   ix->inv_norm = inv;
@@ -405,7 +426,7 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
       fp.out_scores = d_scores + static_cast<size_t>(q0) * k_fetch;
       fp.out_counts = d_counts + q0;
       fp.flags = d_flags + q0;
-      CK(launch_finalize(fp, ix->stream));
+      CK(launch_finalize(fp, ix->f64_on_host, ix->stream));
       ix->stats.kernel_launches++;
     }
   }
@@ -607,7 +628,7 @@ rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long 
     rp.out_counts = d_counts + q0;
     rp.overflow = ix->lg_err.p;
     const int max_cap = *std::max_element(ix->h_lcap.p + q0, ix->h_lcap.p + q0 + Bs);
-    CK(launch_large_rerank(rp, max_cap, ix->stream));
+    CK(launch_large_rerank(rp, max_cap, ix->f64_on_host, ix->stream));
     ix->stats.kernel_launches += max_cap > 0 ? 2 : 1;
   }
   CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
@@ -836,8 +857,10 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
 
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out) {
   if (!out) return fail(RBK_EINVAL, "out is null");
-  if (flags & ~static_cast<uint32_t>(RBK_INDEX_KEEP_F64)) return fail(RBK_EINVAL, "unknown flag");
   *out = nullptr;
+  if (flags & ~static_cast<uint32_t>(RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST)) return fail(RBK_EINVAL, "unknown flag");
+  if ((flags & RBK_INDEX_F64_ON_HOST) && !(flags & RBK_INDEX_KEEP_F64))
+    return fail(RBK_EINVAL, "RBK_INDEX_F64_ON_HOST requires RBK_INDEX_KEEP_F64");
   if (dim < 1 || dim > (1 << 20)) return fail(RBK_EINVAL, "dim out of range");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -857,6 +880,7 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
   ix->dpad = static_cast<int>(round_up(dim, kBlockK));
   ix->device = device;
   ix->keep_f64 = (flags & RBK_INDEX_KEEP_F64) != 0;
+  ix->f64_on_host = (flags & RBK_INDEX_F64_ON_HOST) != 0;
   ix->sm_count = prop.multiProcessorCount;
   memset(&ix->stats, 0, sizeof ix->stats);
   ix->stats.sm_count = ix->sm_count;
@@ -890,7 +914,8 @@ void rbk_index_destroy(rbk_index* ix) {
     cudaFree(ix->inv_norm);
     cudaFree(ix->norm2);
     cudaFree(ix->dead_bits);
-    cudaFree(ix->rows_f64);
+    if (ix->f64_on_host) cudaFreeHost(ix->rows_f64);
+    else cudaFree(ix->rows_f64);
     cudaFree(ix->d_counter);
     ix->stage.release();
     ix->d_slots.release();
@@ -1129,9 +1154,9 @@ rbk_status rbk_index_compact(rbk_index* ix, int64_t* old_to_new, int64_t old_to_
     ix->stats.kernel_launches++;
     CK(cudaMemcpyAsync(ix->rows + d0 * ix->dpad, st_rows, static_cast<size_t>(L) * ix->dpad * 2,
                        cudaMemcpyDeviceToDevice, ix->stream));
-    if (ix->keep_f64)
-      CK(cudaMemcpyAsync(ix->rows_f64 + d0 * ix->dim, st_f64, static_cast<size_t>(L) * ix->dim * 8,
-                         cudaMemcpyDeviceToDevice, ix->stream));
+    if (ix->keep_f64)   // device or mapped host rows (RBK_INDEX_F64_ON_HOST): UVA picks the direction
+      CK(cudaMemcpyAsync(ix->rows_f64 + d0 * ix->dim, st_f64, static_cast<size_t>(L) * ix->dim * 8, cudaMemcpyDefault,
+                         ix->stream));
     CK(cudaMemcpyAsync(ix->norm2 + d0, st_norm2, static_cast<size_t>(L) * 8, cudaMemcpyDeviceToDevice, ix->stream));
     CK(cudaMemcpyAsync(ix->inv_norm + d0, st_inv, static_cast<size_t>(L) * 4, cudaMemcpyDeviceToDevice, ix->stream));
   }
@@ -1152,6 +1177,17 @@ rbk_status rbk_index_compact(rbk_index* ix, int64_t* old_to_new, int64_t old_to_
 int64_t rbk_index_count(const rbk_index* ix) { return ix ? ix->n_live : 0; }
 int64_t rbk_index_size(const rbk_index* ix) { return ix ? ix->n_rows : 0; }
 int32_t rbk_index_dim(const rbk_index* ix) { return ix ? ix->dim : 0; }
+
+rbk_status rbk_index_storage_bytes(const rbk_index* ix, int64_t* device_bytes, int64_t* pinned_host_bytes) {
+  if (!ix) return fail(RBK_EINVAL, "null index");
+  // the allocations of ensure_capacity: rows | inv_norm | norm2 | dead_bits | f64 rows
+  const int64_t cap = ix->cap;
+  const int64_t f64 = ix->keep_f64 ? cap * ix->dim * 8 : 0;
+  const int64_t dev = cap * ix->dpad * 2 + inv_norm_len(cap) * 4 + cap * 8 + (cap + 31) / 32 * 4;
+  if (device_bytes) *device_bytes = dev + (ix->f64_on_host ? 0 : f64);
+  if (pinned_host_bytes) *pinned_host_bytes = ix->f64_on_host ? f64 : 0;
+  return RBK_OK;
+}
 
 rbk_status rbk_index_read_rows_bf16(rbk_index* ix, int64_t first, int64_t n, uint16_t* out) {
   if (!ix || (n > 0 && !out)) return fail(RBK_EINVAL, "null argument");

@@ -203,6 +203,13 @@ __device__ __forceinline__ void for_each_key(const unsigned long long* __restric
   }
 }
 
+// Host-row staging (kHostRows): row pieces each thread keeps in flight.  A mapped host read waits a PCIe round trip,
+// so a block needs many bytes in flight to stream: 256 threads x 8 x 16 B = 32 KB.
+constexpr int kHostLoads = 8;
+
+// kHostRows: rows_f64 is mapped host memory (RBK_INDEX_F64_ON_HOST).  Only the f64 staging differs; the device-tier
+// instantiation compiles to the same code as before the host tier existed.
+template <bool kHostRows>
 __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p) {
   const int ql = blockIdx.x;  // query index inside this launch
   const int tid = threadIdx.x;
@@ -429,6 +436,72 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
         }
         for (; i < len; ++i)
           dot = __dadd_rn(dot, __dmul_rn(s_q[i], bf16_to_f64(reinterpret_cast<const uint16_t*>(mine)[i])));
+      }
+      if (tid == kFinThreads - 1)
+        for (int i = 0; i < len; ++i) na_chain = __dadd_rn(na_chain, __dmul_rn(s_q[i], s_q[i]));
+    }
+  } else if constexpr (kHostRows) {
+    // exact source = f64 rows in mapped host memory: the same chunks walked in the same order, but staged with
+    // 16-byte loads, kHostLoads of them in flight per thread (8-byte ones for odd d, whose rows are not all 16-byte
+    // aligned).  The chunk is even so that every 16-byte piece of an even-d row starts aligned.
+    double* s_rows64 = reinterpret_cast<double*>(s_keys);
+    int chunk = nsel > 0 ? (p.key_cap / nsel - 1) : kQChunk;
+    chunk = (chunk < kQChunk ? chunk : kQChunk) & ~1;
+    const int row_stride = chunk | 1;
+    const bool wide = (p.d & 1) == 0;
+    for (int c0 = 0; c0 < p.d; c0 += chunk) {
+      const int len = p.d - c0 < chunk ? p.d - c0 : chunk;
+      __syncthreads();
+      if (wide) {
+        const int len2 = len >> 1;   // even d, even chunk: len is even
+        for (int i0 = tid; i0 < nsel * len2; i0 += kHostLoads * kFinThreads) {
+          double2 v[kHostLoads];
+#pragma unroll
+          for (int b = 0; b < kHostLoads; ++b) {
+            const int i = i0 + b * kFinThreads;
+            if (i < nsel * len2) {
+              const int rr = i / len2, u = i - rr * len2;
+              const int row = static_cast<int>(key_row(s_sel[rr]));
+              v[b] = __ldg(reinterpret_cast<const double2*>(p.rows_f64 + static_cast<size_t>(row) * p.d + c0) + u);
+            }
+          }
+#pragma unroll
+          for (int b = 0; b < kHostLoads; ++b) {
+            const int i = i0 + b * kFinThreads;
+            if (i < nsel * len2) {
+              const int rr = i / len2, u = i - rr * len2;
+              s_rows64[rr * row_stride + 2 * u] = v[b].x;
+              s_rows64[rr * row_stride + 2 * u + 1] = v[b].y;
+            }
+          }
+        }
+      } else {
+        for (int i0 = tid; i0 < nsel * len; i0 += 2 * kHostLoads * kFinThreads) {
+          double v[2 * kHostLoads];
+#pragma unroll
+          for (int b = 0; b < 2 * kHostLoads; ++b) {
+            const int i = i0 + b * kFinThreads;
+            if (i < nsel * len) {
+              const int rr = i / len, u = i - rr * len;
+              const int row = static_cast<int>(key_row(s_sel[rr]));
+              v[b] = __ldg(p.rows_f64 + static_cast<size_t>(row) * p.d + c0 + u);
+            }
+          }
+#pragma unroll
+          for (int b = 0; b < 2 * kHostLoads; ++b) {
+            const int i = i0 + b * kFinThreads;
+            if (i < nsel * len) {
+              const int rr = i / len, u = i - rr * len;
+              s_rows64[rr * row_stride + u] = v[b];
+            }
+          }
+        }
+      }
+      for (int i = tid; i < len; i += kFinThreads) s_q[i] = __ldg(qv + c0 + i);
+      __syncthreads();
+      if (tid < nsel) {
+        const double* mine = s_rows64 + tid * row_stride;
+        for (int i = 0; i < len; ++i) dot = __dadd_rn(dot, __dmul_rn(s_q[i], mine[i]));
       }
       if (tid == kFinThreads - 1)
         for (int i = 0; i < len; ++i) na_chain = __dadd_rn(na_chain, __dmul_rn(s_q[i], s_q[i]));
@@ -711,17 +784,93 @@ __global__ void __launch_bounds__(256) large_select_kernel(const unsigned int* _
 }
 
 // re-rank, part 1: the reference's fp64 cosine of every emitted row (one thread per candidate).
+// kHostRows (rows_f64 in mapped host memory): a thread walking its own row would issue 32 scattered host reads per
+// warp load.  Instead the block's 256 candidates stage their rows kLsChunk elements at a time in shared memory -
+// consecutive lanes read consecutive 16-byte pieces of one row, kHostLoads pieces in flight per thread - and each
+// thread then walks its own chain from there, in the same order as exact_dot_f64.
+constexpr int kLsChunk = 16;   // doubles per staged row piece (128 bytes)
+
+template <bool kHostRows>
 __global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
   const int q = blockIdx.y;
   const int i = blockIdx.x * 256 + threadIdx.x;
   const int n = min(p.emit_cnt[q], p.emit_cap[q]);
-  if (i >= n) return;
-  const size_t o = static_cast<size_t>(p.emit_off[q]) + i;
-  const int row = p.emit_rows[o];
-  const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
-  const double dot = p.rows_f64 != nullptr ? exact_dot_f64(qv, p.rows_f64 + static_cast<size_t>(row) * p.d, p.d)
-                                           : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
-  p.cand_scores[o] = exact_cosine(dot, p.q_norm2[q], p.row_norm2[row]);
+  if constexpr (!kHostRows) {
+    if (i >= n) return;
+    const size_t o = static_cast<size_t>(p.emit_off[q]) + i;
+    const int row = p.emit_rows[o];
+    const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
+    const double dot = p.rows_f64 != nullptr ? exact_dot_f64(qv, p.rows_f64 + static_cast<size_t>(row) * p.d, p.d)
+                                             : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
+    p.cand_scores[o] = exact_cosine(dot, p.q_norm2[q], p.row_norm2[row]);
+  } else {
+    __shared__ double s_x[256 * (kLsChunk + 1)];   // odd pitch in doubles: conflict-free walks
+    __shared__ double s_q[kLsChunk];
+    __shared__ int s_row[256];
+    const int tid = threadIdx.x;
+    const int first = blockIdx.x * 256;
+    if (first >= n) return;   // uniform over the block
+    const int m = n - first < 256 ? n - first : 256;   // candidates of this block
+    const size_t o = static_cast<size_t>(p.emit_off[q]) + i;
+    if (tid < m) s_row[tid] = p.emit_rows[o];
+    const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
+    const bool wide = (p.d & 1) == 0;   // every row and every even column start 16-byte aligned
+    double dot = 0.0;
+    for (int c0 = 0; c0 < p.d; c0 += kLsChunk) {
+      const int len = p.d - c0 < kLsChunk ? p.d - c0 : kLsChunk;
+      __syncthreads();   // s_row written / the previous chunk consumed
+      if (wide) {
+        const int len2 = len >> 1;
+        for (int i0 = tid; i0 < m * len2; i0 += kHostLoads * 256) {
+          double2 v[kHostLoads];
+#pragma unroll
+          for (int b = 0; b < kHostLoads; ++b) {
+            const int e = i0 + b * 256;
+            if (e < m * len2) {
+              const int rr = e / len2, u = e - rr * len2;
+              v[b] = __ldg(reinterpret_cast<const double2*>(p.rows_f64 + static_cast<size_t>(s_row[rr]) * p.d + c0) + u);
+            }
+          }
+#pragma unroll
+          for (int b = 0; b < kHostLoads; ++b) {
+            const int e = i0 + b * 256;
+            if (e < m * len2) {
+              const int rr = e / len2, u = e - rr * len2;
+              s_x[rr * (kLsChunk + 1) + 2 * u] = v[b].x;
+              s_x[rr * (kLsChunk + 1) + 2 * u + 1] = v[b].y;
+            }
+          }
+        }
+      } else {
+        for (int i0 = tid; i0 < m * len; i0 += 2 * kHostLoads * 256) {
+          double v[2 * kHostLoads];
+#pragma unroll
+          for (int b = 0; b < 2 * kHostLoads; ++b) {
+            const int e = i0 + b * 256;
+            if (e < m * len) {
+              const int rr = e / len, u = e - rr * len;
+              v[b] = __ldg(p.rows_f64 + static_cast<size_t>(s_row[rr]) * p.d + c0 + u);
+            }
+          }
+#pragma unroll
+          for (int b = 0; b < 2 * kHostLoads; ++b) {
+            const int e = i0 + b * 256;
+            if (e < m * len) {
+              const int rr = e / len, u = e - rr * len;
+              s_x[rr * (kLsChunk + 1) + u] = v[b];
+            }
+          }
+        }
+      }
+      if (tid < len) s_q[tid] = __ldg(qv + c0 + tid);
+      __syncthreads();
+      if (tid < m) {
+        const double* mine = s_x + tid * (kLsChunk + 1);
+        for (int e = 0; e < len; ++e) dot = __dadd_rn(dot, __dmul_rn(s_q[e], mine[e]));
+      }
+    }
+    if (tid < m) p.cand_scores[o] = exact_cosine(dot, p.q_norm2[q], p.row_norm2[s_row[tid]]);
+  }
 }
 
 // re-rank, part 2: one block per query keeps the best k_fetch of its candidates by (score desc, row asc) in a
@@ -929,15 +1078,16 @@ cudaError_t launch_prep_queries(const void* src, int src_type, int B, int d, int
   return cudaGetLastError();
 }
 
-cudaError_t launch_finalize(const FinalizeParams& p_in, cudaStream_t stream) {
+cudaError_t launch_finalize(const FinalizeParams& p_in, bool rows_on_host, cudaStream_t stream) {
   if (p_in.B <= 0) return cudaSuccess;
   FinalizeParams p = p_in;
   // >= 2048 keys (16 KB: room for 128 candidate rows x 56 elements per re-rank chunk)
   p.key_cap = p.B <= 160 ? 16384 : (p.B <= 320 ? 8192 : 2048);
   const size_t smem = static_cast<size_t>(p.key_cap) * 8;
-  cudaError_t e = cudaFuncSetAttribute(finalize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
+  auto kernel = rows_on_host ? finalize_kernel<true> : finalize_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
   if (e != cudaSuccess) return e;
-  finalize_kernel<<<p.B, kFinThreads, smem, stream>>>(p);
+  kernel<<<p.B, kFinThreads, smem, stream>>>(p);
   return cudaGetLastError();
 }
 
@@ -968,11 +1118,12 @@ cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init,
   return cudaGetLastError();
 }
 
-cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, cudaStream_t stream) {
+cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, bool rows_on_host, cudaStream_t stream) {
   if (p.B <= 0) return cudaSuccess;
   if (max_cap > 0) {
     dim3 grid(static_cast<unsigned>((max_cap + 255) / 256), static_cast<unsigned>(p.B));
-    large_score_kernel<<<grid, 256, 0, stream>>>(p);
+    if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
+    else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }

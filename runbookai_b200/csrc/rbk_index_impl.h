@@ -82,6 +82,9 @@ struct rbk_index {
   double* norm2 = nullptr;
   double* rows_f64 = nullptr;   // optional exact-source sidecar [cap][dim] (RBK_INDEX_KEEP_F64)
   bool keep_f64 = false;
+  // RBK_INDEX_F64_ON_HOST: rows_f64 is pinned, mapped host memory (one pointer under UVA).  Every write to it is
+  // stream-ordered: a kernel or copy on `stream`, or the host after a synchronisation of `stream`.
+  bool f64_on_host = false;
   unsigned int* dead_bits = nullptr;
   int* d_counter = nullptr;   // [0] tombstone counter, [1] eps_c_max (float bits)
   cudaStream_t own_stream = nullptr, stream = nullptr;

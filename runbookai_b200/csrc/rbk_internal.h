@@ -139,7 +139,9 @@ struct FinalizeParams {
   int* out_counts;        // [B]
   int* flags;             // [B] 1 = not provably exact -> exhaustive fallback
 };
-cudaError_t launch_finalize(const FinalizeParams& p, cudaStream_t stream);
+// rows_on_host: rows_f64 is mapped host memory (RBK_INDEX_F64_ON_HOST); the re-rank stages it with wide loads, more
+// of them in flight, to cover the PCIe round trip.  Same scores either way.
+cudaError_t launch_finalize(const FinalizeParams& p, bool rows_on_host, cudaStream_t stream);
 
 struct ExactParams {
   const int* fail_list;  // [n_fail] query indices
@@ -187,8 +189,9 @@ struct LargeRerankParams {
   int* out_counts;          // [B]
   int* overflow;            // += queries whose emit pass found more rows than C_q (a broken count)
 };
-// max_cap: largest emit_cap of the launch (sizes the scoring grid)
-cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, cudaStream_t stream);
+// max_cap: largest emit_cap of the launch (sizes the scoring grid).  rows_on_host: as for launch_finalize; the
+// scoring kernel then stages its candidates' rows in shared memory with coalesced loads.
+cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, bool rows_on_host, cudaStream_t stream);
 
 // Exact fp64 cosine of every row for B prepared queries: out [B][n_rows], NaN = tombstoned / zero row.
 cudaError_t launch_exact_scores(const uint16_t* rows, const double* rows_f64, const double* row_norm2,

@@ -125,11 +125,19 @@ def shared_index_count() -> int:
 
 
 class VectorStore:
-    def __init__(self, db_path: str, device: int | None = None, index_factory=None, shared: bool = False):
+    def __init__(self, db_path: str, device: int | None = None, index_factory=None, shared: bool = False,
+                 f64_on_host: bool | None = None):
         # index_factory(dim, device) -> object with the _native.Index surface; tests inject a
         # CPU stand-in to exercise the host logic where there is no GPU
-        # keep_f64: the reference stores float64 embeddings; keep them so the re-rank is exact for any input
-        self._index_factory = index_factory or (lambda dim, dev: Index(dim, device=dev, keep_f64=True))
+        # keep_f64: the reference stores float64 embeddings; keep them so the re-rank is exact for any input.
+        # f64_on_host (None: RUNBOOK_KNN_F64_ON_HOST=1 enables): those float64 rows live in pinned host memory instead
+        # of on the GPU - the same answers, about 5x the rows per GPU at d = 1536, host RAM and PCIe reads in the
+        # re-rank instead.  A shared index keeps the placement of the instance that created it.
+        if f64_on_host is None:
+            f64_on_host = os.environ.get("RUNBOOK_KNN_F64_ON_HOST", "0") == "1"
+        self.f64_on_host = on_host = bool(f64_on_host)
+        self._index_factory = index_factory or (
+            lambda dim, dev: Index(dim, device=dev, keep_f64=True, f64_on_host=on_host))
         # one connection, usable from the micro-batcher's worker thread too; serialised by a lock
         self.db = sqlite3.connect(db_path, check_same_thread=False)
         self.db.row_factory = sqlite3.Row

@@ -26,6 +26,14 @@ function devicesFromEnv(): number | number[] {
   return Number(process.env.RUNBOOK_KNN_DEVICE ?? 0);
 }
 
+/**
+ * RUNBOOK_KNN_F64_ON_HOST="1" keeps the float64 rows in pinned host memory instead of on the GPU (RBK_INDEX_F64_ON_HOST):
+ * the same answers, about 5x the rows per GPU at d = 1536, host RAM and PCIe reads in the re-rank instead.
+ */
+function hostRowsFromEnv(): number {
+  return process.env.RUNBOOK_KNN_F64_ON_HOST === '1' ? 1 : 0;
+}
+
 export class GpuEmbeddingIndex {
   private index: any | null = null;
   private idOfSlot: (string | null)[] = [];
@@ -76,7 +84,7 @@ export class GpuEmbeddingIndex {
     this.dim = rows[0].embedding.length / 8;
     const usable = rows.filter((r) => r.embedding.length === this.dim * 8);
     for (const r of rows) if (r.embedding.length !== this.dim * 8) this.badIds.add(r.id);
-    this.index = new RbkIndex(this.dim, this.device, usable.length);
+    this.index = new RbkIndex(this.dim, this.device, usable.length, hostRowsFromEnv());
     // the Buffers go to the addon as they are: it packs them with memcpy and appends in one call
     const first = Number(this.index.appendBlobs(usable.map((r) => r.embedding)));
     usable.forEach((r, i) => this.remember(r.id, first + i));
@@ -86,7 +94,7 @@ export class GpuEmbeddingIndex {
   set(id: string, embedding: number[]): void {
     if (!this.index) {
       this.dim = embedding.length;
-      this.index = new RbkIndex(this.dim, this.device, 0);
+      this.index = new RbkIndex(this.dim, this.device, 0, hostRowsFromEnv());
     }
     const slot = this.slotOfId.get(id);
     if (embedding.length !== this.dim) {
