@@ -544,16 +544,21 @@ __device__ __forceinline__ void run_emit_epilogue(const LargeScanParams& p, cons
 // Bounded-lag lockstep of the QB producers that stream the same corpus range: nobody runs
 // more than kMaxLeadTiles ahead of the slowest, so a tile pulled from HBM by the first
 // reader is still in L2 for the others (keeps DRAM traffic close to 1x the corpus).
-__device__ __forceinline__ void lockstep_pace(volatile int* prog, int QB, int qb, int it, int max_lead) {
+// Whole warp: lane o reads peer o's progress, so all peers cost one L2 round trip, and the warp only spins (re-reading
+// in parallel) while a ballot finds someone behind.  The wait gives up after 2^24 cycles in all (not per peer): it is a
+// hint, and a peer that far behind is not worth more of this CTA's time.
+static_assert(kMaxSubBatch / kBlockM <= 32, "one lane per query block");
+__device__ __forceinline__ void lockstep_pace(volatile int* prog, int QB, int qb, int it, int max_lead, int lane) {
   if (QB <= 1 || (it & 1) != 0) return;   // every other tile: checking every tile costs ~10 % on short kernels
-  prog[qb] = it;
-  for (int o = 0; o < QB; ++o) {
-    if (o == qb) continue;
-    const long long w0 = clock64();
-    while (prog[o] < it - max_lead) {
-      __nanosleep(200);
-      if (clock64() - w0 > (1ll << 24)) break;   // a pacing hint, never a correctness wait
-    }
+  if (lane == 0) prog[qb] = it;
+  const bool peer = lane < QB && lane != qb;
+  const int floor = it - max_lead;
+  bool behind = peer && prog[lane] < floor;
+  const long long w0 = clock64();
+  while (__any_sync(0xFFFFFFFFu, behind)) {
+    __nanosleep(200);
+    if (__shfl_sync(0xFFFFFFFFu, clock64() - w0, 0) > (1ll << 24)) break;   // never a correctness wait
+    behind = peer && prog[lane] < floor;
   }
 }
 

@@ -77,6 +77,47 @@ __device__ unsigned long long g_stage_stats[4];
 __device__ unsigned int g_stage_done;
 #endif
 
+// Development probe (RBK_SCAN_CYCLE_STATS): where a wgmma warpgroup's cycles go.  Its leader thread adds SM-clock
+// deltas into buckets, summed over the launch per warpgroup:
+//   full     waiting on a ring slot's `full` barrier;
+//   mma      fence, HGMMA issue and wait_group until the previous group has retired (tensor work);
+//   handoff  from wait_group returning to the end of the slot releases (the `empty` arrive and, for warpgroup 1,
+//            whose first warp is the producer, the `empty` wait, pacing and TMA issue of the refill);
+//   pace     the part of handoff spent in lockstep_pace (warpgroup 1 only);
+//   tile_end wait_group 0, the last release, the prefilter, the st_empty waits and the row staging.
+// The laps are contiguous, so full + mma + handoff + tile_end is the whole main loop.  The kernel only adds; the host
+// reads and clears the sums with rbk_scan_cycle_stats (no printf: a call inside the kernel makes ptxas serialize the
+// wgmma pipeline, and the probe would time another kernel).  The probe's registers cost the top-k' instantiation
+// about 20 bytes of spills, reloaded at the tile end, none in the k-step loop.  Without the macro CycleProbe is empty
+// and compiles to nothing.
+enum CycleBucket { kCycFull, kCycMma, kCycHandoff, kCycPace, kCycTileEnd, kCycBuckets };
+#ifdef RBK_SCAN_CYCLE_STATS
+__device__ unsigned long long g_cycle_stats[3][2][kCycBuckets + 2];   // [mode][warpgroup][bucket, tiles, units]
+__device__ __forceinline__ uint32_t sm_clock() {
+  uint32_t c;
+  asm volatile("mov.u32 %0, %%clock;" : "=r"(c)::"memory");
+  return c;
+}
+struct CycleProbe {
+  uint32_t t = 0, c[kCycBuckets] = {};
+  __device__ __forceinline__ void mark() { t = sm_clock(); }
+  __device__ __forceinline__ void lap(int b) {   // t .. now into bucket b; now becomes t
+    const uint32_t n = sm_clock();
+    c[b] += n - t;
+    t = n;
+  }
+  __device__ __forceinline__ void add_since(int b, uint32_t t0) { c[b] += sm_clock() - t0; }
+  __device__ __forceinline__ static uint32_t now() { return sm_clock(); }
+};
+#else
+struct CycleProbe {
+  __device__ __forceinline__ void mark() {}
+  __device__ __forceinline__ void lap(int) {}
+  __device__ __forceinline__ void add_since(int, uint32_t) {}
+  __device__ __forceinline__ static uint32_t now() { return 0u; }
+};
+#endif
+
 // kMode 0: top-k' candidate lists (P = ScanParams); kScanCount / kScanEmit: the large-k passes (P = LargeScanParams)
 template <int kMode, typename P>
 __global__ void __launch_bounds__(kScanThreads, 1)
@@ -143,14 +184,16 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
   const int n_iter = t1 - t0;
   const int n_steps = n_iter * n_ks;   // k-steps of the whole unit; step j uses ring slot j % kStages
   volatile int* prog = p.progress + r * p.QB;
+  CycleProbe probe;
   // Load step j into its slot once both warpgroups have released the slot's previous use (whole warp).
   auto issue = [&](int j) {
     if (j >= n_steps) return;
     const int s = j % kStages;
     const int tile = t0 + j / n_ks, ks = j % n_ks;
     mbar_wait(smem_u32(&tail->empty[s]), static_cast<uint32_t>((j / kStages) & 1) ^ 1u);
-    if (ks == 0 && lane == 0) lockstep_pace(prog, p.QB, qb, tile - t0, p.max_lead_tiles);
-    __syncwarp();
+    const uint32_t pace0 = CycleProbe::now();
+    if (ks == 0) lockstep_pace(prog, p.QB, qb, tile - t0, p.max_lead_tiles, lane);
+    probe.add_since(kCycPace, pace0);
     const uint32_t full = smem_u32(&tail->full[s]);
     const uint32_t a_dst = smem_base + s * kStageBytes;
     if (elect_one()) {
@@ -190,10 +233,12 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
 #pragma unroll
   for (int i = 0; i < 128; ++i) acc[i] = 0.f;
   int j = 0;
+  probe.mark();
   for (int i = 0; i < n_iter; ++i) {
     for (int ks = 0; ks < n_ks; ++ks, ++j) {
       const int s = j % kStages;
       mbar_wait(smem_u32(&tail->full[s]), static_cast<uint32_t>((j / kStages) & 1));
+      probe.lap(kCycFull);
       const uint32_t st = smem_base + s * kStageBytes;
       const uint64_t adesc = make_sw128_kmajor_desc(st + wg * (64 * kBlockK * 2));
       const uint64_t bdesc = make_sw128_kmajor_desc(st + kABytes);
@@ -204,7 +249,9 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
                               (ks | k) != 0 ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<1>(acc);   // the previous step's group has retired
+      probe.lap(kCycMma);
       if (ks > 0) release(j - 1);
+      probe.lap(kCycHandoff);
     }
     wgmma_wait<0>(acc);
     release(j - 1);
@@ -272,8 +319,17 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
       mbar_arrive(st_full);
       ++rounds;
     } while (pending != 0ull);
+    probe.lap(kCycTileEnd);
   }
   if (producer && lane == 0 && p.QB > 1) prog[qb] = 0x7FFFFFFF;  // done: never hold a peer back
+#ifdef RBK_SCAN_CYCLE_STATS
+  if (leader) {   // the host reads the sums (rbk_scan_cycle_stats): a call here would serialize the wgmma pipeline
+    for (int b = 0; b < kCycBuckets; ++b)
+      atomicAdd(&g_cycle_stats[kMode][wg][b], static_cast<unsigned long long>(probe.c[b]));
+    atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets], static_cast<unsigned long long>(n_iter));
+    atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets + 1], 1ull);
+  }
+#endif
 #ifdef RBK_SCAN_STAGE_STATS
   if (leader) {
     atomicAdd(&g_stage_stats[0], static_cast<unsigned long long>(n_iter));
@@ -315,3 +371,17 @@ cudaError_t launch_scan_large(const CUtensorMap& tmap_q, const CUtensorMap& tmap
 }
 
 }  // namespace rbk
+
+#ifdef RBK_SCAN_CYCLE_STATS
+// Probe builds only: waits for the current device, copies its cycle sums ([mode][warpgroup][full, mma, handoff, pace,
+// tile_end, tiles, units], 42 values) to out and clears them.  Returns the number of values, or -1 on a CUDA error.
+extern "C" int rbk_scan_cycle_stats(unsigned long long* out) {
+  constexpr int n = 3 * 2 * (rbk::kCycBuckets + 2);
+  static const unsigned long long zero[n] = {};
+  if (cudaDeviceSynchronize() != cudaSuccess ||
+      cudaMemcpyFromSymbol(out, rbk::g_cycle_stats, sizeof(zero)) != cudaSuccess ||
+      cudaMemcpyToSymbol(rbk::g_cycle_stats, zero, sizeof(zero)) != cudaSuccess)
+    return -1;
+  return n;
+}
+#endif
