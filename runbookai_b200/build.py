@@ -44,7 +44,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         return LIB
     LIB.parent.mkdir(parents=True, exist_ok=True)
     cmd = [_nvcc(), *NVCC_FLAGS, *[str(CSRC / s) for s in SOURCES], "-o", str(LIB)]
-    for flag in os.environ.get("RBK_EXTRA_NVCC_FLAGS", "").split():   # development probes, e.g. -DRBK_FIN_PROFILE
+    for flag in os.environ.get("RBK_EXTRA_NVCC_FLAGS", "").split():   # development probes, e.g. -DRBK_SCAN_CYCLE_STATS
         cmd.insert(1, flag)
     if verbose:
         cmd.insert(1, "-Xptxas=-v")

@@ -92,15 +92,6 @@ bool host_source_is_pinned(const void* p) {
   return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
 }
 
-cudaEvent_t get_event(rbk_index* ix, size_t i) {
-  while (ix->ev.size() <= i) {
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    ix->ev.push_back(e);
-  }
-  return ix->ev[i];
-}
-
 // Fold finished (start, stop) pairs into the running totals.  wait = true: block on the pending ones.
 void resolve_scan_events(rbk_index* ix, bool wait) {
   while (ix->tev_tail < ix->tev_head) {
@@ -277,6 +268,95 @@ rbk_status refresh_corpus_tmap(rbk_index* ix) {
   return RBK_OK;
 }
 
+QueryBuffers query_buffers(rbk_index* ix, int q0) {
+  QueryBuffers qb;
+  qb.q_bf16 = ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad;
+  qb.q_f64 = ix->q_f64.p + static_cast<size_t>(q0) * ix->dim;
+  qb.q_norm2 = ix->q_norm2.p + q0;
+  qb.q_inv_norm = ix->q_inv_norm.p + q0;
+  qb.q_eps = ix->q_eps.p + q0;
+  qb.thr_init = ix->thr_init.p + q0;
+  return qb;
+}
+
+// ---- one scan launch per sub-batch of at most kMaxSubBatch queries, in every mode ----
+// A launch's scratch is one buffer, ix->hist, split for a sub-batch of Bs queries as
+//   hist [Bs][kHistBins] | maxbin [Bs] | gthr [Bs] | progress [sm_count + 8]
+// and zeroed before every launch: by the prep kernel for the first sub-batch, by zero_scan_scratch for the others.
+int progress_slots(const rbk_index* ix) { return ix->sm_count + 8; }
+size_t scan_scratch_words(const rbk_index* ix, int Bs) {
+  return static_cast<size_t>(Bs) * kHistBins + 2 * Bs + progress_slots(ix);
+}
+
+// The fields every scan mode shares, for the Bs queries from q0 on.
+void fill_scan_params(rbk_index* ix, int q0, int Bs, int kprime, ScanParams* sp) {
+  const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
+  const int QB = (Bs + kBlockM - 1) / kBlockM;
+  sp->inv_norm_c = ix->inv_norm;
+  sp->thr_init = ix->thr_init.p + q0;
+  sp->inv_norm_q = ix->q_inv_norm.p + q0;
+  sp->hist = ix->hist.p;
+  sp->maxbin = reinterpret_cast<int*>(ix->hist.p + static_cast<size_t>(Bs) * kHistBins);
+  sp->gthr = reinterpret_cast<unsigned int*>(sp->maxbin + Bs);
+  sp->progress = sp->maxbin + 2 * Bs;
+  sp->n_rows = static_cast<int>(ix->n_rows);
+  sp->B = Bs;
+  sp->kprime = kprime;
+  sp->dpad = ix->dpad;
+  sp->max_lead_tiles = ix->max_lead_tiles;
+  sp->QB = QB;
+  sp->R = std::max(1, std::min(ix->sm_count / QB, n_tiles));
+  sp->n_tiles = n_tiles;
+}
+
+LargeScanParams large_scan_params(rbk_index* ix, int q0, int Bs, int k_fetch) {
+  LargeScanParams sp{};
+  fill_scan_params(ix, q0, Bs, k_fetch, &sp);
+  sp.q_eps = ix->q_eps.p + q0;
+  return sp;
+}
+
+cudaError_t zero_scan_scratch(rbk_index* ix, int Bs) {
+  return cudaMemsetAsync(ix->hist.p, 0, sizeof(unsigned int) * scan_scratch_words(ix, Bs), ix->stream);
+}
+
+// The prep kernel for all B queries; it also zeroes the first sub-batch's scan scratch.
+rbk_status prep_queries(rbk_index* ix, const void* d_q, int src_type, int B, double min_score, bool with_norm2) {
+  CK(launch_prep_queries(d_q, src_type, B, ix->dim, ix->dpad, min_score,
+                         ix->keep_f64 ? reinterpret_cast<const float*>(ix->d_counter + 1) : nullptr,
+                         query_buffers(ix, 0), ix->stream, with_norm2, ix->hist.p, std::min(kMaxSubBatch, B),
+                         progress_slots(ix)));
+  ix->stats.kernel_launches++;
+  return RBK_OK;
+}
+
+// Launches one filled sub-batch: its query map, then the scan kernel of kMode (0: the top-k' scan, P = ScanParams;
+// kScanCount / kScanEmit: a large-k pass, P = LargeScanParams) inside a timing pair unless the stream is being captured.
+template <int kMode, typename P>
+rbk_status launch_sub_batch(rbk_index* ix, int q0, const P& sp) {
+  CUtensorMap tmap_q;
+  const int q_rows = static_cast<int>(round_up(sp.B, kBlockM));   // whole query blocks: no out-of-bounds box rows
+  rbk_status st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM);
+  if (st != RBK_OK) return st;
+  cudaEvent_t* tev = ix->capturing ? nullptr : next_scan_events(ix);
+  if (tev) CK(cudaEventRecord(tev[0], ix->stream));
+  if constexpr (kMode == 0) CK(launch_scan(tmap_q, ix->tmap_c, sp, ix->stream));
+  else CK(launch_scan_large(tmap_q, ix->tmap_c, sp, static_cast<LargeScanMode>(kMode), ix->stream));
+  if (tev) CK(cudaEventRecord(tev[1], ix->stream));
+  ix->stats.last_ring_stages = kStages;
+  ix->stats.scan_launches++;
+  ix->stats.kernel_launches++;
+  return RBK_OK;
+}
+
+// Results of a search over an empty index: -1 slots, NaN scores, zero counts.
+rbk_status fill_empty_results(rbk_index* ix, int B, int k_fetch, long long* d_slots, double* d_scores, int* d_counts) {
+  CK(cudaMemsetAsync(d_counts, 0, sizeof(int) * B, ix->stream));
+  CK(cudaMemsetAsync(d_slots, 0xFF, sizeof(long long) * B * k_fetch, ix->stream));   // -1
+  CK(cudaMemsetAsync(d_scores, 0xFF, sizeof(double) * B * k_fetch, ix->stream));     // NaN
+  return RBK_OK;
+}
+
 }  // namespace
 
 // ---- shared with rbk_group.cu (declared in rbk_index_impl.h) ----
@@ -303,9 +383,7 @@ rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem) {
   CK(ix->flags.ensure(B));
   CK(ix->cand.ensure(static_cast<size_t>(ix->sm_count) * kBlockM * kListCap));
   CK(ix->cand_cnt.ensure(static_cast<size_t>(ix->sm_count) * kBlockM));
-  // hist [kMaxSubBatch][kHistBins] | maxbin [kMaxSubBatch] | gthr [kMaxSubBatch] | progress [sm_count + 8]:
-  // one buffer, one memset
-  CK(ix->hist.ensure(static_cast<size_t>(kMaxSubBatch) * kHistBins + 2 * kMaxSubBatch + ix->sm_count + 8));
+  CK(ix->hist.ensure(scan_scratch_words(ix, kMaxSubBatch)));
   return RBK_OK;
 }
 
@@ -324,90 +402,41 @@ rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, i
 
 namespace {
 
-QueryBuffers query_buffers(rbk_index* ix, int q0) {
-  QueryBuffers qb;
-  qb.q_bf16 = ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad;
-  qb.q_f64 = ix->q_f64.p + static_cast<size_t>(q0) * ix->dim;
-  qb.q_norm2 = ix->q_norm2.p + q0;
-  qb.q_inv_norm = ix->q_inv_norm.p + q0;
-  qb.q_eps = ix->q_eps.p + q0;
-  qb.thr_init = ix->thr_init.p + q0;
-  return qb;
-}
-
 // Launch the scan (+ optionally finalize) for every sub-batch.  d_q: device queries.
 rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_fetch, double min_score,
                     long long* d_slots, double* d_scores, int* d_counts, int* d_flags, float* dbg) {
   const int kprime = pick_kprime(ix, k_fetch);
   ix->stats.last_kprime = kprime;
-  // (also zeroes the scan scratch of the first sub-batch; normA is left to the finalize kernel)
-  const int Bs0 = std::min(kMaxSubBatch, B);
-  CK(launch_prep_queries(d_q, src_type, B, ix->dim, ix->dpad, min_score,
-                         ix->keep_f64 ? reinterpret_cast<const float*>(ix->d_counter + 1) : nullptr,
-                         query_buffers(ix, 0), ix->stream, /*with_norm2=*/d_counts == nullptr, ix->hist.p, Bs0,
-                         ix->sm_count + 8));
-  ix->stats.kernel_launches++;
+  // normA is left to the finalize kernel
+  rbk_status st = prep_queries(ix, d_q, src_type, B, min_score, /*with_norm2=*/d_counts == nullptr);
+  if (st != RBK_OK) return st;
   if (ix->n_rows == 0) {
     // nothing to scan: finalize would read unwritten lists; emit empty results directly
     if (d_counts) {
-      CK(cudaMemsetAsync(d_counts, 0, sizeof(int) * B, ix->stream));
-      CK(cudaMemsetAsync(d_slots, 0xFF, sizeof(long long) * B * k_fetch, ix->stream));   // -1
-      CK(cudaMemsetAsync(d_scores, 0xFF, sizeof(double) * B * k_fetch, ix->stream));     // NaN
+      st = fill_empty_results(ix, B, k_fetch, d_slots, d_scores, d_counts);
+      if (st != RBK_OK) return st;
       CK(cudaMemsetAsync(d_flags, 0, sizeof(int) * B, ix->stream));
     }
     return RBK_OK;
   }
-  rbk_status st = refresh_corpus_tmap(ix);
+  st = refresh_corpus_tmap(ix);
   if (st != RBK_OK) return st;
-  const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
   for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
     const int Bs = std::min(kMaxSubBatch, B - q0);
-    const int QB = (Bs + kBlockM - 1) / kBlockM;
-    const int R = std::max(1, std::min(ix->sm_count / QB, n_tiles));
-    CUtensorMap tmap_q;
-    const int q_rows = static_cast<int>(round_up(Bs, kBlockM));   // whole query blocks: no out-of-bounds box rows
-    st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM);
-    if (st != RBK_OK) return st;
+    if (q0 > 0) CK(zero_scan_scratch(ix, Bs));
     ScanParams sp;
-    sp.inv_norm_c = ix->inv_norm;
-    sp.thr_init = ix->thr_init.p + q0;
-    sp.inv_norm_q = ix->q_inv_norm.p + q0;
-    {
-      // per-launch scratch, zeroed with one memset: hist rows of this sub-batch, then maxbin, gthr, progress
-      unsigned int* base = ix->hist.p;
-      sp.hist = base;
-      sp.maxbin = reinterpret_cast<int*>(base + static_cast<size_t>(Bs) * kHistBins);
-      sp.gthr = reinterpret_cast<unsigned int*>(sp.maxbin + Bs);
-      sp.progress = sp.maxbin + 2 * Bs;
-      if (q0 > 0)   // the first sub-batch's scratch was zeroed by the prep kernel
-        CK(cudaMemsetAsync(base, 0,
-                           sizeof(unsigned int) * (static_cast<size_t>(Bs) * kHistBins + 2 * Bs + ix->sm_count + 8),
-                           ix->stream));
-    }
+    fill_scan_params(ix, q0, Bs, kprime, &sp);
     sp.cand = ix->cand.p;
     sp.cand_cnt = ix->cand_cnt.p;
     sp.dbg_scores = dbg ? dbg + static_cast<size_t>(q0) * ix->n_rows : nullptr;
-    sp.n_rows = static_cast<int>(ix->n_rows);
-    sp.B = Bs;
-    sp.kprime = kprime;
-    sp.dpad = ix->dpad;
-    sp.max_lead_tiles = ix->max_lead_tiles;
-    sp.QB = QB;
-    sp.R = R;
-    sp.n_tiles = n_tiles;
-    cudaEvent_t* tev = ix->capturing ? nullptr : next_scan_events(ix);
-    if (tev) CK(cudaEventRecord(tev[0], ix->stream));
-    CK(launch_scan(tmap_q, ix->tmap_c, sp, ix->stream));
-    ix->stats.last_ring_stages = kStages;
-    if (tev) CK(cudaEventRecord(tev[1], ix->stream));
-    ix->stats.scan_launches++;
-    ix->stats.kernel_launches++;
+    st = launch_sub_batch<0>(ix, q0, sp);
+    if (st != RBK_OK) return st;
     if (d_counts) {
       FinalizeParams fp;
       fp.cand = ix->cand.p;
       fp.cand_cnt = ix->cand_cnt.p;
-      fp.QB = QB;
-      fp.R = R;
+      fp.QB = sp.QB;
+      fp.R = sp.R;
       fp.kprime = kprime;
       fp.k_fetch = k_fetch;
       fp.B = Bs;
@@ -483,54 +512,6 @@ rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, i
   ix->stats.queries += B;
   return run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr);
 }
-}  // namespace impl
-}  // namespace rbk
-
-namespace {
-
-// Scan parameters of one sub-batch of the large-k search; the per-launch scratch (hist | maxbin | gthr | progress)
-// is laid out as in run_scan.
-LargeScanParams large_scan_params(rbk_index* ix, int q0, int Bs, int k_fetch, int n_tiles) {
-  LargeScanParams sp{};
-  const int QB = (Bs + kBlockM - 1) / kBlockM;
-  sp.inv_norm_c = ix->inv_norm;
-  sp.thr_init = ix->thr_init.p + q0;
-  sp.inv_norm_q = ix->q_inv_norm.p + q0;
-  sp.hist = ix->hist.p;
-  sp.maxbin = reinterpret_cast<int*>(ix->hist.p + static_cast<size_t>(Bs) * kHistBins);
-  sp.gthr = reinterpret_cast<unsigned int*>(sp.maxbin + Bs);
-  sp.progress = sp.maxbin + 2 * Bs;
-  sp.n_rows = static_cast<int>(ix->n_rows);
-  sp.B = Bs;
-  sp.kprime = k_fetch;
-  sp.dpad = ix->dpad;
-  sp.max_lead_tiles = ix->max_lead_tiles;
-  sp.QB = QB;
-  sp.R = std::max(1, std::min(ix->sm_count / QB, n_tiles));
-  sp.n_tiles = n_tiles;
-  sp.q_eps = ix->q_eps.p + q0;
-  return sp;
-}
-
-rbk_status launch_large_scan(rbk_index* ix, int q0, const LargeScanParams& sp, LargeScanMode mode) {
-  CUtensorMap tmap_q;
-  const int q_rows = static_cast<int>(round_up(sp.B, kBlockM));
-  rbk_status st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM);
-  if (st != RBK_OK) return st;
-  cudaEvent_t* tev = next_scan_events(ix);
-  CK(cudaEventRecord(tev[0], ix->stream));
-  CK(launch_scan_large(tmap_q, ix->tmap_c, sp, mode, ix->stream));
-  CK(cudaEventRecord(tev[1], ix->stream));
-  ix->stats.last_ring_stages = kStages;
-  ix->stats.scan_launches++;
-  ix->stats.kernel_launches++;
-  return RBK_OK;
-}
-
-}  // namespace
-
-namespace rbk {
-namespace impl {
 
 rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, double min_score) {
   ix->stats.searches++;
@@ -545,26 +526,19 @@ rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, doubl
   CK(ix->h_loff.ensure(B));
   CK(ix->h_lerr.ensure(1));
   // normA is computed here: the re-rank has no spare thread to walk the chain beside its candidates
-  const int Bs0 = std::min(kMaxSubBatch, B);
-  CK(launch_prep_queries(d_q, 0, B, ix->dim, ix->dpad, min_score,
-                         ix->keep_f64 ? reinterpret_cast<const float*>(ix->d_counter + 1) : nullptr,
-                         query_buffers(ix, 0), ix->stream, /*with_norm2=*/true, ix->hist.p, Bs0, ix->sm_count + 8));
-  ix->stats.kernel_launches++;
+  rbk_status st = prep_queries(ix, d_q, 0, B, min_score, /*with_norm2=*/true);
+  if (st != RBK_OK) return st;
   if (ix->n_rows == 0) {
     memset(ix->h_lcap.p, 0, sizeof(int) * B);
     return RBK_OK;
   }
-  rbk_status st = refresh_corpus_tmap(ix);
+  st = refresh_corpus_tmap(ix);
   if (st != RBK_OK) return st;
-  const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
   for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
     const int Bs = std::min(kMaxSubBatch, B - q0);
-    if (q0 > 0)   // the first sub-batch's scratch was zeroed by the prep kernel
-      CK(cudaMemsetAsync(ix->hist.p, 0,
-                         sizeof(unsigned int) * (static_cast<size_t>(Bs) * kHistBins + 2 * Bs + ix->sm_count + 8),
-                         ix->stream));
-    const LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch, n_tiles);
-    st = launch_large_scan(ix, q0, sp, kScanCount);
+    if (q0 > 0) CK(zero_scan_scratch(ix, Bs));
+    const LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch);
+    st = launch_sub_batch<kScanCount>(ix, q0, sp);
     if (st != RBK_OK) return st;
     CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Bs, k_fetch, ix->lg_theta.p + q0,
                            ix->lg_cap.p + q0, ix->stream));
@@ -578,12 +552,7 @@ rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long 
                       int* d_counts) {
   CK(cudaMemsetAsync(ix->lg_err.p, 0, sizeof(int), ix->stream));
   CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
-  if (ix->n_rows == 0) {
-    CK(cudaMemsetAsync(d_counts, 0, sizeof(int) * B, ix->stream));
-    CK(cudaMemsetAsync(d_slots, 0xFF, sizeof(long long) * B * k_fetch, ix->stream));   // -1
-    CK(cudaMemsetAsync(d_scores, 0xFF, sizeof(double) * B * k_fetch, ix->stream));     // NaN
-    return RBK_OK;
-  }
+  if (ix->n_rows == 0) return fill_empty_results(ix, B, k_fetch, d_slots, d_scores, d_counts);
   // segment offsets: exclusive prefix sum of C_q
   long long total = 0;
   for (int b = 0; b < B; ++b) {
@@ -594,17 +563,16 @@ rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long 
   CK(ix->lg_scores.ensure(static_cast<size_t>(std::max<long long>(total, 1))));
   CK(cudaMemcpyAsync(ix->lg_off.p, ix->h_loff.p, sizeof(long long) * B, cudaMemcpyHostToDevice, ix->stream));
   CK(cudaMemsetAsync(ix->lg_cnt.p, 0, sizeof(int) * B, ix->stream));
-  const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
   for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
     const int Bs = std::min(kMaxSubBatch, B - q0);
-    LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch, n_tiles);
+    LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch);
     sp.thr_init = ix->lg_theta.p + q0;   // theta_q
     sp.emit_off = ix->lg_off.p + q0;
     sp.emit_cap = ix->lg_cap.p + q0;
     sp.emit_cnt = ix->lg_cnt.p + q0;
     sp.emit_rows = ix->lg_rows.p;
-    CK(cudaMemsetAsync(sp.progress, 0, sizeof(int) * (ix->sm_count + 8), ix->stream));
-    rbk_status st = launch_large_scan(ix, q0, sp, kScanEmit);
+    CK(cudaMemsetAsync(sp.progress, 0, sizeof(int) * progress_slots(ix), ix->stream));
+    rbk_status st = launch_sub_batch<kScanEmit>(ix, q0, sp);
     if (st != RBK_OK) return st;
     LargeRerankParams rp;
     rp.B = Bs;
@@ -656,7 +624,7 @@ void drop_graph(rbk_index* ix) {
 // query is proven exact.  *done = false: something needs the general path (a query's proof failed), which the
 // caller then runs from scratch.
 rbk_status search_graph(rbk_index* ix, const void* q_host, int elem, int B, int k_fetch, double min_score,
-                        size_t blk, size_t off_flags, bool* done) {
+                        const ResultBlock& L, bool* done) {
   *done = false;
   const size_t q_bytes = static_cast<size_t>(B) * ix->dim * elem;
   CK(ix->h_q.ensure(q_bytes));
@@ -675,7 +643,6 @@ rbk_status search_graph(rbk_index* ix, const void* q_host, int elem, int B, int 
   key.slot = ix->slot;
   key.stream = ix->stream;
   unsigned char* base = ix->o_block.p;
-  const size_t nout = static_cast<size_t>(B) * k_fetch;
   if (!ix->graph_exec || memcmp(&key, &ix->graph_key, sizeof key) != 0) {
     drop_graph(ix);
     cudaGraph_t graph = nullptr;
@@ -684,11 +651,10 @@ rbk_status search_graph(rbk_index* ix, const void* q_host, int elem, int B, int 
     cudaError_t e = cudaMemcpyAsync(ix->q_raw.p, ix->h_q.p, q_bytes, cudaMemcpyHostToDevice, ix->stream);
     rbk_status st = RBK_OK;
     if (e == cudaSuccess)
-      st = run_scan(ix, ix->q_raw.p, elem == 8 ? 0 : 1, B, k_fetch, min_score, reinterpret_cast<long long*>(base),
-                    reinterpret_cast<double*>(base + nout * 8), reinterpret_cast<int*>(base + nout * 16),
-                    reinterpret_cast<int*>(base + off_flags), nullptr);
+      st = run_scan(ix, ix->q_raw.p, elem == 8 ? 0 : 1, B, k_fetch, min_score, L.slots(base), L.scores(base),
+                    L.counts(base), L.flags(base), nullptr);
     if (e == cudaSuccess && st == RBK_OK)
-      e = cudaMemcpyAsync(ix->h_block.p, ix->o_block.p, blk, cudaMemcpyDeviceToHost, ix->stream);
+      e = cudaMemcpyAsync(ix->h_block.p, base, L.bytes, cudaMemcpyDeviceToHost, ix->stream);
     ix->capturing = false;
     const cudaError_t e2 = cudaStreamEndCapture(ix->stream, &graph);   // always leave capture mode
     if (st != RBK_OK) {
@@ -712,30 +678,57 @@ rbk_status search_graph(rbk_index* ix, const void* q_host, int elem, int B, int 
     memcpy(&ix->graph_key, &key, sizeof key);
   }
   memcpy(ix->h_q.p, q_host, q_bytes);
-  CK(cudaEventRecord(get_event(ix, 0), ix->stream));
+  CK(cudaEventRecord(ix->ev_start, ix->stream));
   CK(cudaGraphLaunch(ix->graph_exec, ix->stream));
-  CK(cudaEventRecord(get_event(ix, 1), ix->stream));
+  CK(cudaEventRecord(ix->ev_stop, ix->stream));
   CK(cudaStreamSynchronize(ix->stream));   // the one host round trip
   ix->stats.searches++;
   ix->stats.queries += B;
   ix->stats.scan_launches++;
   ix->stats.kernel_launches += 3;           // prep, scan, finalize (inside the graph)
   ix->stats.graph_replays++;
-  const int* h_flags = reinterpret_cast<const int*>(ix->h_block.p + off_flags);
+  const int* h_flags = L.flags(ix->h_block.p);
   for (int b = 0; b < B; ++b)
     if (h_flags[b]) return RBK_OK;          // a proof failed: the general path re-answers the batch
   float total = 0.f;
-  cudaEventElapsedTime(&total, get_event(ix, 0), get_event(ix, 1));
+  cudaEventElapsedTime(&total, ix->ev_start, ix->ev_stop);
   ix->stats.last_total_ms = total;
   *done = true;
   return RBK_OK;
 }
 
-// Whole search, synchronous.  q_host/q_dev: exactly one is non-null.  Host outputs (h_*) may be null
+// Device-time frame of a synchronous search: begin() records the start event before its first work, every host
+// round trip records the stop event and waits, and after the last one finish() takes the time of the whole search
+// and of its scans.
+struct TimedSearch {
+  rbk_index* ix;
+  double scan_ms0 = 0.0;
+  rbk_status begin() {
+    resolve_scan_events(ix, false);
+    scan_ms0 = ix->stats.scan_ms_total;
+    CK(cudaEventRecord(ix->ev_start, ix->stream));
+    return RBK_OK;
+  }
+  rbk_status round_trip() {
+    CK(cudaEventRecord(ix->ev_stop, ix->stream));
+    CK(cudaStreamSynchronize(ix->stream));
+    return RBK_OK;
+  }
+  void finish(float* ms_out) {
+    float total = 0.f;
+    cudaEventElapsedTime(&total, ix->ev_start, ix->ev_stop);
+    resolve_scan_events(ix, true);   // the stream is idle: every pair is final
+    ix->stats.last_total_ms = total;
+    ix->stats.last_scan_ms = static_cast<float>(ix->stats.scan_ms_total - scan_ms0);
+    if (ms_out) *ms_out = total;
+  }
+};
+
+// Whole search, synchronous.  q_host/q_dev: exactly one is non-null.  Host outputs (out_*) may be null
 // (device-output variant); device outputs may be null (host variant uses index scratch).
 rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int elem, int B, int query_dim,
                        int k_fetch, double min_score, long long* d_slots, double* d_scores, int* d_counts,
-                       int64_t* h_slots, double* h_scores, int32_t* h_counts, float* ms_out) {
+                       int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out) {
   rbk_status st = check_search_args(ix, B, q_host || q_dev, query_dim, k_fetch, min_score);
   if (st != RBK_OK) return st;
   std::lock_guard<std::mutex> lk(ix->mu);
@@ -747,42 +740,37 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
   }
   st = ensure_query_scratch(ix, B, elem);
   if (st != RBK_OK) return st;
-  const size_t nout = static_cast<size_t>(B) * k_fetch;
-  // Host-output calls use ONE packed device block (slots | scores | counts | flags) mirrored by one pinned
-  // host block, so results and exactness flags come back in a single D2H copy.
-  const size_t off_scores = nout * 8, off_counts = nout * 16, off_flags = off_counts + static_cast<size_t>(B) * 4;
-  const size_t blk = off_flags + static_cast<size_t>(B) * 4;
+  // Host-output calls use ONE packed device block mirrored by one pinned host block, so results and exactness flags
+  // come back in a single D2H copy.
+  const ResultBlock L(B, k_fetch);
   const bool packed = d_slots == nullptr;
   int* d_flags = ix->flags.p;
   const int* h_flags = nullptr;
   if (packed) {
-    CK(ix->o_block.ensure(blk));
-    CK(ix->h_block.ensure(blk));
-    unsigned char* base = ix->o_block.p;
-    d_slots = reinterpret_cast<long long*>(base);
-    d_scores = reinterpret_cast<double*>(base + off_scores);
-    d_counts = reinterpret_cast<int*>(base + off_counts);
-    d_flags = reinterpret_cast<int*>(base + off_flags);
-    h_flags = reinterpret_cast<const int*>(ix->h_block.p + off_flags);
+    CK(ix->o_block.ensure(L.bytes));
+    CK(ix->h_block.ensure(L.bytes));
+    d_slots = L.slots(ix->o_block.p);
+    d_scores = L.scores(ix->o_block.p);
+    d_counts = L.counts(ix->o_block.p);
+    d_flags = L.flags(ix->o_block.p);
+    h_flags = L.flags(ix->h_block.p);
   } else {
     CK(ix->h_flags.ensure(B));
     h_flags = ix->h_flags.p;
   }
   if (packed && q_host && B <= kBlockM && ix->n_rows > 0 && ix->use_graph) {
     bool done = false;
-    st = search_graph(ix, q_host, elem, B, k_fetch, min_score, blk, off_flags, &done);
+    st = search_graph(ix, q_host, elem, B, k_fetch, min_score, L, &done);
     if (st != RBK_OK) return st;
     if (done) {
       if (ms_out) *ms_out = ix->stats.last_total_ms;
-      memcpy(h_slots, ix->h_block.p, sizeof(int64_t) * nout);
-      memcpy(h_scores, ix->h_block.p + off_scores, sizeof(double) * nout);
-      memcpy(h_counts, ix->h_block.p + off_counts, sizeof(int32_t) * B);
+      L.unpack(ix->h_block.p, out_slots, out_scores, out_counts);
       return RBK_OK;
     }
   }
-  resolve_scan_events(ix, false);
-  const double scan_ms0 = ix->stats.scan_ms_total;
-  CK(cudaEventRecord(get_event(ix, 0), ix->stream));
+  TimedSearch ts{ix};
+  st = ts.begin();
+  if (st != RBK_OK) return st;
   const void* d_q = q_dev;
   if (q_host) {
     CK(cudaMemcpyAsync(ix->q_raw.p, q_host, static_cast<size_t>(B) * ix->dim * elem, cudaMemcpyHostToDevice,
@@ -793,16 +781,18 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
   st = enqueue_search(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags);
   if (st != RBK_OK) return st;
   auto copy_back = [&]() -> cudaError_t {
-    if (packed) return cudaMemcpyAsync(ix->h_block.p, ix->o_block.p, blk, cudaMemcpyDeviceToHost, ix->stream);
+    if (packed) return cudaMemcpyAsync(ix->h_block.p, ix->o_block.p, L.bytes, cudaMemcpyDeviceToHost, ix->stream);
     return cudaMemcpyAsync(ix->h_flags.p, d_flags, sizeof(int) * B, cudaMemcpyDeviceToHost, ix->stream);
   };
-  CK(copy_back());
-  CK(cudaEventRecord(get_event(ix, 1), ix->stream));
-  CK(cudaStreamSynchronize(ix->stream));   // the ONE host round trip of an exact batch
   std::vector<int> fails;
-  for (int b = 0; b < B; ++b)
-    if (h_flags[b]) fails.push_back(b);
-  if (!fails.empty() && ix->stats.last_kprime < kMaxKPrime) {
+  for (;;) {
+    CK(copy_back());
+    st = ts.round_trip();   // the ONE host round trip of an exact batch
+    if (st != RBK_OK) return st;
+    fails.clear();
+    for (int b = 0; b < B; ++b)
+      if (h_flags[b]) fails.push_back(b);
+    if (fails.empty() || ix->stats.last_kprime >= kMaxKPrime) break;
     // A proof fails when more rows tie with the k_fetch-th hit (within the scan's error bound) than the
     // candidate margin holds - duplicated chunks, typically.  Before paying an exhaustive fp64 pass per failing
     // query, scan the batch once more at scan speed with the widest margin (k' = 128): groups of up to ~100
@@ -812,13 +802,7 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
     st = run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr);
     ix->kprime_override = 0;
     if (st != RBK_OK) return st;
-    CK(copy_back());
-    CK(cudaEventRecord(get_event(ix, 1), ix->stream));
-    CK(cudaStreamSynchronize(ix->stream));
     ix->stats.retry_batches++;
-    fails.clear();
-    for (int b = 0; b < B; ++b)
-      if (h_flags[b]) fails.push_back(b);
   }
   if (!fails.empty()) {
     st = run_fallback(ix, fails, k_fetch, min_score, d_slots, d_scores, d_counts);
@@ -826,20 +810,11 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
     // the exhaustive answers are exact by construction: clear the flags the caller may forward
     CK(cudaMemsetAsync(d_flags, 0, sizeof(int) * B, ix->stream));
     if (packed) CK(copy_back());
-    CK(cudaEventRecord(get_event(ix, 1), ix->stream));
-    CK(cudaStreamSynchronize(ix->stream));
+    st = ts.round_trip();
+    if (st != RBK_OK) return st;
   }
-  float total = 0.f;
-  cudaEventElapsedTime(&total, get_event(ix, 0), get_event(ix, 1));
-  resolve_scan_events(ix, true);   // the stream is idle: every pair is final
-  ix->stats.last_total_ms = total;
-  ix->stats.last_scan_ms = static_cast<float>(ix->stats.scan_ms_total - scan_ms0);
-  if (ms_out) *ms_out = total;
-  if (h_slots) {
-    memcpy(h_slots, ix->h_block.p, sizeof(int64_t) * nout);
-    memcpy(h_scores, ix->h_block.p + off_scores, sizeof(double) * nout);
-    memcpy(h_counts, ix->h_block.p + off_counts, sizeof(int32_t) * B);
-  }
+  ts.finish(ms_out);
+  if (out_slots) L.unpack(ix->h_block.p, out_slots, out_scores, out_counts);
   return RBK_OK;
 }
 
@@ -889,6 +864,10 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
     delete ix;
     return cuda_fail(e, "cudaStreamCreate");
   }
+  if ((e = cudaEventCreate(&ix->ev_start)) != cudaSuccess || (e = cudaEventCreate(&ix->ev_stop)) != cudaSuccess) {
+    rbk_index_destroy(ix);
+    return cuda_fail(e, "cudaEventCreate");
+  }
   ix->stream = ix->own_stream;
   e = cudaMalloc(reinterpret_cast<void**>(&ix->d_counter), 2 * sizeof(int));
   if (e == cudaSuccess) e = cudaMemset(ix->d_counter, 0, 2 * sizeof(int));
@@ -931,14 +910,10 @@ void rbk_index_destroy(rbk_index* ix) {
     ix->cand.release();
     ix->cand_cnt.release();
     ix->hist.release();
-    ix->maxbin.release();
-    ix->progress.release();
     ix->flags.release();
     ix->fail_list.release();
-    ix->o_counts.release();
     ix->part_rows.release();
     ix->part_cnt.release();
-    ix->o_slots.release();
     ix->o_scores.release();
     ix->part_scores.release();
     ix->dbg.release();
@@ -955,13 +930,10 @@ void rbk_index_destroy(rbk_index* ix) {
     ix->o_block.release();
     ix->h_block.release();
     ix->h_flags.release();
-    ix->h_counts.release();
-    ix->h_slots.release();
-    ix->h_scores.release();
-    ix->h_f32.release();
     drop_graph(ix);
     ix->h_q.release();
-    for (cudaEvent_t e : ix->ev) cudaEventDestroy(e);
+    if (ix->ev_start) cudaEventDestroy(ix->ev_start);
+    if (ix->ev_stop) cudaEventDestroy(ix->ev_stop);
     for (auto& pr : ix->tev)
       for (cudaEvent_t e : pr)
         if (e) cudaEventDestroy(e);
@@ -1241,35 +1213,27 @@ rbk_status rbk_index_search_large_f64(rbk_index* ix, const double* queries, int3
   }
   st = ensure_query_scratch(ix, B, 8);
   if (st != RBK_OK) return st;
-  const size_t nout = static_cast<size_t>(B) * k_fetch;
-  const size_t blk = nout * 16 + static_cast<size_t>(B) * 4;   // slots | scores | counts
+  const ResultBlock L(B, k_fetch);
+  const size_t blk = L.off_counts + sizeof(int32_t) * B;   // no flags: every answer is exact by construction
   CK(ix->o_block.ensure(blk));
   CK(ix->h_block.ensure(blk));
   unsigned char* base = ix->o_block.p;
-  resolve_scan_events(ix, false);
-  const double scan_ms0 = ix->stats.scan_ms_total;
-  CK(cudaEventRecord(get_event(ix, 0), ix->stream));
+  TimedSearch ts{ix};
+  st = ts.begin();
+  if (st != RBK_OK) return st;
   CK(cudaMemcpyAsync(ix->q_raw.p, queries, static_cast<size_t>(B) * ix->dim * 8, cudaMemcpyHostToDevice, ix->stream));
   st = large_count(ix, ix->q_raw.p, B, k_fetch, min_score);
   if (st != RBK_OK) return st;
   CK(cudaStreamSynchronize(ix->stream));   // C_q sizes the candidate buffer
-  st = large_emit(ix, B, k_fetch, min_score, reinterpret_cast<long long*>(base),
-                  reinterpret_cast<double*>(base + nout * 8), reinterpret_cast<int*>(base + nout * 16));
+  st = large_emit(ix, B, k_fetch, min_score, L.slots(base), L.scores(base), L.counts(base));
   if (st != RBK_OK) return st;
   CK(cudaMemcpyAsync(ix->h_block.p, base, blk, cudaMemcpyDeviceToHost, ix->stream));
-  CK(cudaEventRecord(get_event(ix, 1), ix->stream));
-  CK(cudaStreamSynchronize(ix->stream));
+  st = ts.round_trip();
+  if (st != RBK_OK) return st;
   st = large_check(ix);
   if (st != RBK_OK) return st;
-  float total = 0.f;
-  cudaEventElapsedTime(&total, get_event(ix, 0), get_event(ix, 1));
-  resolve_scan_events(ix, true);
-  ix->stats.last_total_ms = total;
-  ix->stats.last_scan_ms = static_cast<float>(ix->stats.scan_ms_total - scan_ms0);
-  if (kernel_ms_out) *kernel_ms_out = total;
-  memcpy(out_slots, ix->h_block.p, sizeof(int64_t) * nout);
-  memcpy(out_scores, ix->h_block.p + nout * 8, sizeof(double) * nout);
-  memcpy(out_counts, ix->h_block.p + nout * 16, sizeof(int32_t) * B);
+  ts.finish(kernel_ms_out);
+  L.unpack(ix->h_block.p, out_slots, out_scores, out_counts);
   return RBK_OK;
 }
 
@@ -1330,14 +1294,8 @@ rbk_status rbk_merge_topk_device(int32_t device, void* cuda_stream, int32_t G, i
   return RBK_OK;
 }
 
-int64_t rbk_packed_block_bytes(int32_t B, int32_t k_fetch) {
-  const int64_t nk = static_cast<int64_t>(B) * k_fetch;
-  return nk * 16 + 2 * (((static_cast<int64_t>(B) * 4 + 15) / 16) * 16);   // slots | scores | counts | flags
-}
-int64_t rbk_packed_flags_offset(int32_t B, int32_t k_fetch) {
-  const int64_t nk = static_cast<int64_t>(B) * k_fetch;
-  return nk * 16 + ((static_cast<int64_t>(B) * 4 + 15) / 16) * 16;
-}
+int64_t rbk_packed_block_bytes(int32_t B, int32_t k_fetch) { return ResultBlock(B, k_fetch).bytes; }
+int64_t rbk_packed_flags_offset(int32_t B, int32_t k_fetch) { return ResultBlock(B, k_fetch).off_flags; }
 
 rbk_status rbk_merge_topk_packed_device(int32_t device, void* cuda_stream, int32_t G, int32_t B, int32_t k_fetch,
                                         const void* dev_blocks, void* dev_out_slots, void* dev_out_scores,
@@ -1347,12 +1305,11 @@ rbk_status rbk_merge_topk_packed_device(int32_t device, void* cuda_stream, int32
   if (!dev_blocks || !dev_out_slots || !dev_out_scores || !dev_out_counts)
     return fail(RBK_EINVAL, "null device pointer");
   DeviceGuard dg(device);
-  const size_t nk = static_cast<size_t>(B) * k_fetch;
-  const size_t stride = static_cast<size_t>(rbk_packed_block_bytes(B, k_fetch));
+  const ResultBlock L(B, k_fetch);
   const char* base = static_cast<const char*>(dev_blocks);
-  CK(launch_merge_shards(G, B, k_fetch, base, base + nk * 8, base + nk * 16,
-                         dev_out_flags ? base + rbk_packed_flags_offset(B, k_fetch) : nullptr, stride, stride, stride,
-                         stride, static_cast<long long*>(dev_out_slots), static_cast<double*>(dev_out_scores),
+  CK(launch_merge_shards(G, B, k_fetch, base, base + L.off_scores, base + L.off_counts,
+                         dev_out_flags ? base + L.off_flags : nullptr, L.bytes, L.bytes, L.bytes, L.bytes,
+                         static_cast<long long*>(dev_out_slots), static_cast<double*>(dev_out_scores),
                          static_cast<int*>(dev_out_counts), static_cast<int*>(dev_out_flags),
                          static_cast<cudaStream_t>(cuda_stream)));
   return RBK_OK;

@@ -86,7 +86,7 @@ struct rbk_group {
     DevBuf<unsigned char> q, local, all;
   };
   std::vector<Dev> dev;
-  DevBuf<unsigned char> out;     // device 0: slots | scores | counts | flags[B+1]
+  DevBuf<unsigned char> out;     // device 0: the merged block (dirty_word)
   PinBuf<unsigned char> h_out, h_q;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int64_t redone_batches = 0;
@@ -141,13 +141,54 @@ void split_slots(const rbk_group* g, const int64_t* slots, int64_t n, std::vecto
   }
 }
 
+// The merged block on device 0 (g->out) is the packed layout with one more word after the flags: the merge kernel
+// adds the number of queries some shard could not prove to flags[B].
+int64_t dirty_word(const ResultBlock& L) { return L.off_flags + 4 * L.B; }
+int64_t merged_bytes(const ResultBlock& L) { return dirty_word(L) + 4; }
+
+// Stages a batch on every device and enqueues its work there: the buffers for the queries and the packed blocks, the
+// start event, the H2D of the queries to each device from one pinned copy (so that the G copies run concurrently, one
+// per PCIe link), the member's query scratch, then enqueue(d, ix) with the member's lock held and its device current.
+// zero_dirty: the caller reads the dirty count, which the merge kernel adds to - start it from zero (its position
+// depends on B and k_fetch, so a running count across calls of different shapes would be garbage).
+template <typename F>
+rbk_status stage_and_enqueue(rbk_group* g, const void* queries, int elem, const ResultBlock& L, bool zero_dirty,
+                             F&& enqueue) {
+  const int B = static_cast<int>(L.B);
+  const size_t q_bytes = static_cast<size_t>(B) * g->dim * elem;
+  {
+    DeviceGuard dg(g->devices[0]);
+    CK(g->h_q.ensure(q_bytes));
+    CK(g->h_out.ensure(merged_bytes(L)));
+    CK(g->out.ensure(merged_bytes(L)));
+    if (zero_dirty) CK(cudaMemsetAsync(g->out.p + dirty_word(L), 0, 4, g->parts[0]->stream));
+  }
+  memcpy(g->h_q.p, queries, q_bytes);
+  for (int d = 0; d < g->G; ++d) {
+    rbk_index* ix = g->parts[d];
+    std::lock_guard<std::mutex> il(ix->mu);
+    DeviceGuard dg(ix->device);
+    CK(g->dev[d].q.ensure(q_bytes));
+    CK(g->dev[d].local.ensure(L.bytes));
+    if (g->G > 1) CK(g->dev[d].all.ensure(L.bytes * g->G));
+    if (d == 0) CK(cudaEventRecord(g->ev0, ix->stream));
+    CK(cudaMemcpyAsync(g->dev[d].q.p, g->h_q.p, q_bytes, cudaMemcpyHostToDevice, ix->stream));
+    rbk_status st = ensure_query_scratch(ix, B, elem);
+    if (st != RBK_OK) return st;
+    st = enqueue(d, ix);
+    if (st != RBK_OK) return st;
+  }
+  return RBK_OK;
+}
+
 // all-gather of the packed blocks (G > 1) + merge on device 0 into g->out; enqueue only
-rbk_status exchange_and_merge(rbk_group* g, int B, int k_fetch, size_t blk) {
+rbk_status exchange_and_merge(rbk_group* g, const ResultBlock& L, int k_fetch) {
   if (g->G > 1) {
     NcclApi& n = nccl_api();
     NC(n.GroupStart());
     for (int d = 0; d < g->G; ++d) {
-      ncclResult_t r = n.AllGather(g->dev[d].local.p, g->dev[d].all.p, blk, ncclUint8, g->comms[d], g->parts[d]->stream);
+      ncclResult_t r = n.AllGather(g->dev[d].local.p, g->dev[d].all.p, L.bytes, ncclUint8, g->comms[d],
+                                   g->parts[d]->stream);
       if (r != ncclSuccess) {
         n.GroupEnd();
         return nccl_fail(r, "ncclAllGather");
@@ -156,14 +197,21 @@ rbk_status exchange_and_merge(rbk_group* g, int B, int k_fetch, size_t blk) {
     NC(n.GroupEnd());
   }
   DeviceGuard dg(g->devices[0]);
-  const size_t nk = static_cast<size_t>(B) * k_fetch;
   const char* base = reinterpret_cast<const char*>(g->G > 1 ? g->dev[0].all.p : g->dev[0].local.p);
   unsigned char* o = g->out.p;
-  CK(launch_merge_shards(g->G, B, k_fetch, base, base + nk * 8, base + nk * 16,
-                         base + rbk_packed_flags_offset(B, k_fetch), blk, blk, blk, blk,
-                         reinterpret_cast<long long*>(o), reinterpret_cast<double*>(o + nk * 8),
-                         reinterpret_cast<int*>(o + nk * 16), reinterpret_cast<int*>(o + nk * 16 + static_cast<size_t>(B) * 4),
-                         g->parts[0]->stream));
+  CK(launch_merge_shards(g->G, static_cast<int>(L.B), k_fetch, base, base + L.off_scores, base + L.off_counts,
+                         base + L.off_flags, L.bytes, L.bytes, L.bytes, L.bytes, L.slots(o), L.scores(o), L.counts(o),
+                         L.flags(o), g->parts[0]->stream));
+  return RBK_OK;
+}
+
+// D2H of the merged block, the stop event and the host round trip on device 0.
+rbk_status collect(rbk_group* g, const ResultBlock& L) {
+  rbk_index* i0 = g->parts[0];
+  DeviceGuard dg(i0->device);
+  CK(cudaMemcpyAsync(g->h_out.p, g->out.p, merged_bytes(L), cudaMemcpyDeviceToHost, i0->stream));
+  CK(cudaEventRecord(g->ev1, i0->stream));
+  CK(cudaStreamSynchronize(i0->stream));
   return RBK_OK;
 }
 
@@ -176,72 +224,39 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
   if (ms_out) *ms_out = 0.f;
   if (B == 0) return RBK_OK;
   std::lock_guard<std::mutex> lk(g->mu);
-  const size_t q_bytes = static_cast<size_t>(B) * g->dim * elem;
-  const size_t blk = static_cast<size_t>(rbk_packed_block_bytes(B, k_fetch));
-  const size_t off_f = static_cast<size_t>(rbk_packed_flags_offset(B, k_fetch));
-  const size_t nk = static_cast<size_t>(B) * k_fetch;
-  const size_t out_bytes = nk * 16 + (2 * static_cast<size_t>(B) + 1) * 4;
-  {
-    DeviceGuard dg(g->devices[0]);
-    CK(g->h_q.ensure(q_bytes));
-    CK(g->h_out.ensure(out_bytes));
-    CK(g->out.ensure(out_bytes));
-    // the merge kernel ADDS the number of dirty queries to the word after the flags: start every search from zero
-    // (its position depends on B and k_fetch, so a running count across calls of different shapes would be garbage)
-    CK(cudaMemsetAsync(g->out.p + out_bytes - 4, 0, 4, g->parts[0]->stream));
-  }
-  memcpy(g->h_q.p, queries, q_bytes);   // pinned staging: the G H2D copies below run concurrently, one per PCIe link
+  const ResultBlock L(B, k_fetch);
   const int src_type = elem == 8 ? 0 : 1;
-  for (int d = 0; d < g->G; ++d) {
-    rbk_index* ix = g->parts[d];
-    std::lock_guard<std::mutex> il(ix->mu);
-    DeviceGuard dg(ix->device);
-    CK(g->dev[d].q.ensure(q_bytes));
-    CK(g->dev[d].local.ensure(blk));
-    if (g->G > 1) CK(g->dev[d].all.ensure(blk * g->G));
-    if (d == 0) CK(cudaEventRecord(g->ev0, ix->stream));
-    CK(cudaMemcpyAsync(g->dev[d].q.p, g->h_q.p, q_bytes, cudaMemcpyHostToDevice, ix->stream));
-    st = ensure_query_scratch(ix, B, elem);
-    if (st != RBK_OK) return st;
+  st = stage_and_enqueue(g, queries, elem, L, /*zero_dirty=*/true, [&](int d, rbk_index* ix) {
     unsigned char* l = g->dev[d].local.p;
-    st = enqueue_search(ix, g->dev[d].q.p, src_type, B, k_fetch, min_score, reinterpret_cast<long long*>(l),
-                        reinterpret_cast<double*>(l + nk * 8), reinterpret_cast<int*>(l + nk * 16),
-                        reinterpret_cast<int*>(l + off_f));
-    if (st != RBK_OK) return st;
-  }
-  st = exchange_and_merge(g, B, k_fetch, blk);
+    return enqueue_search(ix, g->dev[d].q.p, src_type, B, k_fetch, min_score, L.slots(l), L.scores(l), L.counts(l),
+                          L.flags(l));
+  });
   if (st != RBK_OK) return st;
-  rbk_index* i0 = g->parts[0];
-  {
-    DeviceGuard dg(i0->device);
-    CK(cudaMemcpyAsync(g->h_out.p, g->out.p, out_bytes, cudaMemcpyDeviceToHost, i0->stream));
-    CK(cudaEventRecord(g->ev1, i0->stream));
-    CK(cudaStreamSynchronize(i0->stream));   // the ONE host round trip of an exact batch
-  }
+  st = exchange_and_merge(g, L, k_fetch);
+  if (st != RBK_OK) return st;
+  st = collect(g, L);   // the ONE host round trip of an exact batch
+  if (st != RBK_OK) return st;
   int dirty_total = 0;
-  memcpy(&dirty_total, g->h_out.p + out_bytes - 4, 4);
+  memcpy(&dirty_total, g->h_out.p + dirty_word(L), 4);
   if (dirty_total != 0) {
     // some shard could not prove a query (more near-ties than its candidate margin): every shard re-answers the
     // batch through the synchronous path (wide rescan, then the exhaustive fp64 kernel), and the exchange is redone
     g->redone_batches++;
     for (int d = 0; d < g->G; ++d) {
       unsigned char* l = g->dev[d].local.p;
-      st = rbk_index_search_device(g->parts[d], g->dev[d].q.p, B, k_fetch, min_score, l, l + nk * 8, l + nk * 16);
+      st = rbk_index_search_device(g->parts[d], g->dev[d].q.p, B, k_fetch, min_score, L.slots(l), L.scores(l),
+                                   L.counts(l));
       if (st != RBK_OK) return st;
       DeviceGuard dg(g->parts[d]->device);
-      CK(cudaMemsetAsync(l + off_f, 0, static_cast<size_t>(B) * 4, g->parts[d]->stream));   // exact by construction
+      CK(cudaMemsetAsync(L.flags(l), 0, static_cast<size_t>(B) * 4, g->parts[d]->stream));   // exact by construction
     }
-    st = exchange_and_merge(g, B, k_fetch, blk);
+    st = exchange_and_merge(g, L, k_fetch);
     if (st != RBK_OK) return st;
-    DeviceGuard dg(i0->device);
-    CK(cudaMemcpyAsync(g->h_out.p, g->out.p, out_bytes, cudaMemcpyDeviceToHost, i0->stream));
-    CK(cudaEventRecord(g->ev1, i0->stream));
-    CK(cudaStreamSynchronize(i0->stream));
+    st = collect(g, L);
+    if (st != RBK_OK) return st;
   }
   if (ms_out) cudaEventElapsedTime(ms_out, g->ev0, g->ev1);
-  memcpy(out_slots, g->h_out.p, nk * 8);
-  memcpy(out_scores, g->h_out.p + nk * 8, nk * 8);
-  memcpy(out_counts, g->h_out.p + nk * 16, static_cast<size_t>(B) * 4);
+  L.unpack(g->h_out.p, out_slots, out_scores, out_counts);
   return RBK_OK;
 }
 
@@ -259,32 +274,11 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
   if (ms_out) *ms_out = 0.f;
   if (B == 0) return RBK_OK;
   std::lock_guard<std::mutex> lk(g->mu);
-  const size_t q_bytes = static_cast<size_t>(B) * g->dim * 8;
-  const size_t blk = static_cast<size_t>(rbk_packed_block_bytes(B, k_fetch));
-  const size_t off_f = static_cast<size_t>(rbk_packed_flags_offset(B, k_fetch));
-  const size_t nk = static_cast<size_t>(B) * k_fetch;
-  const size_t out_bytes = nk * 16 + (2 * static_cast<size_t>(B) + 1) * 4;
-  {
-    DeviceGuard dg(g->devices[0]);
-    CK(g->h_q.ensure(q_bytes));
-    CK(g->h_out.ensure(out_bytes));
-    CK(g->out.ensure(out_bytes));
-  }
-  memcpy(g->h_q.p, queries, q_bytes);
-  for (int d = 0; d < g->G; ++d) {
-    rbk_index* ix = g->parts[d];
-    std::lock_guard<std::mutex> il(ix->mu);
-    DeviceGuard dg(ix->device);
-    CK(g->dev[d].q.ensure(q_bytes));
-    CK(g->dev[d].local.ensure(blk));
-    if (g->G > 1) CK(g->dev[d].all.ensure(blk * g->G));
-    if (d == 0) CK(cudaEventRecord(g->ev0, ix->stream));
-    CK(cudaMemcpyAsync(g->dev[d].q.p, g->h_q.p, q_bytes, cudaMemcpyHostToDevice, ix->stream));
-    st = ensure_query_scratch(ix, B, 8);
-    if (st != RBK_OK) return st;
-    st = large_count(ix, g->dev[d].q.p, B, k_fetch, min_score);
-    if (st != RBK_OK) return st;
-  }
+  const ResultBlock L(B, k_fetch);
+  st = stage_and_enqueue(g, queries, 8, L, /*zero_dirty=*/false, [&](int d, rbk_index* ix) {
+    return large_count(ix, g->dev[d].q.p, B, k_fetch, min_score);
+  });
+  if (st != RBK_OK) return st;
   for (int d = 0; d < g->G; ++d) {
     DeviceGuard dg(g->parts[d]->device);
     CK(cudaStreamSynchronize(g->parts[d]->stream));
@@ -294,29 +288,24 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
     std::lock_guard<std::mutex> il(ix->mu);
     DeviceGuard dg(ix->device);
     unsigned char* l = g->dev[d].local.p;
-    st = large_emit(ix, B, k_fetch, min_score, reinterpret_cast<long long*>(l), reinterpret_cast<double*>(l + nk * 8),
-                    reinterpret_cast<int*>(l + nk * 16));
+    st = large_emit(ix, B, k_fetch, min_score, L.slots(l), L.scores(l), L.counts(l));
     if (st != RBK_OK) return st;
-    CK(cudaMemsetAsync(l + off_f, 0, static_cast<size_t>(B) * 4, ix->stream));
+    CK(cudaMemsetAsync(L.flags(l), 0, static_cast<size_t>(B) * 4, ix->stream));
   }
-  st = exchange_and_merge(g, B, k_fetch, blk);
+  st = exchange_and_merge(g, L, k_fetch);
   if (st != RBK_OK) return st;
-  {
-    rbk_index* i0 = g->parts[0];
-    DeviceGuard dg(i0->device);
-    CK(cudaMemcpyAsync(g->h_out.p, g->out.p, out_bytes, cudaMemcpyDeviceToHost, i0->stream));
-    CK(cudaEventRecord(g->ev1, i0->stream));
-  }
+  st = collect(g, L);
+  if (st != RBK_OK) return st;
   for (int d = 0; d < g->G; ++d) {   // every device's overflow counter has landed on the host
-    DeviceGuard dg(g->parts[d]->device);
-    CK(cudaStreamSynchronize(g->parts[d]->stream));
+    if (d > 0) {                     // (collect has waited for device 0)
+      DeviceGuard dg(g->parts[d]->device);
+      CK(cudaStreamSynchronize(g->parts[d]->stream));
+    }
     st = large_check(g->parts[d]);
     if (st != RBK_OK) return st;
   }
   if (ms_out) cudaEventElapsedTime(ms_out, g->ev0, g->ev1);
-  memcpy(out_slots, g->h_out.p, nk * 8);
-  memcpy(out_scores, g->h_out.p + nk * 8, nk * 8);
-  memcpy(out_counts, g->h_out.p + nk * 16, static_cast<size_t>(B) * 4);
+  L.unpack(g->h_out.p, out_slots, out_scores, out_counts);
   return RBK_OK;
 }
 

@@ -2,6 +2,8 @@
 // helpers shared by the two translation units that implement the C ABI: rbk_capi.cu (one index = one GPU) and
 // rbk_group.cu (one group = one index per GPU + the NCCL exchange, all behind one call).
 #pragma once
+#include <string.h>
+
 #include <mutex>
 #include <string>
 #include <vector>
@@ -70,6 +72,28 @@ struct DeviceGuard {
   }
 };
 
+// Byte layout of one search's results as one block, so that they and the exactness flags move in one copy:
+//   slots i64 [B][k_fetch] | scores f64 [B][k_fetch] | counts i32 [B] | flags i32 [B]
+// counts and flags each padded to 16 bytes.  The C ABI publishes it (rbk_packed_block_bytes / rbk_packed_flags_offset):
+// a device group all-gathers these blocks, and so do multi_device.py and the addon.
+struct ResultBlock {
+  int64_t B, nk, off_scores, off_counts, off_flags, bytes;
+  ResultBlock(int32_t B_, int32_t k_fetch)
+      : B(B_), nk(B * k_fetch), off_scores(nk * 8), off_counts(nk * 16), off_flags(off_counts + (B * 4 + 15) / 16 * 16),
+        bytes(off_flags + (B * 4 + 15) / 16 * 16) {}
+  long long* slots(void* base) const { return static_cast<long long*>(base); }
+  double* scores(void* base) const { return reinterpret_cast<double*>(static_cast<char*>(base) + off_scores); }
+  int* counts(void* base) const { return reinterpret_cast<int*>(static_cast<char*>(base) + off_counts); }
+  int* flags(void* base) const { return reinterpret_cast<int*>(static_cast<char*>(base) + off_flags); }
+  // copies a host block out to the caller's arrays
+  void unpack(const void* h, int64_t* out_slots, double* out_scores, int32_t* out_counts) const {
+    const char* p = static_cast<const char*>(h);
+    memcpy(out_slots, p, sizeof(int64_t) * nk);
+    memcpy(out_scores, p + off_scores, sizeof(double) * nk);
+    memcpy(out_counts, p + off_counts, sizeof(int32_t) * B);
+  }
+};
+
 }  // namespace impl
 }  // namespace rbk
 
@@ -101,9 +125,8 @@ struct rbk_index {
   rbk::impl::DevBuf<double> q_f64, q_norm2, q_eps;
   rbk::impl::DevBuf<float> q_inv_norm, thr_init;
   rbk::impl::DevBuf<unsigned long long> cand;
-  rbk::impl::DevBuf<int> cand_cnt, flags, fail_list, o_counts, part_rows, part_cnt, maxbin, progress;
-  rbk::impl::DevBuf<unsigned int> hist;
-  rbk::impl::DevBuf<long long> o_slots;
+  rbk::impl::DevBuf<int> cand_cnt, flags, fail_list, part_rows, part_cnt;
+  rbk::impl::DevBuf<unsigned int> hist;   // the scan's per-launch scratch (split by fill_scan_params)
   rbk::impl::DevBuf<double> o_scores, part_scores;
   rbk::impl::DevBuf<float> dbg;
   // large-k search scratch (grow-only): theta_q, C_q, emit counters, segment offsets, flat candidate rows + scores
@@ -115,22 +138,18 @@ struct rbk_index {
   rbk::impl::PinBuf<long long> h_loff;
   rbk::impl::DevBuf<unsigned char> o_block;
   rbk::impl::PinBuf<unsigned char> h_block;
-  rbk::impl::PinBuf<int> h_flags, h_counts;
-  rbk::impl::PinBuf<long long> h_slots;
-  rbk::impl::PinBuf<double> h_scores;
-  rbk::impl::PinBuf<float> h_f32;
+  rbk::impl::PinBuf<int> h_flags;
   CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
   const void* tmap_c_base = nullptr;
   int64_t tmap_c_rows = -1;
-  std::vector<cudaEvent_t> ev;
+  cudaEvent_t ev_start = nullptr, ev_stop = nullptr;   // device time of a whole synchronous search
   // scan-kernel timing without a host sync per search: (start, stop) event pairs are resolved lazily
   // (rbk_index_stats, or when the ring wraps) into stats.scan_ms_total / stats.scans_timed
   static constexpr int kTimingRing = 64;
   cudaEvent_t tev[kTimingRing][2] = {};
   uint64_t tev_head = 0, tev_tail = 0;   // [tail, head) pending
-  float pending_scan_ms = 0.f;           // scan time of the search being assembled (resolved pairs only)
   // Small batches (B <= 128, host queries in, host results out) replay ONE captured CUDA graph - H2D of the
   // queries, prep, scan, finalize, D2H of the packed block - instead of paying six API calls per search.  The
   // graph bakes in every pointer and scalar it was captured with: `graph_key` is compared before each replay.

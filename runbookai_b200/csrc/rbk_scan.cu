@@ -71,12 +71,6 @@ __device__ __forceinline__ uint32_t quad_bits(uint32_t b) {
   return (b | (b >> 12)) & 0xFFu;
 }
 
-#ifdef RBK_SCAN_STAGE_STATS
-// Development probe: per launch, tiles x warpgroups handed over at all / in more than one round, and rows staged.
-__device__ unsigned long long g_stage_stats[4];
-__device__ unsigned int g_stage_done;
-#endif
-
 // Development probe (RBK_SCAN_CYCLE_STATS): where a wgmma warpgroup's cycles go.  Its leader thread adds SM-clock
 // deltas into buckets, summed over the launch per warpgroup:
 //   full     waiting on a ring slot's `full` barrier;
@@ -226,9 +220,6 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
   float* stage = staging + wg * kStageRows * kScorePitch;
   const uint32_t st_full = smem_u32(&tail->st_full[wg]), st_empty = smem_u32(&tail->st_empty[wg]);
   uint32_t rounds = 0;
-#ifdef RBK_SCAN_STAGE_STATS
-  unsigned long long n_handed = 0, n_multi = 0, n_rows = 0;
-#endif
   float acc[128];
 #pragma unroll
   for (int i = 0; i < 128; ++i) acc[i] = 0.f;
@@ -294,11 +285,6 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
     const uint16_t* wm = tail->wmask[wg][i & 1];
     unsigned long long pending = static_cast<unsigned long long>(wm[0]) | static_cast<unsigned long long>(wm[1]) << 16 |
                                  static_cast<unsigned long long>(wm[2]) << 32 | static_cast<unsigned long long>(wm[3]) << 48;
-#ifdef RBK_SCAN_STAGE_STATS
-    n_handed += pending != 0ull;
-    n_multi += __popcll(pending) > kStageRows;
-    n_rows += __popcll(pending);
-#endif
 
     // Hand the passing rows over, at most kStageRows per round; a tile without any is one round with no rows.
     do {
@@ -328,21 +314,6 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
       atomicAdd(&g_cycle_stats[kMode][wg][b], static_cast<unsigned long long>(probe.c[b]));
     atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets], static_cast<unsigned long long>(n_iter));
     atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets + 1], 1ull);
-  }
-#endif
-#ifdef RBK_SCAN_STAGE_STATS
-  if (leader) {
-    atomicAdd(&g_stage_stats[0], static_cast<unsigned long long>(n_iter));
-    atomicAdd(&g_stage_stats[1], n_handed);
-    atomicAdd(&g_stage_stats[2], n_multi);
-    atomicAdd(&g_stage_stats[3], n_rows);
-    __threadfence();
-    if (atomicAdd(&g_stage_done, 1u) == 2u * gridDim.x - 1u) {
-      printf("[scan stats] mode %d: %llu tile-warpgroups, %llu handed over, %llu in more than one round, %llu rows\n",
-             kMode, g_stage_stats[0], g_stage_stats[1], g_stage_stats[2], g_stage_stats[3]);
-      for (int k = 0; k < 4; ++k) g_stage_stats[k] = 0ull;
-      g_stage_done = 0u;
-    }
   }
 #endif
 }
