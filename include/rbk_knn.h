@@ -177,9 +177,25 @@ rbk_status rbk_index_search_large_f64(rbk_index* idx, const double* queries, int
                                       int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                       int32_t* out_counts, float* kernel_ms_out);
 
-/* More hits than RBK_MAX_K_FETCH_LARGE: the exact fp64 cosine of EVERY row, out_scores[b * size() + slot], NaN for
- * tombstoned / zero rows (which the reference's `>= minScore` drops too, S3).  The host applies the threshold, the
- * stable sort and the cut literally (vector-store.ts:212-221).  One fp64 pass over the corpus per query. */
+/* Any number of hits per query - the reference's VectorStore.search has no ceiling on topK (vector-store.ts:207-221):
+ * exactly the contract of rbk_index_search_large_f64 (same order, threshold, NaN / tombstone rules, bit-identical
+ * fp64 scores, -1 / NaN tail, RBK_EDIM / RBK_EINVAL on the same arguments) for any int32 k_fetch >= 1.
+ * k_fetch <= RBK_MAX_K_FETCH_LARGE runs rbk_index_search_large_f64 itself.  Above it the call keeps
+ * k_eff = min(k_fetch, rbk_index_count()) entries per query on the device (no query can have more hits) and sorts
+ * each query's candidates in global memory after the exact re-score.  Device memory is bounded by a fixed per-pass
+ * budget (256 MiB of candidates and results, at least one query per pass), never by k_fetch: the count scan runs once
+ * for the batch, then the queries go in contiguous groups that fit the budget, each group costing one emit scan.
+ * Results are copied straight into the caller's arrays; kernel_ms_out is the time of the whole call on the device's
+ * stream, these copies included (at pageable-memory speed for ordinary host arrays, B * k_eff * 16 bytes).  Fails with RBK_ECUDA, never with a wrong answer, if an emit
+ * scan finds more rows than the count scan bounded (a bug). */
+rbk_status rbk_index_search_unbounded_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
+                                          int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                          int32_t* out_counts, float* kernel_ms_out);
+
+/* The exact fp64 cosine of EVERY row, out_scores[b * size() + slot], NaN for tombstoned / zero rows (which the
+ * reference's `>= minScore` drops too, S3), for a host that applies the threshold, the stable sort and the cut itself
+ * (vector-store.ts:212-221).  One fp64 pass over the corpus per query and 8 * size() bytes per query to the host; a
+ * search for more hits than RBK_MAX_K_FETCH_LARGE is far cheaper through rbk_index_search_unbounded_f64. */
 rbk_status rbk_index_exact_scores_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
                                       double* out_scores);
 
@@ -252,6 +268,14 @@ rbk_status rbk_group_search_f64(rbk_group* grp, const double* queries, int32_t B
 rbk_status rbk_group_search_large_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
                                       int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                       int32_t* out_counts, float* device_ms_out);
+/* rbk_index_search_unbounded_f64 over the group (any k_fetch >= 1; up to RBK_MAX_K_FETCH_LARGE it is
+ * rbk_group_search_large_f64): the count scan on every GPU and one wait for all of them, then per query group - the
+ * members' candidates and result blocks taken together fit the same per-pass budget - the emit scan, re-score and
+ * sort on every GPU into k_eff = rbk_group_count() entries per query, the all-gather and merge, and the copy into the
+ * caller's arrays.  A one-GPU group never touches NCCL. */
+rbk_status rbk_group_search_unbounded_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
+                                          int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                          int32_t* out_counts, float* device_ms_out);
 
 /* ---- introspection ---- */
 typedef struct {

@@ -208,6 +208,30 @@ int main(int argc, char** argv) {
     }
   }
 
+  // searchUnbounded(): optional unbounded.txt lists k_fetch values (any >= 1); results land in unbounded<i>_*.  One
+  // more call with k_fetch 0 must reject with the library's message.
+  {
+    std::ifstream uf(g_dir + "/unbounded.txt");
+    int ku, i = 0;
+    bool any = false;
+    while (uf >> ku) {
+      any = true;
+      Result ur;
+      if (!search(env, ix, queries, n_q, ku, min_score, &ur, &err, "searchUnbounded"))
+        die("searchUnbounded rejected: " + err);
+      const std::string p = "unbounded" + std::to_string(i++) + "_";
+      write_bin((p + "slots.i64").c_str(), ur.slots.data(), ur.slots.size() * 8);
+      write_bin((p + "scores.f64").c_str(), ur.scores.data(), ur.scores.size() * 8);
+      write_bin((p + "counts.i32").c_str(), ur.counts.data(), ur.counts.size() * 4);
+    }
+    if (any) {
+      Result none;
+      if (search(env, ix, queries, n_q, 0, min_score, &none, &err, "searchUnbounded"))
+        die("searchUnbounded with k_fetch 0 did not reject");
+      log << "err_unbounded " << err << "\n";
+    }
+  }
+
   // ---- error paths: each must surface as a JS exception / rejection with the reference's wording
   {
     std::vector<double> odd(static_cast<size_t>(dim) + 1, 1.0);

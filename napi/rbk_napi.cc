@@ -21,6 +21,7 @@
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
 //   await ix.searchLarge(Float64Array queries, B, kFetch, minScore)   // kFetch up to 4096, same result object
+//   await ix.searchUnbounded(Float64Array queries, B, kFetch, minScore)   // any kFetch >= 1, same result object
 //
 // Build (where Node headers exist):  node-gyp with  libraries: ["-lrbk_knn"], include_dirs: ["../include"].
 #include <node_api.h>
@@ -38,6 +39,9 @@
 // failing to load.
 #pragma weak rbk_index_search_large_f64
 #pragma weak rbk_group_search_large_f64
+// The same for the unbounded search; `searchUnbounded` throws where it is missing.
+#pragma weak rbk_index_search_unbounded_f64
+#pragma weak rbk_group_search_unbounded_f64
 // The same for compaction; `compact` throws where it is missing.  rbk_index_size, which sizes the map, is weak with it
 // so that the method as a whole needs nothing a library without compaction may lack.
 #pragma weak rbk_index_compact
@@ -84,6 +88,14 @@ struct Handle {
                           int32_t* c) {
     return grp ? rbk_group_search_large_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
                : rbk_index_search_large_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
+  }
+  bool has_search_unbounded() const {
+    return grp ? rbk_group_search_unbounded_f64 != nullptr : rbk_index_search_unbounded_f64 != nullptr;
+  }
+  rbk_status search_unbounded(const double* q, int32_t B, int32_t qdim, int32_t k, double ms, int64_t* s, double* v,
+                              int32_t* c) {
+    return grp ? rbk_group_search_unbounded_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
+               : rbk_index_search_unbounded_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
   }
 };
 
@@ -280,11 +292,13 @@ napi_value Count(napi_env env, napi_callback_info info) {
 }
 
 // ---- search: runs on a libuv worker so the JS thread never blocks on the GPU ----
+enum class SearchKind { kScan, kLarge, kUnbounded };   // search / searchLarge / searchUnbounded
+
 struct SearchJob {
   Handle* ix;
   std::vector<double> queries;
   int32_t B, dim, k;
-  bool large;   // searchLarge: rbk_*_search_large_f64
+  SearchKind kind;
   double min_score;
   std::vector<int64_t> slots;
   std::vector<double> scores;
@@ -297,10 +311,11 @@ struct SearchJob {
 
 void search_execute(napi_env, void* data) {
   SearchJob* j = static_cast<SearchJob*>(data);
-  j->st = j->large ? j->ix->search_large(j->queries.data(), j->B, j->dim, j->k, j->min_score, j->slots.data(),
-                                        j->scores.data(), j->counts.data())
-                   : j->ix->search(j->queries.data(), j->B, j->dim, j->k, j->min_score, j->slots.data(),
-                                   j->scores.data(), j->counts.data());
+  auto fn = j->kind == SearchKind::kLarge       ? &Handle::search_large
+            : j->kind == SearchKind::kUnbounded ? &Handle::search_unbounded
+                                                : &Handle::search;
+  j->st = (j->ix->*fn)(j->queries.data(), j->B, j->dim, j->k, j->min_score, j->slots.data(), j->scores.data(),
+                       j->counts.data());
   if (j->st != RBK_OK) j->err = rbk_last_error();   // thread-local: read it on the worker thread
 }
 
@@ -333,12 +348,17 @@ void search_complete(napi_env env, napi_status, void* data) {
   delete j;
 }
 
-napi_value QueueSearch(napi_env env, napi_callback_info info, bool large) {
+napi_value QueueSearch(napi_env env, napi_callback_info info, SearchKind kind) {
   size_t argc = 4;
   napi_value argv[4];
   Handle* ix = unwrap(env, info, &argc, argv);
-  if (large && !ix->has_search_large()) {
+  if (kind == SearchKind::kLarge && !ix->has_search_large()) {
     napi_throw_error(env, nullptr, "searchLarge: this librbk_knn.so has no large-k search (rbk_*_search_large_f64)");
+    return nullptr;
+  }
+  if (kind == SearchKind::kUnbounded && !ix->has_search_unbounded()) {
+    napi_throw_error(env, nullptr,
+                     "searchUnbounded: this librbk_knn.so has no unbounded search (rbk_*_search_unbounded_f64)");
     return nullptr;
   }
   napi_typedarray_type t;
@@ -347,7 +367,7 @@ napi_value QueueSearch(napi_env env, napi_callback_info info, bool large) {
   NAPI_OK(napi_get_typedarray_info(env, argv[0], &t, &len, &data, nullptr, nullptr));
   auto* j = new SearchJob();
   j->ix = ix;
-  j->large = large;
+  j->kind = kind;
   napi_get_value_int32(env, argv[1], &j->B);
   napi_get_value_int32(env, argv[2], &j->k);
   napi_get_value_double(env, argv[3], &j->min_score);   // pass -Infinity for "no threshold"
@@ -364,8 +384,11 @@ napi_value QueueSearch(napi_env env, napi_callback_info info, bool large) {
   return promise;
 }
 
-napi_value Search(napi_env env, napi_callback_info info) { return QueueSearch(env, info, false); }
-napi_value SearchLarge(napi_env env, napi_callback_info info) { return QueueSearch(env, info, true); }
+napi_value Search(napi_env env, napi_callback_info info) { return QueueSearch(env, info, SearchKind::kScan); }
+napi_value SearchLarge(napi_env env, napi_callback_info info) { return QueueSearch(env, info, SearchKind::kLarge); }
+napi_value SearchUnbounded(napi_env env, napi_callback_info info) {
+  return QueueSearch(env, info, SearchKind::kUnbounded);
+}
 
 napi_value Init(napi_env env, napi_value exports) {
   napi_property_descriptor props[] = {
@@ -379,6 +402,7 @@ napi_value Init(napi_env env, napi_value exports) {
       {"count", nullptr, Count, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"search", nullptr, Search, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"searchLarge", nullptr, SearchLarge, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"searchUnbounded", nullptr, SearchUnbounded, nullptr, nullptr, nullptr, napi_default, nullptr},
   };
   napi_value cls;
   NAPI_OK(napi_define_class(env, "RbkIndex", NAPI_AUTO_LENGTH, New, nullptr, sizeof props / sizeof props[0], props, &cls));

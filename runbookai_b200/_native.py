@@ -24,14 +24,14 @@ SYMBOLS = [
     "rbk_index_set_slot_base", "rbk_index_append_f64", "rbk_index_append_f32", "rbk_index_append_bf16",
     "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_compact", "rbk_index_clear",
     "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_storage_bytes", "rbk_index_read_rows_bf16", "rbk_index_search_f64",
-    "rbk_index_search_f32", "rbk_index_search_large_f64", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
+    "rbk_index_search_f32", "rbk_index_search_large_f64", "rbk_index_search_unbounded_f64", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
     "rbk_packed_block_bytes", "rbk_packed_flags_offset",
     "rbk_merge_topk_packed_device", "rbk_index_stats",
     "rbk_index_debug_scores_f32",
     "rbk_group_create", "rbk_group_destroy", "rbk_group_append_f64", "rbk_group_append_f32", "rbk_group_append_bf16",
     "rbk_group_overwrite_f64_batch", "rbk_group_tombstone", "rbk_group_clear", "rbk_group_count", "rbk_group_size",
     "rbk_group_devices", "rbk_group_member", "rbk_group_redone_batches", "rbk_group_search_f32", "rbk_group_search_f64",
-    "rbk_group_search_large_f64",
+    "rbk_group_search_large_f64", "rbk_group_search_unbounded_f64",
 ]
 
 
@@ -85,7 +85,8 @@ def _load() -> C.CDLL:
     lib.rbk_index_dim.restype = i32
     lib.rbk_index_storage_bytes.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     lib.rbk_index_read_rows_bf16.argtypes = [vp, i64, i64, vp]
-    for n in ("rbk_index_search_f64", "rbk_index_search_f32", "rbk_index_search_large_f64"):
+    for n in ("rbk_index_search_f64", "rbk_index_search_f32", "rbk_index_search_large_f64",
+              "rbk_index_search_unbounded_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_search_device.argtypes = [vp, vp, i32, i32, f64, vp, vp, vp]
     lib.rbk_index_exact_scores_f64.argtypes = [vp, vp, i32, i32, vp]
@@ -112,7 +113,8 @@ def _load() -> C.CDLL:
     lib.rbk_group_devices.restype = i32
     lib.rbk_group_member.argtypes = [vp, i32]
     lib.rbk_group_member.restype = vp
-    for n in ("rbk_group_search_f32", "rbk_group_search_f64", "rbk_group_search_large_f64"):
+    for n in ("rbk_group_search_f32", "rbk_group_search_f64", "rbk_group_search_large_f64",
+              "rbk_group_search_unbounded_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_debug_scores_f32.argtypes = [vp, vp, i32, vp]
     return lib
@@ -172,6 +174,14 @@ def _search_any_k(ix, queries, k_fetch: int, min_score):
         slots[b, :len(order)] = order
         scores[b, :len(order)] = sc[b, order]
     return slots, scores, counts, 0.0
+
+
+def _search_any_k_on_device(ix, queries, k_fetch: int, min_score):
+    """search_any_k of Index and Group: every k_fetch on the GPU.  Above RBK_MAX_K_FETCH_LARGE the unbounded search
+    sorts the candidates on the device; up to it, _search_any_k's scan and large-k paths."""
+    if k_fetch > RBK_MAX_K_FETCH_LARGE:
+        return ix.search_unbounded(queries, k_fetch, min_score)
+    return _search_any_k(ix, queries, k_fetch, min_score)
 
 
 class Index:
@@ -307,19 +317,22 @@ class Index:
         """search() for 1 <= k_fetch <= RBK_MAX_K_FETCH_LARGE (f64 queries): count scan, emit scan, exact re-rank."""
         return _search_large(lib.rbk_index_search_large_f64, self._h, queries, k_fetch, min_score)
 
+    def search_unbounded(self, queries, k_fetch: int, min_score: float | None = 0.5):
+        """search() for any k_fetch >= 1 (f64 queries): search_large() up to RBK_MAX_K_FETCH_LARGE; above it the same
+        two scans, then the candidates sorted on the device, at most count() hits per query."""
+        return _search_large(lib.rbk_index_search_unbounded_f64, self._h, queries, k_fetch, min_score)
+
     def exact_scores(self, queries) -> np.ndarray:
-        """float64 [B, size()]: the reference's cosine of every row, NaN for tombstoned / zero rows (k_fetch beyond
-        RBK_MAX_K_FETCH_LARGE)."""
+        """float64 [B, size()]: the reference's cosine of every row, NaN for tombstoned / zero rows."""
         q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
         out = np.empty((q.shape[0], self.size()), dtype=np.float64)
         check(lib.rbk_index_exact_scores_f64(self._h, ptr(q), q.shape[0], q.shape[1], ptr(out)))
         return out
 
     def search_any_k(self, queries, k_fetch: int, min_score: float | None = 0.5):
-        """search() for any k_fetch: search_large() above RBK_MAX_K_FETCH; above RBK_MAX_K_FETCH_LARGE the answer is cut
-        on the host from exact_scores() with the reference's own steps - `>= minScore`, stable descending sort over slot
-        order, slice (vector-store.ts:212-221)."""
-        return _search_any_k(self, queries, k_fetch, min_score)
+        """search() for any k_fetch: search_large() above RBK_MAX_K_FETCH, search_unbounded() above
+        RBK_MAX_K_FETCH_LARGE."""
+        return _search_any_k_on_device(self, queries, k_fetch, min_score)
 
     def search_device(self, q_ptr: int, B: int, k_fetch: int, min_score: float | None, slots_ptr: int,
                       scores_ptr: int, counts_ptr: int) -> None:
@@ -437,6 +450,9 @@ class Group:
     def search_large(self, queries, k_fetch: int, min_score: float | None = 0.5):
         return _search_large(lib.rbk_group_search_large_f64, self._h, queries, k_fetch, min_score)
 
+    def search_unbounded(self, queries, k_fetch: int, min_score: float | None = 0.5):
+        return _search_large(lib.rbk_group_search_unbounded_f64, self._h, queries, k_fetch, min_score)
+
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: every device's exact scores, put back in global slot order (4096-row blocks dealt
         out round-robin)."""
@@ -456,7 +472,7 @@ class Group:
         return out
 
     def search_any_k(self, queries, k_fetch: int, min_score: float | None = 0.5):
-        return _search_any_k(self, queries, k_fetch, min_score)
+        return _search_any_k_on_device(self, queries, k_fetch, min_score)
 
     def stats(self) -> dict:
         out = {"devices": len(self.devices), "redone_batches": lib.rbk_group_redone_batches(self._h)}

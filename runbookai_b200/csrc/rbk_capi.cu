@@ -336,6 +336,9 @@ template <int kMode, typename P>
 rbk_status launch_sub_batch(rbk_index* ix, int q0, const P& sp) {
   CUtensorMap tmap_q;
   const int q_rows = static_cast<int>(round_up(sp.B, kBlockM));   // whole query blocks: no out-of-bounds box rows
+  // every row the map covers must lie inside the query buffer: the scan's TMA loads whole boxes
+  if ((static_cast<size_t>(q0) + q_rows) * ix->dpad > ix->q_bf16.n)
+    return fail(RBK_ECUDA, "scan launch at query " + std::to_string(q0) + " would read past the query buffer");
   rbk_status st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM);
   if (st != RBK_OK) return st;
   cudaEvent_t* tev = ix->capturing ? nullptr : next_scan_events(ix);
@@ -363,13 +366,13 @@ rbk_status fill_empty_results(rbk_index* ix, int B, int k_fetch, long long* d_sl
 namespace rbk {
 namespace impl {
 
-rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem) {
+rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem, int slack_rows) {
   CK(ix->q_raw.ensure(static_cast<size_t>(B) * ix->dim * elem));
   // rows padded to whole query blocks: the scan's TMA boxes are 128 query rows, and a box that hangs over the end of
   // the tensor is zero-FILLED by the TMA unit row by row, which is slow.  With the map covering whole blocks the pad
   // rows are ordinary (zeroed once here) memory; they only ever feed accumulator rows of queries that do not exist.
   {
-    const size_t want = static_cast<size_t>(round_up(B, kBlockM)) * ix->dpad;
+    const size_t want = static_cast<size_t>(round_up(B, kBlockM) + slack_rows) * ix->dpad;
     if (want > ix->q_bf16.n) {
       CK(ix->q_bf16.ensure(want));
       CK(cudaMemsetAsync(ix->q_bf16.p, 0, ix->q_bf16.n * sizeof(uint16_t), ix->stream));
@@ -607,6 +610,109 @@ rbk_status large_check(rbk_index* ix) {
   if (ix->h_lerr.p[0] == 0) return RBK_OK;
   return fail(RBK_ECUDA, "large-k search: the emit scan found more rows than the count scan bounded for " +
                              std::to_string(ix->h_lerr.p[0]) + " queries (the answer is not proven exact)");
+}
+
+std::vector<std::pair<int, int>> split_by_budget(const std::vector<int64_t>& cost) {
+  std::vector<std::pair<int, int>> groups;
+  const int B = static_cast<int>(cost.size());
+  int q0 = 0;
+  int64_t used = 0;
+  for (int b = 0; b < B; ++b) {
+    if (b > q0 && used + cost[b] > kUnboundedBudget) {
+      groups.emplace_back(q0, b);
+      q0 = b;
+      used = 0;
+    }
+    used += cost[b];
+  }
+  if (B > q0) groups.emplace_back(q0, B);
+  return groups;
+}
+
+static int64_t sort_tiles(int cap) { return (cap + kSortTile - 1) / kSortTile; }
+
+rbk_status unbounded_prepare(rbk_index* ix, int B, const std::vector<std::pair<int, int>>& groups) {
+  CK(ix->h_utoff.ensure(B));
+  CK(ix->ub_toff.ensure(B));
+  int64_t max_cand = 1, max_tiles = 1;
+  for (const auto& gr : groups) {
+    int64_t cand = 0, tiles = 0;
+    for (int b = gr.first; b < gr.second; ++b) {
+      ix->h_loff.p[b] = cand;
+      ix->h_utoff.p[b] = static_cast<int>(tiles);
+      cand += ix->h_lcap.p[b];
+      tiles += sort_tiles(ix->h_lcap.p[b]);
+    }
+    max_cand = std::max(max_cand, cand);
+    max_tiles = std::max(max_tiles, tiles);
+  }
+  CK(ix->lg_rows.ensure(static_cast<size_t>(max_cand)));
+  CK(ix->lg_scores.ensure(static_cast<size_t>(max_cand)));
+  CK(ix->ub_rows.ensure(static_cast<size_t>(max_cand)));
+  CK(ix->ub_scores.ensure(static_cast<size_t>(max_cand)));
+  CK(ix->ub_len.ensure(static_cast<size_t>(2 * max_tiles)));
+  CK(cudaMemcpyAsync(ix->lg_off.p, ix->h_loff.p, sizeof(long long) * B, cudaMemcpyHostToDevice, ix->stream));
+  CK(cudaMemcpyAsync(ix->ub_toff.p, ix->h_utoff.p, sizeof(int) * B, cudaMemcpyHostToDevice, ix->stream));
+  CK(cudaMemsetAsync(ix->lg_cnt.p, 0, sizeof(int) * B, ix->stream));
+  CK(cudaMemsetAsync(ix->lg_err.p, 0, sizeof(int), ix->stream));
+  return RBK_OK;
+}
+
+rbk_status unbounded_emit(rbk_index* ix, int q0, int q1, int k_eff, double min_score, long long* d_slots,
+                          double* d_scores, int* d_counts) {
+  if (ix->n_rows == 0) return fill_empty_results(ix, q1 - q0, k_eff, d_slots, d_scores, d_counts);
+  int64_t group_tiles = 0;
+  for (int b = q0; b < q1; ++b) group_tiles += sort_tiles(ix->h_lcap.p[b]);
+  for (int s0 = q0; s0 < q1; s0 += kMaxSubBatch) {
+    const int Bs = std::min(kMaxSubBatch, q1 - s0);
+    LargeScanParams sp = large_scan_params(ix, s0, Bs, k_eff);
+    sp.thr_init = ix->lg_theta.p + s0;   // theta_q of the count pass
+    sp.emit_off = ix->lg_off.p + s0;
+    sp.emit_cap = ix->lg_cap.p + s0;
+    sp.emit_cnt = ix->lg_cnt.p + s0;
+    sp.emit_rows = ix->lg_rows.p;
+    CK(cudaMemsetAsync(sp.progress, 0, sizeof(int) * progress_slots(ix), ix->stream));
+    rbk_status st = launch_sub_batch<kScanEmit>(ix, s0, sp);
+    if (st != RBK_OK) return st;
+    LargeRerankParams rp;
+    rp.B = Bs;
+    rp.d = ix->dim;
+    rp.dpad = ix->dpad;
+    rp.k_fetch = k_eff;
+    rp.min_score = min_score;
+    rp.rows = ix->rows;
+    rp.rows_f64 = ix->rows_f64;
+    rp.row_norm2 = ix->norm2;
+    rp.slot = ix->slot;
+    rp.q_f64 = ix->q_f64.p + static_cast<size_t>(s0) * ix->dim;
+    rp.q_norm2 = ix->q_norm2.p + s0;
+    rp.emit_off = sp.emit_off;
+    rp.emit_cap = sp.emit_cap;
+    rp.emit_cnt = sp.emit_cnt;
+    rp.emit_rows = ix->lg_rows.p;
+    rp.cand_scores = ix->lg_scores.p;
+    rp.out_slots = d_slots + static_cast<size_t>(s0 - q0) * k_eff;
+    rp.out_scores = d_scores + static_cast<size_t>(s0 - q0) * k_eff;
+    rp.out_counts = d_counts + (s0 - q0);
+    rp.overflow = ix->lg_err.p;
+    SegSortScratch ss;
+    ss.tile_off = ix->ub_toff.p + s0;
+    ss.scores = ix->ub_scores.p;
+    ss.rows = ix->ub_rows.p;
+    ss.len[0] = ix->ub_len.p;
+    ss.len[1] = ix->ub_len.p + group_tiles;
+    const int max_cap = *std::max_element(ix->h_lcap.p + s0, ix->h_lcap.p + s0 + Bs);
+    ss.max_tiles = static_cast<int>(sort_tiles(max_cap));
+    int launches = 0;
+    CK(launch_unbounded_rerank(rp, ss, max_cap, ix->f64_on_host, ix->stream, &launches));
+    ix->stats.kernel_launches += launches;
+  }
+  return RBK_OK;
+}
+
+rbk_status unbounded_finish(rbk_index* ix) {
+  CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+  return RBK_OK;
 }
 
 }  // namespace impl
@@ -927,6 +1033,11 @@ void rbk_index_destroy(rbk_index* ix) {
     ix->h_lcap.release();
     ix->h_lerr.release();
     ix->h_loff.release();
+    ix->ub_toff.release();
+    ix->ub_rows.release();
+    ix->ub_len.release();
+    ix->ub_scores.release();
+    ix->h_utoff.release();
     ix->o_block.release();
     ix->h_block.release();
     ix->h_flags.release();
@@ -1234,6 +1345,75 @@ rbk_status rbk_index_search_large_f64(rbk_index* ix, const double* queries, int3
   if (st != RBK_OK) return st;
   ts.finish(kernel_ms_out);
   L.unpack(ix->h_block.p, out_slots, out_scores, out_counts);
+  return RBK_OK;
+}
+
+rbk_status rbk_index_search_unbounded_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
+                                          int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                          int32_t* out_counts, float* kernel_ms_out) {
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, INT32_MAX);
+  if (st != RBK_OK) return st;
+  if (k_fetch <= RBK_MAX_K_FETCH_LARGE)
+    return rbk_index_search_large_f64(ix, queries, B, query_dim, k_fetch, min_score, out_slots, out_scores,
+                                      out_counts, kernel_ms_out);
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  if (kernel_ms_out) *kernel_ms_out = 0.f;
+  if (B == 0) {
+    ix->stats.searches++;
+    return RBK_OK;
+  }
+  // no query can have more hits than there are live rows: every buffer is sized by k_eff
+  const int k_eff = static_cast<int>(std::min<int64_t>(k_fetch, ix->n_live));
+  fill_result_tail(out_slots, out_scores, B, k_fetch, k_eff);
+  if (k_eff == 0) {
+    memset(out_counts, 0, sizeof(int32_t) * B);
+    ix->stats.searches++;
+    ix->stats.queries += B;
+    return RBK_OK;
+  }
+  // a query group may start at any query: kBlockM rows of slack keep its query map inside the buffer
+  st = ensure_query_scratch(ix, B, 8, kBlockM);
+  if (st != RBK_OK) return st;
+  TimedSearch ts{ix};
+  st = ts.begin();
+  if (st != RBK_OK) return st;
+  CK(cudaMemcpyAsync(ix->q_raw.p, queries, static_cast<size_t>(B) * ix->dim * 8, cudaMemcpyHostToDevice, ix->stream));
+  st = large_count(ix, ix->q_raw.p, B, k_eff, min_score);
+  if (st != RBK_OK) return st;
+  CK(cudaStreamSynchronize(ix->stream));   // C_q sizes the candidate buffers and the query groups
+  std::vector<int64_t> cost(B);
+  for (int b = 0; b < B; ++b) cost[b] = ix->h_lcap.p[b] * kUnboundedCandBytes + unbounded_result_bytes(k_eff);
+  const std::vector<std::pair<int, int>> groups = split_by_budget(cost);
+  st = unbounded_prepare(ix, B, groups);
+  if (st != RBK_OK) return st;
+  int max_group = 0;
+  for (const auto& gr : groups) max_group = std::max(max_group, gr.second - gr.first);
+  const ResultBlock L(max_group, k_eff);
+  CK(ix->o_block.ensure(L.off_counts + sizeof(int32_t) * max_group));
+  for (const auto& gr : groups) {
+    const int Bg = gr.second - gr.first;
+    const ResultBlock R(Bg, k_eff);
+    unsigned char* base = ix->o_block.p;
+    st = unbounded_emit(ix, gr.first, gr.second, k_eff, min_score, R.slots(base), R.scores(base), R.counts(base));
+    if (st != RBK_OK) return st;
+    // straight into the caller's rows of k_fetch entries (stream-ordered before the next group reuses the block)
+    const size_t row = sizeof(int64_t) * k_eff, pitch = sizeof(int64_t) * static_cast<size_t>(k_fetch);
+    CK(cudaMemcpy2DAsync(out_slots + static_cast<size_t>(gr.first) * k_fetch, pitch, R.slots(base), row, row, Bg,
+                         cudaMemcpyDeviceToHost, ix->stream));
+    CK(cudaMemcpy2DAsync(out_scores + static_cast<size_t>(gr.first) * k_fetch, pitch, R.scores(base), row, row, Bg,
+                         cudaMemcpyDeviceToHost, ix->stream));
+    CK(cudaMemcpyAsync(out_counts + gr.first, R.counts(base), sizeof(int32_t) * Bg, cudaMemcpyDeviceToHost,
+                       ix->stream));
+  }
+  st = unbounded_finish(ix);
+  if (st != RBK_OK) return st;
+  st = ts.round_trip();
+  if (st != RBK_OK) return st;
+  st = large_check(ix);
+  if (st != RBK_OK) return st;
+  ts.finish(kernel_ms_out);
   return RBK_OK;
 }
 

@@ -967,11 +967,151 @@ __global__ void __launch_bounds__(kTopThreads) large_topk_kernel(LargeRerankPara
   }
 }
 
-// --------------------------------------------------------------------------- all exact scores (k_fetch > 4096)
-// One thread per (row, query): the reference's fp64 cosine of EVERY row, NaN for tombstoned / zero rows.  Serves
-// requests for more hits than the large-k search keeps (k_fetch > RBK_MAX_K_FETCH_LARGE): the host then applies
-// `>= minScore`, the stable sort and the cut literally (vector-store.ts:212-221).  Beyond 4096 hits per query the
-// host-side cut dominates anyway, so simplicity wins over bandwidth here.
+// --------------------------------------------------------------------------- unbounded search: segmented sort
+// Replaces large_topk_kernel when k_fetch exceeds what one block's shared memory holds.  After large_score_kernel a
+// query's segment holds n_q = min(emit_cnt, emit_cap) candidates (row, exact score).  (1) seg_tile_sort_kernel: one
+// block per tile of kSortTile candidates of one query drops what fails `>= min_score` (NaN included), sorts the rest by
+// (score desc, row asc) in shared memory, writes the first min(passing, k_eff) back in place and records that length.
+// (2) seg_merge_kernel, once per doubling: adjacent runs 2r and 2r+1 of a query become run r of twice the width.  Each
+// entry's rank in the merged run is its own index plus the number of entries of the partner run that come before it
+// (binary search; rows are unique, so hit_before is a strict total order and the ranks are a permutation); ranks >= k_eff
+// are dropped, because nothing past position k_eff of a run can reach the answer.  (3) seg_write_kernel: global slots,
+// scores, the -1 / NaN tail and the counts in the [B][k_eff] layout large_topk_kernel writes.
+constexpr int kSortThreads = 512;
+constexpr int kMergeThreads = 256;
+
+__global__ void __launch_bounds__(kSortThreads) seg_tile_sort_kernel(LargeRerankParams p, SegSortScratch s) {
+  extern __shared__ __align__(16) double s_sc[];   // kSortTile scores, then kSortTile rows
+  int* s_rw = reinterpret_cast<int*>(s_sc + kSortTile);
+  __shared__ int s_pass;
+  const int q = blockIdx.y, t = blockIdx.x, tid = threadIdx.x;
+  const int n = min(p.emit_cnt[q], p.emit_cap[q]);
+  const int i0 = t * kSortTile;
+  if (i0 >= n) return;   // uniform: a tile past the segment's end holds nothing and is never read
+  const int m = min(kSortTile, n - i0);
+  int S = 2;             // the bitonic network's width: a power of two >= m
+  while (S < m) S <<= 1;
+  const size_t base = static_cast<size_t>(p.emit_off[q]) + i0;
+  if (tid == 0) s_pass = 0;
+  __syncthreads();
+  int mine = 0;
+  for (int i = tid; i < S; i += kSortThreads) {
+    double sc = -INFINITY;
+    int rw = INT_MAX;    // after every real row, even one scoring -inf
+    if (i < m) {
+      const double v = p.cand_scores[base + i];
+      if (v >= p.min_score) {   // vector-store.ts:212 (NaN fails; -inf = no threshold)
+        sc = v;
+        rw = p.emit_rows[base + i];
+        ++mine;
+      }
+    }
+    s_sc[i] = sc;
+    s_rw[i] = rw;
+  }
+  if (mine) atomicAdd(&s_pass, mine);
+  __syncthreads();
+  for (int k2 = 2; k2 <= S; k2 <<= 1) {
+    for (int st = k2 >> 1; st > 0; st >>= 1) {
+      for (int i = tid; i < S; i += kSortThreads) {
+        const int j = i ^ st;
+        if (j > i) {
+          const bool desc = (i & k2) == 0;
+          const bool j_first = hit_before(s_sc[j], s_rw[j], s_sc[i], s_rw[i]);
+          if (desc ? j_first : !j_first) {
+            const double ts = s_sc[i];
+            s_sc[i] = s_sc[j];
+            s_sc[j] = ts;
+            const int tr = s_rw[i];
+            s_rw[i] = s_rw[j];
+            s_rw[j] = tr;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  const int L = min(s_pass, p.k_fetch);
+  for (int i = tid; i < L; i += kSortThreads) {
+    p.cand_scores[base + i] = s_sc[i];
+    p.emit_rows[base + i] = s_rw[i];
+  }
+  if (tid == 0) s.len[0][s.tile_off[q] + t] = L;
+}
+
+// Merge pass `pass` (0-based): runs of 2^pass tiles -> runs of 2^(pass+1) tiles.  One block per input tile.
+__global__ void __launch_bounds__(kMergeThreads) seg_merge_kernel(LargeRerankParams p, SegSortScratch s, int pass) {
+  const int q = blockIdx.y, t = blockIdx.x, tid = threadIdx.x;
+  const int n = min(p.emit_cnt[q], p.emit_cap[q]);
+  const int nt = (n + kSortTile - 1) / kSortTile;
+  if (t >= nt) return;
+  const int src = pass & 1, dst = src ^ 1;
+  const double* sc_in = src ? s.scores : p.cand_scores;
+  const int* rw_in = src ? s.rows : p.emit_rows;
+  double* sc_out = dst ? s.scores : p.cand_scores;
+  int* rw_out = dst ? s.rows : p.emit_rows;
+  const int w = 1 << pass;                 // tiles per input run
+  const int r = t >> pass, local = t & (w - 1);
+  const int partner = r ^ 1;
+  // (selects, not s.len[src]: a run-time index into the parameter array would copy it to local memory)
+  const int* len_in = (src ? s.len[1] : s.len[0]) + s.tile_off[q];
+  int* len_out = (dst ? s.len[1] : s.len[0]) + s.tile_off[q];
+  const int La = len_in[r * w];
+  const int Lb = partner * w < nt ? len_in[partner * w] : 0;   // the last run of an odd count has no partner: copied
+  const int L = min(La + Lb, p.k_fetch);
+  if (local == 0 && (r & 1) == 0 && tid == 0) len_out[r * w] = L;
+  const size_t seg = static_cast<size_t>(p.emit_off[q]);
+  const size_t mine = seg + static_cast<size_t>(r) * w * kSortTile;
+  const size_t other = seg + static_cast<size_t>(partner) * w * kSortTile;
+  const size_t out = seg + static_cast<size_t>(r >> 1) * 2 * w * kSortTile;
+  // 64-bit positions: with k_eff (< 2^31) entries a run's last tile may end past INT_MAX
+  const long long e1 = min(static_cast<long long>(local + 1) * kSortTile, static_cast<long long>(La));
+  for (long long e = static_cast<long long>(local) * kSortTile + tid; e < e1; e += kMergeThreads) {
+    const double sc = sc_in[mine + e];
+    const int rw = rw_in[mine + e];
+    int lo = 0, hi = Lb;                   // entries of the partner run that come before (sc, rw)
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (hit_before(__ldg(sc_in + other + mid), __ldg(rw_in + other + mid), sc, rw)) lo = mid + 1;
+      else hi = mid;
+    }
+    const long long rank = e + lo;   // La <= k_eff: every rank is >= its own index
+    if (rank < L) {
+      sc_out[out + rank] = sc;
+      rw_out[out + rank] = rw;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) seg_write_kernel(LargeRerankParams p, SegSortScratch s, int final_buf) {
+  const int q = blockIdx.y;
+  const int emitted = p.emit_cnt[q];
+  const int n = min(emitted, p.emit_cap[q]);
+  const int L = n > 0 ? (final_buf ? s.len[1] : s.len[0])[s.tile_off[q]] : 0;
+  const double* sc = final_buf ? s.scores : p.cand_scores;
+  const int* rw = final_buf ? s.rows : p.emit_rows;
+  const size_t seg = static_cast<size_t>(p.emit_off[q]);
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < p.k_fetch; i += gridDim.x * 256ll) {
+    const size_t o = static_cast<size_t>(q) * p.k_fetch + i;
+    if (i < L) {
+      p.out_slots[o] = p.slot.global(rw[seg + i]);
+      p.out_scores[o] = sc[seg + i];
+    } else {
+      p.out_slots[o] = -1;
+      p.out_scores[o] = __longlong_as_double(0x7FF8000000000000ll);
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    p.out_counts[q] = L;
+    if (emitted > p.emit_cap[q]) atomicAdd(p.overflow, 1);   // the count pass missed rows: the answer is not proven
+  }
+}
+
+// --------------------------------------------------------------------------- all exact scores
+// One thread per (row, query): the reference's fp64 cosine of EVERY row, NaN for tombstoned / zero rows, for a host
+// that applies `>= minScore`, the stable sort and the cut itself (vector-store.ts:212-221).  Searches for any number of
+// hits do not need it: rbk_index_search_unbounded_f64 sorts on the device and copies back only the answer, which is far
+// faster than this route's 8 bytes per row and query over PCIe plus a host sort.  Kept simple: one fp64 pass per query.
 __global__ void __launch_bounds__(256) exact_scores_kernel(const uint16_t* __restrict__ rows,
                                                            const double* __restrict__ rows_f64,
                                                            const double* __restrict__ row_norm2,
@@ -1133,6 +1273,41 @@ cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, bool ro
   cudaError_t e = cudaFuncSetAttribute(large_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   large_topk_kernel<<<p.B, kTopThreads, smem, stream>>>(p, S);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_unbounded_rerank(const LargeRerankParams& p, const SegSortScratch& s, int max_cap,
+                                    bool rows_on_host, cudaStream_t stream, int* launches) {
+  *launches = 0;
+  if (p.B <= 0) return cudaSuccess;
+  cudaError_t e;
+  if (max_cap > 0) {
+    dim3 grid(static_cast<unsigned>((max_cap + 255) / 256), static_cast<unsigned>(p.B));
+    if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
+    else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+  }
+  int passes = 0;
+  if (s.max_tiles > 0) {
+    const size_t smem = static_cast<size_t>(kSortTile) * (sizeof(double) + sizeof(int));
+    e = cudaFuncSetAttribute(seg_tile_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const dim3 grid(static_cast<unsigned>(s.max_tiles), static_cast<unsigned>(p.B));
+    seg_tile_sort_kernel<<<grid, kSortThreads, smem, stream>>>(p, s);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    for (; (1 << passes) < s.max_tiles; ++passes) {
+      seg_merge_kernel<<<grid, kMergeThreads, 0, stream>>>(p, s, passes);
+      if ((e = cudaGetLastError()) != cudaSuccess) return e;
+      ++*launches;
+    }
+  }
+  const long long need = (p.k_fetch + 255ll) / 256;
+  const int wblocks = need < 1024 ? static_cast<int>(need) : 1024;
+  seg_write_kernel<<<dim3(static_cast<unsigned>(wblocks), static_cast<unsigned>(p.B)), 256, 0, stream>>>(p, s,
+                                                                                                       passes & 1);
+  ++*launches;
   return cudaGetLastError();
 }
 

@@ -6,6 +6,7 @@
 
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/rbk_knn.h"
@@ -94,6 +95,22 @@ struct ResultBlock {
   }
 };
 
+// Entries [k_eff, k_fetch) of each of the B result rows of k_fetch entries: slot -1, score NaN (an unbounded search
+// keeps at most k_eff = count() hits per query).
+inline void fill_result_tail(int64_t* slots, double* scores, int32_t B, int32_t k_fetch, int32_t k_eff) {
+  if (k_eff >= k_fetch) return;
+  const uint64_t nan_bits = 0x7FF8000000000000ull;   // the quiet NaN the device kernels write
+  double nan;
+  memcpy(&nan, &nan_bits, sizeof nan);
+  for (int32_t b = 0; b < B; ++b) {
+    const size_t o = static_cast<size_t>(b) * k_fetch;
+    for (int32_t i = k_eff; i < k_fetch; ++i) {
+      slots[o + i] = -1;
+      scores[o + i] = nan;
+    }
+  }
+}
+
 }  // namespace impl
 }  // namespace rbk
 
@@ -136,6 +153,10 @@ struct rbk_index {
   rbk::impl::DevBuf<double> lg_scores;
   rbk::impl::PinBuf<int> h_lcap, h_lerr;
   rbk::impl::PinBuf<long long> h_loff;
+  // unbounded search scratch (grow-only): per-query first run-length slot, the sort's second buffer, run lengths
+  rbk::impl::DevBuf<int> ub_toff, ub_rows, ub_len;
+  rbk::impl::DevBuf<double> ub_scores;
+  rbk::impl::PinBuf<int> h_utoff;
   rbk::impl::DevBuf<unsigned char> o_block;
   rbk::impl::PinBuf<unsigned char> h_block;
   rbk::impl::PinBuf<int> h_flags;
@@ -173,8 +194,10 @@ struct rbk_index {
 namespace rbk {
 namespace impl {
 
-// caller holds ix->mu and has the index's device current
-rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem);
+// caller holds ix->mu and has the index's device current.  slack_rows: zeroed bf16 query rows beyond the last whole
+// query block, for callers whose scan launches start at a query that is not a multiple of kBlockM (the unbounded
+// search's query groups): such a launch's query map covers round_up(Bs, kBlockM) rows from its first query.
+rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem, int slack_rows = 0);
 // max_k: RBK_MAX_K_FETCH (the search) or RBK_MAX_K_FETCH_LARGE (the large-k search)
 rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, int k_fetch, double min_score,
                              int max_k = RBK_MAX_K_FETCH);
@@ -191,6 +214,26 @@ rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, doubl
 rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long long* d_slots, double* d_scores,
                       int* d_counts);
 rbk_status large_check(rbk_index* ix);
+
+// Unbounded search (k_fetch > RBK_MAX_K_FETCH_LARGE), built on the same count pass: large_count with k_fetch = k_eff,
+// one host synchronisation, then the queries in contiguous groups whose device storage fits kUnboundedBudget, each
+// group costing one emit scan:
+//   split_by_budget   : the groups, from each query's cost in bytes (at least one query per group);
+//   unbounded_prepare : segment offsets and run-length slots of every query relative to its group, the scratch for
+//                       the largest group, zeroed emit and overflow counters (enqueue only);
+//   unbounded_emit    : emit scan, exact re-score and segmented sort of the queries [q0, q1) into d_slots / d_scores /
+//                       d_counts ([q1 - q0][k_eff]); enqueue only;
+//   unbounded_finish  : the D2H of the overflow counter, for large_check after the next synchronisation.
+constexpr int64_t kUnboundedBudget = 256ll << 20;
+// device bytes per candidate: emit row + exact score (sorted in place) + the sort's second buffer
+constexpr int64_t kUnboundedCandBytes = 4 + 8 + 12;
+// device bytes of one query's result in a packed block of k_eff entries (slots, scores, count, flag)
+inline int64_t unbounded_result_bytes(int k_eff) { return 16ll * k_eff + 8; }
+std::vector<std::pair<int, int>> split_by_budget(const std::vector<int64_t>& cost);
+rbk_status unbounded_prepare(rbk_index* ix, int B, const std::vector<std::pair<int, int>>& groups);
+rbk_status unbounded_emit(rbk_index* ix, int q0, int q1, int k_eff, double min_score, long long* d_slots,
+                          double* d_scores, int* d_counts);
+rbk_status unbounded_finish(rbk_index* ix);
 const char* last_error();
 
 }  // namespace impl

@@ -118,7 +118,7 @@ class MultiDeviceIndex:
             q = q[None, :]
         if q.shape[1] != self.dim:
             raise DimensionError(RBK_EDIM, "Vectors must have the same length")
-        # any k: beyond the scan's candidate lists every device answers from its exact scores (Index.search_any_k)
+        # any k: every device answers on the GPU (Index.search_any_k: the scan, the large-k or the unbounded search)
         res = list(self._pool.map(lambda p: getattr(p, "search_any_k", p.search)(q, k_fetch, min_score), self.parts))
         B, G = q.shape[0], len(self.parts)
         slots = np.concatenate([self._global(g, r[0]) for g, r in enumerate(res)], axis=1)      # [B, G*k]

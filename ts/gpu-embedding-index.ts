@@ -6,7 +6,8 @@
  *
  * NOT COMPILED in the build image (no Node/tsc); `compact()` below is no exception.  It is deliberately
  * tiny: the Map's ordered-key semantics (insertion slot, re-set keeps the slot, delete frees the key and
- * `compact()` later its slot) on top of the N-API addon (napi/rbk_napi.cc -> include/rbk_knn.h).  The
+ * `compact()` later its slot) on top of the N-API addon (napi/rbk_napi.cc -> include/rbk_knn.h).  Searches take any
+ * limit: bestBatch picks the one scan, the large-k search or the unbounded search by size.  The
  * tested mirror of the same bookkeeping is runbookai_b200/vector_store.py (`_set`, `delete_document`,
  * `_load_embeddings`, `compact`).
  * INTEGRATION.md shows the few lines of vector-store.ts that change to use it.
@@ -164,7 +165,8 @@ export class GpuEmbeddingIndex {
    * The same for B queries in ONE device pass (what B sequential search() calls cost the reference): the entry point
    * of the micro-batcher that coalesces concurrent searches of several investigations (SURVEY 8f-3;
    * runbookai_b200/batcher.py is the tested mirror).  limit <= 112 takes one scan (RBK_MAX_K_FETCH); up to 4096
-   * (RBK_MAX_K_FETCH_LARGE) the large-k search (two scans and an exact re-rank).
+   * (RBK_MAX_K_FETCH_LARGE) the large-k search (two scans and an exact re-rank); any larger limit the unbounded search
+   * (the same two scans, the candidates sorted on the GPU), so every topK the reference accepts is answered.
    */
   async bestBatch(queries: number[][], limit: number, minScore: number): Promise<ScoredId[][]> {
     while (this.compacting) await this.compacting; // never search against a table that is being renumbered
@@ -178,9 +180,11 @@ export class GpuEmbeddingIndex {
     this.inFlight++;
     try {
       const { slots, scores, counts } =
-        limit > 112
-          ? await this.index.searchLarge(packed, B, limit, minScore)
-          : await this.index.search(packed, B, limit, minScore);
+        limit > 4096
+          ? await this.index.searchUnbounded(packed, B, limit, minScore)
+          : limit > 112
+            ? await this.index.searchLarge(packed, B, limit, minScore)
+            : await this.index.search(packed, B, limit, minScore);
       return queries.map((_, b) => {
         const out: ScoredId[] = [];
         for (let i = 0; i < counts[b]; i++) {
