@@ -62,7 +62,13 @@ const char* rbk_last_error(void);
 
 /* ---- lifetime: `new VectorStore(dbPath)` / `close()` (vector-store.ts:28-32, :330) ---- */
 /* dim: embedding length (any d >= 1).  device: CUDA ordinal.  capacity_hint: rows to
- * pre-allocate (0 = default); the index grows on demand. */
+ * pre-allocate (0 = default); the index grows on demand.  The device storage sits on virtual address ranges reserved
+ * here for the most rows the device's memory could hold (min(2^31 - 512, total memory / device bytes per row)); a
+ * capacity_hint above that fails with RBK_ENOMEM.  Growth maps more physical memory behind the same addresses: nothing
+ * is copied, so growing to capacity C needs C's storage, not the old and the new at once.  The capacity doubles
+ * (whole 256-row tiles); if the doubled capacity cannot be backed, it grows to exactly the rows needed instead, and
+ * only if that fails too does the call return RBK_ENOMEM, with the index unchanged.  A device without CUDA virtual
+ * memory management fails with RBK_ECUDA. */
 rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, rbk_index** out);
 /* flags: RBK_INDEX_KEEP_F64 keeps, next to the bf16 rows the scan reads, the ORIGINAL values of every appended
  * row as float64 (8*dim bytes per row; f32/bf16 inputs are widened exactly).  The exact re-rank then uses them:
@@ -76,7 +82,8 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * exactness flags, fallback and retry decisions, compaction maps: the same values go through the same operations in
  * the same order, only the bytes come over PCIe.  Device memory per row at d = 1536 drops from 15,372 to 3,084 bytes
  * (about 5x the rows per GPU); host RAM pays 8*dim bytes per row (12 KB at d = 1536), and growing the capacity holds
- * the old and the new buffer at once (peak old + new).  The scan is unchanged.  Cost: each search reads k'*8*dim
+ * the old and the new buffer at once (peak old + new): the host rows are one cudaHostAlloc buffer, reallocated and
+ * copied on growth and on rbk_index_trim, unlike the device buffers, which grow in place.  The scan is unchanged.  Cost: each search reads k'*8*dim
  * bytes of host rows per query (k' = candidates re-ranked, <= 128; about 590 KB at k_fetch 20, d = 1536), the large-k
  * search 8*dim bytes per emitted candidate, and the rare exhaustive fallback / rbk_index_exact_scores_f64 the whole
  * corpus, all at PCIe speed; appends write the rows over PCIe.  Every write to the host rows is stream-ordered (a kernel
@@ -132,6 +139,17 @@ rbk_status rbk_index_tombstone(rbk_index* idx, const int64_t* local_slots, int64
  * because the index's work is stream-ordered; their results carry the OLD slots. */
 rbk_status rbk_index_compact(rbk_index* idx, int64_t* old_to_new, int64_t old_to_new_len);
 rbk_status rbk_index_clear(rbk_index* idx);
+/* Give memory back.  Synchronises the index's stream first, so searches enqueued earlier
+ * (rbk_index_search_device_async) finish before anything they read goes away.  Then sets the capacity to that of a
+ * new index holding size() rows, round_up(max(size(), 1024), 256), and unmaps the device storage beyond it (the pinned
+ * host rows of RBK_INDEX_F64_ON_HOST are reallocated at that capacity); releases every search, compaction and staging
+ * scratch buffer, device and pinned, which the next call that needs one re-grows; and drops the captured search graph
+ * and the corpus tensor map.  Answers never change and nothing is renumbered (unlike rbk_index_compact, so the member
+ * indexes of a group may be trimmed).  Trim after rbk_index_compact or rbk_index_clear to return their slots' bytes.
+ * Storage is unmapped in whole physical chunks of at most 256 MiB: afterwards the mapped device bytes exceed
+ * rbk_index_storage_bytes by less than one chunk per device buffer (five at most).  Growing again maps memory, it does
+ * not copy. */
+rbk_status rbk_index_trim(rbk_index* idx);
 int64_t rbk_index_count(const rbk_index* idx); /* live rows  */
 int64_t rbk_index_size(const rbk_index* idx);  /* slots used, tombstones included */
 int32_t rbk_index_dim(const rbk_index* idx);
@@ -252,6 +270,8 @@ rbk_status rbk_group_append_bf16(rbk_group* grp, const uint16_t* rows, int64_t n
 rbk_status rbk_group_overwrite_f64_batch(rbk_group* grp, const int64_t* slots, int64_t n, const double* rows);
 rbk_status rbk_group_tombstone(rbk_group* grp, const int64_t* slots, int64_t n);
 rbk_status rbk_group_clear(rbk_group* grp);
+/* rbk_index_trim on every member, and the group's own exchange buffers released. */
+rbk_status rbk_group_trim(rbk_group* grp);
 int64_t rbk_group_count(const rbk_group* grp); /* live rows */
 int64_t rbk_group_size(const rbk_group* grp);  /* slots used, tombstones included */
 int32_t rbk_group_devices(const rbk_group* grp);

@@ -2,8 +2,8 @@
 // N-API runtime (mock_napi.cc): loads the module, constructs RbkIndex (one device or a device list, optionally with
 // hostRows), loads rows as
 // SQLite-style BLOBs and as a Float64Array, overwrites, tombstones, counts, searches through the Promise/async-work
-// path, provokes every error path, optionally (compact.txt) tombstones more, compacts and searches again, clears,
-// and lets the finalizer run.  Inputs and outputs are flat binary files in
+// path, provokes every error path, optionally (compact.txt) tombstones more, compacts and searches again, optionally
+// (trim.txt) trims and searches again, clears, and lets the finalizer run.  Inputs and outputs are flat binary files in
 // the directory given as argv[1]; tests/test_napi_addon.py writes the inputs and checks the outputs against the
 // oracle.  Links against librbk_knn.so (GPU test) or against tests/napi_shim (CPU test).
 //
@@ -267,6 +267,7 @@ int main(int argc, char** argv) {
         << "\n";
   }
 
+  Result latest = res;   // the answer of the index as it stands
   // compact(): optional compact.txt lists more slots to tombstone first; then compact() and the same search again,
   // results in compact_*.  On a device-group handle compact() must throw (logged as err_compact).
   {
@@ -294,7 +295,27 @@ int main(int argc, char** argv) {
         write_bin("compact_slots.i64", cr.slots.data(), cr.slots.size() * 8);
         write_bin("compact_scores.f64", cr.scores.data(), cr.scores.size() * 8);
         write_bin("compact_counts.i32", cr.counts.data(), cr.counts.size() * 4);
+        latest = cr;
       }
+    }
+  }
+
+  // trim(): optional trim.txt; trim() and the same search again, results in trim_*, which must equal the answer before
+  // the trim (logged as trim_identical).
+  {
+    std::ifstream tf(g_dir + "/trim.txt");
+    if (tf.good()) {
+      if (!mock::call_method(env, ix, "trim", {}, &r, &err)) die("trim threw: " + err);
+      if (!mock::is_undefined(r)) die("trim returned a value");
+      Result tr;
+      if (!search(env, ix, queries, n_q, k, min_score, &tr, &err)) die("search after trim rejected: " + err);
+      write_bin("trim_slots.i64", tr.slots.data(), tr.slots.size() * 8);
+      write_bin("trim_scores.f64", tr.scores.data(), tr.scores.size() * 8);
+      write_bin("trim_counts.i32", tr.counts.data(), tr.counts.size() * 4);
+      log << "trim_identical "
+          << (tr.slots == latest.slots && tr.counts == latest.counts &&
+              memcmp(tr.scores.data(), latest.scores.data(), latest.scores.size() * 8) == 0)
+          << "\n";
     }
   }
 

@@ -18,6 +18,7 @@
 //   ix.overwriteF64(slot, Float64Array row); ix.overwriteF64Batch(BigInt64Array slots, Float64Array rows)
 //   ix.tombstone(BigInt64Array slots); ix.clear()
 //   ix.compact()                               -> BigInt64Array oldToNew   // reclaim tombstoned slots (one GPU only)
+//   ix.trim()                                  // give unused device memory back (after compact / clear)
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
 //   await ix.searchLarge(Float64Array queries, B, kFetch, minScore)   // kFetch up to 4096, same result object
@@ -46,6 +47,9 @@
 // so that the method as a whole needs nothing a library without compaction may lack.
 #pragma weak rbk_index_compact
 #pragma weak rbk_index_size
+// The same for trim; `trim` throws where it is missing.
+#pragma weak rbk_index_trim
+#pragma weak rbk_group_trim
 
 namespace {
 
@@ -76,6 +80,8 @@ struct Handle {
     return grp ? rbk_group_tombstone(grp, slots, n) : rbk_index_tombstone(ix, slots, n);
   }
   rbk_status clear() { return grp ? rbk_group_clear(grp) : rbk_index_clear(ix); }
+  bool has_trim() const { return grp ? rbk_group_trim != nullptr : rbk_index_trim != nullptr; }
+  rbk_status trim() { return grp ? rbk_group_trim(grp) : rbk_index_trim(ix); }
   int64_t count() const { return grp ? rbk_group_count(grp) : rbk_index_count(ix); }
   rbk_status search(const double* q, int32_t B, int32_t qdim, int32_t k, double ms, int64_t* s, double* v, int32_t* c) {
     return grp ? rbk_group_search_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
@@ -283,6 +289,18 @@ napi_value Compact(napi_env env, napi_callback_info info) {
   return out;
 }
 
+// trim(): capacity down to what the rows need, scratch released; slots and answers unchanged.  Synchronous.
+napi_value Trim(napi_env env, napi_callback_info info) {
+  size_t argc = 0;
+  Handle* h = unwrap(env, info, &argc, nullptr);
+  if (!h->has_trim()) {
+    napi_throw_error(env, nullptr, "trim: this librbk_knn.so has no trim (rbk_index_trim / rbk_group_trim)");
+    return nullptr;
+  }
+  if (h->trim() != RBK_OK) return throw_rbk(env);
+  return nullptr;
+}
+
 napi_value Count(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
@@ -399,6 +417,7 @@ napi_value Init(napi_env env, napi_value exports) {
       {"tombstone", nullptr, Tombstone, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"clear", nullptr, Clear, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"compact", nullptr, Compact, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trim", nullptr, Trim, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"count", nullptr, Count, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"search", nullptr, Search, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"searchLarge", nullptr, SearchLarge, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -22,14 +22,14 @@ RBK_INDEX_F64_ON_HOST = 2
 SYMBOLS = [
     "rbk_abi_version", "rbk_last_error", "rbk_index_create", "rbk_index_create_ex", "rbk_index_destroy", "rbk_index_set_stream",
     "rbk_index_set_slot_base", "rbk_index_append_f64", "rbk_index_append_f32", "rbk_index_append_bf16",
-    "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_compact", "rbk_index_clear",
+    "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_compact", "rbk_index_clear", "rbk_index_trim",
     "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_storage_bytes", "rbk_index_read_rows_bf16", "rbk_index_search_f64",
     "rbk_index_search_f32", "rbk_index_search_large_f64", "rbk_index_search_unbounded_f64", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
     "rbk_packed_block_bytes", "rbk_packed_flags_offset",
     "rbk_merge_topk_packed_device", "rbk_index_stats",
     "rbk_index_debug_scores_f32",
     "rbk_group_create", "rbk_group_destroy", "rbk_group_append_f64", "rbk_group_append_f32", "rbk_group_append_bf16",
-    "rbk_group_overwrite_f64_batch", "rbk_group_tombstone", "rbk_group_clear", "rbk_group_count", "rbk_group_size",
+    "rbk_group_overwrite_f64_batch", "rbk_group_tombstone", "rbk_group_clear", "rbk_group_trim", "rbk_group_count", "rbk_group_size",
     "rbk_group_devices", "rbk_group_member", "rbk_group_redone_batches", "rbk_group_search_f32", "rbk_group_search_f64",
     "rbk_group_search_large_f64", "rbk_group_search_unbounded_f64",
 ]
@@ -78,6 +78,7 @@ def _load() -> C.CDLL:
     lib.rbk_index_tombstone.argtypes = [vp, vp, i64]
     lib.rbk_index_compact.argtypes = [vp, vp, i64]
     lib.rbk_index_clear.argtypes = [vp]
+    lib.rbk_index_trim.argtypes = [vp]
     for n in ("rbk_index_count", "rbk_index_size"):
         getattr(lib, n).argtypes = [vp]
         getattr(lib, n).restype = i64
@@ -106,6 +107,7 @@ def _load() -> C.CDLL:
     lib.rbk_group_overwrite_f64_batch.argtypes = [vp, vp, i64, vp]
     lib.rbk_group_tombstone.argtypes = [vp, vp, i64]
     lib.rbk_group_clear.argtypes = [vp]
+    lib.rbk_group_trim.argtypes = [vp]
     for n in ("rbk_group_count", "rbk_group_size", "rbk_group_redone_batches"):
         getattr(lib, n).argtypes = [vp]
         getattr(lib, n).restype = i64
@@ -275,6 +277,11 @@ class Index:
     def clear(self) -> None:
         check(lib.rbk_index_clear(self._h))
 
+    def trim(self) -> None:
+        """Give memory back: capacity down to what size() rows need (unmapping the device storage beyond it), every
+        scratch buffer released.  Answers and slots do not change; run it after compact() or clear()."""
+        check(lib.rbk_index_trim(self._h))
+
     def count(self) -> int:
         return lib.rbk_index_count(self._h)
 
@@ -421,6 +428,10 @@ class Group:
 
     def clear(self) -> None:
         check(lib.rbk_group_clear(self._h))
+
+    def trim(self) -> None:
+        """Index.trim() on every member; slots do not change."""
+        check(lib.rbk_group_trim(self._h))
 
     def count(self) -> int:
         return lib.rbk_group_count(self._h)

@@ -125,81 +125,232 @@ cudaEvent_t* next_scan_events(rbk_index* ix) {
 
 int64_t inv_norm_len(int64_t cap) { return round_up(cap, kBlockN) + kBlockN; }
 
+// ---- device corpus storage on reserved virtual address ranges (DESIGN.md §3) ----
+// The driver's virtual memory calls, looked up like cuTensorMapEncodeTiled so that the link line stays the runtime's.
+struct VmmApi {
+  bool ok = false;
+  CUresult (*DeviceGetAttribute)(int*, CUdevice_attribute, CUdevice) = nullptr;
+  CUresult (*MemGetAllocationGranularity)(size_t*, const CUmemAllocationProp*, CUmemAllocationGranularity_flags) = nullptr;
+  CUresult (*MemAddressReserve)(CUdeviceptr*, size_t, size_t, CUdeviceptr, unsigned long long) = nullptr;
+  CUresult (*MemAddressFree)(CUdeviceptr, size_t) = nullptr;
+  CUresult (*MemCreate)(CUmemGenericAllocationHandle*, size_t, const CUmemAllocationProp*, unsigned long long) = nullptr;
+  CUresult (*MemRelease)(CUmemGenericAllocationHandle) = nullptr;
+  CUresult (*MemMap)(CUdeviceptr, size_t, size_t, CUmemGenericAllocationHandle, unsigned long long) = nullptr;
+  CUresult (*MemUnmap)(CUdeviceptr, size_t) = nullptr;
+  CUresult (*MemSetAccess)(CUdeviceptr, size_t, const CUmemAccessDesc*, size_t) = nullptr;
+};
+
+const VmmApi& vmm_api() {
+  static VmmApi api;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    bool ok = true;
+    auto get = [&ok](const char* name, auto* fn) {
+      void* p = nullptr;
+      cudaDriverEntryPointQueryResult qres;
+      if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &qres) == cudaSuccess &&
+          qres == cudaDriverEntryPointSuccess && p)
+        *fn = reinterpret_cast<std::remove_pointer_t<decltype(fn)>>(p);
+      else
+        ok = false;
+    };
+    get("cuDeviceGetAttribute", &api.DeviceGetAttribute);
+    get("cuMemGetAllocationGranularity", &api.MemGetAllocationGranularity);
+    get("cuMemAddressReserve", &api.MemAddressReserve);
+    get("cuMemAddressFree", &api.MemAddressFree);
+    get("cuMemCreate", &api.MemCreate);
+    get("cuMemRelease", &api.MemRelease);
+    get("cuMemMap", &api.MemMap);
+    get("cuMemUnmap", &api.MemUnmap);
+    get("cuMemSetAccess", &api.MemSetAccess);
+    api.ok = ok;
+  });
+  return api;
+}
+
+rbk_status cu_fail(CUresult r, const char* what) {
+  return fail(r == CUDA_ERROR_OUT_OF_MEMORY ? RBK_ENOMEM : RBK_ECUDA,
+              std::string(what) + " failed: CUresult " + std::to_string(static_cast<int>(r)));
+}
+
+CUmemAllocationProp vm_prop(int device) {
+  CUmemAllocationProp prop;
+  memset(&prop, 0, sizeof prop);
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = device;
+  return prop;
+}
+
+// Largest physical chunk of one mapping.  A growth maps [old, new) of a buffer in chunks of at most this size (one
+// chunk when the growth is smaller), so growing to a full 80 GB card takes a few hundred map calls, a small index pays
+// one granule (2 MiB on H100) per small buffer, and a trim leaves less than one chunk per buffer mapped beyond the
+// capacity (DESIGN.md §3).
+constexpr size_t kVmChunk = 256ull << 20;
+
+// Unmaps and releases the chunks of r that lie wholly at or beyond `keep` bytes from its base.
+void vm_unmap_from(VmRange* r, size_t keep) {
+  const VmmApi& api = vmm_api();
+  while (!r->chunks.empty() && r->mapped - r->chunks.back().bytes >= keep) {
+    const VmRange::Chunk c = r->chunks.back();
+    r->mapped -= c.bytes;
+    api.MemUnmap(r->base + r->mapped, c.bytes);
+    api.MemRelease(c.handle);
+    r->chunks.pop_back();
+  }
+}
+
+// Backs [base, base + bytes) of r, mapping new chunks after the ones it has.  On failure the chunks this call mapped
+// stay mapped; the caller unmaps them (vm_unmap_from its old `mapped`).
+rbk_status vm_map_to(const rbk_index* ix, VmRange* r, size_t bytes) {
+  const VmmApi& api = vmm_api();
+  const size_t want = static_cast<size_t>(round_up(static_cast<int64_t>(bytes), static_cast<int64_t>(ix->vm_gran)));
+  if (want > r->reserved) return fail(RBK_ENOMEM, "index storage beyond its reserved address range");
+  const size_t max_chunk = std::max(ix->vm_gran, kVmChunk / ix->vm_gran * ix->vm_gran);
+  const CUmemAllocationProp prop = vm_prop(ix->device);
+  CUmemAccessDesc access;
+  memset(&access, 0, sizeof access);
+  access.location = prop.location;
+  access.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  while (r->mapped < want) {
+    const size_t sz = std::min(want - r->mapped, max_chunk);
+    CUmemGenericAllocationHandle h;
+    CUresult res = api.MemCreate(&h, sz, &prop, 0);
+    if (res != CUDA_SUCCESS) return cu_fail(res, "cuMemCreate(index storage)");
+    const CUdeviceptr at = r->base + r->mapped;
+    if ((res = api.MemMap(at, sz, 0, h, 0)) != CUDA_SUCCESS) {
+      api.MemRelease(h);
+      return cu_fail(res, "cuMemMap(index storage)");
+    }
+    r->chunks.push_back({h, sz});
+    r->mapped += sz;
+    if ((res = api.MemSetAccess(at, sz, &access, 1)) != CUDA_SUCCESS) return cu_fail(res, "cuMemSetAccess(index storage)");
+  }
+  return RBK_OK;
+}
+
+// Bytes of each device corpus buffer at capacity `cap` (ix->vm order); 0 for the f64 rows unless they live on the device.
+void storage_at(const rbk_index* ix, int64_t cap, size_t out[rbk_index::kVmBuffers]) {
+  out[0] = static_cast<size_t>(cap) * ix->dpad * 2;
+  out[1] = static_cast<size_t>(inv_norm_len(cap)) * 4;
+  out[2] = static_cast<size_t>(cap) * 8;
+  out[3] = static_cast<size_t>((cap + 31) / 32) * 4;
+  out[4] = ix->keep_f64 && !ix->f64_on_host ? static_cast<size_t>(cap) * ix->dim * 8 : 0;
+}
+
+// Backs every device buffer for `ncap` rows: all of them, or (on failure) none of the chunks this call mapped.
+rbk_status vm_map_capacity(rbk_index* ix, int64_t ncap) {
+  if (ncap > ix->vm_rows)
+    return fail(RBK_ENOMEM, "a capacity of " + std::to_string(ncap) + " rows exceeds the " +
+                                std::to_string(ix->vm_rows) + " this device can hold");
+  size_t want[rbk_index::kVmBuffers], old[rbk_index::kVmBuffers];
+  storage_at(ix, ncap, want);
+  for (int i = 0; i < rbk_index::kVmBuffers; ++i) old[i] = ix->vm[i].mapped;
+  for (int i = 0; i < rbk_index::kVmBuffers; ++i) {
+    rbk_status st = vm_map_to(ix, &ix->vm[i], want[i]);
+    if (st != RBK_OK) {
+      for (int j = 0; j <= i; ++j) vm_unmap_from(&ix->vm[j], old[j]);
+      return st;
+    }
+  }
+  return RBK_OK;
+}
+
+// Reserves the device buffers' address ranges for the largest capacity the device could back.
+rbk_status vm_reserve(rbk_index* ix, size_t total_global_mem) {
+  const VmmApi& api = vmm_api();
+  if (!api.ok) return fail(RBK_ECUDA, "the driver does not provide the CUDA virtual memory management calls");
+  int supported = 0;
+  CUresult res = api.DeviceGetAttribute(&supported, CU_DEVICE_ATTRIBUTE_VIRTUAL_MEMORY_MANAGEMENT_SUPPORTED, ix->device);
+  if (res != CUDA_SUCCESS) return cu_fail(res, "cuDeviceGetAttribute(VIRTUAL_MEMORY_MANAGEMENT_SUPPORTED)");
+  if (!supported)
+    return fail(RBK_ECUDA, "device " + std::to_string(ix->device) +
+                               " does not support CUDA virtual memory management, which the index storage needs");
+  const CUmemAllocationProp prop = vm_prop(ix->device);
+  if ((res = api.MemGetAllocationGranularity(&ix->vm_gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM)) != CUDA_SUCCESS)
+    return cu_fail(res, "cuMemGetAllocationGranularity");
+  // device bytes per row, the tombstone bit rounded up to a byte
+  size_t per_row[rbk_index::kVmBuffers];
+  storage_at(ix, 1, per_row);
+  const int64_t row_bytes = static_cast<int64_t>(per_row[0] + 4 + per_row[2] + 1 + per_row[4]);
+  ix->vm_rows = std::min<int64_t>((1ll << 31) - 2 * kBlockN,
+                                  static_cast<int64_t>(total_global_mem) / row_bytes / kBlockN * kBlockN);
+  size_t bytes[rbk_index::kVmBuffers];
+  storage_at(ix, ix->vm_rows, bytes);
+  for (int i = 0; i < rbk_index::kVmBuffers; ++i) {
+    if (bytes[i] == 0) continue;
+    VmRange& r = ix->vm[i];
+    const size_t len = static_cast<size_t>(round_up(static_cast<int64_t>(bytes[i]), static_cast<int64_t>(ix->vm_gran)));
+    if ((res = api.MemAddressReserve(&r.base, len, 0, 0, 0)) != CUDA_SUCCESS) return cu_fail(res, "cuMemAddressReserve");
+    r.reserved = len;
+  }
+  ix->rows = reinterpret_cast<uint16_t*>(ix->vm[0].base);
+  ix->inv_norm = reinterpret_cast<float*>(ix->vm[1].base);
+  ix->norm2 = reinterpret_cast<double*>(ix->vm[2].base);
+  ix->dead_bits = reinterpret_cast<unsigned int*>(ix->vm[3].base);
+  if (ix->keep_f64 && !ix->f64_on_host) ix->rows_f64 = reinterpret_cast<double*>(ix->vm[4].base);
+  return RBK_OK;
+}
+
+void vm_free(rbk_index* ix) {
+  for (VmRange& r : ix->vm) {
+    vm_unmap_from(&r, 0);
+    if (r.reserved) vmm_api().MemAddressFree(r.base, r.reserved);
+    r = VmRange();
+  }
+}
+
+// RBK_INDEX_F64_ON_HOST: a pinned buffer for `ncap` rows holding the first n_rows rows of the current one, which it
+// replaces (peak: old + new in host RAM).  Synchronises the index stream first, so that every kernel that wrote or read
+// the old rows has finished.
+rbk_status realloc_host_rows(rbk_index* ix, int64_t ncap) {
+  double* r64 = nullptr;
+  // not write-combined: the host reads these rows when the index grows
+  cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&r64), static_cast<size_t>(ncap) * ix->dim * 8,
+                                cudaHostAllocMapped | cudaHostAllocPortable);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaHostAlloc(f64 rows on the host)");
+  void* dp = nullptr;
+  if ((e = cudaHostGetDevicePointer(&dp, r64, 0)) != cudaSuccess || dp != r64) {
+    cudaFreeHost(r64);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaHostGetDevicePointer(f64 rows on the host)");
+    return fail(RBK_ECUDA, "pinned host rows are mapped at another device address (no unified addressing)");
+  }
+  if ((e = cudaStreamSynchronize(ix->stream)) != cudaSuccess) {
+    cudaFreeHost(r64);
+    return cuda_fail(e, "cudaStreamSynchronize");
+  }
+  if (ix->n_rows > 0) memcpy(r64, ix->rows_f64, static_cast<size_t>(ix->n_rows) * ix->dim * 8);
+  if (ix->rows_f64) cudaFreeHost(ix->rows_f64);
+  ix->rows_f64 = r64;
+  return RBK_OK;
+}
+
+// Grows the capacity in place: maps [cap, ncap) of every device buffer and initialises only that region.  Nothing is
+// copied and no pointer moves.
 rbk_status ensure_capacity(rbk_index* ix, int64_t need) {
   if (need <= ix->cap) return RBK_OK;
   if (need >= (1ll << 31) - 2 * kBlockN) return fail(RBK_EINVAL, "an index shard holds at most 2^31 rows");
   // whole 256-row tiles: the corpus tensor maps cover round_up(n_rows, 256) rows, so that no TMA box ever hangs over
   // the end of the tensor (the TMA unit zero-fills out-of-bounds rows one by one - see ensure_query_scratch)
   int64_t ncap = round_up(std::max<int64_t>(need, std::max<int64_t>(ix->cap * 2, 1024)), kBlockN);
-  uint16_t* rows = nullptr;
-  float* inv = nullptr;
-  double* n2 = nullptr;
-  unsigned int* dead = nullptr;
-  double* r64 = nullptr;
-  const size_t dead_words = static_cast<size_t>((ncap + 31) / 32);
-  cudaError_t e;
-  if (ix->keep_f64) {
-    const size_t bytes = static_cast<size_t>(ncap) * ix->dim * 8;
-    if (ix->f64_on_host) {
-      // not write-combined: the host reads these rows when the index grows
-      if ((e = cudaHostAlloc(reinterpret_cast<void**>(&r64), bytes, cudaHostAllocMapped | cudaHostAllocPortable)) !=
-          cudaSuccess)
-        return cuda_fail(e, "cudaHostAlloc(f64 rows on the host)");
-      void* dp = nullptr;
-      if ((e = cudaHostGetDevicePointer(&dp, r64, 0)) != cudaSuccess || dp != r64) {
-        cudaFreeHost(r64);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaHostGetDevicePointer(f64 rows on the host)");
-        return fail(RBK_ECUDA, "pinned host rows are mapped at another device address (no unified addressing)");
-      }
-    } else if ((e = cudaMalloc(reinterpret_cast<void**>(&r64), bytes)) != cudaSuccess) {
-      return cuda_fail(e, "cudaMalloc(f64 sidecar)");
-    }
+  size_t old[rbk_index::kVmBuffers];
+  for (int i = 0; i < rbk_index::kVmBuffers; ++i) old[i] = ix->vm[i].mapped;
+  rbk_status st = vm_map_capacity(ix, ncap);
+  if (st == RBK_ENOMEM && ncap > round_up(need, kBlockN)) {   // the doubled capacity cannot be backed: exactly `need`
+    ncap = round_up(need, kBlockN);
+    st = vm_map_capacity(ix, ncap);
   }
-  auto free_r64 = [&](double* p) {
-    if (ix->f64_on_host) cudaFreeHost(p);
-    else cudaFree(p);
-  };
-  if ((e = cudaMalloc(reinterpret_cast<void**>(&rows), static_cast<size_t>(ncap) * ix->dpad * 2)) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&inv), static_cast<size_t>(inv_norm_len(ncap)) * 4)) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&n2), static_cast<size_t>(ncap) * 8)) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&dead), dead_words * 4)) != cudaSuccess) {
-    cudaFree(rows);
-    cudaFree(inv);
-    cudaFree(n2);
-    cudaFree(dead);
-    free_r64(r64);
-    return cuda_fail(e, "cudaMalloc(index storage)");
+  if (st != RBK_OK) return st;
+  if (ix->f64_on_host && (st = realloc_host_rows(ix, ncap)) != RBK_OK) {
+    for (int i = 0; i < rbk_index::kVmBuffers; ++i) vm_unmap_from(&ix->vm[i], old[i]);
+    return st;
   }
-  cudaStream_t st = ix->stream;
-  CK(cudaMemsetAsync(inv, 0xFF, static_cast<size_t>(inv_norm_len(ncap)) * 4, st));  // all-ones = NaN
-  CK(cudaMemsetAsync(dead, 0, dead_words * 4, st));
+  cudaStream_t s = ix->stream;
+  const int64_t cap = ix->cap;
   // rows not (yet) appended are read by the scan as part of the last tile (their 1/||c|| is NaN: they never match)
-  CK(cudaMemsetAsync(rows + static_cast<size_t>(ix->n_rows) * ix->dpad, 0,
-                     static_cast<size_t>(ncap - ix->n_rows) * ix->dpad * 2, st));
-  if (ix->n_rows > 0) {
-    CK(cudaMemcpyAsync(rows, ix->rows, static_cast<size_t>(ix->n_rows) * ix->dpad * 2, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(inv, ix->inv_norm, static_cast<size_t>(ix->n_rows) * 4, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(n2, ix->norm2, static_cast<size_t>(ix->n_rows) * 8, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dead, ix->dead_bits, static_cast<size_t>((ix->n_rows + 31) / 32) * 4,
-                       cudaMemcpyDeviceToDevice, st));
-    if (r64 && !ix->f64_on_host)
-      CK(cudaMemcpyAsync(r64, ix->rows_f64, static_cast<size_t>(ix->n_rows) * ix->dim * 8, cudaMemcpyDeviceToDevice,
-                         st));
-  }
-  CK(cudaStreamSynchronize(st));
-  // host rows: copied by the host, now that every kernel that wrote or read the old rows has finished
-  if (r64 && ix->f64_on_host && ix->n_rows > 0)
-    memcpy(r64, ix->rows_f64, static_cast<size_t>(ix->n_rows) * ix->dim * 8);
-  cudaFree(ix->rows);
-  cudaFree(ix->inv_norm);
-  cudaFree(ix->norm2);
-  cudaFree(ix->dead_bits);
-  free_r64(ix->rows_f64);
-  ix->rows_f64 = r64;
-  ix->rows = rows;
-  ix->inv_norm = inv;
-  ix->norm2 = n2;
-  ix->dead_bits = dead;
+  CK(cudaMemsetAsync(ix->rows + static_cast<size_t>(cap) * ix->dpad, 0, static_cast<size_t>(ncap - cap) * ix->dpad * 2, s));
+  CK(cudaMemsetAsync(ix->inv_norm + cap, 0xFF, static_cast<size_t>(inv_norm_len(ncap) - cap) * 4, s));   // all-ones = NaN
+  CK(cudaMemsetAsync(ix->dead_bits + cap / 32, 0, static_cast<size_t>(ncap - cap) / 32 * 4, s));   // cap, ncap: x256
   ix->cap = ncap;
   return RBK_OK;
 }
@@ -260,10 +411,9 @@ int pick_kprime(const rbk_index* ix, int k_fetch) {
 
 rbk_status refresh_corpus_tmap(rbk_index* ix) {
   const int64_t map_rows = round_up(ix->n_rows, kBlockN);   // whole tiles (<= cap): no out-of-bounds box rows
-  if (ix->tmap_c_base == ix->rows && ix->tmap_c_rows == map_rows) return RBK_OK;
+  if (ix->tmap_c_rows == map_rows) return RBK_OK;
   rbk_status st = encode_rows_tmap(&ix->tmap_c, ix->rows, map_rows, ix->dpad, kBlockN);
   if (st != RBK_OK) return st;
-  ix->tmap_c_base = ix->rows;
   ix->tmap_c_rows = map_rows;
   return RBK_OK;
 }
@@ -725,6 +875,52 @@ void drop_graph(rbk_index* ix) {
   ix->graph_exec = nullptr;
 }
 
+// Every grow-only scratch buffer (each is re-grown on demand by the next call that needs it) and the captured graph,
+// which bakes in their pointers.  The stream must be idle.
+void release_scratch(rbk_index* ix) {
+  drop_graph(ix);
+  ix->stage.release();
+  ix->d_slots.release();
+  ix->cp_map.release();
+  ix->cp_scan.release();
+  ix->q_raw.release();
+  ix->q_bf16.release();
+  ix->q_f64.release();
+  ix->q_norm2.release();
+  ix->q_eps.release();
+  ix->q_inv_norm.release();
+  ix->thr_init.release();
+  ix->cand.release();
+  ix->cand_cnt.release();
+  ix->hist.release();
+  ix->flags.release();
+  ix->fail_list.release();
+  ix->part_rows.release();
+  ix->part_cnt.release();
+  ix->o_scores.release();
+  ix->part_scores.release();
+  ix->dbg.release();
+  ix->lg_theta.release();
+  ix->lg_cap.release();
+  ix->lg_cnt.release();
+  ix->lg_rows.release();
+  ix->lg_err.release();
+  ix->lg_off.release();
+  ix->lg_scores.release();
+  ix->h_lcap.release();
+  ix->h_lerr.release();
+  ix->h_loff.release();
+  ix->ub_toff.release();
+  ix->ub_rows.release();
+  ix->ub_len.release();
+  ix->ub_scores.release();
+  ix->h_utoff.release();
+  ix->o_block.release();
+  ix->h_block.release();
+  ix->h_flags.release();
+  ix->h_q.release();
+}
+
 // Small-batch fast path of search_core (caller holds the lock; scratch, o_block and h_block are allocated): replay
 // - or first capture - the graph of one whole search.  *done = true: results and flags are in h_block and every
 // query is proven exact.  *done = false: something needs the general path (a query's proof failed), which the
@@ -981,7 +1177,8 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
     rbk_index_destroy(ix);
     return cuda_fail(e, "cudaMalloc");
   }
-  rbk_status st = ensure_capacity(ix, std::max<int64_t>(capacity_hint, 1024));
+  rbk_status st = vm_reserve(ix, prop.totalGlobalMem);
+  if (st == RBK_OK) st = ensure_capacity(ix, std::max<int64_t>(capacity_hint, 1024));
   if (st != RBK_OK) {
     rbk_index_destroy(ix);
     return st;
@@ -995,54 +1192,10 @@ void rbk_index_destroy(rbk_index* ix) {
   {
     DeviceGuard dg(ix->device);
     if (ix->stream) cudaStreamSynchronize(ix->stream);
-    cudaFree(ix->rows);
-    cudaFree(ix->inv_norm);
-    cudaFree(ix->norm2);
-    cudaFree(ix->dead_bits);
+    vm_free(ix);
     if (ix->f64_on_host) cudaFreeHost(ix->rows_f64);
-    else cudaFree(ix->rows_f64);
     cudaFree(ix->d_counter);
-    ix->stage.release();
-    ix->d_slots.release();
-    ix->cp_map.release();
-    ix->cp_scan.release();
-    ix->q_raw.release();
-    ix->q_bf16.release();
-    ix->q_f64.release();
-    ix->q_norm2.release();
-    ix->q_eps.release();
-    ix->q_inv_norm.release();
-    ix->thr_init.release();
-    ix->cand.release();
-    ix->cand_cnt.release();
-    ix->hist.release();
-    ix->flags.release();
-    ix->fail_list.release();
-    ix->part_rows.release();
-    ix->part_cnt.release();
-    ix->o_scores.release();
-    ix->part_scores.release();
-    ix->dbg.release();
-    ix->lg_theta.release();
-    ix->lg_cap.release();
-    ix->lg_cnt.release();
-    ix->lg_rows.release();
-    ix->lg_err.release();
-    ix->lg_off.release();
-    ix->lg_scores.release();
-    ix->h_lcap.release();
-    ix->h_lerr.release();
-    ix->h_loff.release();
-    ix->ub_toff.release();
-    ix->ub_rows.release();
-    ix->ub_len.release();
-    ix->ub_scores.release();
-    ix->h_utoff.release();
-    ix->o_block.release();
-    ix->h_block.release();
-    ix->h_flags.release();
-    drop_graph(ix);
-    ix->h_q.release();
+    release_scratch(ix);
     if (ix->ev_start) cudaEventDestroy(ix->ev_start);
     if (ix->ev_stop) cudaEventDestroy(ix->ev_stop);
     for (auto& pr : ix->tev)
@@ -1257,18 +1410,42 @@ rbk_status rbk_index_compact(rbk_index* ix, int64_t* old_to_new, int64_t old_to_
   return RBK_OK;
 }
 
+rbk_status rbk_index_trim(rbk_index* ix) {
+  if (!ix) return fail(RBK_EINVAL, "null index");
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  CK(cudaStreamSynchronize(ix->stream));   // searches enqueued earlier finish before anything they read goes away
+  // the capacity of a new index holding size() rows; rows, 1/||c|| (NaN), norm2 and tombstone bits beyond size() are
+  // never-appended rows already, so nothing below the new capacity changes
+  const int64_t tcap = round_up(std::max<int64_t>(ix->n_rows, 1024), kBlockN);
+  if (tcap < ix->cap) {
+    if (ix->f64_on_host) {
+      rbk_status st = realloc_host_rows(ix, tcap);
+      if (st != RBK_OK) return st;
+    }
+    size_t keep[rbk_index::kVmBuffers];
+    storage_at(ix, tcap, keep);
+    for (int i = 0; i < rbk_index::kVmBuffers; ++i) vm_unmap_from(&ix->vm[i], keep[i]);
+    ix->cap = tcap;
+  }
+  release_scratch(ix);
+  ix->tmap_c_rows = -1;
+  return RBK_OK;
+}
+
 int64_t rbk_index_count(const rbk_index* ix) { return ix ? ix->n_live : 0; }
 int64_t rbk_index_size(const rbk_index* ix) { return ix ? ix->n_rows : 0; }
 int32_t rbk_index_dim(const rbk_index* ix) { return ix ? ix->dim : 0; }
 
 rbk_status rbk_index_storage_bytes(const rbk_index* ix, int64_t* device_bytes, int64_t* pinned_host_bytes) {
   if (!ix) return fail(RBK_EINVAL, "null index");
-  // the allocations of ensure_capacity: rows | inv_norm | norm2 | dead_bits | f64 rows
-  const int64_t cap = ix->cap;
-  const int64_t f64 = ix->keep_f64 ? cap * ix->dim * 8 : 0;
-  const int64_t dev = cap * ix->dpad * 2 + inv_norm_len(cap) * 4 + cap * 8 + (cap + 31) / 32 * 4;
-  if (device_bytes) *device_bytes = dev + (ix->f64_on_host ? 0 : f64);
-  if (pinned_host_bytes) *pinned_host_bytes = ix->f64_on_host ? f64 : 0;
+  // the buffers of ensure_capacity: rows | inv_norm | norm2 | dead_bits | f64 rows
+  size_t bytes[rbk_index::kVmBuffers];
+  storage_at(ix, ix->cap, bytes);
+  int64_t dev = 0;
+  for (size_t b : bytes) dev += static_cast<int64_t>(b);
+  if (device_bytes) *device_bytes = dev;
+  if (pinned_host_bytes) *pinned_host_bytes = ix->f64_on_host ? ix->cap * ix->dim * 8 : 0;
   return RBK_OK;
 }
 

@@ -552,6 +552,26 @@ rbk_status rbk_group_clear(rbk_group* g) {
   return RBK_OK;
 }
 
+rbk_status rbk_group_trim(rbk_group* g) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  std::lock_guard<std::mutex> lk(g->mu);
+  for (rbk_index* ix : g->parts) {   // synchronises each member's stream, which the group's searches run on
+    rbk_status st = rbk_index_trim(ix);
+    if (st != RBK_OK) return st;
+  }
+  for (size_t d = 0; d < g->parts.size(); ++d) {
+    DeviceGuard dg(g->devices[d]);
+    g->dev[d].q.release();
+    g->dev[d].local.release();
+    g->dev[d].all.release();
+  }
+  DeviceGuard dg(g->devices[0]);
+  g->out.release();
+  g->h_out.release();
+  g->h_q.release();
+  return RBK_OK;
+}
+
 int64_t rbk_group_count(const rbk_group* g) {
   int64_t n = 0;
   if (g)

@@ -62,6 +62,19 @@ struct PinBuf {
   }
 };
 
+// One device corpus buffer on a reserved virtual address range (CUDA virtual memory management).  Physical chunks
+// are mapped from `base` on as the index grows and unmapped from the end by rbk_index_trim, so `base` never moves and
+// a growth copies nothing.
+struct VmRange {
+  struct Chunk {
+    CUmemGenericAllocationHandle handle;
+    size_t bytes;
+  };
+  CUdeviceptr base = 0;
+  size_t reserved = 0, mapped = 0;   // [base, base + mapped) is backed
+  std::vector<Chunk> chunks;         // in address order from base
+};
+
 struct DeviceGuard {
   int prev = -1;
   explicit DeviceGuard(int dev) {
@@ -118,6 +131,12 @@ struct rbk_index {
   int dim = 0, dpad = 0, device = 0, sm_count = 0, margin = 16;
   int64_t cap = 0, n_rows = 0, n_live = 0;
   rbk::SlotLayout slot;      // local row -> global slot (rbk_index_set_slot_base; block-cyclic inside a group)
+  // The device corpus buffers - rows | inv_norm | norm2 | dead_bits | f64 rows (device tier) - each on its own reserved
+  // range, sized for vm_rows rows (the most the device could back); the pointers below are the ranges' bases.
+  static constexpr int kVmBuffers = 5;
+  rbk::impl::VmRange vm[kVmBuffers];
+  int64_t vm_rows = 0;
+  size_t vm_gran = 0;        // allocation granularity of the device
   uint16_t* rows = nullptr;
   float* inv_norm = nullptr;  // padded to a multiple of kBlockN (+ one tile), NaN-filled
   double* norm2 = nullptr;
@@ -163,8 +182,7 @@ struct rbk_index {
   CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
-  const void* tmap_c_base = nullptr;
-  int64_t tmap_c_rows = -1;
+  int64_t tmap_c_rows = -1;   // rows the corpus map covers (-1: none); its base, `rows`, never moves
   cudaEvent_t ev_start = nullptr, ev_stop = nullptr;   // device time of a whole synchronous search
   // scan-kernel timing without a host sync per search: (start, stop) event pairs are resolved lazily
   // (rbk_index_stats, or when the ring wraps) into stats.scan_ms_total / stats.scans_timed

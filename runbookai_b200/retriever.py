@@ -81,7 +81,9 @@ class KnowledgeRetriever:
     def _reclaim(self) -> None:
         """Every mirrored update tombstones the document's old chunks, so a long-running process would otherwise
         keep their device memory and scan time for good.  Once the dead slots reach a quarter of all slots (and at
-        least _COMPACT_MIN_DEAD - below that they cost less than the call) the vector store is compacted."""
+        least _COMPACT_MIN_DEAD - below that they cost less than the call) the vector store is compacted, then
+        trimmed, so the freed slots' device memory goes back too (growing again later maps memory, it copies
+        nothing)."""
         vs = self.vector_store
         ix = vs._index if vs is not None else None
         if ix is None or getattr(ix, "compact", None) is None:
@@ -90,6 +92,7 @@ class KnowledgeRetriever:
         dead = size - ix.count()
         if dead >= _COMPACT_MIN_DEAD and 4 * dead >= size:
             vs.compact()
+            vs.trim()
 
     def _mirror(self, doc: dict) -> None:
         vs = self.vector_store

@@ -496,6 +496,15 @@ class VectorStore:
             self._ids[:] = ids
             return before - ix.size()
 
+    def trim(self) -> None:
+        """Give the device memory of reclaimed slots back: the index's capacity drops to what its rows need and its
+        scratch buffers are released (after compact() or clear()).  No slot moves and no answer changes.  An index
+        without `trim` is left as it is.  Holds the state lock, like compact()."""
+        with self._st.lock:
+            fn = getattr(self._index, "trim", None)
+            if fn is not None:
+                fn()
+
     def get_count(self) -> int:
         """vector-store.ts:302-307."""
         return self.db.execute("SELECT COUNT(*) as count FROM vector_embeddings").fetchone()["count"]

@@ -226,6 +226,15 @@ export class GpuEmbeddingIndex {
     }
   }
 
+  /**
+   * Give unused device memory back (after compact() or clear()): the capacity drops to what the rows need and the
+   * scratch buffers are released.  No slot moves, so searches in flight need no waiting; the native call waits for
+   * the index's queued device work itself.
+   */
+  trim(): void {
+    this.index?.trim();
+  }
+
   private remember(id: string, slot: number): void {
     this.slotOfId.set(id, slot);
     this.idOfSlot[slot] = id;
