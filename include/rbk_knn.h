@@ -110,7 +110,9 @@ rbk_status rbk_index_set_slot_base(rbk_index* idx, int64_t slot_base);
 rbk_status rbk_index_append_f64(rbk_index* idx, const double* rows, int64_t n_rows, int64_t* first_slot_out);
 rbk_status rbk_index_append_f32(rbk_index* idx, const float* rows, int64_t n_rows, int64_t* first_slot_out);
 rbk_status rbk_index_append_bf16(rbk_index* idx, const uint16_t* rows, int64_t n_rows, int64_t* first_slot_out);
-/* Same, rows already in device memory on the index's GPU (bulk load without a PCIe hop). */
+/* Same, rows already in device memory on the index's GPU (bulk load without a PCIe hop).  The rows are read on the
+ * index's stream, which is not ordered after any other stream: work that writes them on another stream (a framework's
+ * current stream, say) must be complete, or that stream must be the index's (rbk_index_set_stream), before the call. */
 rbk_status rbk_index_append_bf16_device(rbk_index* idx, const void* dev_rows, int64_t n_rows,
                                         int64_t* first_slot_out);
 /* f64 rows (the BLOB layout) already on the device, e.g. a sidecar file read with GPUDirect or staged by the host

@@ -1122,6 +1122,16 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
 
 }  // namespace
 
+namespace rbk {
+namespace impl {
+rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, int k_fetch, double min_score,
+                               long long* d_slots, double* d_scores, int* d_counts) {
+  return search_core(ix, nullptr, d_q, elem, B, ix ? ix->dim : 0, k_fetch, min_score, d_slots, d_scores, d_counts,
+                     nullptr, nullptr, nullptr, nullptr);
+}
+}  // namespace impl
+}  // namespace rbk
+
 // =========================================================================== C ABI
 extern "C" {
 

@@ -245,8 +245,9 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
     g->redone_batches++;
     for (int d = 0; d < g->G; ++d) {
       unsigned char* l = g->dev[d].local.p;
-      st = rbk_index_search_device(g->parts[d], g->dev[d].q.p, B, k_fetch, min_score, L.slots(l), L.scores(l),
-                                   L.counts(l));
+      // the staged queries keep the caller's type: f64 ones must not be read as f32
+      st = search_device_exact(g->parts[d], g->dev[d].q.p, elem, B, k_fetch, min_score, L.slots(l), L.scores(l),
+                               L.counts(l));
       if (st != RBK_OK) return st;
       DeviceGuard dg(g->parts[d]->device);
       CK(cudaMemsetAsync(L.flags(l), 0, static_cast<size_t>(B) * 4, g->parts[d]->stream));   // exact by construction

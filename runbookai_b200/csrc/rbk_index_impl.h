@@ -222,6 +222,10 @@ rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, i
 // Enqueue-only search of device-resident queries: no host synchronisation, exactness flags land in d_flags.
 rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, int k_fetch, double min_score,
                           long long* d_slots, double* d_scores, int* d_counts, int* d_flags);
+// Synchronous exact search of device-resident queries of `elem` bytes (8 = f64, 4 = f32), retry and exhaustive
+// fallback included: rbk_index_search_device for either query type.  Takes the index lock itself.
+rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, int k_fetch, double min_score,
+                               long long* d_slots, double* d_scores, int* d_counts);
 // Large-k search of B device-resident f64 queries (caller holds the lock, scratch for B queries is allocated), in
 // two halves around one host synchronisation of the index stream:
 //   large_count: prep, count pass and select per sub-batch, then the D2H of C_q (enqueue only);
