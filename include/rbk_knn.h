@@ -90,6 +90,16 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * or copy on the index stream, or the host after a synchronisation), so searches enqueued earlier never see a
  * half-written row.  The placement is fixed for the index's life. */
 #define RBK_INDEX_F64_ON_HOST 2u
+/* RBK_INDEX_SCAN_F16 (only together with RBK_INDEX_KEEP_F64, else RBK_EINVAL; combines with RBK_INDEX_F64_ON_HOST):
+ * the scan reads fp16 rows instead of bf16, at the same 2 bytes per element.  Each row x (and each query) is stored
+ * scaled by its own power of two, h_i = RNE_f16(x_i * 2^e) with e = 15 - E, E the frexp exponent of max |x_i| over the
+ * finite elements (so max|x| * 2^e is in [2^14, 2^15)); results that would be subnormal are stored as signed zeros.
+ * fp16 keeps 11 significant bits against bf16's 8, so the scan's error bound - whose rounding terms are the angles
+ * between a row or query and its stored copy - is several times tighter (DESIGN.md §6): fewer batches need the wide
+ * retry, and the large-k search emits fewer candidates.  Answers are those of a KEEP_F64 index without the flag: the
+ * same slots and fp64 scores, bit for bit.  The placement is fixed for the index's life; read the stored bits with
+ * rbk_index_read_rows_f16. */
+#define RBK_INDEX_SCAN_F16 16u
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out);
 void rbk_index_destroy(rbk_index* idx); /* NULL is a no-op */
 
@@ -159,8 +169,10 @@ int32_t rbk_index_dim(const rbk_index* idx);
  * float64 rows (KEEP_F64), split by where they live.  Search and compaction scratch are not counted.  Either output
  * may be NULL. */
 rbk_status rbk_index_storage_bytes(const rbk_index* idx, int64_t* device_bytes, int64_t* pinned_host_bytes);
-/* Copy stored rows back (bf16 bits), for tests and for reload sidecars. */
+/* Copy stored rows back (bf16 bits), for tests and for reload sidecars.  RBK_EINVAL on an RBK_INDEX_SCAN_F16 index. */
 rbk_status rbk_index_read_rows_bf16(rbk_index* idx, int64_t first_local_slot, int64_t n_rows, uint16_t* out);
+/* The same for an RBK_INDEX_SCAN_F16 index: the stored, scaled fp16 bits (RBK_EINVAL on any other index). */
+rbk_status rbk_index_read_rows_f16(rbk_index* idx, int64_t first_local_slot, int64_t n_rows, uint16_t* out);
 
 /* ---- search: the scan + sort + cut of VectorStore.search (vector-store.ts:207-221)
  *      and findMostSimilar (embedder.ts:189-202), batched over B queries ---- */
@@ -263,7 +275,8 @@ rbk_status rbk_merge_topk_packed_device(int32_t device, void* cuda_stream, int32
  * and error conventions are those of the rbk_index_* call of the same name. */
 typedef struct rbk_group rbk_group;
 rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_devices, int64_t capacity_hint,
-                            uint32_t flags /* RBK_INDEX_KEEP_F64 [| RBK_INDEX_F64_ON_HOST]: every member */,
+                            uint32_t flags /* RBK_INDEX_KEEP_F64 [| RBK_INDEX_F64_ON_HOST] [| RBK_INDEX_SCAN_F16]:
+                                              every member */,
                             rbk_group** out);
 void rbk_group_destroy(rbk_group* grp); /* NULL is a no-op */
 rbk_status rbk_group_append_f64(rbk_group* grp, const double* rows, int64_t n_rows, int64_t* first_slot_out);

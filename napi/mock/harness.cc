@@ -128,12 +128,16 @@ int main(int argc, char** argv) {
     for (int d : devs) e.push_back(mock::number(env, d));
     dev_arg = mock::array(env, e);
   }
-  // optional host_rows.txt: the constructor's 4th argument (hostRows: float64 rows in pinned host memory)
+  // optional host_rows.txt: the constructor's 4th argument (hostRows: float64 rows in pinned host memory);
+  // optional scan_f16.txt: its 5th (scanF16: the scan reads fp16 rows), with hostRows 0 unless host_rows.txt says
   std::vector<napi_value> ctor_args = {mock::number(env, dim), dev_arg, mock::number(env, n_rows)};
   {
-    std::ifstream hf(g_dir + "/host_rows.txt");
-    int host_rows = 0;
-    if (hf >> host_rows) ctor_args.push_back(mock::number(env, host_rows));
+    std::ifstream hf(g_dir + "/host_rows.txt"), sf(g_dir + "/scan_f16.txt");
+    int host_rows = 0, scan_f16 = 0;
+    const bool have_host = static_cast<bool>(hf >> host_rows);
+    const bool have_f16 = static_cast<bool>(sf >> scan_f16);
+    if (have_host || have_f16) ctor_args.push_back(mock::number(env, host_rows));
+    if (have_f16) ctor_args.push_back(mock::number(env, scan_f16));
   }
   napi_value ix = nullptr;
   if (!mock::construct(env, cls, ctor_args, &ix, &err)) {

@@ -121,21 +121,24 @@ void finalize_index(napi_env, void* data, void*) {
 }
 
 napi_value New(napi_env env, napi_callback_info info) {
-  size_t argc = 4;
-  napi_value argv[4], self;
+  size_t argc = 5;
+  napi_value argv[5], self;
   NAPI_OK(napi_get_cb_info(env, info, &argc, argv, &self, nullptr));
-  int32_t dim = 0, device = 0, host_rows = 0;
+  int32_t dim = 0, device = 0, host_rows = 0, scan_f16 = 0;
   int64_t hint = 0;
   NAPI_OK(napi_get_value_int32(env, argv[0], &dim));
   if (argc > 2) napi_get_value_int64(env, argv[2], &hint);
   if (argc > 3) napi_get_value_int32(env, argv[3], &host_rows);
+  if (argc > 4) napi_get_value_int32(env, argv[4], &scan_f16);
   Handle* h = new Handle();
   h->dim = dim;
   bool is_array = false;
   if (argc > 1) napi_is_array(env, argv[1], &is_array);
   // KEEP_F64: the reference stores float64 embeddings; keep them so results are exact for any input.  hostRows
   // (RUNBOOK_KNN_F64_ON_HOST in ts/gpu-embedding-index.ts): keep them in pinned host memory instead of on the GPU.
-  const uint32_t flags = RBK_INDEX_KEEP_F64 | (host_rows != 0 ? RBK_INDEX_F64_ON_HOST : 0u);
+  // scanF16 (RUNBOOK_KNN_SCAN_F16): the scan reads per-row scaled fp16 rows instead of bf16 (same answers).
+  const uint32_t flags = RBK_INDEX_KEEP_F64 | (host_rows != 0 ? RBK_INDEX_F64_ON_HOST : 0u) |
+                         (scan_f16 != 0 ? RBK_INDEX_SCAN_F16 : 0u);
   rbk_status st;
   if (is_array) {   // [0, 1, ...]: the corpus sharded over these GPUs, one call per search (rbk_group_*)
     uint32_t n = 0;

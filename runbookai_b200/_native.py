@@ -17,13 +17,14 @@ RBK_MAX_K_FETCH = 112
 RBK_MAX_K_FETCH_LARGE = 4096
 RBK_INDEX_KEEP_F64 = 1
 RBK_INDEX_F64_ON_HOST = 2
+RBK_INDEX_SCAN_F16 = 16
 
 # every symbol include/rbk_knn.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "rbk_abi_version", "rbk_last_error", "rbk_index_create", "rbk_index_create_ex", "rbk_index_destroy", "rbk_index_set_stream",
     "rbk_index_set_slot_base", "rbk_index_append_f64", "rbk_index_append_f32", "rbk_index_append_bf16",
     "rbk_index_append_bf16_device", "rbk_index_append_f64_device", "rbk_index_overwrite_f64", "rbk_index_overwrite_f64_batch", "rbk_index_tombstone", "rbk_index_compact", "rbk_index_clear", "rbk_index_trim",
-    "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_storage_bytes", "rbk_index_read_rows_bf16", "rbk_index_search_f64",
+    "rbk_index_count", "rbk_index_size", "rbk_index_dim", "rbk_index_storage_bytes", "rbk_index_read_rows_bf16", "rbk_index_read_rows_f16", "rbk_index_search_f64",
     "rbk_index_search_f32", "rbk_index_search_large_f64", "rbk_index_search_unbounded_f64", "rbk_index_exact_scores_f64", "rbk_index_search_device", "rbk_index_search_device_async", "rbk_merge_topk_device",
     "rbk_packed_block_bytes", "rbk_packed_flags_offset",
     "rbk_merge_topk_packed_device", "rbk_index_stats",
@@ -86,6 +87,7 @@ def _load() -> C.CDLL:
     lib.rbk_index_dim.restype = i32
     lib.rbk_index_storage_bytes.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     lib.rbk_index_read_rows_bf16.argtypes = [vp, i64, i64, vp]
+    lib.rbk_index_read_rows_f16.argtypes = [vp, i64, i64, vp]
     for n in ("rbk_index_search_f64", "rbk_index_search_f32", "rbk_index_search_large_f64",
               "rbk_index_search_unbounded_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
@@ -138,9 +140,10 @@ def ptr(a: np.ndarray | None):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
-def _index_flags(keep_f64: bool, f64_on_host: bool) -> int:
-    """f64_on_host without keep_f64 is passed through: the library rejects it with its own message."""
-    return (RBK_INDEX_KEEP_F64 if keep_f64 else 0) | (RBK_INDEX_F64_ON_HOST if f64_on_host else 0)
+def _index_flags(keep_f64: bool, f64_on_host: bool, scan_f16: bool = False) -> int:
+    """f64_on_host or scan_f16 without keep_f64 is passed through: the library rejects it with its own message."""
+    return ((RBK_INDEX_KEEP_F64 if keep_f64 else 0) | (RBK_INDEX_F64_ON_HOST if f64_on_host else 0)
+            | (RBK_INDEX_SCAN_F16 if scan_f16 else 0))
 
 
 def _search_large(fn, h, queries, k_fetch: int, min_score):
@@ -190,13 +193,16 @@ class Index:
     """Thin object wrapper over rbk_index* (one GPU shard)."""
 
     def __init__(self, dim: int, device: int = 0, capacity_hint: int = 0, keep_f64: bool = False,
-                 f64_on_host: bool = False):
+                 f64_on_host: bool = False, scan_f16: bool = False):
         """keep_f64: RBK_INDEX_KEEP_F64 — exact for arbitrary float64 rows at 8*dim extra bytes per row.
         f64_on_host: RBK_INDEX_F64_ON_HOST — those float64 rows live in pinned host memory instead of on the GPU (same
-        answers; the re-rank reads them over PCIe).  Requires keep_f64."""
+        answers; the re-rank reads them over PCIe).  Requires keep_f64.
+        scan_f16: RBK_INDEX_SCAN_F16 — the scan reads per-row scaled fp16 rows instead of bf16 (same bytes, same
+        answers, a several times tighter error bound, so fewer wide retries).  Requires keep_f64."""
         self._h = None
         h = C.c_void_p()
-        check(lib.rbk_index_create_ex(dim, device, capacity_hint, _index_flags(keep_f64, f64_on_host), C.byref(h)))
+        check(lib.rbk_index_create_ex(dim, device, capacity_hint, _index_flags(keep_f64, f64_on_host, scan_f16),
+                                      C.byref(h)))
         self._h = h
         self.dim = dim
         self.device = device
@@ -299,6 +305,12 @@ class Index:
         check(lib.rbk_index_read_rows_bf16(self._h, first, n, ptr(out)))
         return out
 
+    def read_rows_f16(self, first: int, n: int) -> np.ndarray:
+        """The stored fp16 bits of a scan_f16 index (each row scaled by its own power of two)."""
+        out = np.empty((n, self.dim), dtype=np.uint16)
+        check(lib.rbk_index_read_rows_f16(self._h, first, n, ptr(out)))
+        return out
+
     # -- search
     def search(self, queries, k_fetch: int, min_score: float | None = 0.5):
         """Returns (slots int64 [B,k], scores float64 [B,k], counts int32 [B], device_ms)."""
@@ -371,13 +383,15 @@ class Group:
     """rbk_group*: one corpus sharded over several GPUs behind one handle; the Index surface with GLOBAL slots.
     Every search is one C call: per-GPU scans, one NCCL all-gather, merge on devices[0], one synchronisation."""
 
-    def __init__(self, dim: int, devices, capacity_hint: int = 0, keep_f64: bool = False, f64_on_host: bool = False):
-        """f64_on_host: every member keeps its float64 rows in its own pinned host buffer (see Index)."""
+    def __init__(self, dim: int, devices, capacity_hint: int = 0, keep_f64: bool = False, f64_on_host: bool = False,
+                 scan_f16: bool = False):
+        """f64_on_host: every member keeps its float64 rows in its own pinned host buffer (see Index).
+        scan_f16: every member scans fp16 rows (see Index)."""
         self._h = None
         devs = np.ascontiguousarray(list(devices), dtype=np.int32)
         h = C.c_void_p()
-        check(lib.rbk_group_create(dim, ptr(devs), devs.shape[0], capacity_hint, _index_flags(keep_f64, f64_on_host),
-                                   C.byref(h)))
+        check(lib.rbk_group_create(dim, ptr(devs), devs.shape[0], capacity_hint,
+                                   _index_flags(keep_f64, f64_on_host, scan_f16), C.byref(h)))
         self._h = h
         self.dim = dim
         self.devices = [int(d) for d in devs]

@@ -54,9 +54,9 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2D bf16 row-major [rows][dpad] tensor, box = box_cols columns (one swizzle row: 64 -> 128 B, 32 -> 64 B)
+// 2D bf16 (f16: fp16) row-major [rows][dpad] tensor, box = box_cols columns (one swizzle row: 64 -> 128 B, 32 -> 64 B)
 // x box_rows.
-rbk_status encode_rows_tmap(CUtensorMap* out, const void* base, int64_t rows, int dpad, int box_rows,
+rbk_status encode_rows_tmap(CUtensorMap* out, const void* base, int64_t rows, int dpad, int box_rows, bool f16,
                             int box_cols = kBlockK) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail(RBK_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
@@ -64,7 +64,7 @@ rbk_status encode_rows_tmap(CUtensorMap* out, const void* base, int64_t rows, in
   cuuint64_t gstride[1] = {static_cast<cuuint64_t>(dpad) * 2};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+  CUresult r = fn(out, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE,
                   box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
                                  : (box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE),
@@ -372,7 +372,8 @@ rbk_status append_rows(rbk_index* ix, const void* src, bool is_device, int elem,
     if (elem == 2 && ix->dpad == ix->dim && !ix->keep_f64) {
       CK(cudaMemcpyAsync(dst0, src, static_cast<size_t>(n) * ix->dim * 2, cudaMemcpyDeviceToDevice, ix->stream));
     } else {
-      CK(launch_convert_rows(src, src_type, n, ix->dim, ix->dpad, dst0, dst64, ix->stream));
+      CK(launch_convert_rows(src, src_type, n, ix->dim, ix->dpad, dst0, dst64, ix->stream, nullptr, nullptr, nullptr,
+                             ix->scan_f16));
       ix->stats.kernel_launches++;
     }
   } else {
@@ -384,14 +385,15 @@ rbk_status append_rows(rbk_index* ix, const void* src, bool is_device, int elem,
       const unsigned char* hp = static_cast<const unsigned char*>(src) + static_cast<size_t>(r0) * row_bytes;
       CK(cudaMemcpyAsync(ix->stage.p, hp, static_cast<size_t>(nr) * row_bytes, cudaMemcpyHostToDevice, ix->stream));
       CK(launch_convert_rows(ix->stage.p, src_type, nr, ix->dim, ix->dpad, dst0 + static_cast<size_t>(r0) * ix->dpad,
-                             dst64 ? dst64 + static_cast<size_t>(r0) * ix->dim : nullptr, ix->stream));
+                             dst64 ? dst64 + static_cast<size_t>(r0) * ix->dim : nullptr, ix->stream, nullptr, nullptr,
+                             nullptr, ix->scan_f16));
       ix->stats.kernel_launches++;
       // the staging buffer is reused by the next chunk; pageable H2D copies are already
       // synchronous with respect to the host buffer, the kernel is ordered by the stream
     }
   }
   CK(launch_row_norms(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, ix->n_rows, n, ix->dim, ix->dpad, ix->inv_norm,
-                      ix->norm2, ix->d_counter + 1, ix->stream));
+                      ix->norm2, ix->d_counter + 1, ix->stream, nullptr, nullptr, ix->scan_f16));
   ix->stats.kernel_launches += ix->keep_f64 ? 2 : 1;
   // Host sources: pageable H2D copies have consumed the caller's buffer when cudaMemcpyAsync returns and everything
   // after is stream-ordered, so an append costs no host round trip.  Device sources are read by the copy/convert
@@ -412,7 +414,7 @@ int pick_kprime(const rbk_index* ix, int k_fetch) {
 rbk_status refresh_corpus_tmap(rbk_index* ix) {
   const int64_t map_rows = round_up(ix->n_rows, kBlockN);   // whole tiles (<= cap): no out-of-bounds box rows
   if (ix->tmap_c_rows == map_rows) return RBK_OK;
-  rbk_status st = encode_rows_tmap(&ix->tmap_c, ix->rows, map_rows, ix->dpad, kBlockN);
+  rbk_status st = encode_rows_tmap(&ix->tmap_c, ix->rows, map_rows, ix->dpad, kBlockN, ix->scan_f16);
   if (st != RBK_OK) return st;
   ix->tmap_c_rows = map_rows;
   return RBK_OK;
@@ -475,7 +477,7 @@ rbk_status prep_queries(rbk_index* ix, const void* d_q, int src_type, int B, dou
   CK(launch_prep_queries(d_q, src_type, B, ix->dim, ix->dpad, min_score,
                          ix->keep_f64 ? reinterpret_cast<const float*>(ix->d_counter + 1) : nullptr,
                          query_buffers(ix, 0), ix->stream, with_norm2, ix->hist.p, std::min(kMaxSubBatch, B),
-                         progress_slots(ix)));
+                         progress_slots(ix), ix->scan_f16));
   ix->stats.kernel_launches++;
   return RBK_OK;
 }
@@ -489,12 +491,16 @@ rbk_status launch_sub_batch(rbk_index* ix, int q0, const P& sp) {
   // every row the map covers must lie inside the query buffer: the scan's TMA loads whole boxes
   if ((static_cast<size_t>(q0) + q_rows) * ix->dpad > ix->q_bf16.n)
     return fail(RBK_ECUDA, "scan launch at query " + std::to_string(q0) + " would read past the query buffer");
-  rbk_status st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM);
+  rbk_status st = encode_rows_tmap(&tmap_q, ix->q_bf16.p + static_cast<size_t>(q0) * ix->dpad, q_rows, ix->dpad, kBlockM,
+                                   ix->scan_f16);
   if (st != RBK_OK) return st;
   cudaEvent_t* tev = ix->capturing ? nullptr : next_scan_events(ix);
   if (tev) CK(cudaEventRecord(tev[0], ix->stream));
-  if constexpr (kMode == 0) CK(launch_scan(tmap_q, ix->tmap_c, sp, ix->stream));
-  else CK(launch_scan_large(tmap_q, ix->tmap_c, sp, static_cast<LargeScanMode>(kMode), ix->stream));
+  if constexpr (kMode == 0)
+    CK((ix->scan_f16 ? launch_scan_f16 : launch_scan)(tmap_q, ix->tmap_c, sp, ix->stream));
+  else
+    CK((ix->scan_f16 ? launch_scan_large_f16 : launch_scan_large)(tmap_q, ix->tmap_c, sp,
+                                                                  static_cast<LargeScanMode>(kMode), ix->stream));
   if (tev) CK(cudaEventRecord(tev[1], ix->stream));
   ix->stats.last_ring_stages = kStages;
   ix->stats.scan_launches++;
@@ -1145,9 +1151,12 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out) {
   if (!out) return fail(RBK_EINVAL, "out is null");
   *out = nullptr;
-  if (flags & ~static_cast<uint32_t>(RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST)) return fail(RBK_EINVAL, "unknown flag");
+  if (flags & ~static_cast<uint32_t>(RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16))
+    return fail(RBK_EINVAL, "unknown flag");
   if ((flags & RBK_INDEX_F64_ON_HOST) && !(flags & RBK_INDEX_KEEP_F64))
     return fail(RBK_EINVAL, "RBK_INDEX_F64_ON_HOST requires RBK_INDEX_KEEP_F64");
+  if ((flags & RBK_INDEX_SCAN_F16) && !(flags & RBK_INDEX_KEEP_F64))
+    return fail(RBK_EINVAL, "RBK_INDEX_SCAN_F16 requires RBK_INDEX_KEEP_F64");
   if (dim < 1 || dim > (1 << 20)) return fail(RBK_EINVAL, "dim out of range");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -1168,6 +1177,7 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
   ix->device = device;
   ix->keep_f64 = (flags & RBK_INDEX_KEEP_F64) != 0;
   ix->f64_on_host = (flags & RBK_INDEX_F64_ON_HOST) != 0;
+  ix->scan_f16 = (flags & RBK_INDEX_SCAN_F16) != 0;
   ix->sm_count = prop.multiProcessorCount;
   memset(&ix->stats, 0, sizeof ix->stats);
   ix->stats.sm_count = ix->sm_count;
@@ -1292,9 +1302,9 @@ rbk_status rbk_index_overwrite_f64_batch(rbk_index* ix, const int64_t* slots, in
     CK(cudaMemcpyAsync(ix->stage.p, reinterpret_cast<const unsigned char*>(rows) + static_cast<size_t>(r0) * row_bytes,
                        static_cast<size_t>(nr) * row_bytes, cudaMemcpyHostToDevice, ix->stream));
     CK(launch_convert_rows(ix->stage.p, 0, nr, ix->dim, ix->dpad, ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr,
-                           ix->stream, ix->d_slots.p + r0, ix->dead_bits, ix->d_counter));
+                           ix->stream, ix->d_slots.p + r0, ix->dead_bits, ix->d_counter, ix->scan_f16));
     CK(launch_row_norms(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, 0, nr, ix->dim, ix->dpad, ix->inv_norm,
-                        ix->norm2, ix->d_counter + 1, ix->stream, ix->d_slots.p + r0, ix->dead_bits));
+                        ix->norm2, ix->d_counter + 1, ix->stream, ix->d_slots.p + r0, ix->dead_bits, ix->scan_f16));
     ix->stats.kernel_launches += ix->keep_f64 ? 3 : 2;
   }
   int dead = 0;
@@ -1459,10 +1469,14 @@ rbk_status rbk_index_storage_bytes(const rbk_index* ix, int64_t* device_bytes, i
   return RBK_OK;
 }
 
-rbk_status rbk_index_read_rows_bf16(rbk_index* ix, int64_t first, int64_t n, uint16_t* out) {
+namespace {
+rbk_status read_rows(rbk_index* ix, int64_t first, int64_t n, uint16_t* out, bool f16) {
   if (!ix || (n > 0 && !out)) return fail(RBK_EINVAL, "null argument");
   std::lock_guard<std::mutex> lk(ix->mu);
   DeviceGuard dg(ix->device);
+  if (ix->scan_f16 != f16)
+    return fail(RBK_EINVAL, ix->scan_f16 ? "this index stores fp16 rows (RBK_INDEX_SCAN_F16): use rbk_index_read_rows_f16"
+                                         : "this index stores bf16 rows: use rbk_index_read_rows_bf16");
   if (first < 0 || n < 0 || first + n > ix->n_rows) return fail(RBK_EINVAL, "row range out of bounds");
   if (n == 0) return RBK_OK;
   CK(cudaMemcpy2DAsync(out, static_cast<size_t>(ix->dim) * 2, ix->rows + static_cast<size_t>(first) * ix->dpad,
@@ -1470,6 +1484,14 @@ rbk_status rbk_index_read_rows_bf16(rbk_index* ix, int64_t first, int64_t n, uin
                        cudaMemcpyDeviceToHost, ix->stream));
   CK(cudaStreamSynchronize(ix->stream));
   return RBK_OK;
+}
+}  // namespace
+
+rbk_status rbk_index_read_rows_bf16(rbk_index* ix, int64_t first, int64_t n, uint16_t* out) {
+  return read_rows(ix, first, n, out, false);
+}
+rbk_status rbk_index_read_rows_f16(rbk_index* ix, int64_t first, int64_t n, uint16_t* out) {
+  return read_rows(ix, first, n, out, true);
 }
 
 rbk_status rbk_index_search_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,

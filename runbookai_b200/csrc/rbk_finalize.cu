@@ -12,6 +12,7 @@
 #include <cuda_bf16.h>
 #include <limits.h>
 
+#include "rbk_f16.cuh"
 #include "rbk_internal.h"
 #include "rbk_ptx.cuh"
 
@@ -58,7 +59,11 @@ __device__ __forceinline__ double exact_cosine(double dot, double na, double nb)
 // The exact-scores path, which has no finalize, asks for it.
 // scratch (nullable): the per-launch scan scratch of the FIRST sub-batch - hist [Bs][kHistBins] | maxbin [Bs] |
 // gthr [Bs] | progress [n_progress] - zeroed here, one row per query block, instead of by a separate memset node.
-template <typename SrcT, bool kNorm2>
+// kF16 (RBK_INDEX_SCAN_F16): the scan's copy is the query scaled by its own power of two and rounded to fp16 (the rule
+// of rbk_f16.cuh, applied to the f64 query, or to the f32 one widened exactly); q_inv_norm = 1/||h|| (so it carries
+// the scale) and the angle in q_eps is that of h.  The query stays live or dead (q_inv_norm NaN, thr_init +inf) exactly
+// as in a bf16 index, so that the two tiers take the same decisions on zero, tiny or huge queries.
+template <typename SrcT, bool kNorm2, bool kF16>
 __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restrict__ src, int d, int dpad,
                                                            double min_score, double acc_eps,
                                                            const float* __restrict__ eps_c, QueryBuffers qb,
@@ -77,7 +82,22 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
       for (int i = tid; i < n_progress; i += blockDim.x) tail[2 * Bs + i] = 0u;
   }
   const SrcT* s = src + static_cast<size_t>(q) * d;
+  int e = 0;   // kF16: the query's scale exponent
+  if constexpr (kF16) {
+    __shared__ double red_m[4];
+    double amax = 0.0;
+    for (int i = tid; i < d; i += blockDim.x) {
+      const double a = fabs(static_cast<double>(__ldg(s + i)));
+      if (a < INFINITY) amax = fmax(amax, a);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmax(amax, __shfl_xor_sync(kFull, amax, o));
+    if ((tid & 31) == 0) red_m[tid >> 5] = amax;
+    __syncthreads();
+    e = f16_scale_exp(fmax(fmax(red_m[0], red_m[1]), fmax(red_m[2], red_m[3])));
+  }
   double sb = 0.0, sd = 0.0, sq = 0.0;  // ||bf16(q)||^2, ||q - bf16(q)||^2, ||q||^2 (any order: bounds only)
+  double sh = 0.0, shd = 0.0, sx = 0.0; // kF16: ||h||^2, ||q 2^e - h||^2, ||q 2^e||^2 (any order: bounds only)
   // 8 elements per thread and pass, ALL loads first: the stores below may alias the source as far as the compiler
   // knows, so a load -> store loop exposed one global round trip per element (the kernel took 7.8 us for this)
   for (int i0 = tid; i0 < dpad; i0 += 8 * blockDim.x) {
@@ -101,20 +121,39 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
         sb += xb * xb;
         sd += (x - xb) * (x - xb);
         sq += x * x;
+        if constexpr (kF16) {
+          const double y = scale_pow2(x, e);
+          b = f16_bits_flush(y);
+          const double yh = f16_bits_to_f64(b);
+          sh += yh * yh;
+          shd += (y - yh) * (y - yh);
+          sx += y * y;
+        }
       }
       qb.q_bf16[static_cast<size_t>(q) * dpad + i] = b;
     }
   }
   __shared__ double red_b[4], red_d[4];
+  __shared__ double red_h[4], red_hd[4], red_x[4];
   __shared__ double s_na;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     sb += __shfl_xor_sync(kFull, sb, o);
     sd += __shfl_xor_sync(kFull, sd, o);
+    if constexpr (kF16) {
+      sh += __shfl_xor_sync(kFull, sh, o);
+      shd += __shfl_xor_sync(kFull, shd, o);
+      sx += __shfl_xor_sync(kFull, sx, o);
+    }
   }
   if ((tid & 31) == 0) {
     red_b[tid >> 5] = sb;
     red_d[tid >> 5] = sd;
+    if constexpr (kF16) {
+      red_h[tid >> 5] = sh;
+      red_hd[tid >> 5] = shd;
+      red_x[tid >> 5] = sx;
+    }
   }
   // the reference's normA: index order, multiply then add.  The chain is sequential by contract, so its
   // operands are staged in smem first (a dependent global load per element cost ~23 ns each).
@@ -146,13 +185,26 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
     const double nb2 = red_b[0] + red_b[1] + red_b[2] + red_b[3];
     const double nd2 = red_d[0] + red_d[1] + red_d[2] + red_d[3];
     const bool ok = nb2 > 0.0 && nb2 < INFINITY && na > 0.0 && na < INFINITY;
-    const double inv = ok ? 1.0 / sqrt(nb2) : 0.0;
+    double inv = ok ? 1.0 / sqrt(nb2) : 0.0;
     // angle(q, bf16(q)) <= asin(||q - bf16(q)|| / ||q||); cosine is 1-Lipschitz in the angle
     double ang = 0.0;
     if (ok && nd2 > 0.0) {
       const double ratio = sqrt(nd2 / na) * (1.0 + 1e-9) * (kNorm2 ? 1.0 : 1.0 + 1e-12 * d);   // any-order sum: widen
 
       ang = ratio < 1.0 ? asin(ratio) * (1.0 + 1e-9) : 3.2;
+    }
+    if constexpr (kF16) {
+      // the same bound for h * 2^-e, measured in the scaled domain (the angle does not depend on the scale); a live
+      // query has a finite nonzero bf16 norm, so its h (the largest element in [2^14, 2^15]) has one too
+      const double nh2 = red_h[0] + red_h[1] + red_h[2] + red_h[3];
+      const double nhd2 = red_hd[0] + red_hd[1] + red_hd[2] + red_hd[3];
+      const double nx2 = red_x[0] + red_x[1] + red_x[2] + red_x[3];
+      inv = ok ? 1.0 / sqrt(nh2) : 0.0;
+      ang = 0.0;
+      if (ok && nhd2 > 0.0) {
+        const double ratio = sqrt(nhd2 / nx2) * (1.0 + 1e-9) * (1.0 + 1e-12 * d);   // any-order sums: widen
+        ang = ratio < 1.0 ? asin(ratio) * (1.0 + 1e-9) : 3.2;
+      }
     }
     // + corpus-side quantisation angle when the exact source is an f64 sidecar (0 for bf16-exact corpora)
     const double eps = acc_eps + ang + (eps_c != nullptr ? static_cast<double>(*eps_c) * (1.0 + 1e-6) : 0.0);
@@ -1197,23 +1249,35 @@ __global__ void __launch_bounds__(128) merge_shards_kernel(int G, int B, int k, 
 
 }  // namespace
 
+template <typename SrcT, bool kNorm2>
+void launch_prep_typed(const SrcT* src, bool f16, int B, int d, int dpad, double min_score, double acc_eps,
+                       const float* eps_c, const QueryBuffers& qb, cudaStream_t stream, unsigned int* scratch, int Bs,
+                       int n_progress) {
+  if (f16)
+    prep_queries_kernel<SrcT, kNorm2, true><<<B, 128, 0, stream>>>(src, d, dpad, min_score, acc_eps, eps_c, qb, scratch,
+                                                                   Bs, n_progress);
+  else
+    prep_queries_kernel<SrcT, kNorm2, false><<<B, 128, 0, stream>>>(src, d, dpad, min_score, acc_eps, eps_c, qb,
+                                                                    scratch, Bs, n_progress);
+}
+
 cudaError_t launch_prep_queries(const void* src, int src_type, int B, int d, int dpad, double min_score,
                                 const float* eps_c, const QueryBuffers& qb, cudaStream_t stream, bool with_norm2,
-                                unsigned int* scratch, int Bs, int n_progress) {
+                                unsigned int* scratch, int Bs, int n_progress, bool f16) {
   if (B <= 0) return cudaSuccess;
   const double acc_eps = accumulation_eps(d);
   const double* sd = static_cast<const double*>(src);
   const float* sf = static_cast<const float*>(src);
   if (src_type == 0) {
     if (with_norm2)
-      prep_queries_kernel<double, true><<<B, 128, 0, stream>>>(sd, d, dpad, min_score, acc_eps, eps_c, qb, scratch, Bs, n_progress);
+      launch_prep_typed<double, true>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
     else
-      prep_queries_kernel<double, false><<<B, 128, 0, stream>>>(sd, d, dpad, min_score, acc_eps, eps_c, qb, scratch, Bs, n_progress);
+      launch_prep_typed<double, false>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
   } else {
     if (with_norm2)
-      prep_queries_kernel<float, true><<<B, 128, 0, stream>>>(sf, d, dpad, min_score, acc_eps, eps_c, qb, scratch, Bs, n_progress);
+      launch_prep_typed<float, true>(sf, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
     else
-      prep_queries_kernel<float, false><<<B, 128, 0, stream>>>(sf, d, dpad, min_score, acc_eps, eps_c, qb, scratch, Bs, n_progress);
+      launch_prep_typed<float, false>(sf, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
   }
   return cudaGetLastError();
 }

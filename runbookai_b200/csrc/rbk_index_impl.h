@@ -145,6 +145,10 @@ struct rbk_index {
   // RBK_INDEX_F64_ON_HOST: rows_f64 is pinned, mapped host memory (one pointer under UVA).  Every write to it is
   // stream-ordered: a kernel or copy on `stream`, or the host after a synchronisation of `stream`.
   bool f64_on_host = false;
+  // RBK_INDEX_SCAN_F16: `rows` (and the queries' scan copies) hold per-row scaled fp16 instead of bf16, and the scan
+  // runs its fp16 instantiation (rbk_scan_f16.cu).  Requires keep_f64, so nothing ever decodes these rows as values
+  // except the norm kernels: the re-rank, the fallback and the exact scores read rows_f64.
+  bool scan_f16 = false;
   unsigned int* dead_bits = nullptr;
   int* d_counter = nullptr;   // [0] tombstone counter, [1] eps_c_max (float bits)
   cudaStream_t own_stream = nullptr, stream = nullptr;

@@ -1,7 +1,8 @@
 // rbk_ingest.cu — K3: corpus ingest.  Replaces VectorStore.loadEmbeddings /
 // bufferToFloatArray (reference src/knowledge/store/vector-store.ts:56-88): rows arrive as
 // little-endian float64 (the SQLite BLOB layout), float32 or bf16 and are stored as bf16
-// rows of pitch dpad (= dim rounded up to 8 elements, zero padded) plus, per row,
+// rows of pitch dpad (= dim rounded up to 8 elements, zero padded) - or, for RBK_INDEX_SCAN_F16
+// indexes, as per-row scaled fp16 rows (rbk_f16.cuh) - plus, per row,
 //   inv_norm (fp32)  1/||row||           for the approximate scan (NaN = never matches)
 //   norm2    (fp64)  sum of squares accumulated in index order, multiply-then-add — the
 //                    reference's `normB` (embedder.ts:175-181) bit for bit, reused by the
@@ -9,6 +10,7 @@
 // Both kernels are HBM-bound streams: 16-byte vector loads/stores, no reuse.
 #include <cuda_bf16.h>
 
+#include "rbk_f16.cuh"
 #include "rbk_internal.h"
 
 namespace rbk {
@@ -110,6 +112,65 @@ __global__ void __launch_bounds__(256) convert_rows_kernel(const SrcT* __restric
   }
 }
 
+template <typename SrcT>
+__device__ __forceinline__ double src_to_f64(SrcT v) {   // exact widening of every source type
+  if constexpr (sizeof(SrcT) == 8) return static_cast<double>(v);
+  else if constexpr (sizeof(SrcT) == 4) return static_cast<double>(static_cast<float>(v));
+  else return static_cast<double>(__uint_as_float(static_cast<uint32_t>(v) << 16));
+}
+
+// RBK_INDEX_SCAN_F16 rows (rbk_f16.cuh): the scale needs the row's largest finite magnitude before any element is
+// converted, so one WARP owns a row - pass 1 reduces max |x| over the row (coalesced reads), pass 2 re-reads it (from
+// L1 / L2) and writes the scaled fp16 row in 16-byte stores, plus the f64 sidecar, which such an index always keeps.
+// Same slot_map / dead_bits / n_dead contract as convert_rows_kernel.
+constexpr int kF16ConvThreads = 256;
+template <typename SrcT>
+__global__ void __launch_bounds__(kF16ConvThreads) convert_rows_f16_kernel(
+    const SrcT* __restrict__ src, int64_t n_rows, int d, int dpad, uint16_t* __restrict__ dst,
+    double* __restrict__ dst_f64, const int64_t* __restrict__ slot_map, const unsigned int* __restrict__ dead_bits,
+    int* __restrict__ n_dead) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = static_cast<int64_t>(gridDim.x) * (kF16ConvThreads / 32);
+  for (int64_t srow = blockIdx.x * static_cast<int64_t>(kF16ConvThreads / 32) + (threadIdx.x >> 5); srow < n_rows;
+       srow += warps) {
+    int64_t row = srow;
+    if (slot_map != nullptr) {
+      row = slot_map[srow];
+      if ((dead_bits[row >> 5] >> (row & 31)) & 1u) {
+        if (lane == 0) atomicAdd(n_dead, 1);
+        continue;
+      }
+    }
+    const SrcT* s = src + srow * d;
+    double amax = 0.0;
+    for (int i = lane; i < d; i += 32) {
+      const double a = fabs(src_to_f64(s[i]));
+      if (a < INFINITY) amax = fmax(amax, a);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmax(amax, __shfl_xor_sync(0xFFFFFFFFu, amax, o));
+    const int e = f16_scale_exp(amax);
+    for (int c0 = lane * 8; c0 < dpad; c0 += 32 * 8) {
+      uint16_t o[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        o[j] = 0;
+        if (c0 + j < d) {
+          const double x = src_to_f64(s[c0 + j]);
+          dst_f64[row * d + c0 + j] = x;
+          o[j] = f16_bits_flush(scale_pow2(x, e));
+        }
+      }
+      uint4 out;
+      out.x = o[0] | (static_cast<uint32_t>(o[1]) << 16);
+      out.y = o[2] | (static_cast<uint32_t>(o[3]) << 16);
+      out.z = o[4] | (static_cast<uint32_t>(o[5]) << 16);
+      out.w = o[6] | (static_cast<uint32_t>(o[7]) << 16);
+      *reinterpret_cast<uint4*>(dst + row * dpad + c0) = out;
+    }
+  }
+}
+
 __device__ __forceinline__ double bf16_bits_to_f64(uint32_t h) {
   return static_cast<double>(__uint_as_float(h << 16));
 }
@@ -129,6 +190,8 @@ constexpr int kNormRows = 128;          // rows (= threads) per block
 constexpr int kNormChunk = 128;         // bf16 elements per staged chunk (256 B per row)
 constexpr int kNormPitch16 = kNormChunk / 8 + 1;   // 17 x 16 B per row in smem: odd -> conflict-free walks
 
+// kF16: the rows are RBK_INDEX_SCAN_F16 fp16 bits (inv_norm is that of the stored, scaled values).
+template <bool kF16>
 __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __restrict__ rows_base,
                                                               const double* __restrict__ rows_f64_base,
                                                               const int64_t* __restrict__ slot_map,
@@ -191,8 +254,8 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
         const uint32_t w[4] = {w4.x, w4.y, w4.z, w4.w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const double lo = bf16_bits_to_f64(w[j] & 0xFFFFu);
-          const double hi = bf16_bits_to_f64(w[j] >> 16);
+          const double lo = kF16 ? f16_bits_to_f64(w[j] & 0xFFFFu) : bf16_bits_to_f64(w[j] & 0xFFFFu);
+          const double hi = kF16 ? f16_bits_to_f64(w[j] >> 16) : bf16_bits_to_f64(w[j] >> 16);
           acc = __dadd_rn(acc, __dmul_rn(lo, lo));
           acc = __dadd_rn(acc, __dmul_rn(hi, hi));
         }
@@ -210,15 +273,32 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
 // the values it really stores), again as one sequential chain per row fed from shared memory, and the angle
 // between the f64 row and its bf16 rounding - an upper bound on how far the scan's approximate cosine of this
 // row can be from its true cosine, on top of the other error terms - is folded into *eps_c_max.
+// kF16 (RBK_INDEX_SCAN_F16): the stored rows are fp16 scaled by 2^e, with e recomputed here from the f64 row (a first
+// walk over it for max |x|); the angle folded in is that between x and h * 2^-e, measured in the scaled domain
+// (x * 2^e - h: the same angle).  The row's liveness in the scan must stay what a bf16 index gives it, so that both
+// tiers answer alike: a row whose bf16 rounding has a zero or non-finite norm (elements past float32's range, or all of
+// them below bf16's) gets the NaN inv_norm and the corpus angle such a row gets in a bf16 index.
 constexpr int kNorm64Chunk = 32;        // doubles per staged chunk (256 B per row)
 constexpr int kNorm64Pitch = kNorm64Chunk + 1;
 
+__device__ __forceinline__ float angle_bound(double diff2, double n2) {
+  float eps = 0.f;
+  if (diff2 > 0.0) {
+    const double ratio = (n2 > 0.0 && n2 < INFINITY) ? sqrt(diff2 / n2) * (1.0 + 1e-9) : 2.0;
+    eps = static_cast<float>((ratio < 1.0 ? asin(ratio) : 3.2) * (1.0 + 1e-6));
+    eps = nextafterf(eps, INFINITY);
+  }
+  return eps;
+}
+
+template <bool kF16>
 __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t* __restrict__ rows_base,
                                                                   const double* __restrict__ rows_f64_base,
                                                                   const int64_t* __restrict__ slot_map,
                                                                   const unsigned int* __restrict__ dead_bits,
                                                                   int64_t first_row, int64_t n_items, int d, int dpad,
                                                                   double* __restrict__ norm2_base,
+                                                                  float* __restrict__ inv_norm_base,
                                                                   int* __restrict__ eps_c_max) {
   __shared__ double s_x[kNormRows * kNorm64Pitch];
   __shared__ uint16_t s_b[kNormRows * (kNorm64Chunk + 2)];
@@ -236,20 +316,42 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
   }
   __syncthreads();
   const long long my_row = s_row[tid];
+  int e = 0;
+  if constexpr (kF16) {   // the row's scale: max |x| over the finite elements, staged like the walk below
+    double amax = 0.0;
+    for (int c0 = 0; c0 < d; c0 += kNorm64Chunk) {
+      const int len = d - c0 < kNorm64Chunk ? d - c0 : kNorm64Chunk;
+      for (int i = tid; i < kNormRows * len; i += kNormRows) {
+        const int rr = i / len, el = i - rr * len;
+        const long long row = s_row[rr];
+        s_x[rr * kNorm64Pitch + el] = row >= 0 ? __ldg(rows_f64_base + row * d + c0 + el) : 0.0;
+      }
+      __syncthreads();
+      if (my_row >= 0)
+        for (int i = 0; i < len; ++i) {
+          const double a = fabs(s_x[tid * kNorm64Pitch + i]);
+          if (a < INFINITY) amax = fmax(amax, a);
+        }
+      __syncthreads();
+    }
+    e = f16_scale_exp(amax);
+  }
   double n2 = 0.0, diff2 = 0.0;
+  double h2 = 0.0, hdiff2 = 0.0;    // kF16: ||x 2^e||^2 and ||x 2^e - h||^2 (any order: bounds only)
+  bool b_nonzero = false, b_finite = true;   // kF16: the bf16 rounding of the row has a nonzero / finite norm
   for (int c0 = 0; c0 < d; c0 += kNorm64Chunk) {
     const int len = d - c0 < kNorm64Chunk ? d - c0 : kNorm64Chunk;
     for (int i = tid; i < kNormRows * len; i += kNormRows) {   // consecutive lanes = consecutive elements of a row
-      const int rr = i / len, e = i - rr * len;
+      const int rr = i / len, el = i - rr * len;
       const long long row = s_row[rr];
       double x = 0.0;
       uint16_t bq = 0;
       if (row >= 0) {
-        x = __ldg(rows_f64_base + row * d + c0 + e);
-        bq = __ldg(rows_base + row * dpad + c0 + e);
+        x = __ldg(rows_f64_base + row * d + c0 + el);
+        bq = __ldg(rows_base + row * dpad + c0 + el);
       }
-      s_x[rr * kNorm64Pitch + e] = x;
-      s_b[rr * (kNorm64Chunk + 2) + e] = bq;
+      s_x[rr * kNorm64Pitch + el] = x;
+      s_b[rr * (kNorm64Chunk + 2) + el] = bq;
     }
     __syncthreads();
     if (my_row >= 0) {
@@ -258,19 +360,32 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
       for (int i = 0; i < len; ++i) {
         const double v = mine[i];
         n2 = __dadd_rn(n2, __dmul_rn(v, v));   // the reference's normB for the f64 row
-        const double e = v - bf16_bits_to_f64(mb[i]);
-        diff2 += e * e;
+        if constexpr (kF16) {
+          const double y = scale_pow2(v, e), t = y - f16_bits_to_f64(mb[i]);
+          h2 += y * y;
+          hdiff2 += t * t;
+          const float vb = __bfloat162float(__float2bfloat16_rn(__double2float_rn(v)));   // what a bf16 index stores
+          b_nonzero |= vb != 0.f;
+          b_finite &= fabsf(vb) < INFINITY;
+          const double eb = v - static_cast<double>(vb);
+          diff2 += eb * eb;
+        } else {
+          const double eb = v - bf16_bits_to_f64(mb[i]);
+          diff2 += eb * eb;
+        }
       }
     }
     __syncthreads();
   }
   if (my_row < 0) return;
   norm2_base[my_row] = n2;
-  float eps = 0.f;
-  if (diff2 > 0.0) {
-    const double ratio = (n2 > 0.0 && n2 < INFINITY) ? sqrt(diff2 / n2) * (1.0 + 1e-9) : 2.0;
-    eps = static_cast<float>((ratio < 1.0 ? asin(ratio) : 3.2) * (1.0 + 1e-6));
-    eps = nextafterf(eps, INFINITY);
+  float eps;
+  if constexpr (kF16) {
+    const bool bf16_live = b_nonzero && b_finite;
+    if (!bf16_live) inv_norm_base[my_row] = __uint_as_float(0x7FC00000u);
+    eps = bf16_live ? angle_bound(hdiff2, h2) : angle_bound(diff2, n2);
+  } else {
+    eps = angle_bound(diff2, n2);
   }
   if (eps > 0.f) atomicMax(eps_c_max, __float_as_int(eps));   // non-negative floats order like ints
 }
@@ -301,8 +416,26 @@ int grid_for(int64_t items, int threads, int max_blocks) {
 
 cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, int d, int dpad, uint16_t* dst_rows,
                                 double* dst_f64, cudaStream_t stream, const int64_t* slot_map,
-                                const unsigned int* dead_bits, int* n_dead) {
+                                const unsigned int* dead_bits, int* n_dead, bool f16) {
   if (n_rows <= 0) return cudaSuccess;
+  if (f16) {
+    constexpr int rows_per_block = kF16ConvThreads / 32;
+    int dev = 0, sms = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return e;
+    const int grid = grid_for(n_rows, rows_per_block, sms * 8);
+    if (src_type == 0)
+      convert_rows_f16_kernel<double><<<grid, kF16ConvThreads, 0, stream>>>(
+          static_cast<const double*>(src), n_rows, d, dpad, dst_rows, dst_f64, slot_map, dead_bits, n_dead);
+    else if (src_type == 1)
+      convert_rows_f16_kernel<float><<<grid, kF16ConvThreads, 0, stream>>>(
+          static_cast<const float*>(src), n_rows, d, dpad, dst_rows, dst_f64, slot_map, dead_bits, n_dead);
+    else
+      convert_rows_f16_kernel<uint16_t><<<grid, kF16ConvThreads, 0, stream>>>(
+          static_cast<const uint16_t*>(src), n_rows, d, dpad, dst_rows, dst_f64, slot_map, dead_bits, n_dead);
+    return cudaGetLastError();
+  }
   const int64_t total = n_rows * (dpad >> 3);
   int dev = 0, sms = 0;
   cudaError_t e = cudaGetDevice(&dev);
@@ -325,15 +458,26 @@ cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, i
 
 cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_base, int64_t first_row, int64_t n_items,
                              int d, int dpad, float* inv_norm_base, double* norm2_base, int* eps_c_max,
-                             cudaStream_t stream, const int64_t* slot_map, const unsigned int* dead_bits) {
+                             cudaStream_t stream, const int64_t* slot_map, const unsigned int* dead_bits, bool f16) {
   if (n_items <= 0) return cudaSuccess;
+  if (f16 && rows_f64_base == nullptr) return cudaErrorInvalidValue;   // the fp16 tier always keeps the f64 rows
   const unsigned blocks = static_cast<unsigned>((n_items + kNormRows - 1) / kNormRows);
-  row_norms_kernel<<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits, first_row, n_items,
-                                                     d, dpad, inv_norm_base, norm2_base, eps_c_max);
+  if (f16)
+    row_norms_kernel<true><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits, first_row,
+                                                             n_items, d, dpad, inv_norm_base, norm2_base, eps_c_max);
+  else
+    row_norms_kernel<false><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits, first_row,
+                                                              n_items, d, dpad, inv_norm_base, norm2_base, eps_c_max);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || rows_f64_base == nullptr) return e;
-  row_norms_f64_kernel<<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits, first_row,
-                                                         n_items, d, dpad, norm2_base, eps_c_max);
+  if (f16)
+    row_norms_f64_kernel<true><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits,
+                                                                 first_row, n_items, d, dpad, norm2_base, inv_norm_base,
+                                                                 eps_c_max);
+  else
+    row_norms_f64_kernel<false><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits,
+                                                                  first_row, n_items, d, dpad, norm2_base,
+                                                                  inv_norm_base, eps_c_max);
   return cudaGetLastError();
 }
 

@@ -57,23 +57,31 @@ struct LargeScanParams : ScanParams {
 enum LargeScanMode { kScanCount = 1, kScanEmit = 2 };
 cudaError_t launch_scan_large(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const LargeScanParams& p,
                               LargeScanMode mode, cudaStream_t stream);
+// The same kernels with fp16 operands (rbk_scan_f16.cu), for indexes created with RBK_INDEX_SCAN_F16: both tensor maps
+// are then CU_TENSOR_MAP_DATA_TYPE_FLOAT16 maps of per-row scaled fp16 rows.
+cudaError_t launch_scan_f16(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const ScanParams& p,
+                            cudaStream_t stream);
+cudaError_t launch_scan_large_f16(const CUtensorMap& tmap_q, const CUtensorMap& tmap_c, const LargeScanParams& p,
+                                  LargeScanMode mode, cudaStream_t stream);
 
 // ---- ingest (rbk_ingest.cu) ----
 // src element type: 0 = f64, 1 = f32, 2 = bf16 bits.  src is device memory, row pitch = d.
 // dst_f64 (nullable): exact-source sidecar rows, pitch d.
 // slot_map (nullable, bulk overwrite): dst_rows / dst_f64 are the index's row 0 and source row r lands in row
 // slot_map[r]; rows whose slot is tombstoned (dead_bits) are skipped and counted in *n_dead.
+// f16: store the rows by the RBK_INDEX_SCAN_F16 rule (rbk_f16.cuh) instead of as bf16; dst_f64 is then required.
 cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, int d, int dpad,
                                 uint16_t* dst_rows, double* dst_f64, cudaStream_t stream,
                                 const int64_t* slot_map = nullptr, const unsigned int* dead_bits = nullptr,
-                                int* n_dead = nullptr);
+                                int* n_dead = nullptr, bool f16 = false);
 // Norms of rows [first_row, first_row + n_items) of the index (or, with slot_map, of rows slot_map[i]; tombstoned
 // ones skipped).  All array arguments are the index's BASE pointers.  rows_f64_base (nullable): when given,
 // norm2 comes from it and the bf16-vs-f64 angle bound is max-ed into *eps_c_max (float bits in an int).
+// f16: the rows are RBK_INDEX_SCAN_F16 fp16 rows (rows_f64_base required); the angle is that of their rounding.
 cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_base, int64_t first_row,
                              int64_t n_items, int d, int dpad, float* inv_norm_base, double* norm2_base,
                              int* eps_c_max, cudaStream_t stream, const int64_t* slot_map = nullptr,
-                             const unsigned int* dead_bits = nullptr);
+                             const unsigned int* dead_bits = nullptr, bool f16 = false);
 cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows, float* inv_norm,
                              unsigned int* dead_bits, int* n_killed, cudaStream_t stream);
 
@@ -92,10 +100,10 @@ cudaError_t launch_compact_gather(const uint16_t* rows, const double* rows_f64, 
 
 // ---- query preparation + finalize + exhaustive fallback + shard merge (rbk_finalize.cu) ----
 struct QueryBuffers {
-  uint16_t* q_bf16;    // [B][dpad]
+  uint16_t* q_bf16;    // [B][dpad] the scan's copy: bf16, or scaled fp16 for an RBK_INDEX_SCAN_F16 index
   double* q_f64;       // [B][d]
   double* q_norm2;     // [B] exact sequential sum of squares of the f64 query (reference's normA)
-  float* q_inv_norm;   // [B] 1/||bf16(q)||  (approximate-score scaling)
+  float* q_inv_norm;   // [B] 1/||bf16(q)||, or 1/||h|| of the scaled fp16 copy (it carries the scale 2^-e)
   double* q_eps;       // [B] bound on |approx - exact| cosine for this query
   float* thr_init;     // [B]
 };
@@ -104,9 +112,11 @@ struct QueryBuffers {
 // with_norm2: also run the sequential normA chain (only the exact-scores path, which has no finalize kernel; a
 // search leaves it to finalize).  scratch (nullable): hist | maxbin | gthr | progress of the first sub-batch (Bs
 // queries, n_progress pacing slots), zeroed by the kernel.
+// f16: the scan's copy follows the RBK_INDEX_SCAN_F16 rule (rbk_f16.cuh) and q_eps holds the angle of that rounding;
+// a query is live (finite q_inv_norm) exactly when it would be for a bf16 index.
 cudaError_t launch_prep_queries(const void* src, int src_type, int B, int d, int dpad, double min_score,
                                 const float* eps_c, const QueryBuffers& qb, cudaStream_t stream, bool with_norm2,
-                                unsigned int* scratch, int Bs, int n_progress);
+                                unsigned int* scratch, int Bs, int n_progress, bool f16 = false);
 
 // local row -> global slot.  Contiguous shards: slot_base + row.  A group that deals rows out block-cyclically over
 // G devices (rbk_group.cu): device g's local row r is global slot ((r / block) * G + g) * block + r % block - still

@@ -37,9 +37,10 @@ def _bucket(chunks) -> dict:
 
 
 class KnowledgeRetriever:
-    def __init__(self, config: dict, device: int | None = None, vector_store=None):
+    def __init__(self, config: dict, device: int | None = None, vector_store=None, scan_f16: bool | None = None):
         """config: {storePath, sources: [callable(since) -> iterable of documents], vectorStorePath?}
-        (retriever/index.ts:19-39)."""
+        (retriever/index.ts:19-39).  scan_f16: the vector store's scan precision (see VectorStore; None:
+        RUNBOOK_KNN_SCAN_F16)."""
         self.config = config
         d = os.path.dirname(config["storePath"])
         if d:
@@ -51,7 +52,7 @@ class KnowledgeRetriever:
             self._hybrid = HybridRetriever({"storePath": config["storePath"],
                                             "vectorStorePath": config.get("vectorStorePath")
                                             or os.path.join(d or ".", "vectors.db")},
-                                           fts_store=self.store, device=device)
+                                           fts_store=self.store, device=device, scan_f16=scan_f16)
             if vector_store is not None:       # tests inject a store built on the CPU stand-in index
                 if self._hybrid.vector_store is not None:
                     self._hybrid.vector_store.close()

@@ -126,18 +126,24 @@ def shared_index_count() -> int:
 
 class VectorStore:
     def __init__(self, db_path: str, device: int | None = None, index_factory=None, shared: bool = False,
-                 f64_on_host: bool | None = None):
+                 f64_on_host: bool | None = None, scan_f16: bool | None = None):
         # index_factory(dim, device) -> object with the _native.Index surface; tests inject a
         # CPU stand-in to exercise the host logic where there is no GPU
         # keep_f64: the reference stores float64 embeddings; keep them so the re-rank is exact for any input.
         # f64_on_host (None: RUNBOOK_KNN_F64_ON_HOST=1 enables): those float64 rows live in pinned host memory instead
         # of on the GPU - the same answers, about 5x the rows per GPU at d = 1536, host RAM and PCIe reads in the
         # re-rank instead.  A shared index keeps the placement of the instance that created it.
+        # scan_f16 (None: RUNBOOK_KNN_SCAN_F16=1 enables): the scan reads per-row scaled fp16 rows instead of bf16 - the
+        # same answers and bytes, a tighter error bound, so fewer batches need the wide retry.  A shared index keeps the
+        # setting of the instance that created it.
         if f64_on_host is None:
             f64_on_host = os.environ.get("RUNBOOK_KNN_F64_ON_HOST", "0") == "1"
+        if scan_f16 is None:
+            scan_f16 = os.environ.get("RUNBOOK_KNN_SCAN_F16", "0") == "1"
         self.f64_on_host = on_host = bool(f64_on_host)
+        self.scan_f16 = f16 = bool(scan_f16)
         self._index_factory = index_factory or (
-            lambda dim, dev: Index(dim, device=dev, keep_f64=True, f64_on_host=on_host))
+            lambda dim, dev: Index(dim, device=dev, keep_f64=True, f64_on_host=on_host, scan_f16=f16))
         # one connection, usable from the micro-batcher's worker thread too; serialised by a lock
         self.db = sqlite3.connect(db_path, check_same_thread=False)
         self.db.row_factory = sqlite3.Row
@@ -616,12 +622,13 @@ class VectorStore:
 
 
 def create_vector_store(base_dir: str = ".runbook", device: int | None = None, index_factory=None,
-                        shared: bool | None = None) -> VectorStore:
+                        shared: bool | None = None, scan_f16: bool | None = None) -> VectorStore:
     """vector-store.ts:338-341.  shared (default on; RUNBOOK_KNN_SHARED_INDEX=0 turns it off): call sites
-    that build and close a store per use attach to the process-wide index of that db instead of re-uploading."""
+    that build and close a store per use attach to the process-wide index of that db instead of re-uploading.
+    scan_f16: see VectorStore (None: RUNBOOK_KNN_SCAN_F16)."""
     if shared is None:
         shared = os.environ.get("RUNBOOK_KNN_SHARED_INDEX", "1") != "0"
-    return VectorStore(f"{base_dir}/vectors.db", device, index_factory, shared=shared)
+    return VectorStore(f"{base_dir}/vectors.db", device, index_factory, shared=shared, scan_f16=scan_f16)
 
 
 createVectorStore = create_vector_store

@@ -35,6 +35,14 @@ function hostRowsFromEnv(): number {
   return process.env.RUNBOOK_KNN_F64_ON_HOST === '1' ? 1 : 0;
 }
 
+/**
+ * RUNBOOK_KNN_SCAN_F16="1" makes the scan read per-row scaled fp16 rows instead of bf16 (RBK_INDEX_SCAN_F16): the same
+ * answers and bytes per row, a tighter error bound, so fewer batches are rescanned with the wide candidate margin.
+ */
+function scanF16FromEnv(): number {
+  return process.env.RUNBOOK_KNN_SCAN_F16 === '1' ? 1 : 0;
+}
+
 export class GpuEmbeddingIndex {
   private index: any | null = null;
   private idOfSlot: (string | null)[] = [];
@@ -85,7 +93,7 @@ export class GpuEmbeddingIndex {
     this.dim = rows[0].embedding.length / 8;
     const usable = rows.filter((r) => r.embedding.length === this.dim * 8);
     for (const r of rows) if (r.embedding.length !== this.dim * 8) this.badIds.add(r.id);
-    this.index = new RbkIndex(this.dim, this.device, usable.length, hostRowsFromEnv());
+    this.index = new RbkIndex(this.dim, this.device, usable.length, hostRowsFromEnv(), scanF16FromEnv());
     // the Buffers go to the addon as they are: it packs them with memcpy and appends in one call
     const first = Number(this.index.appendBlobs(usable.map((r) => r.embedding)));
     usable.forEach((r, i) => this.remember(r.id, first + i));
@@ -95,7 +103,7 @@ export class GpuEmbeddingIndex {
   set(id: string, embedding: number[]): void {
     if (!this.index) {
       this.dim = embedding.length;
-      this.index = new RbkIndex(this.dim, this.device, 0, hostRowsFromEnv());
+      this.index = new RbkIndex(this.dim, this.device, 0, hostRowsFromEnv(), scanF16FromEnv());
     }
     const slot = this.slotOfId.get(id);
     if (embedding.length !== this.dim) {
