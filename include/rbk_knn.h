@@ -202,9 +202,14 @@ rbk_status rbk_index_search_device(rbk_index* idx, const void* dev_queries_f32, 
  * which becomes k_fetch = 4000 through the hybrid retriever): exactly the contract of rbk_index_search_f64 - same
  * order, threshold, NaN / tombstone rules and bit-identical fp64 scores - for 1 <= k_fetch <= 4096.  k_fetch <= 112
  * is accepted too and gives the same answer as rbk_index_search_f64.  Two scans of the corpus (count, then emit the
- * rows the count proved may belong to the answer) and an exact fp64 re-rank of those rows; one extra host round trip
- * between the scans.  Host queries and outputs, synchronous; batches over 1024 queries are split.  Fails with
- * RBK_ECUDA, never with a wrong answer, if the emit scan finds more rows than the count scan bounded (a bug). */
+ * rows the count proved may belong to the answer), an exact fp64 re-rank of those rows and the cut to k_fetch in
+ * shared memory; one extra host round trip between the scans.  Host queries and outputs, synchronous; batches over
+ * 1024 queries are split.  Device memory is bounded by a fixed per-pass budget (256 MiB of candidates and results, at
+ * least one query per pass): the count scan runs once for the batch, then the queries go in contiguous groups that fit
+ * the budget, each group costing one emit scan and one copy of its results to the host through a pinned buffer the
+ * index keeps (rbk_index_trim releases it).  kernel_ms_out is the time of the whole call on the device's stream.
+ * Fails with RBK_ECUDA, never with a wrong answer, if an emit scan finds more rows than the count scan bounded (a
+ * bug). */
 rbk_status rbk_index_search_large_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
                                       int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                       int32_t* out_counts, float* kernel_ms_out);
@@ -212,14 +217,12 @@ rbk_status rbk_index_search_large_f64(rbk_index* idx, const double* queries, int
 /* Any number of hits per query - the reference's VectorStore.search has no ceiling on topK (vector-store.ts:207-221):
  * exactly the contract of rbk_index_search_large_f64 (same order, threshold, NaN / tombstone rules, bit-identical
  * fp64 scores, -1 / NaN tail, RBK_EDIM / RBK_EINVAL on the same arguments) for any int32 k_fetch >= 1.
- * k_fetch <= RBK_MAX_K_FETCH_LARGE runs rbk_index_search_large_f64 itself.  Above it the call keeps
- * k_eff = min(k_fetch, rbk_index_count()) entries per query on the device (no query can have more hits) and sorts
- * each query's candidates in global memory after the exact re-score.  Device memory is bounded by a fixed per-pass
- * budget (256 MiB of candidates and results, at least one query per pass), never by k_fetch: the count scan runs once
- * for the batch, then the queries go in contiguous groups that fit the budget, each group costing one emit scan.
- * Results are copied straight into the caller's arrays; kernel_ms_out is the time of the whole call on the device's
- * stream, these copies included (at pageable-memory speed for ordinary host arrays, B * k_eff * 16 bytes).  Fails with RBK_ECUDA, never with a wrong answer, if an emit
- * scan finds more rows than the count scan bounded (a bug). */
+ * k_fetch <= RBK_MAX_K_FETCH_LARGE runs rbk_index_search_large_f64 itself.  Above it the same pipeline keeps
+ * k_eff = min(k_fetch, rbk_index_count()) entries per query on the device (no query can have more hits) and, in
+ * place of the cut in shared memory, sorts each query's candidates in global memory after the exact re-score; the
+ * per-pass budget, the query groups and the pinned copy-back are the same, so device memory never grows with k_fetch.
+ * Fails with RBK_ECUDA, never with a wrong answer, if an emit scan finds more rows than the count scan bounded (a
+ * bug). */
 rbk_status rbk_index_search_unbounded_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
                                           int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                           int32_t* out_counts, float* kernel_ms_out);
@@ -298,16 +301,16 @@ rbk_status rbk_group_search_f32(rbk_group* grp, const float* queries, int32_t B,
 rbk_status rbk_group_search_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
                                 double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts,
                                 float* device_ms_out);
-/* rbk_index_search_large_f64 over the group: the count scan on every GPU, one wait for all of them, the emit scan and
- * re-rank on every GPU, then the same all-gather and merge as rbk_group_search_f64. */
+/* rbk_index_search_large_f64 over the group: the count scan on every GPU and one wait for all of them, then per query
+ * group - the members' candidates and result blocks taken together fit the same per-pass budget - the emit scan,
+ * re-rank and cut on every GPU, the same all-gather and merge as rbk_group_search_f64, and the copy into the caller's
+ * arrays.  A one-GPU group never touches NCCL. */
 rbk_status rbk_group_search_large_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
                                       int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                       int32_t* out_counts, float* device_ms_out);
 /* rbk_index_search_unbounded_f64 over the group (any k_fetch >= 1; up to RBK_MAX_K_FETCH_LARGE it is
- * rbk_group_search_large_f64): the count scan on every GPU and one wait for all of them, then per query group - the
- * members' candidates and result blocks taken together fit the same per-pass budget - the emit scan, re-score and
- * sort on every GPU into k_eff = rbk_group_count() entries per query, the all-gather and merge, and the copy into the
- * caller's arrays.  A one-GPU group never touches NCCL. */
+ * rbk_group_search_large_f64): the pipeline of rbk_group_search_large_f64, with the sort in global memory as the cut
+ * and k_eff = min(k_fetch, rbk_group_count()) entries per query on every GPU. */
 rbk_status rbk_group_search_unbounded_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
                                           int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                           int32_t* out_counts, float* device_ms_out);

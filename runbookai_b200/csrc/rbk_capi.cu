@@ -522,13 +522,14 @@ rbk_status fill_empty_results(rbk_index* ix, int B, int k_fetch, long long* d_sl
 namespace rbk {
 namespace impl {
 
-rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem, int slack_rows) {
+rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem) {
   CK(ix->q_raw.ensure(static_cast<size_t>(B) * ix->dim * elem));
   // rows padded to whole query blocks: the scan's TMA boxes are 128 query rows, and a box that hangs over the end of
   // the tensor is zero-FILLED by the TMA unit row by row, which is slow.  With the map covering whole blocks the pad
   // rows are ordinary (zeroed once here) memory; they only ever feed accumulator rows of queries that do not exist.
+  // One more block of them lets a large-k search's query group start its map at any query.
   {
-    const size_t want = static_cast<size_t>(round_up(B, kBlockM) + slack_rows) * ix->dpad;
+    const size_t want = static_cast<size_t>(round_up(B, kBlockM) + kBlockM) * ix->dpad;
     if (want > ix->q_bf16.n) {
       CK(ix->q_bf16.ensure(want));
       CK(cudaMemsetAsync(ix->q_bf16.p, 0, ix->q_bf16.n * sizeof(uint16_t), ix->stream));
@@ -672,10 +673,10 @@ rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, i
   return run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr);
 }
 
-rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, double min_score) {
+rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double min_score) {
   ix->stats.searches++;
   ix->stats.queries += B;
-  ix->stats.last_kprime = k_fetch;
+  ix->stats.last_kprime = k_eff;
   CK(ix->lg_theta.ensure(B));
   CK(ix->lg_cap.ensure(B));
   CK(ix->lg_cnt.ensure(B));
@@ -696,69 +697,14 @@ rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, doubl
   for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
     const int Bs = std::min(kMaxSubBatch, B - q0);
     if (q0 > 0) CK(zero_scan_scratch(ix, Bs));
-    const LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch);
+    const LargeScanParams sp = large_scan_params(ix, q0, Bs, k_eff);
     st = launch_sub_batch<kScanCount>(ix, q0, sp);
     if (st != RBK_OK) return st;
-    CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Bs, k_fetch, ix->lg_theta.p + q0,
+    CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Bs, k_eff, ix->lg_theta.p + q0,
                            ix->lg_cap.p + q0, ix->stream));
     ix->stats.kernel_launches++;
   }
   CK(cudaMemcpyAsync(ix->h_lcap.p, ix->lg_cap.p, sizeof(int) * B, cudaMemcpyDeviceToHost, ix->stream));
-  return RBK_OK;
-}
-
-rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long long* d_slots, double* d_scores,
-                      int* d_counts) {
-  CK(cudaMemsetAsync(ix->lg_err.p, 0, sizeof(int), ix->stream));
-  CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
-  if (ix->n_rows == 0) return fill_empty_results(ix, B, k_fetch, d_slots, d_scores, d_counts);
-  // segment offsets: exclusive prefix sum of C_q
-  long long total = 0;
-  for (int b = 0; b < B; ++b) {
-    ix->h_loff.p[b] = total;
-    total += ix->h_lcap.p[b];
-  }
-  CK(ix->lg_rows.ensure(static_cast<size_t>(std::max<long long>(total, 1))));
-  CK(ix->lg_scores.ensure(static_cast<size_t>(std::max<long long>(total, 1))));
-  CK(cudaMemcpyAsync(ix->lg_off.p, ix->h_loff.p, sizeof(long long) * B, cudaMemcpyHostToDevice, ix->stream));
-  CK(cudaMemsetAsync(ix->lg_cnt.p, 0, sizeof(int) * B, ix->stream));
-  for (int q0 = 0; q0 < B; q0 += kMaxSubBatch) {
-    const int Bs = std::min(kMaxSubBatch, B - q0);
-    LargeScanParams sp = large_scan_params(ix, q0, Bs, k_fetch);
-    sp.thr_init = ix->lg_theta.p + q0;   // theta_q
-    sp.emit_off = ix->lg_off.p + q0;
-    sp.emit_cap = ix->lg_cap.p + q0;
-    sp.emit_cnt = ix->lg_cnt.p + q0;
-    sp.emit_rows = ix->lg_rows.p;
-    CK(cudaMemsetAsync(sp.progress, 0, sizeof(int) * progress_slots(ix), ix->stream));
-    rbk_status st = launch_sub_batch<kScanEmit>(ix, q0, sp);
-    if (st != RBK_OK) return st;
-    LargeRerankParams rp;
-    rp.B = Bs;
-    rp.d = ix->dim;
-    rp.dpad = ix->dpad;
-    rp.k_fetch = k_fetch;
-    rp.min_score = min_score;
-    rp.rows = ix->rows;
-    rp.rows_f64 = ix->rows_f64;
-    rp.row_norm2 = ix->norm2;
-    rp.slot = ix->slot;
-    rp.q_f64 = ix->q_f64.p + static_cast<size_t>(q0) * ix->dim;
-    rp.q_norm2 = ix->q_norm2.p + q0;
-    rp.emit_off = sp.emit_off;
-    rp.emit_cap = sp.emit_cap;
-    rp.emit_cnt = sp.emit_cnt;
-    rp.emit_rows = ix->lg_rows.p;
-    rp.cand_scores = ix->lg_scores.p;
-    rp.out_slots = d_slots + static_cast<size_t>(q0) * k_fetch;
-    rp.out_scores = d_scores + static_cast<size_t>(q0) * k_fetch;
-    rp.out_counts = d_counts + q0;
-    rp.overflow = ix->lg_err.p;
-    const int max_cap = *std::max_element(ix->h_lcap.p + q0, ix->h_lcap.p + q0 + Bs);
-    CK(launch_large_rerank(rp, max_cap, ix->f64_on_host, ix->stream));
-    ix->stats.kernel_launches += max_cap > 0 ? 2 : 1;
-  }
-  CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
   return RBK_OK;
 }
 
@@ -774,7 +720,7 @@ std::vector<std::pair<int, int>> split_by_budget(const std::vector<int64_t>& cos
   int q0 = 0;
   int64_t used = 0;
   for (int b = 0; b < B; ++b) {
-    if (b > q0 && used + cost[b] > kUnboundedBudget) {
+    if (b > q0 && used + cost[b] > kLargeBudget) {
       groups.emplace_back(q0, b);
       q0 = b;
       used = 0;
@@ -787,38 +733,45 @@ std::vector<std::pair<int, int>> split_by_budget(const std::vector<int64_t>& cos
 
 static int64_t sort_tiles(int cap) { return (cap + kSortTile - 1) / kSortTile; }
 
-rbk_status unbounded_prepare(rbk_index* ix, int B, const std::vector<std::pair<int, int>>& groups) {
-  CK(ix->h_utoff.ensure(B));
-  CK(ix->ub_toff.ensure(B));
+rbk_status large_prepare(rbk_index* ix, int B, bool sorted, const std::vector<std::pair<int, int>>& groups) {
+  if (sorted) {
+    CK(ix->h_utoff.ensure(B));
+    CK(ix->ub_toff.ensure(B));
+  }
   int64_t max_cand = 1, max_tiles = 1;
   for (const auto& gr : groups) {
     int64_t cand = 0, tiles = 0;
     for (int b = gr.first; b < gr.second; ++b) {
       ix->h_loff.p[b] = cand;
-      ix->h_utoff.p[b] = static_cast<int>(tiles);
       cand += ix->h_lcap.p[b];
-      tiles += sort_tiles(ix->h_lcap.p[b]);
+      if (sorted) {
+        ix->h_utoff.p[b] = static_cast<int>(tiles);
+        tiles += sort_tiles(ix->h_lcap.p[b]);
+      }
     }
     max_cand = std::max(max_cand, cand);
     max_tiles = std::max(max_tiles, tiles);
   }
   CK(ix->lg_rows.ensure(static_cast<size_t>(max_cand)));
   CK(ix->lg_scores.ensure(static_cast<size_t>(max_cand)));
-  CK(ix->ub_rows.ensure(static_cast<size_t>(max_cand)));
-  CK(ix->ub_scores.ensure(static_cast<size_t>(max_cand)));
-  CK(ix->ub_len.ensure(static_cast<size_t>(2 * max_tiles)));
   CK(cudaMemcpyAsync(ix->lg_off.p, ix->h_loff.p, sizeof(long long) * B, cudaMemcpyHostToDevice, ix->stream));
-  CK(cudaMemcpyAsync(ix->ub_toff.p, ix->h_utoff.p, sizeof(int) * B, cudaMemcpyHostToDevice, ix->stream));
+  if (sorted) {
+    CK(ix->ub_rows.ensure(static_cast<size_t>(max_cand)));
+    CK(ix->ub_scores.ensure(static_cast<size_t>(max_cand)));
+    CK(ix->ub_len.ensure(static_cast<size_t>(2 * max_tiles)));
+    CK(cudaMemcpyAsync(ix->ub_toff.p, ix->h_utoff.p, sizeof(int) * B, cudaMemcpyHostToDevice, ix->stream));
+  }
   CK(cudaMemsetAsync(ix->lg_cnt.p, 0, sizeof(int) * B, ix->stream));
   CK(cudaMemsetAsync(ix->lg_err.p, 0, sizeof(int), ix->stream));
   return RBK_OK;
 }
 
-rbk_status unbounded_emit(rbk_index* ix, int q0, int q1, int k_eff, double min_score, long long* d_slots,
-                          double* d_scores, int* d_counts) {
+rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, double min_score, long long* d_slots,
+                      double* d_scores, int* d_counts) {
   if (ix->n_rows == 0) return fill_empty_results(ix, q1 - q0, k_eff, d_slots, d_scores, d_counts);
   int64_t group_tiles = 0;
-  for (int b = q0; b < q1; ++b) group_tiles += sort_tiles(ix->h_lcap.p[b]);
+  if (sorted)
+    for (int b = q0; b < q1; ++b) group_tiles += sort_tiles(ix->h_lcap.p[b]);
   for (int s0 = q0; s0 < q1; s0 += kMaxSubBatch) {
     const int Bs = std::min(kMaxSubBatch, q1 - s0);
     LargeScanParams sp = large_scan_params(ix, s0, Bs, k_eff);
@@ -851,22 +804,24 @@ rbk_status unbounded_emit(rbk_index* ix, int q0, int q1, int k_eff, double min_s
     rp.out_scores = d_scores + static_cast<size_t>(s0 - q0) * k_eff;
     rp.out_counts = d_counts + (s0 - q0);
     rp.overflow = ix->lg_err.p;
-    SegSortScratch ss;
-    ss.tile_off = ix->ub_toff.p + s0;
-    ss.scores = ix->ub_scores.p;
-    ss.rows = ix->ub_rows.p;
-    ss.len[0] = ix->ub_len.p;
-    ss.len[1] = ix->ub_len.p + group_tiles;
     const int max_cap = *std::max_element(ix->h_lcap.p + s0, ix->h_lcap.p + s0 + Bs);
-    ss.max_tiles = static_cast<int>(sort_tiles(max_cap));
+    SegSortScratch ss;
+    if (sorted) {
+      ss.tile_off = ix->ub_toff.p + s0;
+      ss.scores = ix->ub_scores.p;
+      ss.rows = ix->ub_rows.p;
+      ss.len[0] = ix->ub_len.p;
+      ss.len[1] = ix->ub_len.p + group_tiles;
+      ss.max_tiles = static_cast<int>(sort_tiles(max_cap));
+    }
     int launches = 0;
-    CK(launch_unbounded_rerank(rp, ss, max_cap, ix->f64_on_host, ix->stream, &launches));
+    CK(launch_large_rerank(rp, sorted ? &ss : nullptr, max_cap, ix->f64_on_host, ix->stream, &launches));
     ix->stats.kernel_launches += launches;
   }
   return RBK_OK;
 }
 
-rbk_status unbounded_finish(rbk_index* ix) {
+rbk_status large_finish(rbk_index* ix) {
   CK(cudaMemcpyAsync(ix->h_lerr.p, ix->lg_err.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
   return RBK_OK;
 }
@@ -1518,11 +1473,15 @@ rbk_status rbk_index_search_device(rbk_index* ix, const void* dev_queries_f32, i
                      static_cast<int*>(dev_out_counts), nullptr, nullptr, nullptr, nullptr);
 }
 
-rbk_status rbk_index_search_large_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
-                                      int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
-                                      int32_t* out_counts, float* kernel_ms_out) {
+namespace {
+// The large-k search for k_fetch in [1, max_k] (rbk_index_impl.h): the count scan, one wait, then per query group
+// the emit scan and the cut into o_block, its D2H into the pinned h_block, a wait, and the copy into the caller's rows
+// of k_fetch entries.
+rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
+                        double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
+                        float* kernel_ms_out) {
   if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
-  rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, RBK_MAX_K_FETCH_LARGE);
+  rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
   if (st != RBK_OK) return st;
   std::lock_guard<std::mutex> lk(ix->mu);
   DeviceGuard dg(ix->device);
@@ -1531,59 +1490,17 @@ rbk_status rbk_index_search_large_f64(rbk_index* ix, const double* queries, int3
     ix->stats.searches++;
     return RBK_OK;
   }
-  st = ensure_query_scratch(ix, B, 8);
-  if (st != RBK_OK) return st;
-  const ResultBlock L(B, k_fetch);
-  const size_t blk = L.off_counts + sizeof(int32_t) * B;   // no flags: every answer is exact by construction
-  CK(ix->o_block.ensure(blk));
-  CK(ix->h_block.ensure(blk));
-  unsigned char* base = ix->o_block.p;
-  TimedSearch ts{ix};
-  st = ts.begin();
-  if (st != RBK_OK) return st;
-  CK(cudaMemcpyAsync(ix->q_raw.p, queries, static_cast<size_t>(B) * ix->dim * 8, cudaMemcpyHostToDevice, ix->stream));
-  st = large_count(ix, ix->q_raw.p, B, k_fetch, min_score);
-  if (st != RBK_OK) return st;
-  CK(cudaStreamSynchronize(ix->stream));   // C_q sizes the candidate buffer
-  st = large_emit(ix, B, k_fetch, min_score, L.slots(base), L.scores(base), L.counts(base));
-  if (st != RBK_OK) return st;
-  CK(cudaMemcpyAsync(ix->h_block.p, base, blk, cudaMemcpyDeviceToHost, ix->stream));
-  st = ts.round_trip();
-  if (st != RBK_OK) return st;
-  st = large_check(ix);
-  if (st != RBK_OK) return st;
-  ts.finish(kernel_ms_out);
-  L.unpack(ix->h_block.p, out_slots, out_scores, out_counts);
-  return RBK_OK;
-}
-
-rbk_status rbk_index_search_unbounded_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
-                                          int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
-                                          int32_t* out_counts, float* kernel_ms_out) {
-  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
-  rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, INT32_MAX);
-  if (st != RBK_OK) return st;
-  if (k_fetch <= RBK_MAX_K_FETCH_LARGE)
-    return rbk_index_search_large_f64(ix, queries, B, query_dim, k_fetch, min_score, out_slots, out_scores,
-                                      out_counts, kernel_ms_out);
-  std::lock_guard<std::mutex> lk(ix->mu);
-  DeviceGuard dg(ix->device);
-  if (kernel_ms_out) *kernel_ms_out = 0.f;
-  if (B == 0) {
-    ix->stats.searches++;
-    return RBK_OK;
-  }
-  // no query can have more hits than there are live rows: every buffer is sized by k_eff
-  const int k_eff = static_cast<int>(std::min<int64_t>(k_fetch, ix->n_live));
-  fill_result_tail(out_slots, out_scores, B, k_fetch, k_eff);
+  const bool sorted = k_fetch > RBK_MAX_K_FETCH_LARGE;
+  // the sort's buffers are sized by k_eff: no query can have more hits than there are live rows
+  const int k_eff = sorted ? static_cast<int>(std::min<int64_t>(k_fetch, ix->n_live)) : k_fetch;
   if (k_eff == 0) {
+    fill_result_tail(out_slots, out_scores, B, k_fetch, 0);
     memset(out_counts, 0, sizeof(int32_t) * B);
     ix->stats.searches++;
     ix->stats.queries += B;
     return RBK_OK;
   }
-  // a query group may start at any query: kBlockM rows of slack keep its query map inside the buffer
-  st = ensure_query_scratch(ix, B, 8, kBlockM);
+  st = ensure_query_scratch(ix, B, 8);
   if (st != RBK_OK) return st;
   TimedSearch ts{ix};
   st = ts.begin();
@@ -1593,37 +1510,47 @@ rbk_status rbk_index_search_unbounded_f64(rbk_index* ix, const double* queries, 
   if (st != RBK_OK) return st;
   CK(cudaStreamSynchronize(ix->stream));   // C_q sizes the candidate buffers and the query groups
   std::vector<int64_t> cost(B);
-  for (int b = 0; b < B; ++b) cost[b] = ix->h_lcap.p[b] * kUnboundedCandBytes + unbounded_result_bytes(k_eff);
+  for (int b = 0; b < B; ++b) cost[b] = ix->h_lcap.p[b] * large_cand_bytes(sorted) + large_result_bytes(k_eff);
   const std::vector<std::pair<int, int>> groups = split_by_budget(cost);
-  st = unbounded_prepare(ix, B, groups);
+  st = large_prepare(ix, B, sorted, groups);
   if (st != RBK_OK) return st;
   int max_group = 0;
   for (const auto& gr : groups) max_group = std::max(max_group, gr.second - gr.first);
-  const ResultBlock L(max_group, k_eff);
-  CK(ix->o_block.ensure(L.off_counts + sizeof(int32_t) * max_group));
+  // no flags: every answer is exact by construction
+  const size_t blk = ResultBlock(max_group, k_eff).off_counts + sizeof(int32_t) * max_group;
+  CK(ix->o_block.ensure(blk));
+  CK(ix->h_block.ensure(blk));
   for (const auto& gr : groups) {
-    const int Bg = gr.second - gr.first;
-    const ResultBlock R(Bg, k_eff);
+    const ResultBlock R(gr.second - gr.first, k_eff);
     unsigned char* base = ix->o_block.p;
-    st = unbounded_emit(ix, gr.first, gr.second, k_eff, min_score, R.slots(base), R.scores(base), R.counts(base));
+    st = large_emit(ix, gr.first, gr.second, sorted, k_eff, min_score, R.slots(base), R.scores(base), R.counts(base));
+    if (st == RBK_OK && gr.second == B) st = large_finish(ix);   // the overflow count rides the last round trip
     if (st != RBK_OK) return st;
-    // straight into the caller's rows of k_fetch entries (stream-ordered before the next group reuses the block)
-    const size_t row = sizeof(int64_t) * k_eff, pitch = sizeof(int64_t) * static_cast<size_t>(k_fetch);
-    CK(cudaMemcpy2DAsync(out_slots + static_cast<size_t>(gr.first) * k_fetch, pitch, R.slots(base), row, row, Bg,
-                         cudaMemcpyDeviceToHost, ix->stream));
-    CK(cudaMemcpy2DAsync(out_scores + static_cast<size_t>(gr.first) * k_fetch, pitch, R.scores(base), row, row, Bg,
-                         cudaMemcpyDeviceToHost, ix->stream));
-    CK(cudaMemcpyAsync(out_counts + gr.first, R.counts(base), sizeof(int32_t) * Bg, cudaMemcpyDeviceToHost,
-                       ix->stream));
+    CK(cudaMemcpyAsync(ix->h_block.p, base, R.off_counts + sizeof(int32_t) * R.B, cudaMemcpyDeviceToHost, ix->stream));
+    st = ts.round_trip();
+    if (st != RBK_OK) return st;
+    const size_t o = static_cast<size_t>(gr.first) * k_fetch;
+    R.unpack_rows(ix->h_block.p, k_fetch, out_slots + o, out_scores + o, out_counts + gr.first);
   }
-  st = unbounded_finish(ix);
-  if (st != RBK_OK) return st;
-  st = ts.round_trip();
-  if (st != RBK_OK) return st;
   st = large_check(ix);
   if (st != RBK_OK) return st;
   ts.finish(kernel_ms_out);
   return RBK_OK;
+}
+}  // namespace
+
+rbk_status rbk_index_search_large_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
+                                      int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* kernel_ms_out) {
+  return search_large(ix, queries, B, query_dim, k_fetch, min_score, RBK_MAX_K_FETCH_LARGE, out_slots, out_scores,
+                      out_counts, kernel_ms_out);
+}
+
+rbk_status rbk_index_search_unbounded_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
+                                          int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
+                                          int32_t* out_counts, float* kernel_ms_out) {
+  return search_large(ix, queries, B, query_dim, k_fetch, min_score, INT32_MAX, out_slots, out_scores, out_counts,
+                      kernel_ms_out);
 }
 
 rbk_status rbk_index_exact_scores_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,

@@ -1322,26 +1322,8 @@ cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init,
   return cudaGetLastError();
 }
 
-cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, bool rows_on_host, cudaStream_t stream) {
-  if (p.B <= 0) return cudaSuccess;
-  if (max_cap > 0) {
-    dim3 grid(static_cast<unsigned>((max_cap + 255) / 256), static_cast<unsigned>(p.B));
-    if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
-    else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-  }
-  int S = 2048;
-  while (S < p.k_fetch + kTopThreads) S <<= 1;
-  const size_t smem = static_cast<size_t>(S) * (sizeof(double) + sizeof(int));
-  cudaError_t e = cudaFuncSetAttribute(large_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  large_topk_kernel<<<p.B, kTopThreads, smem, stream>>>(p, S);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_unbounded_rerank(const LargeRerankParams& p, const SegSortScratch& s, int max_cap,
-                                    bool rows_on_host, cudaStream_t stream, int* launches) {
+cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
+                                bool rows_on_host, cudaStream_t stream, int* launches) {
   *launches = 0;
   if (p.B <= 0) return cudaSuccess;
   cudaError_t e;
@@ -1352,6 +1334,17 @@ cudaError_t launch_unbounded_rerank(const LargeRerankParams& p, const SegSortScr
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
   }
+  if (!sort) {   // the cut in shared memory, one block per query
+    int S = 2048;
+    while (S < p.k_fetch + kTopThreads) S <<= 1;
+    const size_t smem = static_cast<size_t>(S) * (sizeof(double) + sizeof(int));
+    e = cudaFuncSetAttribute(large_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    large_topk_kernel<<<p.B, kTopThreads, smem, stream>>>(p, S);
+    ++*launches;
+    return cudaGetLastError();
+  }
+  const SegSortScratch& s = *sort;
   int passes = 0;
   if (s.max_tiles > 0) {
     const size_t smem = static_cast<size_t>(kSortTile) * (sizeof(double) + sizeof(int));

@@ -151,10 +151,9 @@ int64_t merged_bytes(const ResultBlock& L) { return dirty_word(L) + 4; }
 // per PCIe link), the member's query scratch, then enqueue(d, ix) with the member's lock held and its device current.
 // zero_dirty: the caller reads the dirty count, which the merge kernel adds to - start it from zero (its position
 // depends on B and k_fetch, so a running count across calls of different shapes would be garbage).
-// q_slack_rows: as for ensure_query_scratch.
 template <typename F>
 rbk_status stage_and_enqueue(rbk_group* g, const void* queries, int elem, const ResultBlock& L, bool zero_dirty,
-                             F&& enqueue, int q_slack_rows = 0) {
+                             F&& enqueue) {
   const int B = static_cast<int>(L.B);
   const size_t q_bytes = static_cast<size_t>(B) * g->dim * elem;
   {
@@ -174,7 +173,7 @@ rbk_status stage_and_enqueue(rbk_group* g, const void* queries, int elem, const 
     if (g->G > 1) CK(g->dev[d].all.ensure(L.bytes * g->G));
     if (d == 0) CK(cudaEventRecord(g->ev0, ix->stream));
     CK(cudaMemcpyAsync(g->dev[d].q.p, g->h_q.p, q_bytes, cudaMemcpyHostToDevice, ix->stream));
-    rbk_status st = ensure_query_scratch(ix, B, elem, q_slack_rows);
+    rbk_status st = ensure_query_scratch(ix, B, elem);
     if (st != RBK_OK) return st;
     st = enqueue(d, ix);
     if (st != RBK_OK) return st;
@@ -262,82 +261,32 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
   return RBK_OK;
 }
 
-// Large-k search over the group: count scan + select on every device, ONE wait for all of them (C_q sizes each
-// device's candidate buffer), emit scan + exact re-rank on every device into its packed block (flags zero: the
-// answers are exact by construction), then the all-gather and merge of group_search.
+// Large-k search over the group, k_fetch in [1, max_k] (the pipeline and the k_eff / cut rule of rbk_index_impl.h):
+// the count scan on every device and ONE wait for all of them, then the queries in contiguous groups whose candidates
+// on all devices together, plus the result blocks they move, fit kLargeBudget.  Per query group: emit scan, exact
+// re-score and cut on every device into its packed block of k_eff entries per query (flags zero: the answers are
+// exact by construction), the all-gather and merge of group_search, and the copy into the caller's rows of k_fetch
+// entries.
 rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
-                              double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts,
+                              double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
                               float* ms_out) {
   if (!g) return fail(RBK_EINVAL, "null group");
   if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
-  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score,
-                                    RBK_MAX_K_FETCH_LARGE);
+  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
   if (st != RBK_OK) return st;
   if (ms_out) *ms_out = 0.f;
   if (B == 0) return RBK_OK;
   std::lock_guard<std::mutex> lk(g->mu);
-  const ResultBlock L(B, k_fetch);
-  st = stage_and_enqueue(g, queries, 8, L, /*zero_dirty=*/false, [&](int d, rbk_index* ix) {
-    return large_count(ix, g->dev[d].q.p, B, k_fetch, min_score);
-  });
-  if (st != RBK_OK) return st;
-  for (int d = 0; d < g->G; ++d) {
-    DeviceGuard dg(g->parts[d]->device);
-    CK(cudaStreamSynchronize(g->parts[d]->stream));
-  }
-  for (int d = 0; d < g->G; ++d) {
-    rbk_index* ix = g->parts[d];
-    std::lock_guard<std::mutex> il(ix->mu);
-    DeviceGuard dg(ix->device);
-    unsigned char* l = g->dev[d].local.p;
-    st = large_emit(ix, B, k_fetch, min_score, L.slots(l), L.scores(l), L.counts(l));
-    if (st != RBK_OK) return st;
-    CK(cudaMemsetAsync(L.flags(l), 0, static_cast<size_t>(B) * 4, ix->stream));
-  }
-  st = exchange_and_merge(g, L, k_fetch);
-  if (st != RBK_OK) return st;
-  st = collect(g, L);
-  if (st != RBK_OK) return st;
-  for (int d = 0; d < g->G; ++d) {   // every device's overflow counter has landed on the host
-    if (d > 0) {                     // (collect has waited for device 0)
-      DeviceGuard dg(g->parts[d]->device);
-      CK(cudaStreamSynchronize(g->parts[d]->stream));
-    }
-    st = large_check(g->parts[d]);
-    if (st != RBK_OK) return st;
-  }
-  if (ms_out) cudaEventElapsedTime(ms_out, g->ev0, g->ev1);
-  L.unpack(g->h_out.p, out_slots, out_scores, out_counts);
-  return RBK_OK;
-}
-
-// Unbounded search over the group (k_fetch > RBK_MAX_K_FETCH_LARGE; below it, group_search_large): the count scan on
-// every device and ONE wait for all of them, then the queries in contiguous groups whose candidates on all devices
-// together, plus the result blocks they move, fit kUnboundedBudget.  Per query group: emit scan, exact re-score and
-// segmented sort on every device into its packed block of k_eff = count() entries per query, the all-gather and merge
-// of group_search, and the copy into the caller's rows of k_fetch entries.
-rbk_status group_search_unbounded(rbk_group* g, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
-                                  double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts,
-                                  float* ms_out) {
-  if (!g) return fail(RBK_EINVAL, "null group");
-  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
-  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score, INT32_MAX);
-  if (st != RBK_OK) return st;
-  if (k_fetch <= RBK_MAX_K_FETCH_LARGE)
-    return group_search_large(g, queries, B, query_dim, k_fetch, min_score, out_slots, out_scores, out_counts, ms_out);
-  if (ms_out) *ms_out = 0.f;
-  if (B == 0) return RBK_OK;
-  std::lock_guard<std::mutex> lk(g->mu);
-  const int k_eff = static_cast<int>(std::min<int64_t>(k_fetch, rbk_group_count(g)));
-  fill_result_tail(out_slots, out_scores, B, k_fetch, k_eff);
+  const bool sorted = k_fetch > RBK_MAX_K_FETCH_LARGE;
+  const int k_eff = sorted ? static_cast<int>(std::min<int64_t>(k_fetch, rbk_group_count(g))) : k_fetch;
   if (k_eff == 0) {
+    fill_result_tail(out_slots, out_scores, B, k_fetch, 0);
     memset(out_counts, 0, sizeof(int32_t) * B);
     return RBK_OK;
   }
-  // query groups may start at any query: kBlockM rows of query slack on every member (ensure_query_scratch)
-  st = stage_and_enqueue(
-      g, queries, 8, ResultBlock(B, 1), /*zero_dirty=*/false,
-      [&](int d, rbk_index* ix) { return large_count(ix, g->dev[d].q.p, B, k_eff, min_score); }, kBlockM);
+  st = stage_and_enqueue(g, queries, 8, ResultBlock(B, 1), /*zero_dirty=*/false, [&](int d, rbk_index* ix) {
+    return large_count(ix, g->dev[d].q.p, B, k_eff, min_score);
+  });
   if (st != RBK_OK) return st;
   for (int d = 0; d < g->G; ++d) {
     DeviceGuard dg(g->parts[d]->device);
@@ -347,8 +296,8 @@ rbk_status group_search_unbounded(rbk_group* g, const double* queries, int32_t B
   // the merged block
   std::vector<int64_t> cost(B);
   for (int b = 0; b < B; ++b) {
-    cost[b] = (g->G + 2) * unbounded_result_bytes(k_eff);
-    for (rbk_index* ix : g->parts) cost[b] += ix->h_lcap.p[b] * kUnboundedCandBytes;
+    cost[b] = (g->G + 2) * large_result_bytes(k_eff);
+    for (rbk_index* ix : g->parts) cost[b] += ix->h_lcap.p[b] * large_cand_bytes(sorted);
   }
   const std::vector<std::pair<int, int>> groups = split_by_budget(cost);
   int max_group = 0;
@@ -365,7 +314,7 @@ rbk_status group_search_unbounded(rbk_group* g, const double* queries, int32_t B
     DeviceGuard dg(ix->device);
     CK(g->dev[d].local.ensure(Lmax.bytes));
     if (g->G > 1) CK(g->dev[d].all.ensure(Lmax.bytes * g->G));
-    st = unbounded_prepare(ix, B, groups);
+    st = large_prepare(ix, B, sorted, groups);
     if (st != RBK_OK) return st;
   }
   for (const auto& gr : groups) {
@@ -376,7 +325,8 @@ rbk_status group_search_unbounded(rbk_group* g, const double* queries, int32_t B
       std::lock_guard<std::mutex> il(ix->mu);
       DeviceGuard dg(ix->device);
       unsigned char* l = g->dev[d].local.p;
-      st = unbounded_emit(ix, gr.first, gr.second, k_eff, min_score, L.slots(l), L.scores(l), L.counts(l));
+      st = large_emit(ix, gr.first, gr.second, sorted, k_eff, min_score, L.slots(l), L.scores(l), L.counts(l));
+      if (st == RBK_OK && gr.second == B) st = large_finish(ix);   // the overflow count rides the last round trip
       if (st != RBK_OK) return st;
       CK(cudaMemsetAsync(L.flags(l), 0, static_cast<size_t>(Bg) * 4, ix->stream));
     }
@@ -384,22 +334,15 @@ rbk_status group_search_unbounded(rbk_group* g, const double* queries, int32_t B
     if (st != RBK_OK) return st;
     st = collect(g, L);
     if (st != RBK_OK) return st;
-    unsigned char* h = g->h_out.p;
-    for (int b = 0; b < Bg; ++b) {
-      const size_t src = static_cast<size_t>(b) * k_eff, dst = static_cast<size_t>(gr.first + b) * k_fetch;
-      memcpy(out_slots + dst, L.slots(h) + src, sizeof(int64_t) * k_eff);
-      memcpy(out_scores + dst, L.scores(h) + src, sizeof(double) * k_eff);
-    }
-    memcpy(out_counts + gr.first, L.counts(h), sizeof(int32_t) * Bg);
+    const size_t o = static_cast<size_t>(gr.first) * k_fetch;
+    L.unpack_rows(g->h_out.p, k_fetch, out_slots + o, out_scores + o, out_counts + gr.first);
   }
-  for (int d = 0; d < g->G; ++d) {   // every device's overflow counter
-    rbk_index* ix = g->parts[d];
-    std::lock_guard<std::mutex> il(ix->mu);
-    DeviceGuard dg(ix->device);
-    st = unbounded_finish(ix);
-    if (st != RBK_OK) return st;
-    CK(cudaStreamSynchronize(ix->stream));
-    st = large_check(ix);
+  for (int d = 0; d < g->G; ++d) {   // every device's overflow counter has landed on the host
+    if (d > 0) {                     // (collect has waited for device 0)
+      DeviceGuard dg(g->parts[d]->device);
+      CK(cudaStreamSynchronize(g->parts[d]->stream));
+    }
+    st = large_check(g->parts[d]);
     if (st != RBK_OK) return st;
   }
   if (ms_out) cudaEventElapsedTime(ms_out, g->ev0, g->ev1);
@@ -597,14 +540,14 @@ rbk_status rbk_group_search_f64(rbk_group* g, const double* queries, int32_t B, 
 rbk_status rbk_group_search_large_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,
                                       int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                       int32_t* out_counts, float* device_ms_out) {
-  return group_search_large(g, queries, B, query_dim, k_fetch, min_score, out_slots, out_scores, out_counts,
-                            device_ms_out);
+  return group_search_large(g, queries, B, query_dim, k_fetch, min_score, RBK_MAX_K_FETCH_LARGE, out_slots, out_scores,
+                            out_counts, device_ms_out);
 }
 rbk_status rbk_group_search_unbounded_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,
                                           int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                           int32_t* out_counts, float* device_ms_out) {
-  return group_search_unbounded(g, queries, B, query_dim, k_fetch, min_score, out_slots, out_scores, out_counts,
-                                device_ms_out);
+  return group_search_large(g, queries, B, query_dim, k_fetch, min_score, INT32_MAX, out_slots, out_scores, out_counts,
+                            device_ms_out);
 }
 
 }  // extern "C"

@@ -86,6 +86,22 @@ struct DeviceGuard {
   }
 };
 
+// Entries [k_eff, k_fetch) of each of the B result rows of k_fetch entries: slot -1, score NaN (a large-k search
+// keeps at most k_eff = count() hits per query).
+inline void fill_result_tail(int64_t* slots, double* scores, int32_t B, int32_t k_fetch, int32_t k_eff) {
+  if (k_eff >= k_fetch) return;
+  const uint64_t nan_bits = 0x7FF8000000000000ull;   // the quiet NaN the device kernels write
+  double nan;
+  memcpy(&nan, &nan_bits, sizeof nan);
+  for (int32_t b = 0; b < B; ++b) {
+    const size_t o = static_cast<size_t>(b) * k_fetch;
+    for (int32_t i = k_eff; i < k_fetch; ++i) {
+      slots[o + i] = -1;
+      scores[o + i] = nan;
+    }
+  }
+}
+
 // Byte layout of one search's results as one block, so that they and the exactness flags move in one copy:
 //   slots i64 [B][k_fetch] | scores f64 [B][k_fetch] | counts i32 [B] | flags i32 [B]
 // counts and flags each padded to 16 bytes.  The C ABI publishes it (rbk_packed_block_bytes / rbk_packed_flags_offset):
@@ -106,23 +122,19 @@ struct ResultBlock {
     memcpy(out_scores, p + off_scores, sizeof(double) * nk);
     memcpy(out_counts, p + off_counts, sizeof(int32_t) * B);
   }
-};
-
-// Entries [k_eff, k_fetch) of each of the B result rows of k_fetch entries: slot -1, score NaN (an unbounded search
-// keeps at most k_eff = count() hits per query).
-inline void fill_result_tail(int64_t* slots, double* scores, int32_t B, int32_t k_fetch, int32_t k_eff) {
-  if (k_eff >= k_fetch) return;
-  const uint64_t nan_bits = 0x7FF8000000000000ull;   // the quiet NaN the device kernels write
-  double nan;
-  memcpy(&nan, &nan_bits, sizeof nan);
-  for (int32_t b = 0; b < B; ++b) {
-    const size_t o = static_cast<size_t>(b) * k_fetch;
-    for (int32_t i = k_eff; i < k_fetch; ++i) {
-      slots[o + i] = -1;
-      scores[o + i] = nan;
+  // copies a host block of k entries per query out to the caller's rows of k_fetch >= k entries, out_* pointing at
+  // the block's first query; entries [k, k_fetch) of each row get slot -1, score NaN
+  void unpack_rows(const void* h, int32_t k_fetch, int64_t* out_slots, double* out_scores, int32_t* out_counts) const {
+    const char* p = static_cast<const char*>(h);
+    const int64_t k = B > 0 ? nk / B : 0;
+    for (int64_t b = 0; b < B; ++b) {
+      memcpy(out_slots + b * k_fetch, p + sizeof(int64_t) * b * k, sizeof(int64_t) * k);
+      memcpy(out_scores + b * k_fetch, p + off_scores + sizeof(double) * b * k, sizeof(double) * k);
     }
+    memcpy(out_counts, p + off_counts, sizeof(int32_t) * B);
+    fill_result_tail(out_slots, out_scores, static_cast<int32_t>(B), k_fetch, static_cast<int32_t>(k));
   }
-}
+};
 
 }  // namespace impl
 }  // namespace rbk
@@ -176,7 +188,8 @@ struct rbk_index {
   rbk::impl::DevBuf<double> lg_scores;
   rbk::impl::PinBuf<int> h_lcap, h_lerr;
   rbk::impl::PinBuf<long long> h_loff;
-  // unbounded search scratch (grow-only): per-query first run-length slot, the sort's second buffer, run lengths
+  // segmented sort scratch (grow-only, k_fetch > RBK_MAX_K_FETCH_LARGE only): per-query first run-length slot, the
+  // sort's second buffer, run lengths
   rbk::impl::DevBuf<int> ub_toff, ub_rows, ub_len;
   rbk::impl::DevBuf<double> ub_scores;
   rbk::impl::PinBuf<int> h_utoff;
@@ -216,11 +229,11 @@ struct rbk_index {
 namespace rbk {
 namespace impl {
 
-// caller holds ix->mu and has the index's device current.  slack_rows: zeroed bf16 query rows beyond the last whole
-// query block, for callers whose scan launches start at a query that is not a multiple of kBlockM (the unbounded
-// search's query groups): such a launch's query map covers round_up(Bs, kBlockM) rows from its first query.
-rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem, int slack_rows = 0);
-// max_k: RBK_MAX_K_FETCH (the search) or RBK_MAX_K_FETCH_LARGE (the large-k search)
+// caller holds ix->mu and has the index's device current.  The scan's query buffer keeps kBlockM zeroed rows beyond
+// the last whole query block, so that a scan launch may start at any query (a large-k search's query groups): such a
+// launch's query map covers round_up(Bs, kBlockM) rows from its first query.
+rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem);
+// max_k: RBK_MAX_K_FETCH (the search), RBK_MAX_K_FETCH_LARGE or INT32_MAX (the large-k searches)
 rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, int k_fetch, double min_score,
                              int max_k = RBK_MAX_K_FETCH);
 // Enqueue-only search of device-resident queries: no host synchronisation, exactness flags land in d_flags.
@@ -230,36 +243,32 @@ rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, i
 // fallback included: rbk_index_search_device for either query type.  Takes the index lock itself.
 rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, int k_fetch, double min_score,
                                long long* d_slots, double* d_scores, int* d_counts);
-// Large-k search of B device-resident f64 queries (caller holds the lock, scratch for B queries is allocated), in
-// two halves around one host synchronisation of the index stream:
-//   large_count: prep, count pass and select per sub-batch, then the D2H of C_q (enqueue only);
-//   large_emit : (after the stream has been synchronised) segment offsets on the host, emit pass and exact re-rank
-//                per sub-batch into d_slots / d_scores / d_counts, then the D2H of the overflow counter (enqueue only);
-//   large_check: (after the next synchronisation) RBK_ECUDA if any query emitted more rows than its bound.
-rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_fetch, double min_score);
-rbk_status large_emit(rbk_index* ix, int B, int k_fetch, double min_score, long long* d_slots, double* d_scores,
-                      int* d_counts);
-rbk_status large_check(rbk_index* ix);
-
-// Unbounded search (k_fetch > RBK_MAX_K_FETCH_LARGE), built on the same count pass: large_count with k_fetch = k_eff,
-// one host synchronisation, then the queries in contiguous groups whose device storage fits kUnboundedBudget, each
-// group costing one emit scan:
-//   split_by_budget   : the groups, from each query's cost in bytes (at least one query per group);
-//   unbounded_prepare : segment offsets and run-length slots of every query relative to its group, the scratch for
-//                       the largest group, zeroed emit and overflow counters (enqueue only);
-//   unbounded_emit    : emit scan, exact re-score and segmented sort of the queries [q0, q1) into d_slots / d_scores /
-//                       d_counts ([q1 - q0][k_eff]); enqueue only;
-//   unbounded_finish  : the D2H of the overflow counter, for large_check after the next synchronisation.
-constexpr int64_t kUnboundedBudget = 256ll << 20;
-// device bytes per candidate: emit row + exact score (sorted in place) + the sort's second buffer
-constexpr int64_t kUnboundedCandBytes = 4 + 8 + 12;
+// Large-k search of B device-resident f64 queries (caller holds the lock, scratch for B queries is allocated), for
+// any k_fetch above the scan's: the count scan, one host synchronisation, then the queries in contiguous groups whose
+// device storage fits kLargeBudget, each group costing one emit scan.  `sorted` (the caller's k_fetch is above
+// RBK_MAX_K_FETCH_LARGE) picks the cut: the segmented sort in global memory, or one block per query in shared memory.
+// k_eff is the number of entries kept per query: min(k_fetch, count()) when sorted, else k_fetch.
+//   large_count   : prep, count pass and select per sub-batch at k_eff, then the D2H of C_q (enqueue only);
+//   split_by_budget: (after the stream has been synchronised) the groups, from each query's cost in bytes (at least
+//                   one query per group);
+//   large_prepare : segment offsets (and, sorted, run-length slots) of every query relative to its group, the scratch
+//                   for the largest group, zeroed emit and overflow counters (enqueue only);
+//   large_emit    : emit scan, exact re-score and cut of the queries [q0, q1) into d_slots / d_scores / d_counts
+//                   ([q1 - q0][k_eff]); enqueue only;
+//   large_finish  : the D2H of the overflow counter (enqueue only);
+//   large_check   : (after the next synchronisation) RBK_ECUDA if any query emitted more rows than its bound.
+rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double min_score);
+constexpr int64_t kLargeBudget = 256ll << 20;
+// device bytes per candidate: emit row + exact score (sorted in place), and the sort's second buffer
+inline int64_t large_cand_bytes(bool sorted) { return sorted ? 4 + 8 + 12 : 4 + 8; }
 // device bytes of one query's result in a packed block of k_eff entries (slots, scores, count, flag)
-inline int64_t unbounded_result_bytes(int k_eff) { return 16ll * k_eff + 8; }
+inline int64_t large_result_bytes(int k_eff) { return 16ll * k_eff + 8; }
 std::vector<std::pair<int, int>> split_by_budget(const std::vector<int64_t>& cost);
-rbk_status unbounded_prepare(rbk_index* ix, int B, const std::vector<std::pair<int, int>>& groups);
-rbk_status unbounded_emit(rbk_index* ix, int q0, int q1, int k_eff, double min_score, long long* d_slots,
-                          double* d_scores, int* d_counts);
-rbk_status unbounded_finish(rbk_index* ix);
+rbk_status large_prepare(rbk_index* ix, int B, bool sorted, const std::vector<std::pair<int, int>>& groups);
+rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, double min_score, long long* d_slots,
+                      double* d_scores, int* d_counts);
+rbk_status large_finish(rbk_index* ix);
+rbk_status large_check(rbk_index* ix);
 const char* last_error();
 
 }  // namespace impl

@@ -192,22 +192,19 @@ struct LargeRerankParams {
   const long long* emit_off;
   const int* emit_cap;
   const int* emit_cnt;
-  int* emit_rows;           // written only by the unbounded search's in-place tile sort
+  int* emit_rows;           // written only by the segmented sort's in-place tile sort
   double* cand_scores;      // parallel to emit_rows
   long long* out_slots;     // [B][k_fetch]
   double* out_scores;       // [B][k_fetch]
   int* out_counts;          // [B]
   int* overflow;            // += queries whose emit pass found more rows than C_q (a broken count)
 };
-// max_cap: largest emit_cap of the launch (sizes the scoring grid).  rows_on_host: as for launch_finalize; the
-// scoring kernel then stages its candidates' rows in shared memory with coalesced loads.
-cudaError_t launch_large_rerank(const LargeRerankParams& p, int max_cap, bool rows_on_host, cudaStream_t stream);
 
-// ---- unbounded search (rbk_finalize.cu): the large-k re-score, then a segmented sort in global memory ----
-// Each query's segment of emit_rows / cand_scores is cut into tiles of kSortTile candidates (never two queries in one
-// tile); every tile is sorted in shared memory, then adjacent sorted runs of the same query are merged pairwise, one
-// pass per doubling, every run truncated to k_fetch entries.  The two buffers ping-pong: [0] is emit_rows /
-// cand_scores themselves (each tile is sorted in place), [1] is the scratch below.
+// The cut of k_fetch > RBK_MAX_K_FETCH_LARGE: a segmented sort in global memory.  Each query's segment of emit_rows /
+// cand_scores is cut into tiles of kSortTile candidates (never two queries in one tile); every tile is sorted in
+// shared memory, then adjacent sorted runs of the same query are merged pairwise, one pass per doubling, every run
+// truncated to k_fetch entries.  The two buffers ping-pong: [0] is emit_rows / cand_scores themselves (each tile is
+// sorted in place), [1] is the scratch below.
 constexpr int kSortTile = 4096;
 struct SegSortScratch {
   const int* tile_off;   // [B] first run-length slot of query q (tiles of the queries before it, in this group)
@@ -216,10 +213,13 @@ struct SegSortScratch {
   int* len[2];           // per-run passing lengths, one slot per tile (a run's length sits at its first tile)
   int max_tiles;         // most tiles of one query in this launch (sizes the grids and the number of passes)
 };
-// p.k_fetch is k_eff (the entries kept per query); out_* are [B][k_eff], filled with -1 / NaN past the count.
+// The exact fp64 re-score of every emitted candidate, then the cut to p.k_fetch entries per query, filled with
+// -1 / NaN past the count: in shared memory, one block per query (sort null, p.k_fetch <= RBK_MAX_K_FETCH_LARGE), or
+// the segmented sort above.  max_cap: largest emit_cap of the launch (sizes the scoring grid).  rows_on_host: as for
+// launch_finalize; the scoring kernel then stages its candidates' rows in shared memory with coalesced loads.
 // *launches: kernels enqueued.
-cudaError_t launch_unbounded_rerank(const LargeRerankParams& p, const SegSortScratch& s, int max_cap,
-                                    bool rows_on_host, cudaStream_t stream, int* launches);
+cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
+                                bool rows_on_host, cudaStream_t stream, int* launches);
 
 // Exact fp64 cosine of every row for B prepared queries: out [B][n_rows], NaN = tombstoned / zero row.
 cudaError_t launch_exact_scores(const uint16_t* rows, const double* rows_f64, const double* row_norm2,

@@ -143,7 +143,8 @@ def test_batch_split_into_query_groups(rb, oracle_mod):
     """200k rows x 48 queries x k_fetch 200k: the candidates and results (~8 MB per query) exceed the per-pass budget,
     so the batch is answered in several query groups - one emit scan each - and stays exact.  The groups start at
     queries that are not multiples of the scan's 128-query block (33 per group on an index, 18 on a one-GPU group);
-    each group's scan must stay inside the query buffer, which the library checks before every launch."""
+    each group's scan must stay inside the query buffer, which the library checks before every launch.  Then the same
+    for the large-k search at k_fetch 4096."""
     from runbookai_b200 import _native, synth
     n, d, B, k = 200_000, 64, 48, 200_000
     corpus = synth.random_corpus(n, d, 421)
@@ -163,6 +164,23 @@ def test_batch_split_into_query_groups(rb, oracle_mod):
         before = g.stats()["scan_launches"]
         assert bit_equal(g.search_unbounded(q, k, None), got)
         assert g.stats()["scan_launches"] - before >= 3
+    # The large-k search (k_fetch <= 4096, the cut in shared memory) keeps the same budget: 1M rows that are all
+    # power-of-two multiples of one direction tie for every query along it (the fp64 arithmetic scales exactly), so
+    # C_q = n and 32 queries' candidates (12 bytes each, ~380 MB) need two query groups.
+    n, B, k = 1_000_000, 32, 4096
+    rng = np.random.default_rng(423)
+    u = synth.bf16_round(synth.random_queries(1, d, 424)[0]).astype(np.float64)
+    scale = np.exp2(rng.integers(-3, 4, n))[:, None]
+    corpus = synth.f32_to_bf16_bits((u * scale).astype(np.float32))
+    q = u * np.exp2(rng.integers(-2, 3, B))[:, None]
+    want = oracle(oracle_mod, corpus, q, k, None)
+    with rb.Index(d) as ix, rb.Group(d, [0]) as g:
+        for h in (ix, g):
+            h.append_bf16(corpus)
+            before = h.stats()["scan_launches"]
+            got = h.search_large(q, k, None)
+            assert h.stats()["scan_launches"] - before >= 3                # one count scan, at least two emit scans
+            check(got, *want)
 
 
 def test_host_rows_equal_device_rows(rb):
