@@ -74,7 +74,12 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * row as float64 (8*dim bytes per row; f32/bf16 inputs are widened exactly).  The exact re-rank then uses them:
  * results are the reference's fp64 cosine bit for bit for ARBITRARY float64 embeddings (the SQLite BLOBs of
  * vector-store.ts:71-88), not only for bf16-representable ones.  The scan's error bound grows by the largest
- * angle between a row and its bf16 rounding, so more queries may take the exhaustive path on near-tied data. */
+ * angle between a row and its bf16 rounding, so more queries may take the exhaustive path on near-tied data.
+ * The scan's bound covers only rows and queries whose largest finite element m has 2^-40 <= m < 2^40 (the scan band,
+ * DESIGN.md §6).  A query the reference scores (finite, not all zero) outside the band skips the scan and is answered
+ * by the exhaustive kernel.  Once ANY such row has been stored (in any tier; it stays so until rbk_index_clear), every
+ * top-k search of the index takes the exhaustive kernel and every large-k search re-scores every live row: exact, at
+ * the cost of the whole corpus per query. */
 #define RBK_INDEX_KEEP_F64 1u
 /* RBK_INDEX_F64_ON_HOST (only together with RBK_INDEX_KEEP_F64, else RBK_EINVAL): the [capacity][dim] float64 rows
  * live in pinned, mapped host memory (cudaHostAlloc Mapped | Portable) instead of on the GPU; every other buffer stays
@@ -97,7 +102,8 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * fp16 keeps 11 significant bits against bf16's 8, so the scan's error bound - whose rounding terms are the angles
  * between a row or query and its stored copy - is several times tighter (DESIGN.md §6): fewer batches need the wide
  * retry, and the large-k search emits fewer candidates.  Answers are those of a KEEP_F64 index without the flag: the
- * same slots and fp64 scores, bit for bit.  The placement is fixed for the index's life; read the stored bits with
+ * same slots and fp64 scores, bit for bit, including the scan-band rule above (decided on the float64 row or query,
+ * not on the scaled copy).  The placement is fixed for the index's life; read the stored bits with
  * rbk_index_read_rows_f16. */
 #define RBK_INDEX_SCAN_F16 16u
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out);

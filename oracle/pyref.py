@@ -21,7 +21,7 @@ def cosine_similarity(a, b):
         na += a[i] * a[i]
         nb += b[i] * b[i]
     den = math.sqrt(na) * math.sqrt(nb)
-    if den == 0.0:  # JS: x/0 -> NaN (0/0) or +-Infinity; only 0/0 can occur here
+    if den == 0.0:  # JS: x/0 -> NaN (0/0) or +-Infinity (a norm that underflows to 0 while the dot does not)
         return float("nan") if dot == 0.0 or dot != dot else math.copysign(float("inf"), dot)
     return dot / den
 

@@ -475,7 +475,7 @@ cudaError_t zero_scan_scratch(rbk_index* ix, int Bs) {
 // The prep kernel for all B queries; it also zeroes the first sub-batch's scan scratch.
 rbk_status prep_queries(rbk_index* ix, const void* d_q, int src_type, int B, double min_score, bool with_norm2) {
   CK(launch_prep_queries(d_q, src_type, B, ix->dim, ix->dpad, min_score,
-                         ix->keep_f64 ? reinterpret_cast<const float*>(ix->d_counter + 1) : nullptr,
+                         reinterpret_cast<const float*>(ix->d_counter + 1),
                          query_buffers(ix, 0), ix->stream, with_norm2, ix->hist.p, std::min(kMaxSubBatch, B),
                          progress_slots(ix), ix->scan_f16));
   ix->stats.kernel_launches++;
@@ -700,8 +700,8 @@ rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double 
     const LargeScanParams sp = large_scan_params(ix, q0, Bs, k_eff);
     st = launch_sub_batch<kScanCount>(ix, q0, sp);
     if (st != RBK_OK) return st;
-    CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Bs, k_eff, ix->lg_theta.p + q0,
-                           ix->lg_cap.p + q0, ix->stream));
+    CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Bs, k_eff, static_cast<int>(ix->n_rows),
+                           ix->lg_theta.p + q0, ix->lg_cap.p + q0, ix->stream));
     ix->stats.kernel_launches++;
   }
   CK(cudaMemcpyAsync(ix->h_lcap.p, ix->lg_cap.p, sizeof(int) * B, cudaMemcpyDeviceToHost, ix->stream));
@@ -783,6 +783,12 @@ rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, dou
     CK(cudaMemsetAsync(sp.progress, 0, sizeof(int) * progress_slots(ix), ix->stream));
     rbk_status st = launch_sub_batch<kScanEmit>(ix, s0, sp);
     if (st != RBK_OK) return st;
+    // a query whose bound proves nothing has C_q = n_rows (large_select); only then is there anything to emit
+    if (std::find(ix->h_lcap.p + s0, ix->h_lcap.p + s0 + Bs, static_cast<int>(ix->n_rows)) != ix->h_lcap.p + s0 + Bs) {
+      CK(launch_large_emit_all(ix->q_eps.p + s0, ix->dead_bits, ix->n_rows, Bs, sp.emit_off, sp.emit_cnt,
+                               ix->lg_rows.p, ix->stream));
+      ix->stats.kernel_launches++;
+    }
     LargeRerankParams rp;
     rp.B = Bs;
     rp.d = ix->dim;

@@ -97,6 +97,7 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
     e = f16_scale_exp(fmax(fmax(red_m[0], red_m[1]), fmax(red_m[2], red_m[3])));
   }
   double sb = 0.0, sd = 0.0, sq = 0.0;  // ||bf16(q)||^2, ||q - bf16(q)||^2, ||q||^2 (any order: bounds only)
+  double fmx = 0.0, bad = 0.0;           // max |x| over the finite elements; 1 if any element is not finite
   double sh = 0.0, shd = 0.0, sx = 0.0; // kF16: ||h||^2, ||q 2^e - h||^2, ||q 2^e||^2 (any order: bounds only)
   // 8 elements per thread and pass, ALL loads first: the stores below may alias the source as far as the compiler
   // knows, so a load -> store loop exposed one global round trip per element (the kernel took 7.8 us for this)
@@ -115,6 +116,8 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
       if (i < d) {
         const double x = xs[u];
         qb.q_f64[static_cast<size_t>(q) * d + i] = x;
+        if (fabs(x) < INFINITY) fmx = fmax(fmx, fabs(x));
+        else bad = 1.0;
         const __nv_bfloat16 h = __float2bfloat16_rn(__double2float_rn(x));
         b = __bfloat16_as_ushort(h);
         const double xb = static_cast<double>(__bfloat162float(h));
@@ -133,13 +136,15 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
       qb.q_bf16[static_cast<size_t>(q) * dpad + i] = b;
     }
   }
-  __shared__ double red_b[4], red_d[4];
+  __shared__ double red_b[4], red_d[4], red_m2[4], red_bad[4];
   __shared__ double red_h[4], red_hd[4], red_x[4];
   __shared__ double s_na;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     sb += __shfl_xor_sync(kFull, sb, o);
     sd += __shfl_xor_sync(kFull, sd, o);
+    fmx = fmax(fmx, __shfl_xor_sync(kFull, fmx, o));
+    bad = fmax(bad, __shfl_xor_sync(kFull, bad, o));
     if constexpr (kF16) {
       sh += __shfl_xor_sync(kFull, sh, o);
       shd += __shfl_xor_sync(kFull, shd, o);
@@ -149,6 +154,8 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
   if ((tid & 31) == 0) {
     red_b[tid >> 5] = sb;
     red_d[tid >> 5] = sd;
+    red_m2[tid >> 5] = fmx;
+    red_bad[tid >> 5] = bad;
     if constexpr (kF16) {
       red_h[tid >> 5] = sh;
       red_hd[tid >> 5] = shd;
@@ -185,6 +192,12 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
     const double nb2 = red_b[0] + red_b[1] + red_b[2] + red_b[3];
     const double nd2 = red_d[0] + red_d[1] + red_d[2] + red_d[3];
     const bool ok = nb2 > 0.0 && nb2 < INFINITY && na > 0.0 && na < INFINITY;
+    // A query the reference scores (finite, not all zero) whose largest element lies outside the scan band is left
+    // to the exhaustive kernel (DESIGN.md §6): its bf16 copy may be zero or infinite, its fp32 products may leave
+    // fp32's range, its normA may underflow or overflow.  Inside the band none of that happens, and ok holds.
+    const double qmax = fmax(fmax(red_m2[0], red_m2[1]), fmax(red_m2[2], red_m2[3]));
+    const bool ref_live = fmax(fmax(red_bad[0], red_bad[1]), fmax(red_bad[2], red_bad[3])) == 0.0 && qmax > 0.0;
+    const bool off_band = ref_live && !in_scan_band(qmax);
     double inv = ok ? 1.0 / sqrt(nb2) : 0.0;
     // angle(q, bf16(q)) <= asin(||q - bf16(q)|| / ||q||); cosine is 1-Lipschitz in the angle
     double ang = 0.0;
@@ -207,14 +220,17 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
       }
     }
     // + corpus-side quantisation angle when the exact source is an f64 sidecar (0 for bf16-exact corpora)
-    const double eps = acc_eps + ang + (eps_c != nullptr ? static_cast<double>(*eps_c) * (1.0 + 1e-6) : 0.0);
+    const double eps = off_band ? INFINITY
+                                : acc_eps + ang + (eps_c != nullptr ? static_cast<double>(*eps_c) * (1.0 + 1e-6) : 0.0);
     if (kNorm2) qb.q_norm2[q] = na;   // (else: written by the finalize kernel, bit-exact)
     qb.q_eps[q] = eps;
     const float invf = ok ? static_cast<float>(inv) : __uint_as_float(0x7FC00000u);
     qb.q_inv_norm[q] = invf;
     float thr;
-    if (!ok) {
-      thr = INFINITY;  // zero / non-finite query: cosine is NaN for every row (S3) -> nothing matches
+    if (!ok || !(eps < kEpsNone)) {
+      // zero / non-finite query: cosine is NaN for every row (S3) -> nothing matches; or a bound that proves
+      // nothing: the scan is skipped and the query is answered exactly (finalize flags it, large_select emits all)
+      thr = INFINITY;
     } else if (min_score == -INFINITY) {
       thr = -INFINITY;
     } else {
@@ -624,7 +640,9 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
     p.out_counts[ql] = count;
     // ---- proof of exactness (DESIGN.md §6) ----
     bool ok;
-    if (tau_raw == -INFINITY) {
+    if (!(p.q.q_eps[ql] < kEpsNone)) {
+      ok = false;  // the scan's bound proves nothing for this query (prep_queries): the exhaustive kernel answers it
+    } else if (tau_raw == -INFINITY) {
       ok = true;  // nothing was ever dropped except by thr_init (provably below min_score)
     } else {
       const double bound = static_cast<double>(tau_raw) * static_cast<double>(p.q.q_inv_norm[ql]) + p.q.q_eps[ql];
@@ -786,7 +804,8 @@ __global__ void __launch_bounds__(256) large_select_kernel(const unsigned int* _
                                                            const float* __restrict__ thr_init,
                                                            const float* __restrict__ inv_norm_q,
                                                            const double* __restrict__ q_eps, int k_fetch,
-                                                           float* __restrict__ theta, int* __restrict__ cap) {
+                                                           int n_rows, float* __restrict__ theta,
+                                                           int* __restrict__ cap) {
   const int q = blockIdx.x;
   const int tid = threadIdx.x;
   __shared__ unsigned int s_grp[256];          // suffix sums over groups of 4 bins
@@ -815,6 +834,11 @@ __global__ void __launch_bounds__(256) large_select_kernel(const unsigned int* _
   __syncthreads();
   if (tid != 0) return;
   const float ti = thr_init[q];
+  if (!(q_eps[q] < kEpsNone)) {   // the bound proves nothing: no scan, every live row is a candidate (large_emit_all)
+    theta[q] = INFINITY;
+    cap[q] = n_rows;
+    return;
+  }
   if (!(ti < INFINITY)) {   // zero / non-finite query: nothing matches
     theta[q] = INFINITY;
     cap[q] = 0;
@@ -833,6 +857,24 @@ __global__ void __launch_bounds__(256) large_select_kernel(const unsigned int* _
   // the bin of a row with a >= th is >= this one: same float expression as hist_add
   const int b = static_cast<int>((th * inv + 1.0f) * (kHistBins * 0.5f));
   cap[q] = static_cast<int>(s_suf[min(max(b, 0), kHistBins - 1)]);
+}
+
+// The candidates of a query whose bound proves nothing (large_select gave it theta = +inf and C_q = n_rows, so the
+// emit scan wrote nothing for it): every row that is not tombstoned, in any order - the re-rank sorts them.
+__global__ void __launch_bounds__(256) large_emit_all_kernel(const double* __restrict__ q_eps,
+                                                             const unsigned int* __restrict__ dead_bits,
+                                                             int64_t n_rows, const long long* __restrict__ emit_off,
+                                                             int* __restrict__ emit_cnt, int* __restrict__ emit_rows) {
+  const int q = blockIdx.y;
+  if (q_eps[q] < kEpsNone) return;
+  const int64_t row = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x;
+  const bool take = row < n_rows && !((dead_bits[row >> 5] >> (row & 31)) & 1u);
+  const unsigned int m = __ballot_sync(kFull, take);
+  const int lane = threadIdx.x & 31;
+  int base = 0;
+  if (lane == 0 && m != 0u) base = atomicAdd(emit_cnt + q, __popc(m));
+  base = __shfl_sync(kFull, base, 0);
+  if (take) emit_rows[emit_off[q] + base + __popc(m & ((1u << lane) - 1u))] = static_cast<int>(row);
 }
 
 // re-rank, part 1: the reference's fp64 cosine of every emitted row (one thread per candidate).
@@ -1316,9 +1358,18 @@ cudaError_t launch_exact_scores(const uint16_t* rows, const double* rows_f64, co
 }
 
 cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init, const float* inv_norm_q,
-                                const double* q_eps, int B, int k_fetch, float* theta, int* cap, cudaStream_t stream) {
+                                const double* q_eps, int B, int k_fetch, int n_rows, float* theta, int* cap,
+                                cudaStream_t stream) {
   if (B <= 0) return cudaSuccess;
-  large_select_kernel<<<B, 256, 0, stream>>>(hist, thr_init, inv_norm_q, q_eps, k_fetch, theta, cap);
+  large_select_kernel<<<B, 256, 0, stream>>>(hist, thr_init, inv_norm_q, q_eps, k_fetch, n_rows, theta, cap);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_large_emit_all(const double* q_eps, const unsigned int* dead_bits, int64_t n_rows, int B,
+                                  const long long* emit_off, int* emit_cnt, int* emit_rows, cudaStream_t stream) {
+  if (B <= 0 || n_rows <= 0) return cudaSuccess;
+  dim3 grid(static_cast<unsigned>((n_rows + 255) / 256), static_cast<unsigned>(B));
+  large_emit_all_kernel<<<grid, 256, 0, stream>>>(q_eps, dead_bits, n_rows, emit_off, emit_cnt, emit_rows);
   return cudaGetLastError();
 }
 

@@ -215,7 +215,7 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
   }
   __syncthreads();
   const long long my_row = s_row[tid];
-  double acc = 0.0;
+  double acc = 0.0, amax = 0.0;   // amax: largest |element| (a bf16 index's scan band, DESIGN.md §6)
   const int n16 = dpad >> 3;                         // 16-byte pieces per row
   constexpr int kPieces = kNormChunk / 8;            // 16-byte pieces per row and chunk; = pieces per thread and chunk
   // piece index i of a chunk -> (row i / len16, unit i % len16): consecutive lanes = consecutive units of a row;
@@ -258,6 +258,7 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
           const double hi = kF16 ? f16_bits_to_f64(w[j] >> 16) : bf16_bits_to_f64(w[j] >> 16);
           acc = __dadd_rn(acc, __dmul_rn(lo, lo));
           acc = __dadd_rn(acc, __dmul_rn(hi, hi));
+          if (!kF16) amax = fmax(amax, fmax(fabs(lo), fabs(hi)));
         }
       }
     }
@@ -266,7 +267,11 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
   if (my_row < 0) return;
   const bool ok = acc > 0.0 && acc < INFINITY;
   inv_norm_base[my_row] = ok ? static_cast<float>(1.0 / sqrt(acc)) : __uint_as_float(0x7FC00000u);
-  if (rows_f64_base == nullptr) norm2_base[my_row] = acc;
+  if (rows_f64_base == nullptr) {
+    norm2_base[my_row] = acc;
+    // a bf16 row the reference scores but the scan's bound does not cover: no first pass proves anything any more
+    if (!kF16 && ok && !in_scan_band(amax)) atomicMax(eps_c_max, __float_as_int(kEpsOffBand));
+  }
 }
 
 // Exact-source sidecar indexes (RBK_INDEX_KEEP_F64): norm2 comes from the f64 row (the reference's normB for
@@ -337,6 +342,7 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
     e = f16_scale_exp(amax);
   }
   double n2 = 0.0, diff2 = 0.0;
+  double xmax = 0.0, bad = 0.0;     // largest finite |x|; 1 if some element is not finite
   double h2 = 0.0, hdiff2 = 0.0;    // kF16: ||x 2^e||^2 and ||x 2^e - h||^2 (any order: bounds only)
   bool b_nonzero = false, b_finite = true;   // kF16: the bf16 rounding of the row has a nonzero / finite norm
   for (int c0 = 0; c0 < d; c0 += kNorm64Chunk) {
@@ -360,6 +366,8 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
       for (int i = 0; i < len; ++i) {
         const double v = mine[i];
         n2 = __dadd_rn(n2, __dmul_rn(v, v));   // the reference's normB for the f64 row
+        if (fabs(v) < INFINITY) xmax = fmax(xmax, fabs(v));
+        else bad = 1.0;
         if constexpr (kF16) {
           const double y = scale_pow2(v, e), t = y - f16_bits_to_f64(mb[i]);
           h2 += y * y;
@@ -387,6 +395,9 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
   } else {
     eps = angle_bound(diff2, n2);
   }
+  // a row the reference scores (finite, not all zero) outside the scan band: its scan copy may be dead or its normB
+  // may underflow or overflow, so no first pass on this index proves anything any more (DESIGN.md §6)
+  if (bad == 0.0 && xmax > 0.0 && !in_scan_band(xmax)) eps = fmaxf(eps, kEpsOffBand);
   if (eps > 0.f) atomicMax(eps_c_max, __float_as_int(eps));   // non-negative floats order like ints
 }
 

@@ -178,8 +178,13 @@ cudaError_t launch_exact_fallback(const ExactParams& p, cudaStream_t stream);
 
 // ---- large-k search (rbk_finalize.cu): select between the two scan passes, exact re-rank after them ----
 // theta [B] (raw domain) and cap [B] (C_q) from the count pass's histograms hist [B][kHistBins].
+// A query whose q_eps is not below kEpsNone gets theta = +inf (the emit scan skips it) and C_q = n_rows; then
+// launch_large_emit_all writes every live row into its segment.
 cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init, const float* inv_norm_q,
-                                const double* q_eps, int B, int k_fetch, float* theta, int* cap, cudaStream_t stream);
+                                const double* q_eps, int B, int k_fetch, int n_rows, float* theta, int* cap,
+                                cudaStream_t stream);
+cudaError_t launch_large_emit_all(const double* q_eps, const unsigned int* dead_bits, int64_t n_rows, int B,
+                                  const long long* emit_off, int* emit_cnt, int* emit_rows, cudaStream_t stream);
 struct LargeRerankParams {
   int B, d, dpad, k_fetch;
   double min_score;
@@ -235,5 +240,18 @@ cudaError_t launch_merge_shards(int G, int B, int k_fetch, const void* slots, co
 
 // Bound on the fp32 tensor-core accumulation + scaling error of an approximate cosine.
 inline double accumulation_eps(int d) { return (double)(d + 8) * (1.0 / 4194304.0); }  // (d+8) * 2^-22
+
+// The scan band (DESIGN.md §6): the scan's bound holds for a query or row whose largest finite element m has
+// 2^-40 <= m < 2^40.  Then its bf16 copy is live, every product of two such copies' elements is below 2^81 (no fp32
+// overflow for any d < 2^46), the elements that underflow in fp32 products change an approximate cosine by at most
+// d 2^-126 / 2^-80 = d 2^-46 (far inside accumulation_eps), and normA / normB cannot underflow or overflow in float64.
+// Outside it, a query the reference scores, or any such row in the index, gets a bound of kEpsNone or more: the
+// first pass never proves it and the large-k search re-scores every live row.
+constexpr double kScanBandLo = 9.094947017729282e-13;   // 2^-40
+constexpr double kScanBandHi = 1099511627776.0;         // 2^40
+__host__ __device__ inline bool in_scan_band(double m) { return m >= kScanBandLo && m < kScanBandHi; }
+// A bound this wide (the whole range of a cosine) proves nothing; 3.2 is what an off-band row folds in.
+constexpr double kEpsNone = 2.0;
+constexpr float kEpsOffBand = 3.2f;
 
 }  // namespace rbk
