@@ -153,7 +153,7 @@ rbk_status rbk_index_tombstone(rbk_index* idx, const int64_t* local_slots, int64
  * slot_base is kept, so global slots stay slot_base + local.  Capacity is kept: later appends reuse the reclaimed
  * slots.  Without tombstones nothing moves and the identity map is returned.  Staging is one 64 MB buffer, allocated
  * before the first row moves (RBK_ENOMEM leaves the index untouched).  Not available for the member indexes of a
- * group (RBK_EINVAL).  Synchronous.  Searches enqueued before the call (rbk_index_search_device_async) run first,
+ * group (RBK_EINVAL): rbk_group_compact compacts them together.  Synchronous.  Searches enqueued before the call (rbk_index_search_device_async) run first,
  * because the index's work is stream-ordered; their results carry the OLD slots. */
 rbk_status rbk_index_compact(rbk_index* idx, int64_t* old_to_new, int64_t old_to_new_len);
 rbk_status rbk_index_clear(rbk_index* idx);
@@ -294,6 +294,20 @@ rbk_status rbk_group_append_bf16(rbk_group* grp, const uint16_t* rows, int64_t n
 rbk_status rbk_group_overwrite_f64_batch(rbk_group* grp, const int64_t* slots, int64_t n, const double* rows);
 rbk_status rbk_group_tombstone(rbk_group* grp, const int64_t* slots, int64_t n);
 rbk_status rbk_group_clear(rbk_group* grp);
+/* Reclaim the slots of tombstoned rows across the group: rbk_index_compact in GLOBAL slots.  The live rows move down
+ * to global slots 0 .. rbk_group_count()-1 in their current global order, moving between devices where the
+ * block-cyclic layout puts their new slot elsewhere; afterwards every member holds exactly the rows and per-row state
+ * that a new group of the same devices and flags would hold after appending the survivors in order, size() ==
+ * count(), and later appends land at count().  old_to_new (nullable) receives, for every global slot s <
+ * rbk_group_size() before the call, its new global slot, or -1 if s was tombstoned; old_to_new_len must then be >=
+ * that size (RBK_EINVAL otherwise, group untouched).  No slot or score changes except through the map.  Every
+ * allocation (one staging buffer of 64 MB, or one 4096-row block if that is more, per member) happens before the first
+ * row moves (RBK_ENOMEM leaves the group untouched); tombstone bits that disagree with a member's count() return
+ * RBK_ECUDA before anything moves.  Every member's corpus-side error bound becomes the largest of them (answers are
+ * unchanged; retry and fallback counts may differ from those of a new group).  Capacity is kept: follow with
+ * rbk_group_trim to return it.  Without tombstones nothing moves and the identity map is returned.  Synchronous; uses
+ * no NCCL.  The members themselves refuse rbk_index_compact (RBK_EINVAL). */
+rbk_status rbk_group_compact(rbk_group* grp, int64_t* old_to_new, int64_t old_to_new_len);
 /* rbk_index_trim on every member, and the group's own exchange buffers released. */
 rbk_status rbk_group_trim(rbk_group* grp);
 int64_t rbk_group_count(const rbk_group* grp); /* live rows */

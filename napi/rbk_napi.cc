@@ -17,7 +17,7 @@
 //   ix.appendBlobs(Buffer[] blobs)             -> firstSlot     // SQLite f64-LE BLOBs, packed in C++: no JS copies
 //   ix.overwriteF64(slot, Float64Array row); ix.overwriteF64Batch(BigInt64Array slots, Float64Array rows)
 //   ix.tombstone(BigInt64Array slots); ix.clear()
-//   ix.compact()                               -> BigInt64Array oldToNew   // reclaim tombstoned slots (one GPU only)
+//   ix.compact()                               -> BigInt64Array oldToNew   // reclaim tombstoned slots
 //   ix.trim()                                  // give unused device memory back (after compact / clear)
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
@@ -47,6 +47,10 @@
 // so that the method as a whole needs nothing a library without compaction may lack.
 #pragma weak rbk_index_compact
 #pragma weak rbk_index_size
+// Compaction of a device group came later still; `compact` on a group handle throws where it is missing.
+// rbk_group_size sizes its map.
+#pragma weak rbk_group_compact
+#pragma weak rbk_group_size
 // The same for trim; `trim` throws where it is missing.
 #pragma weak rbk_index_trim
 #pragma weak rbk_group_trim
@@ -271,23 +275,24 @@ napi_value Clear(napi_env env, napi_callback_info info) {
 }
 
 // compact() -> BigInt64Array old_to_new: reclaim the slots of tombstoned rows; old slot s now lives at
-// old_to_new[s] (-1 = it was deleted).  Synchronous.  Single-device handles only.
+// old_to_new[s] (-1 = it was deleted).  Synchronous.  On a device group the slots are global ones.
 napi_value Compact(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
-  if (h->grp) {
+  if (h->grp && (rbk_group_compact == nullptr || rbk_group_size == nullptr)) {
     napi_throw_error(env, nullptr, "compaction is not available for a device group");
     return nullptr;
   }
-  if (rbk_index_compact == nullptr || rbk_index_size == nullptr) {
+  if (!h->grp && (rbk_index_compact == nullptr || rbk_index_size == nullptr)) {
     napi_throw_error(env, nullptr, "compact: this librbk_knn.so has no compaction (rbk_index_compact)");
     return nullptr;
   }
-  const int64_t n = rbk_index_size(h->ix);
+  const int64_t n = h->grp ? rbk_group_size(h->grp) : rbk_index_size(h->ix);
   napi_value ab, out;
   void* p = nullptr;
   NAPI_OK(napi_create_arraybuffer(env, (size_t)n * 8, &p, &ab));
-  if (rbk_index_compact(h->ix, static_cast<int64_t*>(p), n) != RBK_OK) return throw_rbk(env);
+  int64_t* map = static_cast<int64_t*>(p);
+  if ((h->grp ? rbk_group_compact(h->grp, map, n) : rbk_index_compact(h->ix, map, n)) != RBK_OK) return throw_rbk(env);
   NAPI_OK(napi_create_typedarray(env, napi_bigint64_array, (size_t)n, ab, 0, &out));
   return out;
 }

@@ -30,7 +30,7 @@ SYMBOLS = [
     "rbk_merge_topk_packed_device", "rbk_index_stats",
     "rbk_index_debug_scores_f32",
     "rbk_group_create", "rbk_group_destroy", "rbk_group_append_f64", "rbk_group_append_f32", "rbk_group_append_bf16",
-    "rbk_group_overwrite_f64_batch", "rbk_group_tombstone", "rbk_group_clear", "rbk_group_trim", "rbk_group_count", "rbk_group_size",
+    "rbk_group_overwrite_f64_batch", "rbk_group_tombstone", "rbk_group_clear", "rbk_group_compact", "rbk_group_trim", "rbk_group_count", "rbk_group_size",
     "rbk_group_devices", "rbk_group_member", "rbk_group_redone_batches", "rbk_group_search_f32", "rbk_group_search_f64",
     "rbk_group_search_large_f64", "rbk_group_search_unbounded_f64",
 ]
@@ -109,6 +109,7 @@ def _load() -> C.CDLL:
     lib.rbk_group_overwrite_f64_batch.argtypes = [vp, vp, i64, vp]
     lib.rbk_group_tombstone.argtypes = [vp, vp, i64]
     lib.rbk_group_clear.argtypes = [vp]
+    lib.rbk_group_compact.argtypes = [vp, vp, i64]
     lib.rbk_group_trim.argtypes = [vp]
     for n in ("rbk_group_count", "rbk_group_size", "rbk_group_redone_batches"):
         getattr(lib, n).argtypes = [vp]
@@ -442,6 +443,13 @@ class Group:
 
     def clear(self) -> None:
         check(lib.rbk_group_clear(self._h))
+
+    def compact(self) -> np.ndarray:
+        """Index.compact() in global slots: the live rows move down to slots 0 .. count()-1 in their current order,
+        between devices where the block-cyclic layout says so.  Returns old_to_new, int64 [size() before the call]."""
+        out = np.empty(self.size(), dtype=np.int64)
+        check(lib.rbk_group_compact(self._h, ptr(out), out.shape[0]))
+        return out
 
     def trim(self) -> None:
         """Index.trim() on every member; slots do not change."""

@@ -1096,6 +1096,63 @@ rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, 
   return search_core(ix, nullptr, d_q, elem, B, ix ? ix->dim : 0, k_fetch, min_score, d_slots, d_scores, d_counts,
                      nullptr, nullptr, nullptr, nullptr);
 }
+
+int64_t compact_row_bytes(const rbk_index* ix) {
+  return static_cast<int64_t>(ix->dpad) * 2 + (ix->keep_f64 ? static_cast<int64_t>(ix->dim) * 8 : 0) + 12;
+}
+
+rbk_status compact_alloc(rbk_index* ix, int64_t C, int64_t chunk_rows, CompactStage* st) {
+  const int64_t n = ix->n_rows, row_bytes = compact_row_bytes(ix);
+  const int64_t n_words = (n + 31) / 32, n_blocks = (n_words + 1023) / 1024, n_chunks = (n + chunk_rows - 1) / chunk_rows;
+  CK(ix->stage.ensure(static_cast<size_t>(C * row_bytes)));
+  CK(ix->cp_map.ensure(static_cast<size_t>(n)));
+  CK(ix->cp_scan.ensure(static_cast<size_t>(n_words + n_blocks + n_chunks + 1)));
+  unsigned char* p = ix->stage.p;
+  st->rows = reinterpret_cast<uint16_t*>(p);
+  st->f64 = reinterpret_cast<double*>(p + C * ix->dpad * 2);
+  st->norm2 = reinterpret_cast<double*>(p + C * (row_bytes - 12));
+  st->inv = reinterpret_cast<float*>(p + C * (row_bytes - 4));
+  return RBK_OK;
+}
+
+rbk_status compact_map(rbk_index* ix, int64_t chunk_rows, int* h_chunk_pref, int64_t* h_map) {
+  const int64_t n = ix->n_rows;
+  const int64_t n_words = (n + 31) / 32, n_blocks = (n_words + 1023) / 1024, n_chunks = (n + chunk_rows - 1) / chunk_rows;
+  int* word_pref = ix->cp_scan.p;
+  int* block_sum = word_pref + n_words;
+  int* chunk_pref_d = block_sum + n_blocks;
+  CK(launch_compact_map(ix->dead_bits, n, chunk_rows, word_pref, block_sum, ix->cp_map.p, chunk_pref_d, ix->stream));
+  ix->stats.kernel_launches += 3;
+  CK(cudaMemcpyAsync(h_chunk_pref, chunk_pref_d, sizeof(int) * (n_chunks + 1), cudaMemcpyDeviceToHost, ix->stream));
+  if (h_map) CK(cudaMemcpyAsync(h_map, ix->cp_map.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, ix->stream));
+  return RBK_OK;
+}
+
+rbk_status compact_gather(rbk_index* ix, const CompactStage& st, int64_t s0, int64_t n, int64_t rank0) {
+  CK(launch_compact_gather(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, ix->norm2, ix->inv_norm, ix->cp_map.p, s0,
+                           n, rank0, ix->dim, ix->dpad, st.rows, st.f64, st.norm2, st.inv, ix->sm_count, ix->stream));
+  ix->stats.kernel_launches++;
+  return RBK_OK;
+}
+
+rbk_status compact_tail(rbk_index* ix, int64_t n_new) {
+  // the tail looks like never-appended rows: zero bf16 rows (read by the scan's last tile), NaN 1/||c||, no tombstones
+  const int64_t n = ix->n_rows;
+  CK(cudaMemsetAsync(ix->rows + n_new * ix->dpad, 0, static_cast<size_t>(n - n_new) * ix->dpad * 2, ix->stream));
+  CK(cudaMemsetAsync(ix->inv_norm + n_new, 0xFF, static_cast<size_t>(n - n_new) * 4, ix->stream));
+  CK(cudaMemsetAsync(ix->dead_bits, 0, static_cast<size_t>((n + 31) / 32) * 4, ix->stream));
+  return RBK_OK;
+}
+
+void compact_commit(rbk_index* ix, int64_t n_new) {
+  ix->n_rows = n_new;
+  ix->n_live = n_new;
+  // caches keyed on the corpus: the captured search graph (GraphKey.n_rows) and the corpus tensor map (map_rows) are
+  // dropped here so that the next search rebuilds them; the large-k scratch is sized per call from C_q, not from the
+  // corpus, and the fallback / exact-scores / debug buffers from n_rows at each call.
+  drop_graph(ix);
+  ix->tmap_c_rows = -1;
+}
 }  // namespace impl
 }  // namespace rbk
 
@@ -1325,39 +1382,25 @@ rbk_status rbk_index_compact(rbk_index* ix, int64_t* old_to_new, int64_t old_to_
   const int64_t n = ix->n_rows, n_live = ix->n_live;
   if (old_to_new && old_to_new_len < n) return fail(RBK_EINVAL, "old_to_new_len is shorter than size()");
   if (ix->slot.block != 0)   // block-cyclic rows: moving them would break the group's slot layout
-    return fail(RBK_EINVAL, "compaction is not available for a member of a device group");
+    return fail(RBK_EINVAL, "compaction is not available for a member of a device group (use rbk_group_compact)");
   if (n_live == n) {         // no tombstones (or an empty index): nothing moves, every cache stays valid
     for (int64_t s = 0; old_to_new && s < n; ++s) old_to_new[s] = s;
     return RBK_OK;
   }
   // Staging chunk: whole 32-row words, 64 MB (the append path's staging size) of packed rows.
-  //   stage = bf16 rows [C][dpad] | f64 rows [C][dim] (KEEP_F64) | norm2 [C] | inv_norm [C]
-  const int64_t row_bytes = static_cast<int64_t>(ix->dpad) * 2 + (ix->keep_f64 ? static_cast<int64_t>(ix->dim) * 8 : 0) + 12;
-  const int64_t C = std::min(round_up(n, 32), std::max<int64_t>(32, (64ll << 20) / row_bytes / 32 * 32));
+  const int64_t C = std::min(round_up(n, 32), std::max<int64_t>(32, (64ll << 20) / compact_row_bytes(ix) / 32 * 32));
   const int64_t n_chunks = (n + C - 1) / C;
-  const int64_t n_words = (n + 31) / 32, n_blocks = (n_words + 1023) / 1024;
   // every allocation before the first row moves: RBK_ENOMEM leaves the index untouched
-  CK(ix->stage.ensure(static_cast<size_t>(C * row_bytes)));
-  CK(ix->cp_map.ensure(static_cast<size_t>(n)));
-  CK(ix->cp_scan.ensure(static_cast<size_t>(n_words + n_blocks + n_chunks + 1)));
-  int* word_pref = ix->cp_scan.p;
-  int* block_sum = word_pref + n_words;
-  int* chunk_pref_d = block_sum + n_blocks;
+  CompactStage st;
+  rbk_status s = compact_alloc(ix, C, C, &st);
+  if (s != RBK_OK) return s;
   std::vector<int> chunk_pref(static_cast<size_t>(n_chunks + 1));
-  CK(launch_compact_map(ix->dead_bits, n, C, word_pref, block_sum, ix->cp_map.p, chunk_pref_d, ix->stream));
-  ix->stats.kernel_launches += 3;
-  CK(cudaMemcpyAsync(chunk_pref.data(), chunk_pref_d, sizeof(int) * (n_chunks + 1), cudaMemcpyDeviceToHost, ix->stream));
-  if (old_to_new)
-    CK(cudaMemcpyAsync(old_to_new, ix->cp_map.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, ix->stream));
+  s = compact_map(ix, C, chunk_pref.data(), old_to_new);
+  if (s != RBK_OK) return s;
   CK(cudaStreamSynchronize(ix->stream));
   if (chunk_pref[n_chunks] != n_live)
     return fail(RBK_ECUDA, "compaction: the tombstone bits count " + std::to_string(chunk_pref[n_chunks]) +
                                " live rows, the index " + std::to_string(n_live) + " (the index was not changed)");
-  unsigned char* st = ix->stage.p;
-  uint16_t* st_rows = reinterpret_cast<uint16_t*>(st);
-  double* st_f64 = reinterpret_cast<double*>(st + C * ix->dpad * 2);
-  double* st_norm2 = reinterpret_cast<double*>(st + C * (row_bytes - 12));
-  float* st_inv = reinterpret_cast<float*>(st + C * (row_bytes - 4));
   // In place, stable, one chunk of sources at a time.  Chunk [s0, s1) holds L live rows that land at [d0, d0 + L) with
   // d0 + L <= s1: the copies overwrite only rows of this chunk and of earlier ones, all already staged, never a
   // source of a later chunk.  Chunks before the first tombstone (d0 == s0, L == s1 - s0) do not move.
@@ -1365,29 +1408,20 @@ rbk_status rbk_index_compact(rbk_index* ix, int64_t* old_to_new, int64_t old_to_
     const int64_t s0 = c * C, s1 = std::min(n, s0 + C);
     const int64_t d0 = chunk_pref[c], L = chunk_pref[c + 1] - d0;
     if ((d0 == s0 && L == s1 - s0) || L == 0) continue;
-    CK(launch_compact_gather(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, ix->norm2, ix->inv_norm, ix->cp_map.p,
-                             s0, s1 - s0, d0, ix->dim, ix->dpad, st_rows, st_f64, st_norm2, st_inv, ix->sm_count,
-                             ix->stream));
-    ix->stats.kernel_launches++;
-    CK(cudaMemcpyAsync(ix->rows + d0 * ix->dpad, st_rows, static_cast<size_t>(L) * ix->dpad * 2,
+    s = compact_gather(ix, st, s0, s1 - s0, d0);
+    if (s != RBK_OK) return s;
+    CK(cudaMemcpyAsync(ix->rows + d0 * ix->dpad, st.rows, static_cast<size_t>(L) * ix->dpad * 2,
                        cudaMemcpyDeviceToDevice, ix->stream));
     if (ix->keep_f64)   // device or mapped host rows (RBK_INDEX_F64_ON_HOST): UVA picks the direction
-      CK(cudaMemcpyAsync(ix->rows_f64 + d0 * ix->dim, st_f64, static_cast<size_t>(L) * ix->dim * 8, cudaMemcpyDefault,
+      CK(cudaMemcpyAsync(ix->rows_f64 + d0 * ix->dim, st.f64, static_cast<size_t>(L) * ix->dim * 8, cudaMemcpyDefault,
                          ix->stream));
-    CK(cudaMemcpyAsync(ix->norm2 + d0, st_norm2, static_cast<size_t>(L) * 8, cudaMemcpyDeviceToDevice, ix->stream));
-    CK(cudaMemcpyAsync(ix->inv_norm + d0, st_inv, static_cast<size_t>(L) * 4, cudaMemcpyDeviceToDevice, ix->stream));
+    CK(cudaMemcpyAsync(ix->norm2 + d0, st.norm2, static_cast<size_t>(L) * 8, cudaMemcpyDeviceToDevice, ix->stream));
+    CK(cudaMemcpyAsync(ix->inv_norm + d0, st.inv, static_cast<size_t>(L) * 4, cudaMemcpyDeviceToDevice, ix->stream));
   }
-  // the tail looks like never-appended rows: zero bf16 rows (read by the scan's last tile), NaN 1/||c||, no tombstones
-  CK(cudaMemsetAsync(ix->rows + n_live * ix->dpad, 0, static_cast<size_t>(n - n_live) * ix->dpad * 2, ix->stream));
-  CK(cudaMemsetAsync(ix->inv_norm + n_live, 0xFF, static_cast<size_t>(n - n_live) * 4, ix->stream));
-  CK(cudaMemsetAsync(ix->dead_bits, 0, static_cast<size_t>(n_words) * 4, ix->stream));
+  s = compact_tail(ix, n_live);
+  if (s != RBK_OK) return s;
   CK(cudaStreamSynchronize(ix->stream));
-  ix->n_rows = n_live;
-  // caches keyed on the corpus: the captured search graph (GraphKey.n_rows) and the corpus tensor map (map_rows) are
-  // dropped here so that the next search rebuilds them; the large-k scratch is sized per call from C_q, not from the
-  // corpus, and the fallback / exact-scores / debug buffers from n_rows at each call.
-  drop_graph(ix);
-  ix->tmap_c_rows = -1;
+  compact_commit(ix, n_live);
   return RBK_OK;
 }
 

@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <memory>
 
+#include "rbk_group_plan.h"
 #include "rbk_index_impl.h"
 
 using namespace rbk;
@@ -349,6 +350,172 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
   return RBK_OK;
 }
 
+// One compaction's events, one pair per member; destroyed on every return.
+struct CompactEvents {
+  std::vector<cudaEvent_t> gathered, copied;
+  explicit CompactEvents(int G) : gathered(G, nullptr), copied(G, nullptr) {}
+  ~CompactEvents() {
+    for (cudaEvent_t e : gathered)
+      if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : copied)
+      if (e) cudaEventDestroy(e);
+  }
+};
+
+// rbk_group_compact: the plan of rbk_group_plan.h, run chunk by chunk.  Every member packs its survivors of the chunk
+// into its own staging (the gather kernel of rbk_index_compact) and records `gathered`; every receiver waits for the
+// senders it reads, copies their segments into its own rows on its own stream and records `copied`; a sender waits for
+// the receivers that read its staging before it refills it.
+rbk_status group_compact(rbk_group* g, int64_t* old_to_new, int64_t old_to_new_len) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  std::lock_guard<std::mutex> lk(g->mu);
+  const int G = g->G;
+  const int64_t n = g->n_slots, block = g->block;
+  if (old_to_new && old_to_new_len < n) return fail(RBK_EINVAL, "old_to_new_len is shorter than rbk_group_size()");
+  std::vector<std::unique_lock<std::mutex>> member_locks;
+  member_locks.reserve(G);
+  for (rbk_index* ix : g->parts) member_locks.emplace_back(ix->mu);
+  int64_t n_live = 0;
+  for (int d = 0; d < G; ++d) {
+    if (g->parts[d]->n_rows != group_plan::member_rows(G, block, n, d))
+      return fail(RBK_EINVAL, "group placement out of step with a member index");
+    n_live += g->parts[d]->n_live;
+  }
+  if (n_live == n) {   // no tombstones (or an empty group): nothing moves
+    for (int64_t s = 0; old_to_new && s < n; ++s) old_to_new[s] = s;
+    return RBK_OK;
+  }
+  // A member stages whole blocks, 64 MB of packed rows or one block if that is more; a chunk is R rounds of G blocks,
+  // so that each member's share of it is at most R blocks of consecutive local rows.
+  const int64_t R = std::max<int64_t>(1, (64ll << 20) / (block * compact_row_bytes(g->parts[0])));
+  // every allocation before the first row moves: RBK_ENOMEM leaves the group untouched
+  std::vector<CompactStage> stage(G);
+  std::vector<std::vector<int>> pref(G);
+  std::vector<std::vector<int64_t>> local_map(G);
+  std::vector<int> eps(G, 0);
+  CompactEvents ev(G);
+  for (int d = 0; d < G; ++d) {
+    rbk_index* ix = g->parts[d];
+    DeviceGuard dg(ix->device);
+    rbk_status st = compact_alloc(ix, R * block, block, &stage[d]);
+    if (st != RBK_OK) return st;
+    CK(cudaEventCreateWithFlags(&ev.gathered[d], cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&ev.copied[d], cudaEventDisableTiming));
+    pref[d].assign(static_cast<size_t>((ix->n_rows + block - 1) / block + 1), 0);
+    if (old_to_new) local_map[d].resize(static_cast<size_t>(ix->n_rows));
+  }
+  // 1. Map: each member's liveness scan, per-block survivor counts (map chunk = one block) and its eps_c_max.
+  for (int d = 0; d < G; ++d) {
+    rbk_index* ix = g->parts[d];
+    DeviceGuard dg(ix->device);
+    if (ix->n_rows > 0) {
+      rbk_status st = compact_map(ix, block, pref[d].data(), old_to_new ? local_map[d].data() : nullptr);
+      if (st != RBK_OK) return st;
+    }
+    CK(cudaMemcpyAsync(&eps[d], ix->d_counter + 1, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+  }
+  for (int d = 0; d < G; ++d) {
+    DeviceGuard dg(g->parts[d]->device);
+    CK(cudaStreamSynchronize(g->parts[d]->stream));
+  }
+  for (int d = 0; d < G; ++d)
+    if (pref[d].back() != g->parts[d]->n_live)
+      return fail(RBK_ECUDA, "compaction: the tombstone bits of device " + std::to_string(g->devices[d]) + " count " +
+                                 std::to_string(pref[d].back()) + " live rows, its index " +
+                                 std::to_string(g->parts[d]->n_live) + " (the group was not changed)");
+  const int64_t nb = (n + block - 1) / block;
+  std::vector<int64_t> block_live(static_cast<size_t>(nb));
+  for (int64_t b = 0; b < nb; ++b) {
+    const std::vector<int>& p = pref[b % G];
+    block_live[b] = p[b / G + 1] - p[b / G];
+  }
+  // 2. Plan, and the caller's map: a survivor's new slot is its block's base plus its rank within the block.
+  const group_plan::Plan plan = group_plan::make_plan(G, block, n, block_live, R * G);
+  if (old_to_new) {
+    std::vector<const int64_t*> rank(G);
+    std::vector<const int*> block_pref(G);
+    for (int d = 0; d < G; ++d) {
+      rank[d] = local_map[d].data();
+      block_pref[d] = pref[d].data();
+    }
+    group_plan::fill_old_to_new(G, block, n, plan, rank, block_pref, old_to_new);
+  }
+  // A moved row carries its share of the corpus-side error bound (and the off-band marker) to its new device: every
+  // member takes the largest, which only widens the bound.
+  const int eps_max = *std::max_element(eps.begin(), eps.end());   // non-negative floats order like ints
+  // Peer access makes the cross-device copies direct; without it they are still correct, staged by the driver.
+  for (int d = 0; d < G; ++d)
+    for (int e = 0; e < G; ++e) {
+      int can = 0;
+      if (d == e || cudaDeviceCanAccessPeer(&can, g->devices[d], g->devices[e]) != cudaSuccess || !can) continue;
+      DeviceGuard dg(g->devices[d]);
+      if (cudaDeviceEnablePeerAccess(g->devices[e], 0) != cudaSuccess) cudaGetLastError();   // already enabled
+    }
+  cudaGetLastError();
+  // 3. Move.  pending[e][r]: receiver r has read e's staging since e's last gather.
+  std::vector<std::vector<char>> pending(G, std::vector<char>(G, 0));
+  for (const group_plan::Chunk& c : plan.chunks) {
+    for (int e = 0; e < G; ++e) {
+      if (c.staged[e] == 0) continue;
+      rbk_index* ix = g->parts[e];
+      DeviceGuard dg(ix->device);
+      for (int r = 0; r < G; ++r)
+        if (pending[e][r]) {
+          CK(cudaStreamWaitEvent(ix->stream, ev.copied[r], 0));
+          pending[e][r] = 0;
+        }
+      rbk_status st = compact_gather(ix, stage[e], c.g0[e], c.gn[e], c.rank0[e]);
+      if (st != RBK_OK) return st;
+      CK(cudaEventRecord(ev.gathered[e], ix->stream));
+    }
+    for (int d = 0; d < G; ++d) {
+      rbk_index* ix = g->parts[d];
+      DeviceGuard dg(ix->device);
+      std::vector<char> waited(G, 0);
+      bool wrote = false;
+      for (const group_plan::Segment& s : c.segs) {
+        if (s.dst != d) continue;
+        if (s.src != d && !waited[s.src]) {
+          CK(cudaStreamWaitEvent(ix->stream, ev.gathered[s.src], 0));
+          waited[s.src] = 1;
+        }
+        const CompactStage& ss = stage[s.src];
+        // device, peer or mapped host rows (RBK_INDEX_F64_ON_HOST): UVA picks the direction
+        CK(cudaMemcpyAsync(ix->rows + s.dst_row * ix->dpad, ss.rows + s.src_off * ix->dpad,
+                           static_cast<size_t>(s.len) * ix->dpad * 2, cudaMemcpyDefault, ix->stream));
+        if (ix->keep_f64)
+          CK(cudaMemcpyAsync(ix->rows_f64 + s.dst_row * ix->dim, ss.f64 + s.src_off * ix->dim,
+                             static_cast<size_t>(s.len) * ix->dim * 8, cudaMemcpyDefault, ix->stream));
+        CK(cudaMemcpyAsync(ix->norm2 + s.dst_row, ss.norm2 + s.src_off, static_cast<size_t>(s.len) * 8,
+                           cudaMemcpyDefault, ix->stream));
+        CK(cudaMemcpyAsync(ix->inv_norm + s.dst_row, ss.inv + s.src_off, static_cast<size_t>(s.len) * 4,
+                           cudaMemcpyDefault, ix->stream));
+        wrote = true;
+      }
+      if (!wrote) continue;
+      CK(cudaEventRecord(ev.copied[d], ix->stream));
+      for (int e = 0; e < G; ++e)
+        if (waited[e]) pending[e][d] = 1;
+    }
+  }
+  // 4. Finish: every member holds the slots below n_live that the layout gives it.
+  for (int d = 0; d < G; ++d) {
+    rbk_index* ix = g->parts[d];
+    DeviceGuard dg(ix->device);
+    rbk_status st = compact_tail(ix, group_plan::member_rows(G, block, n_live, d));
+    if (st != RBK_OK) return st;
+    CK(cudaMemcpyAsync(ix->d_counter + 1, &eps_max, sizeof(int), cudaMemcpyHostToDevice, ix->stream));
+  }
+  for (int d = 0; d < G; ++d) {
+    rbk_index* ix = g->parts[d];
+    DeviceGuard dg(ix->device);
+    CK(cudaStreamSynchronize(ix->stream));
+    compact_commit(ix, group_plan::member_rows(G, block, n_live, d));
+  }
+  g->n_slots = n_live;
+  return RBK_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -514,6 +681,10 @@ rbk_status rbk_group_trim(rbk_group* g) {
   g->h_out.release();
   g->h_q.release();
   return RBK_OK;
+}
+
+rbk_status rbk_group_compact(rbk_group* g, int64_t* old_to_new, int64_t old_to_new_len) {
+  return group_compact(g, old_to_new, old_to_new_len);
 }
 
 int64_t rbk_group_count(const rbk_group* g) {

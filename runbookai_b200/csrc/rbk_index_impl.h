@@ -269,6 +269,30 @@ rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, dou
                       double* d_scores, int* d_counts);
 rbk_status large_finish(rbk_index* ix);
 rbk_status large_check(rbk_index* ix);
+
+// The steps of a compaction, shared by rbk_index_compact and rbk_group_compact (caller holds ix->mu and has the index's
+// device current).  Staging of C rows, packed: bf16 (or fp16) rows [C][dpad] | f64 rows [C][dim] (KEEP_F64) | norm2 [C]
+// | inv_norm [C].
+struct CompactStage {
+  uint16_t* rows;
+  double* f64;
+  double* norm2;
+  float* inv;
+};
+int64_t compact_row_bytes(const rbk_index* ix);
+// Every allocation of the compaction: the staging of C rows, and the liveness scan's scratch for map chunks of
+// chunk_rows rows (a multiple of 32).
+rbk_status compact_alloc(rbk_index* ix, int64_t C, int64_t chunk_rows, CompactStage* st);
+// Enqueues the liveness scan of rows [0, n_rows): ix->cp_map (each row's rank among the live rows, -1 if tombstoned)
+// and its D2H copies: h_chunk_pref [ceil(n_rows / chunk_rows) + 1] (live rows before each map chunk, then all of them)
+// and, when h_map is not null, cp_map itself [n_rows].  The caller synchronises the stream.
+rbk_status compact_map(rbk_index* ix, int64_t chunk_rows, int* h_chunk_pref, int64_t* h_map);
+// Enqueues the packing of the live rows among rows [s0, s0 + n) into staging rows cp_map[s] - rank0.
+rbk_status compact_gather(rbk_index* ix, const CompactStage& st, int64_t s0, int64_t n, int64_t rank0);
+// Enqueues the reset of rows [n_new, n_rows) to never-appended rows and clears every tombstone bit.
+rbk_status compact_tail(rbk_index* ix, int64_t n_new);
+// After the stream has been synchronised: the index holds n_new live rows; drops the caches keyed on the corpus.
+void compact_commit(rbk_index* ix, int64_t n_new);
 const char* last_error();
 
 }  // namespace impl

@@ -84,7 +84,7 @@ class KnowledgeRetriever:
         keep their device memory and scan time for good.  Once the dead slots reach a quarter of all slots (and at
         least _COMPACT_MIN_DEAD - below that they cost less than the call) the vector store is compacted, then
         trimmed, so the freed slots' device memory goes back too (growing again later maps memory, it copies
-        nothing)."""
+        nothing).  A single-GPU index and a device group are reclaimed alike; an index without `compact` is skipped."""
         vs = self.vector_store
         ix = vs._index if vs is not None else None
         if ix is None or getattr(ix, "compact", None) is None:

@@ -480,7 +480,8 @@ class VectorStore:
     def compact(self) -> int:
         """Give the slots of deleted rows back (the reference's `Map.delete` frees its entry; a tombstone does not):
         the device index moves its live rows down in Map order and the slot <-> id table follows its old_to_new map.
-        Returns the number of slots reclaimed.  An index without `compact` (a device group) is left as it is.  The
+        Returns the number of slots reclaimed.  A device group compacts in global slots, moving rows between its
+        GPUs; an index without `compact` is left as it is.  The
         SQLite table, the reload sidecar (which describes the table, not slots) and `bad_ids` do not change.  Holds
         the state lock, like every search, so no search maps its slots through a half-updated table."""
         with self._st.lock:

@@ -209,7 +209,8 @@ export class GpuEmbeddingIndex {
    * Give the slots of deleted ids back (the reference's Map.delete frees its entry; a tombstone alone does not): the
    * device index moves its live rows down in Map order and returns oldToNew, through which slotOfId and idOfSlot are
    * renumbered.  Holds back new bestBatch calls and waits for those in flight first, so no search result is ever mapped
-   * through the other table.  Returns the number of slots reclaimed.  Throws for a device group (RUNBOOK_KNN_DEVICES).
+   * through the other table.  Returns the number of slots reclaimed.  A device group (RUNBOOK_KNN_DEVICES) compacts
+   * the same way, in global slots, moving rows between its GPUs; only a library built before group compaction throws.
    */
   async compact(): Promise<number> {
     while (this.compacting) await this.compacting;
