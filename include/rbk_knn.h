@@ -44,6 +44,8 @@ extern "C" {
 /* Largest k_fetch of the large-k search (rbk_index_search_large_f64): 4 * limit for the reference's largest
  * limit (1000, knowledge-context.ts:150). */
 #define RBK_MAX_K_FETCH_LARGE 4096
+/* Widest row an index or group accepts: 1 <= dim <= RBK_MAX_DIM, else RBK_EINVAL. */
+#define RBK_MAX_DIM (1 << 20)
 
 typedef struct rbk_index rbk_index;
 
@@ -61,8 +63,9 @@ int rbk_abi_version(void);
 const char* rbk_last_error(void);
 
 /* ---- lifetime: `new VectorStore(dbPath)` / `close()` (vector-store.ts:28-32, :330) ---- */
-/* dim: embedding length (any d >= 1).  device: CUDA ordinal.  capacity_hint: rows to
- * pre-allocate (0 = default); the index grows on demand.  The device storage sits on virtual address ranges reserved
+/* dim: embedding length, 1 <= dim <= RBK_MAX_DIM (RBK_EINVAL outside, checked before the device).  device: CUDA
+ * ordinal.  capacity_hint: rows to pre-allocate (0 = default; at least 1024 rows are mapped at creation, about 2*dim
+ * bytes each, 10*dim with RBK_INDEX_KEEP_F64: 2 GiB and 10 GiB at RBK_MAX_DIM); the index grows on demand.  The device storage sits on virtual address ranges reserved
  * here for the most rows the device's memory could hold (min(2^31 - 512, total memory / device bytes per row)); a
  * capacity_hint above that fails with RBK_ENOMEM.  Growth maps more physical memory behind the same addresses: nothing
  * is copied, so growing to capacity C needs C's storage, not the old and the new at once.  The capacity doubles

@@ -1175,7 +1175,7 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
     return fail(RBK_EINVAL, "RBK_INDEX_F64_ON_HOST requires RBK_INDEX_KEEP_F64");
   if ((flags & RBK_INDEX_SCAN_F16) && !(flags & RBK_INDEX_KEEP_F64))
     return fail(RBK_EINVAL, "RBK_INDEX_SCAN_F16 requires RBK_INDEX_KEEP_F64");
-  if (dim < 1 || dim > (1 << 20)) return fail(RBK_EINVAL, "dim out of range");
+  if (dim < 1 || dim > RBK_MAX_DIM) return fail(RBK_EINVAL, "dim out of range");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev == 0)

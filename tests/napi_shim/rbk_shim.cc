@@ -36,7 +36,7 @@ const char* rbk_last_error(void) { return g_err.c_str(); }
 int rbk_abi_version(void) { return RBK_ABI_VERSION; }
 
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t, uint32_t, rbk_index** out) {
-  if (dim < 1) return fail(RBK_EINVAL, "dim out of range");
+  if (dim < 1 || dim > RBK_MAX_DIM) return fail(RBK_EINVAL, "dim out of range");
   if (device != 0) return fail(RBK_EINVAL, "device ordinal out of range");
   *out = new rbk_index();
   (*out)->dim = dim;
@@ -99,7 +99,7 @@ rbk_status rbk_index_search_f64(rbk_index* ix, const double* queries, int32_t B,
 // the group family: same behaviour behind the other handle type (global slots = insertion order)
 rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_devices, int64_t, uint32_t, rbk_group** out) {
   if (!device_ids || n_devices < 1) return fail(RBK_EINVAL, "bad device list");
-  if (dim < 1) return fail(RBK_EINVAL, "dim out of range");
+  if (dim < 1 || dim > RBK_MAX_DIM) return fail(RBK_EINVAL, "dim out of range");
   *out = new rbk_group();
   (*out)->ix.dim = dim;
   return RBK_OK;
