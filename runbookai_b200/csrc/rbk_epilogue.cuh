@@ -544,21 +544,24 @@ __device__ __forceinline__ void run_emit_epilogue(const LargeScanParams& p, cons
 // Bounded-lag lockstep of the QB producers that stream the same corpus range: nobody runs
 // more than kMaxLeadTiles ahead of the slowest, so a tile pulled from HBM by the first
 // reader is still in L2 for the others (keeps DRAM traffic close to 1x the corpus).
-// Whole warp: lane o reads peer o's progress, so all peers cost one L2 round trip, and the warp only spins (re-reading
-// in parallel) while a ballot finds someone behind.  The wait gives up after 2^24 cycles in all (not per peer): it is a
-// hint, and a peer that far behind is not worth more of this CTA's time.
+// Whole warp, before tile `it` of the unit is loaded: lane o answers for peer o (`peer`: the lane has one), and `seen`
+// is that peer's progress as the lane read it a few k-steps ago (lockstep_peek), so the usual case costs no L2 round
+// trip here.  Progress only rises: a peer that was not behind then is not behind now.  Only when a ballot finds someone
+// behind does the warp re-read, all peers in parallel, and spin while one still is.  The wait gives up after 2^24
+// cycles in all (not per peer): it is a hint, and a peer that far behind is not worth more of this CTA's time.
 static_assert(kMaxSubBatch / kBlockM <= 32, "one lane per query block");
-__device__ __forceinline__ void lockstep_pace(volatile int* prog, int QB, int qb, int it, int max_lead, int lane) {
-  if (QB <= 1 || (it & 1) != 0) return;   // every other tile: checking every tile costs ~10 % on short kernels
+__device__ __forceinline__ void lockstep_peek(const volatile int* prog, int lane, bool peer, int& seen) {
+  if (peer) seen = prog[lane];   // no use of the value here: the load is in flight while the warp goes on
+}
+__device__ __forceinline__ void lockstep_pace(volatile int* prog, int qb, int it, int max_lead, int lane, bool peer,
+                                              int seen) {
   if (lane == 0) prog[qb] = it;
-  const bool peer = lane < QB && lane != qb;
   const int floor = it - max_lead;
-  bool behind = peer && prog[lane] < floor;
+  if (!__any_sync(0xFFFFFFFFu, peer && seen < floor)) return;
   const long long w0 = clock64();
-  while (__any_sync(0xFFFFFFFFu, behind)) {
-    __nanosleep(200);
+  while (__any_sync(0xFFFFFFFFu, peer && prog[lane] < floor)) {
     if (__shfl_sync(0xFFFFFFFFu, clock64() - w0, 0) > (1ll << 24)) break;   // never a correctness wait
-    behind = peer && prog[lane] < floor;
+    __nanosleep(200);
   }
 }
 

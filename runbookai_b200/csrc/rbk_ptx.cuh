@@ -48,6 +48,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// Adds 1 to a shared-memory counter and returns its old value.  acq_rel at CTA scope: the add releases what this thread
+// did or observed before it and acquires what every earlier adder had released, as an mbarrier arrive + wait pair does.
+__device__ __forceinline__ uint32_t smem_inc_acq_rel(uint32_t addr) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"(addr) : "memory");
+  return old;
+}
+
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");

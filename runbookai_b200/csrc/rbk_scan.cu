@@ -46,9 +46,10 @@ cudaError_t launch_scan_large(const CUtensorMap& tmap_q, const CUtensorMap& tmap
 
 #ifdef RBK_SCAN_CYCLE_STATS
 // Probe builds only: waits for the current device, copies its cycle sums ([mode][warpgroup][full, mma, handoff, pace,
-// tile_end, tiles, units], 42 values) to out and clears them.  Returns the number of values, or -1 on a CUDA error.
+// refill, tile_end, fetch, tiles, units, fetch_waits, refills], 66 values) to out and clears them.  Returns the number
+// of values, or -1 on a CUDA error.
 extern "C" int rbk_scan_cycle_stats(unsigned long long* out) {
-  constexpr int n = 3 * 2 * (rbk::kCycBuckets + 2);
+  constexpr int n = 3 * 2 * (rbk::kCycBuckets + rbk::kCycCounters);
   static const unsigned long long zero[n] = {};
   if (cudaDeviceSynchronize() != cudaSuccess ||
       cudaMemcpyFromSymbol(out, rbk::g_cycle_stats, sizeof(zero)) != cudaSuccess ||

@@ -36,7 +36,10 @@ struct SmemTail {
   StageHeader hdr[2];
   uint16_t wmask[2][2][4];     // [warpgroup][tile parity][warp] queries of the warp that pass the prefilter
   unsigned long long full[kStages];
-  unsigned long long empty[kStages];
+  uint32_t released[kStages];   // releases of the slot so far, two per use (one per wgmma warpgroup)
+#if RBK_SCAN_PROBE
+  uint32_t issue_clk[kStages];  // SM clock at the slot's last TMA issue
+#endif
   unsigned long long invc_full[2][2];
   unsigned long long st_full[2];
   unsigned long long st_empty[2];
@@ -74,25 +77,29 @@ __device__ __forceinline__ uint32_t quad_bits(uint32_t b) {
 // deltas into buckets, summed over the launch per warpgroup:
 //   full     waiting on a ring slot's `full` barrier;
 //   mma      fence, HGMMA issue and wait_group until the previous group has retired (tensor work);
-//   handoff  from wait_group returning to the end of the slot releases (the `empty` arrive and, for warpgroup 1,
-//            whose first warp is the producer, the `empty` wait, pacing and TMA issue of the refill);
-//   pace     the part of handoff spent in lockstep_pace (warpgroup 1 only);
-//   tile_end wait_group 0, the last release, the prefilter, the st_empty waits and the row staging.
+//   handoff  from wait_group returning to the end of the slot release: pacing (warpgroup 1), the release count and,
+//            in the warpgroup that released the slot last, the TMA issue of its refill.  Nobody waits here for the
+//            other warpgroup;
+//   pace     the part of handoff spent on lockstep (warpgroup 1 only: its first warp paces the CTA);
+//   refill   the part of handoff its leader spent issuing refills, `refills` of them;
+//   tile_end wait_group 0, the last release, the prefilter, the st_empty waits and the row staging;
+//   fetch    not a lap: over the `fetch_waits` full waits that found the barrier still pending, cycles from the slot's
+//            TMA issue (either warpgroup's) to the wait's return, i.e. how long a copy that is waited for takes.
 // The laps are contiguous, so full + mma + handoff + tile_end is the whole main loop.  The kernel only adds; the host
 // reads and clears the sums with rbk_scan_cycle_stats (no printf: a call inside the kernel makes ptxas serialize the
 // wgmma pipeline, and the probe would time another kernel).  The probe's registers cost the top-k' instantiation
-// about 20 bytes of spills, reloaded at the tile end, none in the k-step loop.  Without the macro CycleProbe is empty
-// and compiles to nothing.
-enum CycleBucket { kCycFull, kCycMma, kCycHandoff, kCycPace, kCycTileEnd, kCycBuckets };
+// about 20 bytes of spills.  Without the macro CycleProbe is empty and compiles to nothing.
+enum CycleBucket { kCycFull, kCycMma, kCycHandoff, kCycPace, kCycRefill, kCycTileEnd, kCycFetch, kCycBuckets };
+constexpr int kCycCounters = 4;   // after the buckets: tiles, units, fetch_waits, refills
 #if RBK_SCAN_PROBE
-__device__ unsigned long long g_cycle_stats[3][2][kCycBuckets + 2];   // [mode][warpgroup][bucket, tiles, units]
+__device__ unsigned long long g_cycle_stats[3][2][kCycBuckets + kCycCounters];   // [mode][warpgroup][...]
 __device__ __forceinline__ uint32_t sm_clock() {
   uint32_t c;
   asm volatile("mov.u32 %0, %%clock;" : "=r"(c)::"memory");
   return c;
 }
 struct CycleProbe {
-  uint32_t t = 0, c[kCycBuckets] = {};
+  uint32_t t = 0, c[kCycBuckets] = {}, fetch_waits = 0, refills = 0;
   __device__ __forceinline__ void mark() { t = sm_clock(); }
   __device__ __forceinline__ void lap(int b) {   // t .. now into bucket b; now becomes t
     const uint32_t n = sm_clock();
@@ -100,6 +107,14 @@ struct CycleProbe {
     t = n;
   }
   __device__ __forceinline__ void add_since(int b, uint32_t t0) { c[b] += sm_clock() - t0; }
+  __device__ __forceinline__ void refilled(uint32_t t0) {
+    add_since(kCycRefill, t0);
+    ++refills;
+  }
+  __device__ __forceinline__ void fetched(uint32_t issue_clk) {   // a full wait that blocked has returned
+    add_since(kCycFetch, issue_clk);
+    ++fetch_waits;
+  }
   __device__ __forceinline__ static uint32_t now() { return sm_clock(); }
 };
 #else
@@ -107,6 +122,7 @@ struct CycleProbe {
   __device__ __forceinline__ void mark() {}
   __device__ __forceinline__ void lap(int) {}
   __device__ __forceinline__ void add_since(int, uint32_t) {}
+  __device__ __forceinline__ void refilled(uint32_t) {}
   __device__ __forceinline__ static uint32_t now() { return 0u; }
 };
 #endif
@@ -138,7 +154,7 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
     tma_prefetch_desc(&tmap_c);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(smem_u32(&tail->full[s]), 1);
-      mbar_init(smem_u32(&tail->empty[s]), 2);   // one arrive per wgmma warpgroup
+      tail->released[s] = 0u;
     }
     for (int w = 0; w < 2; ++w) {
       mbar_init(smem_u32(&tail->invc_full[w][0]), 1);
@@ -173,33 +189,54 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
   setmaxnreg_inc<kMmaRegs>();
   const int wg = wgroup - 1;
   const bool leader = (threadIdx.x & 127) == 0;
-  const bool producer = warp == 4;
   const int n_iter = t1 - t0;
-  const int n_steps = n_iter * n_ks;   // k-steps of the whole unit; step j uses ring slot j % kStages
   volatile int* prog = p.progress + r * p.QB;
   CycleProbe probe;
-  // Load step j into its slot once both warpgroups have released the slot's previous use (whole warp).
-  auto issue = [&](int j) {
-    if (j >= n_steps) return;
-    const int s = j % kStages;
-    const int tile = t0 + j / n_ks, ks = j % n_ks;
-    mbar_wait(smem_u32(&tail->empty[s]), static_cast<uint32_t>((j / kStages) & 1) ^ 1u);
-    const uint32_t pace0 = CycleProbe::now();
-    if (ks == 0) lockstep_pace(prog, p.QB, qb, tile - t0, p.max_lead_tiles, lane);
-    probe.add_since(kCycPace, pace0);
+  // Load k-slab ks of tile t0 + it into ring slot s (one thread).
+  auto issue = [&](int s, int it, int ks) {
+    const uint32_t issue0 = CycleProbe::now();
+#if RBK_SCAN_PROBE
+    tail->issue_clk[s] = issue0;
+#endif
     const uint32_t full = smem_u32(&tail->full[s]);
     const uint32_t a_dst = smem_base + s * kStageBytes;
-    if (elect_one()) {
-      mbar_arrive_expect_tx(full, kStageBytes);
-      tma_load_2d(a_dst, &tmap_q, full, ks * kBlockK, qb * kBlockM);
-      tma_load_2d(a_dst + kABytes, &tmap_c, full, ks * kBlockK, tile * kBlockN);
-    }
-    __syncwarp();
+    mbar_arrive_expect_tx(full, kStageBytes);
+    tma_load_2d(a_dst, &tmap_q, full, ks * kBlockK, qb * kBlockM);
+    tma_load_2d(a_dst + kABytes, &tmap_c, full, ks * kBlockK, (t0 + it) * kBlockN);
+    probe.refilled(issue0);
   };
-  // a step's slot is released (and refilled kStages steps ahead) once its wgmma group has retired
-  auto release = [&](int j) {
-    if (leader) mbar_arrive(smem_u32(&tail->empty[j % kStages]));
-    if (producer) issue(j + kStages);
+  // Lockstep is the business of warpgroup 1's first warp: it holds back its own release of the slot that a paced
+  // tile's first k-slab goes into, and with it the refill, whichever warpgroup issues that.  Its lanes read the
+  // peers' progress two refills earlier (as early as the tile before when n_ks < 3), so the check itself waits for
+  // no load.  seen starts as "nobody behind": the first check of a unit whose tiles are one k-slab is skipped.
+  const bool pacer = warp == 4 && p.QB > 1;
+  const bool peer = lane < p.QB && lane != qb;
+  const int peek_ks = n_ks > 2 ? n_ks - 2 : 0;
+  int seen = 0x7FFFFFFF;
+  // The step that refills the slot released next: k-slab r_ks of tile t0 + r_it (kStages steps after the released one).
+  int r_it = kStages / n_ks, r_ks = kStages % n_ks;
+  // Slot s is released by a warpgroup once its wgmma group on it has retired.  The warpgroup that does so last
+  // refills it there and then, from its leader thread, and nobody waits for the other: the leaders count releases in
+  // released[s], two per use of the slot, so the one whose add returns an odd count is the second.  Ordering: the
+  // leader's wgmma_wait has retired its warpgroup's reads of the slot before its add; the add is acq_rel at CTA scope,
+  // so the second leader's add has acquired the first one's, and its TMA issue follows in program order - the chain
+  // an `empty` mbarrier (arrive, arrive, wait, issue) would give.  Measured against that mbarrier kept for the
+  // ordering beside a relaxed add (arrive, add, and a wait by the second), this is the faster of the two (DESIGN §7).
+  // A warpgroup that runs ahead stops at a `full` wait.
+  auto release = [&](int s) {
+    // every other tile: pacing every tile costs ~10 % on short kernels
+    if (pacer && r_ks == 0 && (r_it & 1) == 0 && r_it < n_iter) {
+      const uint32_t pace0 = CycleProbe::now();
+      lockstep_pace(prog, qb, r_it, p.max_lead_tiles, lane, peer, seen);
+      probe.add_since(kCycPace, pace0);
+    }
+    if (leader && (smem_inc_acq_rel(smem_u32(&tail->released[s])) & 1u) != 0u && r_it < n_iter) issue(s, r_it, r_ks);
+    // after the add: its release fence would wait for the load
+    if (pacer && r_ks == peek_ks && (r_it & 1) != 0) lockstep_peek(prog, lane, peer, seen);
+    if (++r_ks == n_ks) {
+      r_ks = 0;
+      ++r_it;
+    }
   };
   // 1/||c|| of tile t0 + i for this warpgroup's prefilter, into buffer i & 1
   auto load_invc = [&](int i) {
@@ -208,8 +245,8 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
     mbar_arrive_expect_tx(bar, kBlockN * 4);
     bulk_load(smem_u32(tail->invc[wg][i & 1]), p.inv_norm_c + static_cast<size_t>(t0 + i) * kBlockN, kBlockN * 4, bar);
   };
-  if (producer)
-    for (int j = 0; j < kStages; ++j) issue(j);
+  if (leader && wg == 0)
+    for (int j = 0; j < kStages && j / n_ks < n_iter; ++j) issue(j, j / n_ks, j % n_ks);
   load_invc(0);
   load_invc(1);
   // this thread's accumulator rows: query qw0 (d[4j + 0..1]) and qw1 (d[4j + 2..3]) of the warpgroup's 64
@@ -227,7 +264,14 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
   for (int i = 0; i < n_iter; ++i) {
     for (int ks = 0; ks < n_ks; ++ks, ++j) {
       const int s = j % kStages;
-      mbar_wait(smem_u32(&tail->full[s]), static_cast<uint32_t>((j / kStages) & 1));
+      const uint32_t full = smem_u32(&tail->full[s]), parity = static_cast<uint32_t>((j / kStages) & 1);
+#if RBK_SCAN_PROBE
+      const bool blocked = leader && !mbar_try_wait(full, parity);
+#endif
+      mbar_wait(full, parity);
+#if RBK_SCAN_PROBE
+      if (blocked) probe.fetched(tail->issue_clk[s]);
+#endif
       probe.lap(kCycFull);
       const uint32_t st = smem_base + s * kStageBytes;
       const uint64_t adesc = make_sw128_kmajor_desc(st + wg * (64 * kBlockK * 2));
@@ -239,11 +283,11 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
       wgmma_commit();
       wgmma_wait<1>(acc);   // the previous step's group has retired
       probe.lap(kCycMma);
-      if (ks > 0) release(j - 1);
+      if (ks > 0) release((j - 1) % kStages);
       probe.lap(kCycHandoff);
     }
     wgmma_wait<0>(acc);
-    release(j - 1);
+    release((j - 1) % kStages);
 
     // Prefilter: scores = accumulator * 1/||c|| (the very multiply the epilogue used to do), then each row's maximum
     // against the threshold its epilogue thread last published.  fmaxf drops the NaN of dead rows.
@@ -305,13 +349,15 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ 
     } while (pending != 0ull);
     probe.lap(kCycTileEnd);
   }
-  if (producer && lane == 0 && p.QB > 1) prog[qb] = 0x7FFFFFFF;  // done: never hold a peer back
+  if (pacer && lane == 0) prog[qb] = 0x7FFFFFFF;  // done: never hold a peer back
 #if RBK_SCAN_PROBE
   if (leader) {   // the host reads the sums (rbk_scan_cycle_stats): a call here would serialize the wgmma pipeline
     for (int b = 0; b < kCycBuckets; ++b)
       atomicAdd(&g_cycle_stats[kMode][wg][b], static_cast<unsigned long long>(probe.c[b]));
     atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets], static_cast<unsigned long long>(n_iter));
     atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets + 1], 1ull);
+    atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets + 2], static_cast<unsigned long long>(probe.fetch_waits));
+    atomicAdd(&g_cycle_stats[kMode][wg][kCycBuckets + 3], static_cast<unsigned long long>(probe.refills));
   }
 #endif
 }

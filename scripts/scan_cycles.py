@@ -7,8 +7,9 @@ Builds the library with -DRBK_SCAN_CYCLE_STATS into a temporary copy of the pack
 replaced), then, per workload, generates bench.py's corpus and queries in a child process and runs one warm-up search
 and `--launches` searches.  After each search it reads (and clears) the probe's sums with `rbk_scan_cycle_stats`, and
 writes DIR/scan_cycles.json: per workload and launch the raw sums of each wgmma warpgroup, and the median over the
-launches of each bucket per (tile, warpgroup), in SM cycles.  `unit` is the whole main loop (the sum of the buckets
-other than pace).  Each launch also carries the probe kernel's time (CUDA events, `last_scan_ms`) and the SM clock the
+launches of each bucket per (tile, warpgroup), in SM cycles.  `unit` is the whole main loop (full + mma + handoff +
+tile_end; pace and refill are parts of handoff).  `fetch` is per blocked `full` wait, not per tile: the cycles from
+the slot's TMA issue to the wait's return, with `fetch_waits` such waits per tile.  Each launch also carries the probe kernel's time (CUDA events, `last_scan_ms`) and the SM clock the
 two imply (`unit` cycles per CTA over that time): compare that time with bench.py's `kernel_ms` of the default build
 to see how far the probe's clock reads moved the kernel.
 """
@@ -25,8 +26,9 @@ import tempfile
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
-BUCKETS = ("full", "mma", "handoff", "pace", "tile_end")
-FIELDS = BUCKETS + ("tiles", "units")
+BUCKETS = ("full", "mma", "handoff", "pace", "refill", "tile_end", "fetch")
+LAPS = ("full", "mma", "handoff", "tile_end")      # contiguous: they sum to the main loop
+FIELDS = BUCKETS + ("tiles", "units", "fetch_waits", "refills")
 
 
 def build_probe(pkg_dir: Path) -> Path:
@@ -93,17 +95,20 @@ def child(pkg_root: str, workload: str, launches: int) -> None:
 
 
 def per_tile(rec: dict) -> dict:
-    """Cycles per (tile, warpgroup), both warpgroups averaged; pace is warpgroup 1's alone."""
+    """Cycles per (tile, warpgroup), both warpgroups averaged, and each warpgroup's own where they differ by role."""
     w1, w2 = rec["wg1"], rec["wg2"]
     tiles = w1["tiles"] + w2["tiles"]
-    res = {b: (w1[b] + w2[b]) / tiles for b in BUCKETS if b != "pace"}
-    res["pace"] = w1["pace"] / w1["tiles"]
-    res["unit"] = sum(res[b] for b in ("full", "mma", "handoff", "tile_end"))
-    for b in ("full", "handoff"):
-        res[b + "_wg1"] = w1[b] / w1["tiles"]
-        res[b + "_wg2"] = w2[b] / w2["tiles"]
+    res = {b: (w1[b] + w2[b]) / tiles for b in LAPS}
+    res["unit"] = sum(res[b] for b in LAPS)
+    for name, w in (("wg1", w1), ("wg2", w2)):
+        for b in ("full", "handoff", "pace", "refill"):
+            res[f"{b}_{name}"] = w[b] / w["tiles"]
+        res[f"refills_{name}"] = w["refills"] / w["tiles"]
+        res[f"fetch_waits_{name}"] = w["fetch_waits"] / w["tiles"]
+    waits = w1["fetch_waits"] + w2["fetch_waits"]
+    res["fetch_per_blocked_wait"] = (w1["fetch"] + w2["fetch"]) / waits if waits else 0.0
     # the SM clock that this many cycles per CTA in the probe kernel's event time implies
-    unit_per_cta = sum(w1[b] + w2[b] for b in ("full", "mma", "handoff", "tile_end")) / (w1["units"] + w2["units"])
+    unit_per_cta = sum(w1[b] + w2[b] for b in LAPS) / (w1["units"] + w2["units"])
     res["implied_sm_mhz"] = unit_per_cta / (rec["last_scan_ms"] * 1e3)
     res["scan_ms"] = rec["last_scan_ms"]
     return res
