@@ -96,7 +96,7 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * search 8*dim bytes per emitted candidate, and the rare exhaustive fallback / rbk_index_exact_scores_f64 the whole
  * corpus, all at PCIe speed; appends write the rows over PCIe.  Every write to the host rows is stream-ordered (a kernel
  * or copy on the index stream, or the host after a synchronisation), so searches enqueued earlier never see a
- * half-written row.  The placement is fixed for the index's life. */
+ * half-written row.  The placement is fixed until rbk_index_set_tier. */
 #define RBK_INDEX_F64_ON_HOST 2u
 /* RBK_INDEX_SCAN_F16 (only together with RBK_INDEX_KEEP_F64, else RBK_EINVAL; combines with RBK_INDEX_F64_ON_HOST):
  * the scan reads fp16 rows instead of bf16, at the same 2 bytes per element.  Each row x (and each query) is stored
@@ -106,11 +106,44 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * between a row or query and its stored copy - is several times tighter (DESIGN.md §6): fewer batches need the wide
  * retry, and the large-k search emits fewer candidates.  Answers are those of a KEEP_F64 index without the flag: the
  * same slots and fp64 scores, bit for bit, including the scan-band rule above (decided on the float64 row or query,
- * not on the scaled copy).  The placement is fixed for the index's life; read the stored bits with
+ * not on the scaled copy).  The placement is fixed until rbk_index_set_tier; read the stored bits with
  * rbk_index_read_rows_f16. */
 #define RBK_INDEX_SCAN_F16 16u
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out);
 void rbk_index_destroy(rbk_index* idx); /* NULL is a no-op */
+/* The index's creation flags as they are now (RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16); 0 for
+ * NULL. */
+uint32_t rbk_index_flags(const rbk_index* idx);
+/* Change the storage tier of a float64-backed index in place, from the float64 rows it holds: move them between the
+ * device and pinned host memory (RBK_INDEX_F64_ON_HOST) and switch the scan between bf16 and fp16 (RBK_INDEX_SCAN_F16),
+ * without reloading.
+ *   - flags: a flag set rbk_index_create_ex accepts, with the index's own RBK_INDEX_KEEP_F64 bit (a float64 copy cannot
+ *     be made from bf16 rows, and dropping it would change the answers); anything else returns RBK_EINVAL with the index
+ *     untouched.  The current flags are a no-op (RBK_OK).  The member indexes of a group refuse the call (RBK_EINVAL):
+ *     rbk_group_set_tier changes them together.
+ *   - Every answer stays bit for bit: slots, fp64 scores, counts, -1 / NaN tails, exactness flags, compaction maps; so
+ *     do size(), count(), slot_base, the capacity and the stats counters.
+ *   - Afterwards the index is what rbk_index_create_ex with `flags`, fed the same calls, would be: the same stored scan
+ *     bits (tombstoned slots included; the one exception is a NaN element of a bf16 input, whose payload bits the bf16
+ *     tier's direct copy kept and a re-derivation does not), inv_norm and norm2, rbk_index_storage_bytes, and the
+ *     row ceiling that later growth can reach, min(2^31 - 512, total device memory / device bytes per row) of the new
+ *     tier.  Moving the rows to the host maps the device buffers' existing physical memory at new, larger address
+ *     ranges (nothing is copied, peak device memory does not grow).
+ *   - The corpus-side error bound is recomputed under the new scan type as the largest angle over every stored slot,
+ *     live or tombstoned (a change of placement alone keeps it).  It is never larger than that of an index created
+ *     with `flags`; after overwrites or compaction it may be smaller, and then fewer batches may take the wide retry or
+ *     the fallback.  Once an off-band row has been stored (see RBK_INDEX_KEEP_F64), the bound stays one that proves
+ *     nothing until rbk_index_clear.
+ *   - Every allocation - the pinned [capacity][dim] buffer, the device memory of the float64 rows, the new address
+ *     ranges - happens before anything changes: RBK_ENOMEM (and RBK_EINVAL) leaves the index exactly as it was.
+ *     Moving the rows to the device fails so when the capacity is above the device tier's row ceiling (rbk_index_trim
+ *     first, or stay).  That guarantee covers the allocations only: a CUDA error while the rows move (RBK_ECUDA,
+ *     which poisons the context anyway) may leave the index part-way changed; the allocations it no longer needs are
+ *     released.
+ *   - Synchronous.  Searches enqueued earlier (rbk_index_search_device_async) finish first, on the old tier, because the
+ *     index's work is stream-ordered.  Cost: one pass of the float64 rows from one side of PCIe to the other (placement),
+ *     and the ingest kernels over every stored row (scan type; they read the rows over PCIe when they are on the host). */
+rbk_status rbk_index_set_tier(rbk_index* idx, uint32_t flags);
 
 /* Run all device work of this index on the given cudaStream_t (NULL = the index's own
  * stream).  Lets a host framework time the engine with events on its current stream. */
@@ -313,6 +346,10 @@ rbk_status rbk_group_clear(rbk_group* grp);
 rbk_status rbk_group_compact(rbk_group* grp, int64_t* old_to_new, int64_t old_to_new_len);
 /* rbk_index_trim on every member, and the group's own exchange buffers released. */
 rbk_status rbk_group_trim(rbk_group* grp);
+/* rbk_index_set_tier on every member together (read the flags of any member with rbk_index_flags): every member's
+ * allocations happen before any member changes, so RBK_ENOMEM leaves the whole group as it was.  Synchronous; uses no
+ * NCCL. */
+rbk_status rbk_group_set_tier(rbk_group* grp, uint32_t flags);
 int64_t rbk_group_count(const rbk_group* grp); /* live rows */
 int64_t rbk_group_size(const rbk_group* grp);  /* slots used, tombstones included */
 int32_t rbk_group_devices(const rbk_group* grp);

@@ -3,7 +3,8 @@
 // hostRows), loads rows as
 // SQLite-style BLOBs and as a Float64Array, overwrites, tombstones, counts, searches through the Promise/async-work
 // path, provokes every error path, optionally (compact.txt) tombstones more, compacts and searches again, optionally
-// (trim.txt) trims and searches again, clears, and lets the finalizer run.  Inputs and outputs are flat binary files in
+// (trim.txt) trims and searches again, optionally (set_tier.txt) changes the storage tier between searches, clears, and
+// lets the finalizer run.  Inputs and outputs are flat binary files in
 // the directory given as argv[1]; tests/test_napi_addon.py writes the inputs and checks the outputs against the
 // oracle.  Links against librbk_knn.so (GPU test) or against tests/napi_shim (CPU test).
 //
@@ -188,6 +189,52 @@ int main(int argc, char** argv) {
   write_bin("slots.i64", res.slots.data(), res.slots.size() * 8);
   write_bin("scores.f64", res.scores.data(), res.scores.size() * 8);
   write_bin("counts.i32", res.counts.data(), res.counts.size() * 4);
+
+  // setTier() / tier: optional set_tier.txt "f64OnHost scanF16" (0 or 1 each).  Reads `tier`, changes both, searches
+  // again (results in tier_*, logged as tier_identical), flips scanF16 alone and searches again (tier_partial_identical),
+  // then passes a number where a boolean belongs (err_set_tier_type).  A library without tier changes: err_set_tier.
+  {
+    std::ifstream sf(g_dir + "/set_tier.txt");
+    int host = 0, f16 = 0;
+    if (sf >> host >> f16) {
+      napi_value t = nullptr;
+      auto log_tier = [&](const char* key) {
+        if (!mock::get_accessor(env, ix, "tier", &t, &err)) return false;
+        log << key << " " << mock::as_bool(mock::get_property(env, t, "f64OnHost")) << " "
+            << mock::as_bool(mock::get_property(env, t, "scanF16")) << "\n";
+        return true;
+      };
+      auto same_as_first = [&](const Result& x) {
+        return x.slots == res.slots && x.counts == res.counts &&
+               memcmp(x.scores.data(), res.scores.data(), res.scores.size() * 8) == 0;
+      };
+      if (!log_tier("tier_before")) {
+        log << "err_set_tier " << err << "\n";
+      } else {
+        napi_value arg = mock::object(env, {{"f64OnHost", mock::boolean(env, host != 0)},
+                                            {"scanF16", mock::boolean(env, f16 != 0)}});
+        if (!mock::call_method(env, ix, "setTier", {arg}, &r, &err)) die("setTier threw: " + err);
+        if (!mock::is_undefined(r)) die("setTier returned a value");
+        log_tier("tier_after");
+        Result tr;
+        if (!search(env, ix, queries, n_q, k, min_score, &tr, &err)) die("search after setTier rejected: " + err);
+        write_bin("tier_slots.i64", tr.slots.data(), tr.slots.size() * 8);
+        write_bin("tier_scores.f64", tr.scores.data(), tr.scores.size() * 8);
+        write_bin("tier_counts.i32", tr.counts.data(), tr.counts.size() * 4);
+        log << "tier_identical " << same_as_first(tr) << "\n";
+        if (!mock::call_method(env, ix, "setTier", {mock::object(env, {{"scanF16", mock::boolean(env, f16 == 0)}})}, &r,
+                               &err))
+          die("setTier({scanF16}) threw: " + err);
+        log_tier("tier_partial");
+        Result pr;
+        if (!search(env, ix, queries, n_q, k, min_score, &pr, &err)) die("search after setTier rejected: " + err);
+        log << "tier_partial_identical " << same_as_first(pr) << "\n";
+        if (mock::call_method(env, ix, "setTier", {mock::object(env, {{"f64OnHost", mock::number(env, 1)}})}, &r, &err))
+          die("setTier with a number did not throw");
+        log << "err_set_tier_type " << err << "\n";
+      }
+    }
+  }
 
   // searchLarge(): optional large.txt lists k_fetch values (up to 4096); results land in large<i>_*.  One more call
   // with k_fetch 4097 must reject with the library's message.

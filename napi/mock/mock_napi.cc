@@ -9,7 +9,7 @@
 
 namespace {
 
-enum Kind { kUndefined, kNumber, kString, kObject, kArray, kArrayBuffer, kTypedArray, kBuffer, kClass, kPromise, kError };
+enum Kind { kUndefined, kBoolean, kNumber, kString, kObject, kArray, kArrayBuffer, kTypedArray, kBuffer, kClass, kPromise, kError };
 
 struct Val {
   Kind kind = kUndefined;
@@ -25,6 +25,7 @@ struct Val {
   // class
   napi_callback ctor = nullptr;
   std::map<std::string, napi_callback> methods;
+  std::map<std::string, napi_callback> getters;
   Val* cls = nullptr;                       // instance -> its class
   // wrapped native pointer
   void* native = nullptr;
@@ -117,10 +118,40 @@ napi_status napi_define_class(napi_env env, const char* utf8name, size_t, napi_c
   c->str = utf8name;
   c->ctor = constructor;
   for (size_t i = 0; i < property_count; ++i) {
-    if (!properties[i].utf8name || !properties[i].method) return napi_invalid_arg;
-    c->methods[properties[i].utf8name] = properties[i].method;
+    if (!properties[i].utf8name || (!properties[i].method == !properties[i].getter)) return napi_invalid_arg;
+    if (properties[i].method) c->methods[properties[i].utf8name] = properties[i].method;
+    else c->getters[properties[i].utf8name] = properties[i].getter;
   }
   *result = N(c);
+  return napi_ok;
+}
+
+napi_status napi_get_boolean(napi_env env, bool value, napi_value* result) {
+  Val* b = env->make(kBoolean);
+  b->num = value ? 1 : 0;
+  *result = N(b);
+  return napi_ok;
+}
+
+napi_status napi_get_value_bool(napi_env, napi_value value, bool* result) {
+  Val* v = V(value);
+  if (!v || v->kind != kBoolean) return napi_boolean_expected;
+  *result = v->num != 0;
+  return napi_ok;
+}
+
+napi_status napi_has_named_property(napi_env, napi_value object, const char* utf8name, bool* result) {
+  Val* o = V(object);
+  if (!o || o->kind != kObject) return napi_object_expected;
+  *result = o->props.count(utf8name) != 0;
+  return napi_ok;
+}
+
+napi_status napi_get_named_property(napi_env, napi_value object, const char* utf8name, napi_value* result) {
+  Val* o = V(object);
+  if (!o || o->kind != kObject) return napi_object_expected;
+  auto it = o->props.find(utf8name);
+  *result = it == o->props.end() ? nullptr : N(it->second);
   return napi_ok;
 }
 
@@ -369,6 +400,29 @@ bool call_method(napi_env env, napi_value object, const char* name, const std::v
   }
   return invoke(env, o->cls->methods[name], o, args, out, error);
 }
+
+bool get_accessor(napi_env env, napi_value object, const char* name, napi_value* out, std::string* error) {
+  Val* o = V(object);
+  if (!o || !o->cls || !o->cls->getters.count(name)) {
+    if (error) *error = std::string(name) + " is not a getter";
+    return false;
+  }
+  return invoke(env, o->cls->getters[name], o, {}, out, error);
+}
+
+napi_value boolean(napi_env env, bool v) {
+  napi_value out = nullptr;
+  napi_get_boolean(env, v, &out);
+  return out;
+}
+
+napi_value object(napi_env env, const std::vector<std::pair<std::string, napi_value>>& props) {
+  Val* o = env->make(kObject);
+  for (const auto& p : props) o->props[p.first] = V(p.second);
+  return N(o);
+}
+
+int as_bool(napi_value v) { return V(v) && V(v)->kind == kBoolean ? (V(v)->num != 0) : -1; }
 
 void run_event_loop(napi_env env) {
   while (!env->queue.empty()) {

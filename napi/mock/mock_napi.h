@@ -3,6 +3,7 @@
 #define RBK_MOCK_NAPI_H_
 
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "node_api.h"
@@ -18,12 +19,16 @@ napi_value number(napi_env env, double v);
 napi_value array(napi_env env, const std::vector<napi_value>& elems);
 napi_value buffer(napi_env env, const void* bytes, size_t n);                                  // Node Buffer
 napi_value typed_array(napi_env env, napi_typedarray_type t, const void* data, size_t length);  // copies the data
+napi_value boolean(napi_env env, bool v);
+napi_value object(napi_env env, const std::vector<std::pair<std::string, napi_value>>& props);   // { name: value, ... }
 
 // exports.<name>;  new cls(args...);  obj.method(args...).  A thrown exception comes back as false + message.
 napi_value get_property(napi_env env, napi_value object, const char* name);
 bool construct(napi_env env, napi_value cls, const std::vector<napi_value>& args, napi_value* out, std::string* error);
 bool call_method(napi_env env, napi_value object, const char* name, const std::vector<napi_value>& args,
                  napi_value* out, std::string* error);
+// obj.name through a getter the class defines
+bool get_accessor(napi_env env, napi_value object, const char* name, napi_value* out, std::string* error);
 
 // the event loop: run every queued async work item (execute on a second thread, complete on this one)
 void run_event_loop(napi_env env);
@@ -31,6 +36,7 @@ void run_event_loop(napi_env env);
 // reading results
 bool is_undefined(napi_value v);
 double as_number(napi_value v);
+int as_bool(napi_value v);   // 1 true, 0 false, -1 not a boolean
 // promise: 0 pending, 1 fulfilled, 2 rejected; *value = resolution / rejection
 int promise_state(napi_value promise, napi_value* value);
 std::string error_message(napi_value error);

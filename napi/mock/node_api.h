@@ -100,6 +100,10 @@ napi_status napi_unwrap(napi_env env, napi_value js_object, void** result);
 napi_status napi_define_class(napi_env env, const char* utf8name, size_t length, napi_callback constructor, void* data,
                               size_t property_count, const napi_property_descriptor* properties, napi_value* result);
 // -- reading values
+napi_status napi_get_boolean(napi_env env, bool value, napi_value* result);
+napi_status napi_get_value_bool(napi_env env, napi_value value, bool* result);
+napi_status napi_has_named_property(napi_env env, napi_value object, const char* utf8name, bool* result);
+napi_status napi_get_named_property(napi_env env, napi_value object, const char* utf8name, napi_value* result);
 napi_status napi_get_value_int32(napi_env env, napi_value value, int32_t* result);
 napi_status napi_get_value_int64(napi_env env, napi_value value, int64_t* result);
 napi_status napi_get_value_double(napi_env env, napi_value value, double* result);

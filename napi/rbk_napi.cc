@@ -19,6 +19,8 @@
 //   ix.tombstone(BigInt64Array slots); ix.clear()
 //   ix.compact()                               -> BigInt64Array oldToNew   // reclaim tombstoned slots
 //   ix.trim()                                  // give unused device memory back (after compact / clear)
+//   ix.setTier({ f64OnHost, scanF16 })         // move the float64 rows / switch the scan in place (omitted: kept)
+//   ix.tier                                    -> { f64OnHost: boolean, scanF16: boolean }
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
 //   await ix.searchLarge(Float64Array queries, B, kFetch, minScore)   // kFetch up to 4096, same result object
@@ -54,6 +56,11 @@
 // The same for trim; `trim` throws where it is missing.
 #pragma weak rbk_index_trim
 #pragma weak rbk_group_trim
+// The same for tier changes; `setTier` and `tier` throw where they are missing.
+#pragma weak rbk_index_flags
+#pragma weak rbk_index_set_tier
+#pragma weak rbk_group_set_tier
+#pragma weak rbk_group_member
 
 namespace {
 
@@ -87,6 +94,12 @@ struct Handle {
   bool has_trim() const { return grp ? rbk_group_trim != nullptr : rbk_index_trim != nullptr; }
   rbk_status trim() { return grp ? rbk_group_trim(grp) : rbk_index_trim(ix); }
   int64_t count() const { return grp ? rbk_group_count(grp) : rbk_index_count(ix); }
+  bool has_tier() const {
+    return rbk_index_flags != nullptr &&
+           (grp ? rbk_group_set_tier != nullptr && rbk_group_member != nullptr : rbk_index_set_tier != nullptr);
+  }
+  uint32_t flags() { return rbk_index_flags(grp ? rbk_group_member(grp, 0) : ix); }   // a group's members share them
+  rbk_status set_tier(uint32_t flags) { return grp ? rbk_group_set_tier(grp, flags) : rbk_index_set_tier(ix, flags); }
   rbk_status search(const double* q, int32_t B, int32_t qdim, int32_t k, double ms, int64_t* s, double* v, int32_t* c) {
     return grp ? rbk_group_search_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
                : rbk_index_search_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
@@ -309,6 +322,59 @@ napi_value Trim(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+bool require_tier(napi_env env, Handle* h) {
+  if (h->has_tier()) return true;
+  napi_throw_error(env, nullptr, "setTier: this librbk_knn.so has no tier change (rbk_index_set_tier / rbk_group_set_tier)");
+  return false;
+}
+
+// setTier({ f64OnHost, scanF16 }): rbk_index_set_tier / rbk_group_set_tier.  A key that is absent keeps its setting;
+// one that is present must be a boolean.  Synchronous; answers do not change.
+napi_value SetTier(napi_env env, napi_callback_info info) {
+  size_t argc = 1;
+  napi_value argv[1] = {nullptr};
+  Handle* h = unwrap(env, info, &argc, argv);
+  if (!require_tier(env, h)) return nullptr;
+  uint32_t flags = h->flags();
+  const struct {
+    const char* name;
+    uint32_t bit;
+  } keys[] = {{"f64OnHost", RBK_INDEX_F64_ON_HOST}, {"scanF16", RBK_INDEX_SCAN_F16}};
+  for (const auto& k : keys) {
+    bool has = false;
+    if (argc < 1 || napi_has_named_property(env, argv[0], k.name, &has) != napi_ok) {
+      napi_throw_type_error(env, nullptr, "setTier: the argument must be an object { f64OnHost, scanF16 }");
+      return nullptr;
+    }
+    if (!has) continue;
+    napi_value v;
+    bool on = false;
+    NAPI_OK(napi_get_named_property(env, argv[0], k.name, &v));
+    if (napi_get_value_bool(env, v, &on) != napi_ok) {
+      napi_throw_type_error(env, nullptr, (std::string("setTier: ") + k.name + " must be a boolean").c_str());
+      return nullptr;
+    }
+    flags = on ? (flags | k.bit) : (flags & ~k.bit);
+  }
+  if (h->set_tier(flags) != RBK_OK) return throw_rbk(env);
+  return nullptr;
+}
+
+// tier -> { f64OnHost, scanF16 }: where the float64 rows live and which scan the index runs, as they are now.
+napi_value GetTier(napi_env env, napi_callback_info info) {
+  size_t argc = 0;
+  Handle* h = unwrap(env, info, &argc, nullptr);
+  if (!require_tier(env, h)) return nullptr;
+  const uint32_t flags = h->flags();
+  napi_value out, host, f16;
+  NAPI_OK(napi_create_object(env, &out));
+  NAPI_OK(napi_get_boolean(env, (flags & RBK_INDEX_F64_ON_HOST) != 0, &host));
+  NAPI_OK(napi_get_boolean(env, (flags & RBK_INDEX_SCAN_F16) != 0, &f16));
+  NAPI_OK(napi_set_named_property(env, out, "f64OnHost", host));
+  NAPI_OK(napi_set_named_property(env, out, "scanF16", f16));
+  return out;
+}
+
 napi_value Count(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
@@ -426,6 +492,8 @@ napi_value Init(napi_env env, napi_value exports) {
       {"clear", nullptr, Clear, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"compact", nullptr, Compact, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trim", nullptr, Trim, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"setTier", nullptr, SetTier, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"tier", nullptr, nullptr, GetTier, nullptr, nullptr, napi_default, nullptr},
       {"count", nullptr, Count, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"search", nullptr, Search, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"searchLarge", nullptr, SearchLarge, nullptr, nullptr, nullptr, napi_default, nullptr},

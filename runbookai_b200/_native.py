@@ -33,6 +33,7 @@ SYMBOLS = [
     "rbk_group_overwrite_f64_batch", "rbk_group_tombstone", "rbk_group_clear", "rbk_group_compact", "rbk_group_trim", "rbk_group_count", "rbk_group_size",
     "rbk_group_devices", "rbk_group_member", "rbk_group_redone_batches", "rbk_group_search_f32", "rbk_group_search_f64",
     "rbk_group_search_large_f64", "rbk_group_search_unbounded_f64",
+    "rbk_index_flags", "rbk_index_set_tier", "rbk_group_set_tier",
 ]
 
 
@@ -122,6 +123,10 @@ def _load() -> C.CDLL:
               "rbk_group_search_unbounded_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_debug_scores_f32.argtypes = [vp, vp, i32, vp]
+    lib.rbk_index_flags.argtypes = [vp]
+    lib.rbk_index_flags.restype = C.c_uint32
+    lib.rbk_index_set_tier.argtypes = [vp, C.c_uint32]
+    lib.rbk_group_set_tier.argtypes = [vp, C.c_uint32]
     return lib
 
 
@@ -145,6 +150,20 @@ def _index_flags(keep_f64: bool, f64_on_host: bool, scan_f16: bool = False) -> i
     """f64_on_host or scan_f16 without keep_f64 is passed through: the library rejects it with its own message."""
     return ((RBK_INDEX_KEEP_F64 if keep_f64 else 0) | (RBK_INDEX_F64_ON_HOST if f64_on_host else 0)
             | (RBK_INDEX_SCAN_F16 if scan_f16 else 0))
+
+
+def _tier_flags(current: int, f64_on_host, scan_f16) -> int:
+    """The flag set of a tier change from the current one: None keeps a setting, RBK_INDEX_KEEP_F64 stays as it is
+    (an index without it is refused by the library with its own message)."""
+    flags = int(current)
+    for value, bit, name in ((f64_on_host, RBK_INDEX_F64_ON_HOST, "f64_on_host"),
+                             (scan_f16, RBK_INDEX_SCAN_F16, "scan_f16")):
+        if value is None:
+            continue
+        if not isinstance(value, (bool, np.bool_)):
+            raise TypeError(f"{name} must be a bool or None, not {type(value).__name__}")
+        flags = flags | bit if value else flags & ~bit
+    return flags
 
 
 def _search_large(fn, h, queries, k_fetch: int, min_score):
@@ -227,6 +246,17 @@ class Index:
 
     def set_slot_base(self, base: int) -> None:
         check(lib.rbk_index_set_slot_base(self._h, base))
+
+    @property
+    def flags(self) -> int:
+        """The creation flags as they are now (RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16)."""
+        return int(lib.rbk_index_flags(self._h))
+
+    def set_tier(self, *, f64_on_host: bool | None = None, scan_f16: bool | None = None) -> None:
+        """Change the storage tier in place (rbk_index_set_tier): move the float64 rows between the GPU and pinned host
+        memory, switch the scan between bf16 and fp16.  None keeps a setting.  Needs keep_f64; answers do not change.
+        Raises RbkError(RBK_ENOMEM) with the index unchanged when the new tier cannot be backed."""
+        check(lib.rbk_index_set_tier(self._h, _tier_flags(self.flags, f64_on_host, scan_f16)))
 
     # -- mutation
     def _append(self, fn, rows: np.ndarray) -> int:
@@ -454,6 +484,16 @@ class Group:
     def trim(self) -> None:
         """Index.trim() on every member; slots do not change."""
         check(lib.rbk_group_trim(self._h))
+
+    @property
+    def flags(self) -> int:
+        """The members' creation flags as they are now (they share them)."""
+        return int(lib.rbk_index_flags(C.c_void_p(lib.rbk_group_member(self._h, 0))))
+
+    def set_tier(self, *, f64_on_host: bool | None = None, scan_f16: bool | None = None) -> None:
+        """Index.set_tier() on every member together: every member's allocations come first, so RBK_ENOMEM leaves the
+        whole group as it was."""
+        check(lib.rbk_group_set_tier(self._h, _tier_flags(self.flags, f64_on_host, scan_f16)))
 
     def count(self) -> int:
         return lib.rbk_group_count(self._h)

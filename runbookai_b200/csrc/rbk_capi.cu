@@ -229,13 +229,25 @@ rbk_status vm_map_to(const rbk_index* ix, VmRange* r, size_t bytes) {
   return RBK_OK;
 }
 
-// Bytes of each device corpus buffer at capacity `cap` (ix->vm order); 0 for the f64 rows unless they live on the device.
-void storage_at(const rbk_index* ix, int64_t cap, size_t out[rbk_index::kVmBuffers]) {
+// Bytes of each device corpus buffer at capacity `cap` (ix->vm order); 0 for the f64 rows unless they live on the device
+// (f64_dev: they would, -1: the index's own tier).
+void storage_at(const rbk_index* ix, int64_t cap, size_t out[rbk_index::kVmBuffers], int f64_dev = -1) {
+  if (f64_dev < 0) f64_dev = ix->keep_f64 && !ix->f64_on_host;
   out[0] = static_cast<size_t>(cap) * ix->dpad * 2;
   out[1] = static_cast<size_t>(inv_norm_len(cap)) * 4;
   out[2] = static_cast<size_t>(cap) * 8;
   out[3] = static_cast<size_t>((cap + 31) / 32) * 4;
-  out[4] = ix->keep_f64 && !ix->f64_on_host ? static_cast<size_t>(cap) * ix->dim * 8 : 0;
+  out[4] = f64_dev ? static_cast<size_t>(cap) * ix->dim * 8 : 0;
+}
+
+// The most rows the device's memory could back with the f64 rows on the device (f64_dev) or not: the row ceiling of a
+// tier, min(2^31 - 512, total memory / device bytes per row) in whole tiles.
+int64_t tier_vm_rows(const rbk_index* ix, bool f64_dev) {
+  // device bytes per row, the tombstone bit rounded up to a byte
+  size_t per_row[rbk_index::kVmBuffers];
+  storage_at(ix, 1, per_row, f64_dev);
+  const int64_t row_bytes = static_cast<int64_t>(per_row[0] + 4 + per_row[2] + 1 + per_row[4]);
+  return std::min<int64_t>((1ll << 31) - 2 * kBlockN, static_cast<int64_t>(ix->total_mem) / row_bytes / kBlockN * kBlockN);
 }
 
 // Backs every device buffer for `ncap` rows: all of them, or (on failure) none of the chunks this call mapped.
@@ -269,12 +281,8 @@ rbk_status vm_reserve(rbk_index* ix, size_t total_global_mem) {
   const CUmemAllocationProp prop = vm_prop(ix->device);
   if ((res = api.MemGetAllocationGranularity(&ix->vm_gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM)) != CUDA_SUCCESS)
     return cu_fail(res, "cuMemGetAllocationGranularity");
-  // device bytes per row, the tombstone bit rounded up to a byte
-  size_t per_row[rbk_index::kVmBuffers];
-  storage_at(ix, 1, per_row);
-  const int64_t row_bytes = static_cast<int64_t>(per_row[0] + 4 + per_row[2] + 1 + per_row[4]);
-  ix->vm_rows = std::min<int64_t>((1ll << 31) - 2 * kBlockN,
-                                  static_cast<int64_t>(total_global_mem) / row_bytes / kBlockN * kBlockN);
+  ix->total_mem = total_global_mem;
+  ix->vm_rows = tier_vm_rows(ix, ix->keep_f64 && !ix->f64_on_host);
   size_t bytes[rbk_index::kVmBuffers];
   storage_at(ix, ix->vm_rows, bytes);
   for (int i = 0; i < rbk_index::kVmBuffers; ++i) {
@@ -298,6 +306,54 @@ void vm_free(rbk_index* ix) {
     if (r.reserved) vmm_api().MemAddressFree(r.base, r.reserved);
     r = VmRange();
   }
+}
+
+// Reserves an empty range of at least `bytes` (whole granules) into *r.
+rbk_status vm_reserve_range(const rbk_index* ix, size_t bytes, VmRange* r) {
+  *r = VmRange();
+  const size_t len = static_cast<size_t>(round_up(static_cast<int64_t>(bytes), static_cast<int64_t>(ix->vm_gran)));
+  const CUresult res = vmm_api().MemAddressReserve(&r->base, len, 0, 0, 0);
+  if (res != CUDA_SUCCESS) return cu_fail(res, "cuMemAddressReserve");
+  r->reserved = len;
+  return RBK_OK;
+}
+
+// Unmaps every chunk of r and frees its address range; the physical chunks are NOT released (another range maps them).
+void vm_drop_mapping(VmRange* r) {
+  const VmmApi& api = vmm_api();
+  size_t off = 0;
+  for (const VmRange::Chunk& c : r->chunks) {
+    api.MemUnmap(r->base + off, c.bytes);
+    off += c.bytes;
+  }
+  if (r->reserved) api.MemAddressFree(r->base, r->reserved);
+  *r = VmRange();
+}
+
+// A second mapping of src's physical chunks, in the same order, on a new range of `bytes` (>= src.mapped): the same
+// memory at another address, nothing copied.  On failure nothing is left reserved or mapped.
+rbk_status vm_alias(const rbk_index* ix, const VmRange& src, size_t bytes, VmRange* out) {
+  rbk_status st = vm_reserve_range(ix, bytes, out);
+  if (st != RBK_OK) return st;
+  const VmmApi& api = vmm_api();
+  CUmemAccessDesc access;
+  memset(&access, 0, sizeof access);
+  access.location = vm_prop(ix->device).location;
+  access.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  for (const VmRange::Chunk& c : src.chunks) {
+    const CUdeviceptr at = out->base + out->mapped;
+    CUresult res = api.MemMap(at, c.bytes, 0, c.handle, 0);
+    if (res == CUDA_SUCCESS) {
+      out->chunks.push_back(c);
+      out->mapped += c.bytes;
+      res = api.MemSetAccess(at, c.bytes, &access, 1);
+    }
+    if (res != CUDA_SUCCESS) {
+      vm_drop_mapping(out);
+      return cu_fail(res, "cuMemMap(index storage, new address range)");
+    }
+  }
+  return RBK_OK;
 }
 
 // RBK_INDEX_F64_ON_HOST: a pinned buffer for `ncap` rows holding the first n_rows rows of the current one, which it
@@ -1153,6 +1209,172 @@ void compact_commit(rbk_index* ix, int64_t n_new) {
   drop_graph(ix);
   ix->tmap_c_rows = -1;
 }
+
+uint32_t index_flags(const rbk_index* ix) {
+  return (ix->keep_f64 ? RBK_INDEX_KEEP_F64 : 0u) | (ix->f64_on_host ? RBK_INDEX_F64_ON_HOST : 0u) |
+         (ix->scan_f16 ? RBK_INDEX_SCAN_F16 : 0u);
+}
+
+rbk_status check_flags(uint32_t flags) {
+  if (flags & ~static_cast<uint32_t>(RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16))
+    return fail(RBK_EINVAL, "unknown flag");
+  if ((flags & RBK_INDEX_F64_ON_HOST) && !(flags & RBK_INDEX_KEEP_F64))
+    return fail(RBK_EINVAL, "RBK_INDEX_F64_ON_HOST requires RBK_INDEX_KEEP_F64");
+  if ((flags & RBK_INDEX_SCAN_F16) && !(flags & RBK_INDEX_KEEP_F64))
+    return fail(RBK_EINVAL, "RBK_INDEX_SCAN_F16 requires RBK_INDEX_KEEP_F64");
+  return RBK_OK;
+}
+
+rbk_status tier_check(const rbk_index* ix, uint32_t flags) {
+  rbk_status st = check_flags(flags);
+  if (st != RBK_OK) return st;
+  if (((flags & RBK_INDEX_KEEP_F64) != 0) != ix->keep_f64)
+    return fail(RBK_EINVAL, ix->keep_f64 ? "a tier change keeps the float64 rows: RBK_INDEX_KEEP_F64 cannot be dropped"
+                                         : "a tier change cannot add RBK_INDEX_KEEP_F64: this index holds no float64 rows");
+  return RBK_OK;
+}
+
+rbk_status tier_prepare(rbk_index* ix, uint32_t flags, TierPlan* p) {
+  *p = TierPlan();
+  p->flags = flags;
+  const bool host = (flags & RBK_INDEX_F64_ON_HOST) != 0;
+  p->to_host = host && !ix->f64_on_host;
+  p->to_device = !host && ix->f64_on_host;
+  p->rescan = ((flags & RBK_INDEX_SCAN_F16) != 0) != ix->scan_f16;
+  p->vm_rows = ix->vm_rows;
+  // searches enqueued earlier finish on the old tier; the corpus-side bound is read once they have
+  CK(cudaMemcpyAsync(&p->eps_bits, ix->d_counter + 1, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+  CK(cudaStreamSynchronize(ix->stream));
+  if (p->to_host) {
+    // the pinned rows, as realloc_host_rows allocates them
+    cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&p->host_rows), static_cast<size_t>(ix->cap) * ix->dim * 8,
+                                  cudaHostAllocMapped | cudaHostAllocPortable);
+    if (e != cudaSuccess) {
+      p->host_rows = nullptr;
+      return cuda_fail(e, "cudaHostAlloc(f64 rows on the host)");
+    }
+    void* dp = nullptr;
+    if ((e = cudaHostGetDevicePointer(&dp, p->host_rows, 0)) != cudaSuccess || dp != p->host_rows) {
+      tier_abort(ix, p);
+      if (e != cudaSuccess) return cuda_fail(e, "cudaHostGetDevicePointer(f64 rows on the host)");
+      return fail(RBK_ECUDA, "pinned host rows are mapped at another device address (no unified addressing)");
+    }
+    // The ceiling rises: buffers 0-3 get ranges sized for the host tier's vm_rows, and their chunks are mapped there
+    // too.  Nothing is copied, and no physical memory is added.
+    p->vm_rows = tier_vm_rows(ix, false);
+    size_t want[rbk_index::kVmBuffers];
+    storage_at(ix, p->vm_rows, want, 0);
+    for (int i = 0; i < 4; ++i) {
+      if (ix->vm[i].reserved >= static_cast<size_t>(round_up(static_cast<int64_t>(want[i]),
+                                                              static_cast<int64_t>(ix->vm_gran))))
+        continue;   // an index created on the host tier, or moved there before, has the larger range already
+      rbk_status st = vm_alias(ix, ix->vm[i], want[i], &p->vm[i]);
+      if (st != RBK_OK) {
+        tier_abort(ix, p);
+        return st;
+      }
+      p->alias[i] = true;
+    }
+  } else if (p->to_device) {
+    const int64_t dev_rows = tier_vm_rows(ix, true);
+    if (ix->cap > dev_rows)
+      return fail(RBK_ENOMEM, "a capacity of " + std::to_string(ix->cap) + " rows exceeds the " +
+                                  std::to_string(dev_rows) + " this device can hold with the float64 rows on it");
+    p->vm_rows = dev_rows;
+    size_t want[rbk_index::kVmBuffers];
+    storage_at(ix, dev_rows, want, 1);
+    rbk_status st = vm_reserve_range(ix, want[4], &p->vm[4]);
+    if (st != RBK_OK) return st;
+    storage_at(ix, ix->cap, want, 1);
+    if ((st = vm_map_to(ix, &p->vm[4], want[4])) != RBK_OK) {
+      tier_abort(ix, p);
+      return st;
+    }
+  }
+  return RBK_OK;
+}
+
+void tier_abort(rbk_index* ix, TierPlan* p) {
+  (void)ix;
+  if (p->host_rows) cudaFreeHost(p->host_rows);
+  p->host_rows = nullptr;
+  for (int i = 0; i < 4; ++i)
+    if (p->alias[i]) {
+      vm_drop_mapping(&p->vm[i]);   // the chunks stay the index's
+      p->alias[i] = false;
+    }
+  if (p->vm[4].reserved) {
+    vm_unmap_from(&p->vm[4], 0);
+    vmm_api().MemAddressFree(p->vm[4].base, p->vm[4].reserved);
+    p->vm[4] = VmRange();
+  }
+}
+
+namespace {
+// Re-derives the scan copy of rows [0, n_rows) - tombstoned ones too - from the float64 rows with the ingest kernels,
+// and eps_c_max as the largest angle over them.  1/||c|| stays NaN for tombstoned rows.  A bound that proves nothing (an
+// off-band or non-finite row has been stored) stays so until rbk_index_clear, whatever rows the index holds now.
+rbk_status tier_rescan(rbk_index* ix, bool f16, int eps_bits) {
+  float eps;
+  memcpy(&eps, &eps_bits, sizeof eps);
+  const int eps0 = eps >= kEpsNone ? eps_bits : 0;
+  CK(cudaMemcpyAsync(ix->d_counter + 1, &eps0, sizeof(int), cudaMemcpyHostToDevice, ix->stream));   // pageable: staged
+  CK(launch_convert_rows(ix->rows_f64, 0, ix->n_rows, ix->dim, ix->dpad, ix->rows, nullptr, ix->stream, nullptr, nullptr,
+                         nullptr, f16));
+  CK(launch_row_norms(ix->rows, ix->rows_f64, 0, ix->n_rows, ix->dim, ix->dpad, ix->inv_norm, ix->norm2,
+                      ix->d_counter + 1, ix->stream, nullptr, ix->dead_bits, f16));
+  ix->scan_f16 = f16;
+  return RBK_OK;
+}
+}  // namespace
+
+rbk_status tier_commit(rbk_index* ix, TierPlan* p) {
+  const bool f16 = (p->flags & RBK_INDEX_SCAN_F16) != 0;
+  const size_t f64_bytes = static_cast<size_t>(ix->n_rows) * ix->dim * 8;
+  rbk_status st = RBK_OK;
+  if (p->rescan && !ix->f64_on_host) {   // while the f64 rows are on the device: no PCIe reads
+    if ((st = tier_rescan(ix, f16, p->eps_bits)) != RBK_OK) return st;
+    p->rescan = false;
+  }
+  if (p->to_host) {
+    if (f64_bytes) CK(cudaMemcpyAsync(p->host_rows, ix->rows_f64, f64_bytes, cudaMemcpyDeviceToHost, ix->stream));
+    CK(cudaStreamSynchronize(ix->stream));
+    for (int i = 0; i < 4; ++i) {
+      if (!p->alias[i]) continue;
+      vm_drop_mapping(&ix->vm[i]);   // the old addresses; the chunks now belong to the new range
+      ix->vm[i] = std::move(p->vm[i]);
+      p->vm[i] = VmRange();
+      p->alias[i] = false;
+    }
+    vm_unmap_from(&ix->vm[4], 0);
+    if (ix->vm[4].reserved) vmm_api().MemAddressFree(ix->vm[4].base, ix->vm[4].reserved);
+    ix->vm[4] = VmRange();
+    ix->rows = reinterpret_cast<uint16_t*>(ix->vm[0].base);
+    ix->inv_norm = reinterpret_cast<float*>(ix->vm[1].base);
+    ix->norm2 = reinterpret_cast<double*>(ix->vm[2].base);
+    ix->dead_bits = reinterpret_cast<unsigned int*>(ix->vm[3].base);
+    ix->rows_f64 = p->host_rows;
+    p->host_rows = nullptr;
+    ix->f64_on_host = true;
+  } else if (p->to_device) {
+    double* dev = reinterpret_cast<double*>(p->vm[4].base);
+    if (f64_bytes) CK(cudaMemcpyAsync(dev, ix->rows_f64, f64_bytes, cudaMemcpyHostToDevice, ix->stream));
+    CK(cudaStreamSynchronize(ix->stream));
+    cudaFreeHost(ix->rows_f64);
+    ix->vm[4] = std::move(p->vm[4]);
+    p->vm[4] = VmRange();
+    ix->rows_f64 = dev;
+    ix->f64_on_host = false;
+  }
+  ix->vm_rows = p->vm_rows;
+  if (p->rescan && (st = tier_rescan(ix, f16, p->eps_bits)) != RBK_OK) return st;
+  CK(cudaStreamSynchronize(ix->stream));
+  // every cache keyed on the old tier or the old pointers: the captured graph (its scan instantiation and pointers)
+  // and the corpus tensor map (its data type and base); the other scratch buffers hold no corpus pointer
+  drop_graph(ix);
+  ix->tmap_c_rows = -1;
+  return RBK_OK;
+}
 }  // namespace impl
 }  // namespace rbk
 
@@ -1169,12 +1391,8 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out) {
   if (!out) return fail(RBK_EINVAL, "out is null");
   *out = nullptr;
-  if (flags & ~static_cast<uint32_t>(RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16))
-    return fail(RBK_EINVAL, "unknown flag");
-  if ((flags & RBK_INDEX_F64_ON_HOST) && !(flags & RBK_INDEX_KEEP_F64))
-    return fail(RBK_EINVAL, "RBK_INDEX_F64_ON_HOST requires RBK_INDEX_KEEP_F64");
-  if ((flags & RBK_INDEX_SCAN_F16) && !(flags & RBK_INDEX_KEEP_F64))
-    return fail(RBK_EINVAL, "RBK_INDEX_SCAN_F16 requires RBK_INDEX_KEEP_F64");
+  rbk_status fst = check_flags(flags);
+  if (fst != RBK_OK) return fst;
   if (dim < 1 || dim > RBK_MAX_DIM) return fail(RBK_EINVAL, "dim out of range");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -1446,6 +1664,22 @@ rbk_status rbk_index_trim(rbk_index* ix) {
   release_scratch(ix);
   ix->tmap_c_rows = -1;
   return RBK_OK;
+}
+
+uint32_t rbk_index_flags(const rbk_index* ix) { return ix ? index_flags(ix) : 0u; }
+
+rbk_status rbk_index_set_tier(rbk_index* ix, uint32_t flags) {
+  if (!ix) return fail(RBK_EINVAL, "null index");
+  std::lock_guard<std::mutex> lk(ix->mu);
+  if (ix->slot.block != 0)
+    return fail(RBK_EINVAL, "a tier change is not available for a member of a device group (use rbk_group_set_tier)");
+  rbk_status st = tier_check(ix, flags);
+  if (st != RBK_OK || flags == index_flags(ix)) return st;
+  DeviceGuard dg(ix->device);
+  TierPlan plan;
+  if ((st = tier_prepare(ix, flags, &plan)) != RBK_OK) return st;
+  if ((st = tier_commit(ix, &plan)) != RBK_OK) tier_abort(ix, &plan);   // a CUDA error: release what was not taken over
+  return st;
 }
 
 int64_t rbk_index_count(const rbk_index* ix) { return ix ? ix->n_live : 0; }

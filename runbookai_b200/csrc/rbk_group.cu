@@ -687,6 +687,45 @@ rbk_status rbk_group_compact(rbk_group* g, int64_t* old_to_new, int64_t old_to_n
   return group_compact(g, old_to_new, old_to_new_len);
 }
 
+// rbk_index_set_tier on every member: every member's allocations (tier_prepare) before any member changes, as
+// rbk_group_compact allocates before the first row moves.
+rbk_status rbk_group_set_tier(rbk_group* g, uint32_t flags) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  std::lock_guard<std::mutex> lk(g->mu);
+  std::vector<std::unique_lock<std::mutex>> member_locks;
+  member_locks.reserve(g->G);
+  for (rbk_index* ix : g->parts) member_locks.emplace_back(ix->mu);
+  for (rbk_index* ix : g->parts) {
+    rbk_status st = tier_check(ix, flags);
+    if (st != RBK_OK) return st;
+  }
+  if (flags == index_flags(g->parts[0])) return RBK_OK;   // the members share their flags
+  std::vector<TierPlan> plans(g->G);
+  for (int d = 0; d < g->G; ++d) {
+    DeviceGuard dg(g->devices[d]);
+    rbk_status st = tier_prepare(g->parts[d], flags, &plans[d]);
+    if (st != RBK_OK) {
+      for (int e = 0; e < d; ++e) {
+        DeviceGuard dge(g->devices[e]);
+        tier_abort(g->parts[e], &plans[e]);
+      }
+      return st;
+    }
+  }
+  for (int d = 0; d < g->G; ++d) {
+    DeviceGuard dg(g->devices[d]);
+    rbk_status st = tier_commit(g->parts[d], &plans[d]);
+    if (st != RBK_OK) {   // a CUDA error: release what no member has taken over
+      for (int e = d; e < g->G; ++e) {
+        DeviceGuard dge(g->devices[e]);
+        tier_abort(g->parts[e], &plans[e]);
+      }
+      return st;
+    }
+  }
+  return RBK_OK;
+}
+
 int64_t rbk_group_count(const rbk_group* g) {
   int64_t n = 0;
   if (g)

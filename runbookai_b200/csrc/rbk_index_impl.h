@@ -63,8 +63,9 @@ struct PinBuf {
 };
 
 // One device corpus buffer on a reserved virtual address range (CUDA virtual memory management).  Physical chunks
-// are mapped from `base` on as the index grows and unmapped from the end by rbk_index_trim, so `base` never moves and
-// a growth copies nothing.
+// are mapped from `base` on as the index grows and unmapped from the end by rbk_index_trim, so `base` does not move and
+// a growth copies nothing.  The one exception is rbk_index_set_tier moving the f64 rows to the host: it maps the same
+// chunks at a larger range (raising the row ceiling) and the base pointers move there.
 struct VmRange {
   struct Chunk {
     CUmemGenericAllocationHandle handle;
@@ -149,6 +150,7 @@ struct rbk_index {
   rbk::impl::VmRange vm[kVmBuffers];
   int64_t vm_rows = 0;
   size_t vm_gran = 0;        // allocation granularity of the device
+  size_t total_mem = 0;      // the device's memory, which sets vm_rows for each storage tier
   uint16_t* rows = nullptr;
   float* inv_norm = nullptr;  // padded to a multiple of kBlockN (+ one tile), NaN-filled
   double* norm2 = nullptr;
@@ -199,7 +201,7 @@ struct rbk_index {
   CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
-  int64_t tmap_c_rows = -1;   // rows the corpus map covers (-1: none); its base, `rows`, never moves
+  int64_t tmap_c_rows = -1;   // rows the corpus map covers (-1: none); its base, `rows`, moves only in rbk_index_set_tier
   cudaEvent_t ev_start = nullptr, ev_stop = nullptr;   // device time of a whole synchronous search
   // scan-kernel timing without a host sync per search: (start, stop) event pairs are resolved lazily
   // (rbk_index_stats, or when the ring wraps) into stats.scan_ms_total / stats.scans_timed
@@ -293,6 +295,31 @@ rbk_status compact_gather(rbk_index* ix, const CompactStage& st, int64_t s0, int
 rbk_status compact_tail(rbk_index* ix, int64_t n_new);
 // After the stream has been synchronised: the index holds n_new live rows; drops the caches keyed on the corpus.
 void compact_commit(rbk_index* ix, int64_t n_new);
+
+// The steps of a storage tier change, shared by rbk_index_set_tier and rbk_group_set_tier (caller holds ix->mu and has
+// the index's device current).  tier_prepare makes every allocation the change needs and changes nothing the index
+// shows: the pinned rows and the larger address ranges, their physical chunks mapped there a second time (device to
+// host), or the device f64 range, mapped for cap rows (host to device).  Then exactly one of tier_abort, which releases
+// what tier_prepare made, or tier_commit, which moves the rows, re-derives the scan copy when its type changes, and drops
+// every cache keyed on the old tier or the old pointers.  A tier_commit that fails (a CUDA error only) leaves what it
+// has not yet taken over in the plan, for tier_abort; the index itself may then be part-way changed.
+struct TierPlan {
+  uint32_t flags = 0;
+  bool to_host = false, to_device = false, rescan = false;
+  int64_t vm_rows = 0;                  // the ceiling of the new tier
+  double* host_rows = nullptr;          // to_host: the pinned [cap][dim] buffer
+  bool alias[rbk_index::kVmBuffers] = {};
+  VmRange vm[rbk_index::kVmBuffers];    // to_host: buffers 0-3 re-reserved (where alias[i]); to_device: buffer 4
+  int eps_bits = 0;                     // eps_c_max before the change (float bits)
+};
+uint32_t index_flags(const rbk_index* ix);
+// RBK_EINVAL for a flag set rbk_index_create_ex refuses (check_flags, which it shares), or one the index cannot move to
+// (the KEEP_F64 bit must stay; group membership is the caller's).
+rbk_status check_flags(uint32_t flags);
+rbk_status tier_check(const rbk_index* ix, uint32_t flags);
+rbk_status tier_prepare(rbk_index* ix, uint32_t flags, TierPlan* p);
+void tier_abort(rbk_index* ix, TierPlan* p);
+rbk_status tier_commit(rbk_index* ix, TierPlan* p);
 const char* last_error();
 
 }  // namespace impl

@@ -121,7 +121,8 @@ __device__ __forceinline__ double src_to_f64(SrcT v) {   // exact widening of ev
 
 // RBK_INDEX_SCAN_F16 rows (rbk_f16.cuh): the scale needs the row's largest finite magnitude before any element is
 // converted, so one WARP owns a row - pass 1 reduces max |x| over the row (coalesced reads), pass 2 re-reads it (from
-// L1 / L2) and writes the scaled fp16 row in 16-byte stores, plus the f64 sidecar, which such an index always keeps.
+// L1 / L2) and writes the scaled fp16 row in 16-byte stores, plus the f64 sidecar, which such an index always keeps
+// (dst_f64 null: the source IS the sidecar, when a tier change re-derives the scan copy from it).
 // Same slot_map / dead_bits / n_dead contract as convert_rows_kernel.
 constexpr int kF16ConvThreads = 256;
 template <typename SrcT>
@@ -157,7 +158,7 @@ __global__ void __launch_bounds__(kF16ConvThreads) convert_rows_f16_kernel(
         o[j] = 0;
         if (c0 + j < d) {
           const double x = src_to_f64(s[c0 + j]);
-          dst_f64[row * d + c0 + j] = x;
+          if (dst_f64 != nullptr) dst_f64[row * d + c0 + j] = x;
           o[j] = f16_bits_flush(scale_pow2(x, e));
         }
       }
@@ -209,7 +210,7 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
     long long row = -1;
     if (item < n_items) {
       row = slot_map ? slot_map[item] : first_row + item;
-      if (slot_map && ((dead_bits[row >> 5] >> (row & 31)) & 1u)) row = -1;   // tombstoned slots stay dead
+      if (dead_bits && ((dead_bits[row >> 5] >> (row & 31)) & 1u)) row = -1;   // tombstoned slots stay dead
     }
     s_row[tid] = row;
   }
@@ -472,6 +473,8 @@ cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_b
                              cudaStream_t stream, const int64_t* slot_map, const unsigned int* dead_bits, bool f16) {
   if (n_items <= 0) return cudaSuccess;
   if (f16 && rows_f64_base == nullptr) return cudaErrorInvalidValue;   // the fp16 tier always keeps the f64 rows
+  // dead_bits without slot_map (a tier change): the f64 kernel folds every row's angle in, tombstoned or not
+  if (!slot_map && dead_bits && rows_f64_base == nullptr) return cudaErrorInvalidValue;
   const unsigned blocks = static_cast<unsigned>((n_items + kNormRows - 1) / kNormRows);
   if (f16)
     row_norms_kernel<true><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits, first_row,

@@ -69,7 +69,8 @@ cudaError_t launch_scan_large_f16(const CUtensorMap& tmap_q, const CUtensorMap& 
 // dst_f64 (nullable): exact-source sidecar rows, pitch d.
 // slot_map (nullable, bulk overwrite): dst_rows / dst_f64 are the index's row 0 and source row r lands in row
 // slot_map[r]; rows whose slot is tombstoned (dead_bits) are skipped and counted in *n_dead.
-// f16: store the rows by the RBK_INDEX_SCAN_F16 rule (rbk_f16.cuh) instead of as bf16; dst_f64 is then required.
+// f16: store the rows by the RBK_INDEX_SCAN_F16 rule (rbk_f16.cuh) instead of as bf16.  dst_f64 null with f16 only
+// when src is the index's own f64 rows (a tier change re-deriving the scan copy).
 cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, int d, int dpad,
                                 uint16_t* dst_rows, double* dst_f64, cudaStream_t stream,
                                 const int64_t* slot_map = nullptr, const unsigned int* dead_bits = nullptr,
@@ -78,6 +79,8 @@ cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, i
 // ones skipped).  All array arguments are the index's BASE pointers.  rows_f64_base (nullable): when given,
 // norm2 comes from it and the bf16-vs-f64 angle bound is max-ed into *eps_c_max (float bits in an int).
 // f16: the rows are RBK_INDEX_SCAN_F16 fp16 rows (rows_f64_base required); the angle is that of their rounding.
+// dead_bits without slot_map (rows_f64_base required; a tier change re-deriving every stored row): every row's norm2
+// and angle are computed, but a tombstoned row's inv_norm stays NaN.
 cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_base, int64_t first_row,
                              int64_t n_items, int d, int dpad, float* inv_norm_base, double* norm2_base,
                              int* eps_c_max, cudaStream_t stream, const int64_t* slot_map = nullptr,

@@ -42,7 +42,7 @@ from typing import Sequence
 import numpy as np
 
 from . import embedder as _emb
-from ._native import RBK_EDIM, RBK_MAX_K_FETCH, DimensionError, Index
+from ._native import RBK_EDIM, RBK_INDEX_F64_ON_HOST, RBK_INDEX_SCAN_F16, RBK_MAX_K_FETCH, DimensionError, Index
 
 SCHEMA = """
       CREATE TABLE IF NOT EXISTS vector_embeddings (
@@ -132,18 +132,20 @@ class VectorStore:
         # keep_f64: the reference stores float64 embeddings; keep them so the re-rank is exact for any input.
         # f64_on_host (None: RUNBOOK_KNN_F64_ON_HOST=1 enables): those float64 rows live in pinned host memory instead
         # of on the GPU - the same answers, about 5x the rows per GPU at d = 1536, host RAM and PCIe reads in the
-        # re-rank instead.  A shared index keeps the placement of the instance that created it.
+        # re-rank instead.  A shared index keeps the placement of the instance that created it, until set_tier().
         # scan_f16 (None: RUNBOOK_KNN_SCAN_F16=1 enables): the scan reads per-row scaled fp16 rows instead of bf16 - the
         # same answers and bytes, a tighter error bound, so fewer batches need the wide retry.  A shared index keeps the
-        # setting of the instance that created it.
+        # setting of the instance that created it, until set_tier().
         if f64_on_host is None:
             f64_on_host = os.environ.get("RUNBOOK_KNN_F64_ON_HOST", "0") == "1"
         if scan_f16 is None:
             scan_f16 = os.environ.get("RUNBOOK_KNN_SCAN_F16", "0") == "1"
-        self.f64_on_host = on_host = bool(f64_on_host)
-        self.scan_f16 = f16 = bool(scan_f16)
+        # what this instance asks for; the index, once there is one, reports its own tier (f64_on_host / scan_f16)
+        self._want_f64_on_host = bool(f64_on_host)
+        self._want_scan_f16 = bool(scan_f16)
         self._index_factory = index_factory or (
-            lambda dim, dev: Index(dim, device=dev, keep_f64=True, f64_on_host=on_host, scan_f16=f16))
+            lambda dim, dev: Index(dim, device=dev, keep_f64=True, f64_on_host=self._want_f64_on_host,
+                                   scan_f16=self._want_scan_f16))
         # one connection, usable from the micro-batcher's worker thread too; serialised by a lock
         self.db = sqlite3.connect(db_path, check_same_thread=False)
         self.db.row_factory = sqlite3.Row
@@ -204,6 +206,49 @@ class VectorStore:
     @property
     def _ids(self):
         return self._st.ids
+
+    def _index_flags(self) -> int | None:
+        """The index's flags, or None before there is an index (or for an index that does not report them)."""
+        st = getattr(self, "_st", None)
+        ix = st.index if st is not None else None
+        flags = getattr(ix, "flags", None) if ix is not None else None
+        return None if flags is None else int(flags)
+
+    @property
+    def f64_on_host(self) -> bool:
+        """Whether the float64 rows live in pinned host memory: the index's tier once there is one (a shared index's may
+        have been chosen or changed by another instance), else what this instance asked for."""
+        flags = self._index_flags()
+        return self._want_f64_on_host if flags is None else bool(flags & RBK_INDEX_F64_ON_HOST)
+
+    @property
+    def scan_f16(self) -> bool:
+        """Whether the scan reads fp16 rows: the index's tier once there is one, else what this instance asked for."""
+        flags = self._index_flags()
+        return self._want_scan_f16 if flags is None else bool(flags & RBK_INDEX_SCAN_F16)
+
+    def set_tier(self, f64_on_host: bool | None = None, scan_f16: bool | None = None) -> None:
+        """Change the storage tier of the index in place, from the float64 rows it already holds (no reload from
+        SQLite): f64_on_host moves them between the GPU and pinned host memory, scan_f16 switches the scan between bf16
+        and fp16.  None keeps a setting.  Answers do not change.  Holds the state lock, so a shared index changes for
+        every instance attached to it.  Before the first row there is no index yet: the request applies to the index
+        this instance creates.  Nothing is automatic: an append that fails with RBK_ENOMEM still raises, and the caller
+        decides whether to move the rows to host memory and retry; an RBK_ENOMEM here leaves the index as it was."""
+        for name, value in (("f64_on_host", f64_on_host), ("scan_f16", scan_f16)):
+            if value is not None and not isinstance(value, (bool, np.bool_)):
+                raise TypeError(f"{name} must be a bool or None, not {type(value).__name__}")
+        with self._st.lock:
+            ix = self._index
+            if ix is not None:
+                fn = getattr(ix, "set_tier", None)
+                if fn is None:
+                    raise NotImplementedError(f"{type(ix).__name__} has no storage tiers to change")
+                fn(f64_on_host=None if f64_on_host is None else bool(f64_on_host),
+                   scan_f16=None if scan_f16 is None else bool(scan_f16))
+            if f64_on_host is not None:
+                self._want_f64_on_host = bool(f64_on_host)
+            if scan_f16 is not None:
+                self._want_scan_f16 = bool(scan_f16)
 
     @property
     def _slot_of(self):

@@ -244,6 +244,23 @@ export class GpuEmbeddingIndex {
     this.index?.trim();
   }
 
+  /**
+   * Change the storage tier of the loaded index in place (rbk_index_set_tier / rbk_group_set_tier): `f64OnHost` moves
+   * the float64 rows between the GPU and pinned host memory, `scanF16` switches the scan between bf16 and fp16.  An
+   * omitted key keeps its setting.  Answers and slots do not change, so nothing is remapped; the native call waits
+   * for the index's queued device work itself.  Nothing is automatic: an append that throws for lack of device memory
+   * is the caller's to retry after `setTier({ f64OnHost: true })`.  Throws (with the index unchanged) if the new tier
+   * cannot be backed, and against a library built before tier changes.
+   */
+  setTier(tier: { f64OnHost?: boolean; scanF16?: boolean }): void {
+    this.index?.setTier(tier);
+  }
+
+  /** Where the float64 rows live and which scan runs, as they are now; null before the first row is loaded. */
+  get tier(): { f64OnHost: boolean; scanF16: boolean } | null {
+    return this.index ? this.index.tier : null;
+  }
+
   private remember(id: string, slot: number): void {
     this.slotOfId.set(id, slot);
     this.idOfSlot[slot] = id;
