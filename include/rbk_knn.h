@@ -316,8 +316,11 @@ rbk_status rbk_merge_topk_packed_device(int32_t device, void* cuda_stream, int32
  * rbk_group_search_*.  Slots are GLOBAL insertion indices, exactly as for a single index; results are identical
  * to a single index holding the same rows (ids and fp64 scores bit for bit, ties by ascending slot).
  * NCCL is looked up at run time (dlopen "libnccl.so.2"); a group of more than one GPU fails with RBK_ENCCL if it
- * is missing, a one-GPU group never touches it.  Mutation and search semantics, limits (k_fetch <= RBK_MAX_K_FETCH)
- * and error conventions are those of the rbk_index_* call of the same name. */
+ * is missing, a one-GPU group never touches it.  device_ids may name a device more than once (e.g. {0, 0, 0}: three
+ * members on GPU 0, each with its own stream): such a group creates no NCCL communicator and gathers the members'
+ * blocks to device_ids[0] with device copies instead; its answers are those of any other group.  Mutation and search
+ * semantics, limits (k_fetch <= RBK_MAX_K_FETCH) and error conventions are those of the rbk_index_* call of the same
+ * name. */
 typedef struct rbk_group rbk_group;
 rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_devices, int64_t capacity_hint,
                             uint32_t flags /* RBK_INDEX_KEEP_F64 [| RBK_INDEX_F64_ON_HOST] [| RBK_INDEX_SCAN_F16]:

@@ -34,6 +34,16 @@ const char* last_error() { return g_err_storage.c_str(); }
 }  // namespace rbk
 using namespace rbk::impl;
 
+// fill_empty_results' slots and scores (outside the anonymous namespaces: nvcc's host stub for a kernel inside one
+// cannot tell this file's several apart)
+static __global__ void empty_results_kernel(long long* slots, double* scores, int64_t n) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    slots[i] = -1;
+    scores[i] = __longlong_as_double(0x7FF8000000000000ll);
+  }
+}
+
 namespace {
 
 
@@ -564,11 +574,16 @@ rbk_status launch_sub_batch(rbk_index* ix, int q0, const P& sp) {
   return RBK_OK;
 }
 
-// Results of a search over an empty index: -1 slots, NaN scores, zero counts.
+// Results of a search over an empty index: -1 slots, zero counts, and NaN scores with the bits every other path
+// writes (the quiet NaN 0x7FF8000000000000), so an empty index answers byte for byte as an empty group does.
 rbk_status fill_empty_results(rbk_index* ix, int B, int k_fetch, long long* d_slots, double* d_scores, int* d_counts) {
   CK(cudaMemsetAsync(d_counts, 0, sizeof(int) * B, ix->stream));
-  CK(cudaMemsetAsync(d_slots, 0xFF, sizeof(long long) * B * k_fetch, ix->stream));   // -1
-  CK(cudaMemsetAsync(d_scores, 0xFF, sizeof(double) * B * k_fetch, ix->stream));     // NaN
+  const int64_t n = static_cast<int64_t>(B) * k_fetch;
+  if (n > 0) {
+    empty_results_kernel<<<static_cast<unsigned>(std::min<int64_t>((n + 255) / 256, 1024)), 256, 0, ix->stream>>>(
+        d_slots, d_scores, n);
+    CK(cudaGetLastError());
+  }
   return RBK_OK;
 }
 

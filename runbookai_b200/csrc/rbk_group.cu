@@ -9,7 +9,9 @@
 //     ->  ONE ncclAllGather of the packed per-GPU blocks (results + exactness flags) over NVLink
 //     ->  merge kernel on GPU 0  ->  one D2H, one host synchronisation.
 // NCCL is resolved with dlopen("libnccl.so.2") on first use, so the library itself has no link-time dependency on
-// it and a one-GPU group never needs it.  Exact per-shard fp64 scores make the merge exact; local row order is
+// it and a one-GPU group never needs it.  A device list that names a device more than once (co-located members, e.g.
+// a G-member group on one GPU) has no communicator: member 0's stream waits for each member's block and copies it.
+// Exact per-shard fp64 scores make the merge exact; local row order is
 // global slot order within a device, so the (score desc, slot asc) tie-break survives (SlotLayout, rbk_internal.h).
 #include <dlfcn.h>
 #include <nccl.h>   // types and enums only: every NCCL symbol is looked up at run time
@@ -81,10 +83,11 @@ struct rbk_group {
   int64_t n_slots = 0;           // global slots handed out (tombstones included)
   std::vector<int> devices;
   std::vector<rbk_index*> parts;
-  std::vector<ncclComm_t> comms; // empty for G == 1
+  std::vector<ncclComm_t> comms; // empty for G == 1 and for a device list with a repeat (co-located members)
   std::mutex mu;
   struct Dev {
     DevBuf<unsigned char> q, local, all;
+    cudaEvent_t enqueued = nullptr;   // co-located members: the member's block is written (recorded on its stream)
   };
   std::vector<Dev> dev;
   DevBuf<unsigned char> out;     // device 0: the merged block (dirty_word)
@@ -147,6 +150,10 @@ void split_slots(const rbk_group* g, const int64_t* slots, int64_t n, std::vecto
 int64_t dirty_word(const ResultBlock& L) { return L.off_flags + 4 * L.B; }
 int64_t merged_bytes(const ResultBlock& L) { return dirty_word(L) + 4; }
 
+// Member d's buffer for the gathered blocks: every member's with NCCL, only member 0's when members are co-located
+// (exchange_and_merge copies the blocks there).
+bool needs_all(const rbk_group* g, int d) { return g->G > 1 && (d == 0 || !g->comms.empty()); }
+
 // Stages a batch on every device and enqueues its work there: the buffers for the queries and the packed blocks, the
 // start event, the H2D of the queries to each device from one pinned copy (so that the G copies run concurrently, one
 // per PCIe link), the member's query scratch, then enqueue(d, ix) with the member's lock held and its device current.
@@ -171,7 +178,7 @@ rbk_status stage_and_enqueue(rbk_group* g, const void* queries, int elem, const 
     DeviceGuard dg(ix->device);
     CK(g->dev[d].q.ensure(q_bytes));
     CK(g->dev[d].local.ensure(L.bytes));
-    if (g->G > 1) CK(g->dev[d].all.ensure(L.bytes * g->G));
+    if (needs_all(g, d)) CK(g->dev[d].all.ensure(L.bytes * g->G));
     if (d == 0) CK(cudaEventRecord(g->ev0, ix->stream));
     CK(cudaMemcpyAsync(g->dev[d].q.p, g->h_q.p, q_bytes, cudaMemcpyHostToDevice, ix->stream));
     rbk_status st = ensure_query_scratch(ix, B, elem);
@@ -182,9 +189,25 @@ rbk_status stage_and_enqueue(rbk_group* g, const void* queries, int elem, const 
   return RBK_OK;
 }
 
-// all-gather of the packed blocks (G > 1) + merge on device 0 into g->out; enqueue only
+// all-gather of the packed blocks (G > 1) + merge on device 0 into g->out; enqueue only.  Co-located members (a device
+// list with a repeat, no communicator): member 0's stream waits for every member's block and copies it into its own
+// `all` buffer.
 rbk_status exchange_and_merge(rbk_group* g, const ResultBlock& L, int k_fetch) {
-  if (g->G > 1) {
+  if (g->G > 1 && g->comms.empty()) {
+    for (int d = 1; d < g->G; ++d) {
+      DeviceGuard dg(g->devices[d]);
+      CK(cudaEventRecord(g->dev[d].enqueued, g->parts[d]->stream));
+    }
+    DeviceGuard dg(g->devices[0]);
+    cudaStream_t s0 = g->parts[0]->stream;
+    for (int d = 0; d < g->G; ++d) {
+      if (d > 0) CK(cudaStreamWaitEvent(s0, g->dev[d].enqueued, 0));
+      // Member d writes its block again (the next call, query group or re-answer) only after collect() has
+      // synchronised s0, which orders that write after this copy: a change that drops that synchronisation must make
+      // member d's stream wait for the copy instead.
+      CK(cudaMemcpyAsync(g->dev[0].all.p + d * L.bytes, g->dev[d].local.p, L.bytes, cudaMemcpyDefault, s0));
+    }
+  } else if (g->G > 1) {
     NcclApi& n = nccl_api();
     NC(n.GroupStart());
     for (int d = 0; d < g->G; ++d) {
@@ -314,7 +337,7 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
     std::lock_guard<std::mutex> il(ix->mu);
     DeviceGuard dg(ix->device);
     CK(g->dev[d].local.ensure(Lmax.bytes));
-    if (g->G > 1) CK(g->dev[d].all.ensure(Lmax.bytes * g->G));
+    if (needs_all(g, d)) CK(g->dev[d].all.ensure(Lmax.bytes * g->G));
     st = large_prepare(ix, B, sorted, groups);
     if (st != RBK_OK) return st;
   }
@@ -447,7 +470,9 @@ rbk_status group_compact(rbk_group* g, int64_t* old_to_new, int64_t old_to_new_l
   for (int d = 0; d < G; ++d)
     for (int e = 0; e < G; ++e) {
       int can = 0;
-      if (d == e || cudaDeviceCanAccessPeer(&can, g->devices[d], g->devices[e]) != cudaSuccess || !can) continue;
+      if (g->devices[d] == g->devices[e] ||   // co-located members: no peer to enable
+          cudaDeviceCanAccessPeer(&can, g->devices[d], g->devices[e]) != cudaSuccess || !can)
+        continue;
       DeviceGuard dg(g->devices[d]);
       if (cudaDeviceEnablePeerAccess(g->devices[e], 0) != cudaSuccess) cudaGetLastError();   // already enabled
     }
@@ -525,9 +550,9 @@ rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_de
   if (!out) return fail(RBK_EINVAL, "out is null");
   *out = nullptr;
   if (!device_ids || n_devices < 1 || n_devices > 64) return fail(RBK_EINVAL, "bad device list");
+  bool repeat = false;   // NCCL refuses two ranks on one device: such a group exchanges its blocks by copies
   for (int a = 0; a < n_devices; ++a)
-    for (int b = a + 1; b < n_devices; ++b)
-      if (device_ids[a] == device_ids[b]) return fail(RBK_EINVAL, "a device may appear only once in a group");
+    for (int b = a + 1; b < n_devices; ++b) repeat = repeat || device_ids[a] == device_ids[b];
   std::unique_ptr<rbk_group> g(new (std::nothrow) rbk_group());
   if (!g) return fail(RBK_ENOMEM, "out of host memory");
   g->dim = dim;
@@ -550,7 +575,7 @@ rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_de
     ix->slot.g = d;
     g->parts.push_back(ix);
   }
-  if (n_devices > 1) {
+  if (n_devices > 1 && !repeat) {
     NcclApi& n = nccl_api();
     if (!n.ok) {
       destroy_parts();
@@ -571,6 +596,13 @@ rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_de
       return fail(RBK_ECUDA, "cudaEventCreate");
     }
   }
+  for (int d = 1; repeat && d < n_devices; ++d) {
+    DeviceGuard dg(g->devices[d]);
+    if (cudaEventCreateWithFlags(&g->dev[d].enqueued, cudaEventDisableTiming) != cudaSuccess) {
+      rbk_group_destroy(g.release());
+      return fail(RBK_ECUDA, "cudaEventCreate");
+    }
+  }
   *out = g.release();
   return RBK_OK;
 }
@@ -583,6 +615,7 @@ void rbk_group_destroy(rbk_group* g) {
     g->dev[d].q.release();
     g->dev[d].local.release();
     g->dev[d].all.release();
+    if (g->dev[d].enqueued) cudaEventDestroy(g->dev[d].enqueued);
   }
   if (!g->comms.empty()) {
     NcclApi& n = nccl_api();

@@ -19,6 +19,13 @@ def load_golden():
     return g
 
 
+def group_devices(n):
+    """A device list for an n-member group: one GPU each when the machine has n (the NCCL exchange), else n members
+    co-located on GPU 0 (the copy exchange), so every G > 1 path runs on a one-GPU machine too."""
+    import torch
+    return list(range(n)) if torch.cuda.device_count() >= n else [0] * n
+
+
 class OracleIndex:
     """CPU stand-in with the _native.Index surface, backed by the oracle.  Lets the CPU
     suite exercise the host logic (VectorStore, sharded merge) without a GPU.  Rows are

@@ -369,14 +369,12 @@ def test_fallback_block_split(rb, oracle_mod, tier, n_rand, above):
 
 def test_one_gpu_group_re_answers_through_the_fallback(rb, oracle_mod):
     """A Group whose member cannot prove a query re-answers the batch; at d = 1536 with KEEP_F64 that re-answer goes
-    through the exhaustive kernel.  Two GPUs are used when the machine has them."""
-    import torch
+    through the exhaustive kernel.  A group of one member and one of two (on one GPU when the machine has one)."""
+    from common import group_devices
     d, k = 1536, 20
     rng = np.random.default_rng(4)
     rows, q, _, _ = tie_corpus(rng, d, 9000, above=[3, 0, 9], group_size=150, q_per_group=5)
-    for devices in ([0], [0, 1]):
-        if torch.cuda.device_count() < len(devices):
-            continue
+    for devices in (group_devices(1), group_devices(2)):
         with rb.Group(d, devices, keep_f64=True) as g:
             g.append_f64(rows)
             f0 = g.stats()["fallback_queries"]

@@ -224,15 +224,13 @@ def test_infinity_and_signed_zero_ties_in_every_sort(rb, oracle_mod, tier):
 # --------------------------------------------------------------------------- a Group
 @pytest.mark.parametrize("n_dev", [1, 2])
 def test_group_across_the_range(rb, oracle_mod, n_dev):
-    import torch
-    if torch.cuda.device_count() < n_dev:
-        pytest.skip(f"needs {n_dev} GPUs")
+    from common import group_devices
     d = 100
     rng, rows = plain_corpus(d, "device", 77)
     q = rows[rng.choice(N_PLAIN, len(LADDER))] + 0.1 * rng.standard_normal((len(LADDER), d))
     q = np.stack([scaled(q[i], e) for i, e in enumerate(LADDER)])
     allrows = np.concatenate([rows, ladder_rows(rng, rows, q[LADDER.index(0)][None, :], "device")])
-    with rb.Group(d, list(range(n_dev)), keep_f64=True) as g:
+    with rb.Group(d, group_devices(n_dev), keep_f64=True) as g:
         g.append_f64(allrows)
         all_routes(oracle_mod, g, allrows, None, q, f"group on {n_dev} GPUs", group=True)
 

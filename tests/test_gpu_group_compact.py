@@ -146,14 +146,11 @@ def test_one_gpu_group_large_corpus_takes_many_staging_chunks(rb, oracle_mod):
             assert (s[b, :c[b]] == es[b, :c[b]]).all() and v[b, :c[b]].tobytes() == ev[b, :c[b]].tobytes()
 
 
-# --------------------------------------------------------------------------- two or more GPUs
+# --------------------------------------------------------------------------- two or more members
 def group_devices(n_dev):
-    have = n_devices()
-    if have < 2:
-        pytest.skip("needs >= 2 GPUs")
-    if n_dev == 0 and have == 2:
-        pytest.skip("all visible GPUs are the two of the other case")
-    return list(range(have if n_dev == 0 else 2))
+    """n_dev members (0: every visible GPU, at least three members), co-located where the machine has too few GPUs."""
+    import common
+    return common.group_devices(max(n_devices(), 3) if n_dev == 0 else n_dev)
 
 
 @pytest.mark.parametrize("n_dev", [2, 0], ids=["two", "all"])

@@ -222,11 +222,10 @@ def test_storage_bytes(rb):
         assert same(dev.search(rows[:5], 20, None)[1], host.search(rows[:5], 20, None)[1])
 
 
-@pytest.mark.parametrize("devs", [[0], [0, 1]], ids=["one_gpu", "two_gpus"])
-def test_groups(rb, oracle_mod, devs):
-    import torch
-    if torch.cuda.device_count() < len(devs):
-        pytest.skip("needs >= 2 GPUs")
+@pytest.mark.parametrize("n_dev", [1, 2], ids=["one_gpu", "two_gpus"])
+def test_groups(rb, oracle_mod, n_dev):
+    from common import group_devices
+    devs = group_devices(n_dev)
     n, d = 9000, 192
     rng = np.random.default_rng(5)
     corpus = rng.standard_normal((n, d))

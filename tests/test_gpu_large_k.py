@@ -246,14 +246,12 @@ def test_one_gpu_group(rb, oracle_mod):
 
 
 def test_two_gpu_group(rb, oracle_mod):
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs")
+    from common import group_devices
     from runbookai_b200 import synth
     n, d = 50_000, 512
     corpus = synth.random_corpus(n, d, 81)
     q = synth.random_queries(4, d, 82).astype(np.float64)
-    with rb.Group(d, [0, 1]) as g:
+    with rb.Group(d, group_devices(2)) as g:
         g.append_bf16(corpus)
         check(g.search_large(q, 1000, None), *oracle_bf16(oracle_mod, corpus, q, 1000, None))
 

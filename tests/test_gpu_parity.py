@@ -159,10 +159,10 @@ def test_multi_device_index_single_process(rb, oracle_mod):
 def test_group_one_handle_many_gpus_matches_oracle(rb, oracle_mod):
     """rbk_group_*: the in-library multi-GPU index (one host process, one call per search: per-GPU scans, ONE
     ncclAllGather of the packed blocks, merge kernel, one synchronisation).  Two GPUs when the box has them (NCCL
-    path), else a one-GPU group (same code minus the collective).  Rows are dealt out in 4096-row blocks, so appends
+    path), else two members on one GPU (the copy exchange).  Rows are dealt out in 4096-row blocks, so appends
     straddle blocks and devices; ties across devices, tombstones, bulk overwrite and the dirty-flag re-answer path
     (a tie group larger than any candidate margin) are all checked against the oracle on the whole corpus."""
-    import torch
+    from common import group_devices
     from runbookai_b200 import Group, synth
     n, d = 30_000, 256
     corpus = synth.random_corpus(n, d, 141)
@@ -170,7 +170,7 @@ def test_group_one_handle_many_gpus_matches_oracle(rb, oracle_mod):
     synth.plant_neighbours(corpus, q, 12, 143)
     corpus[4096 + 7] = corpus[5]                           # exact tie across the first block boundary (= across devices)
     corpus[3 * 4096 + 1] = corpus[5]
-    devs = [0, 1] if torch.cuda.device_count() > 1 else [0]
+    devs = group_devices(2)
     with Group(d, devs) as g:
         for r0 in range(0, n, 7000):                       # appends that straddle blocks and devices
             assert g.append_bf16(corpus[r0:r0 + 7000]) == r0

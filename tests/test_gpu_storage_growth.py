@@ -321,12 +321,10 @@ def test_trim_returns_memory_and_keeps_answers(rb, oracle_mod):
 
 @pytest.mark.parametrize("n_dev", [1, 2])
 def test_group_trim_after_clear(rb, oracle_mod, n_dev):
-    import torch
-    if torch.cuda.device_count() < n_dev:
-        pytest.skip(f"needs {n_dev} GPUs")
+    from common import group_devices
     d = 128
     rng = np.random.default_rng(12)
-    with rb.Group(d, list(range(n_dev)), keep_f64=True) as g:
+    with rb.Group(d, group_devices(n_dev), keep_f64=True) as g:
         rows = rng.standard_normal((30000, d))
         g.append_f64(rows)
         g.clear()

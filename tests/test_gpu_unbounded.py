@@ -241,14 +241,12 @@ def test_one_gpu_group_equals_a_single_index(rb):
 
 
 def test_two_gpu_group_equals_a_single_index(rb):
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs")
+    from common import group_devices
     from runbookai_b200 import synth
     n, d = 50_000, 128
     corpus = synth.random_corpus(n, d, 461)
     q = synth.random_queries(4, d, 462).astype(np.float64)
-    with rb.Group(d, [0, 1]) as g, rb.Index(d) as ix:
+    with rb.Group(d, group_devices(2)) as g, rb.Index(d) as ix:
         for h in (g, ix):
             h.append_bf16(corpus)
             h.tombstone(np.arange(5, n, 17))

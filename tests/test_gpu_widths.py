@@ -382,10 +382,8 @@ def test_width_above_the_limit_is_rejected(rb):
 def test_group_answers_like_an_index(rb, oracle_mod, d, tier, n_dev):
     """A group and an index fed the same calls (more than one 4096-row block, so a second GPU holds rows): the same
     answers bit for bit on every route, the same compaction map, the same answers after trim, and the oracle's."""
-    import torch
+    from common import group_devices
     from runbookai_b200 import synth
-    if torch.cuda.device_count() < n_dev:
-        pytest.skip(f"needs {n_dev} GPUs")
     n = 5000
     rng = np.random.default_rng(d + n_dev)
     q = rng.standard_normal((6, d))
@@ -398,7 +396,7 @@ def test_group_answers_like_an_index(rb, oracle_mod, d, tier, n_dev):
         corpus[rng.choice(n, 30, replace=False)] = q[np.arange(30) % 6] + 0.3 * rng.standard_normal((30, d))
     live = runs_dead(n, rng, 0.4)
     live[4096:4200] = 0
-    with make(rb, d, tier, rb.Group, devices=list(range(n_dev))) as g, make(rb, d, tier) as ix:
+    with make(rb, d, tier, rb.Group, devices=group_devices(n_dev)) as g, make(rb, d, tier) as ix:
         for h in (g, ix):
             h.append_bf16(corpus) if tier == "bf16" else h.append_f64(corpus)
             h.tombstone(np.flatnonzero(live == 0))
