@@ -24,7 +24,7 @@ import numpy as np
 
 from . import embedder as _emb
 from ._native import RBK_EDIM, RBK_MAX_K_FETCH, DimensionError
-from .vector_store import NOT_CONFIGURED, VectorStore
+from .vector_store import NOT_CONFIGURED, VectorStore, js_or
 
 
 class MicroBatcher:
@@ -95,7 +95,7 @@ class MicroBatcher:
             st = self.store
             # callers that want more than the scan's candidate lists hold (topK > 56) take the large-k path of
             # VectorStore.search on their own; everybody else shares one device pass
-            big = [b for b in batch if 2 * (b[1].get("topK") or b[1].get("top_k") or 10) > RBK_MAX_K_FETCH]
+            big = [b for b in batch if 2 * js_or(b[1].get("topK"), b[1].get("top_k"), 10) > RBK_MAX_K_FETCH]
             for q_, o_, f_ in big:
                 try:
                     f_.set_result(st.search(q_, o_))
@@ -108,8 +108,8 @@ class MicroBatcher:
             qvec = np.asarray(_emb.embed_texts([b[0] for b in batch]), dtype=np.float64)
             # one device pass: fetch enough for the most demanding caller, strictest-common threshold = the
             # LOWEST minScore; each caller's own cut and threshold are re-applied below (S4, S5, S7)
-            top_ks = [o.get("topK") or o.get("top_k") or 10 for _, o, _ in batch]
-            mins = [o.get("minScore") or o.get("min_score") or 0.5 for _, o, _ in batch]
+            top_ks = [js_or(o.get("topK"), o.get("top_k"), 10) for _, o, _ in batch]
+            mins = [js_or(o.get("minScore"), o.get("min_score"), 0.5) for _, o, _ in batch]
             k_fetch = 2 * max(top_ks)
             with st._st.lock:   # state checks, scan and slot -> id lookup against the same table (the index may be shared)
                 if st._index is None or not st._ids:

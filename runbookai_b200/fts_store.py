@@ -9,7 +9,7 @@ import json
 import re
 import sqlite3
 
-from .vector_store import RetrievedChunk
+from .vector_store import RetrievedChunk, js_or
 
 SCHEMA = """
       CREATE TABLE IF NOT EXISTS documents (
@@ -66,7 +66,7 @@ class KnowledgeStore:
     def search(self, query, options: dict | None = None) -> list[RetrievedChunk]:
         """sqlite.ts:125-209."""
         o = options or {}
-        limit = o.get("limit") or 10
+        limit = js_or(o.get("limit"), 10)
         safe = query if isinstance(query, str) else str(query or "")
         type_filter = [t for t in (o.get("typeFilter") or []) if isinstance(t, str)]
         service_filter = [s for s in (o.get("serviceFilter") or []) if isinstance(s, str)]

@@ -11,7 +11,7 @@ from dataclasses import replace
 from typing import Sequence
 
 from . import embedder as _emb
-from .vector_store import RetrievedChunk, VectorStore, create_vector_store
+from .vector_store import RetrievedChunk, VectorStore, create_vector_store, js_or
 
 
 def reciprocal_rank_fusion(fts_results: Sequence[RetrievedChunk], vector_results: Sequence[RetrievedChunk],
@@ -54,7 +54,7 @@ class HybridRetriever:
         """hybrid-search.ts:54-100."""
         o = dict(options or {})
         o.update(kw)
-        top_k = o.get("topK") or 10
+        top_k = js_or(o.get("topK"), 10)
         mode = o.get("mode") or ("hybrid" if self.has_vector_search() else "fts")
         tf, sf = o.get("typeFilter"), o.get("serviceFilter")
         if mode == "fts" or not self.has_vector_search():

@@ -69,6 +69,15 @@ _SIDECAR_VERSION = 2
 _TAIL_ROWS = 64
 
 
+def js_or(*values):
+    """JavaScript's `a || b || ...`: the first value JavaScript counts as truthy, else the last one.  Python's `or`
+    agrees on None, False, 0, -0.0 and "", but counts NaN as true, where `NaN || 0.5` is 0.5."""
+    for v in values[:-1]:
+        if v and v == v:
+            return v
+    return values[-1]
+
+
 @dataclass
 class RetrievedChunk:
     """src/knowledge/types.ts:250-259."""
@@ -616,8 +625,8 @@ class VectorStore:
         o.update(kw)
         if not _emb.is_embedder_configured():
             raise RuntimeError(NOT_CONFIGURED)                       # :197-199
-        top_k = o.get("topK") or o.get("top_k") or 10                # :201  (0/None -> 10)
-        min_score = o.get("minScore") or o.get("min_score") or 0.5   # :202  (0/None -> 0.5)
+        top_k = js_or(o.get("topK"), o.get("top_k"), 10)                # :201  (0/None/NaN -> 10)
+        min_score = js_or(o.get("minScore"), o.get("min_score"), 0.5)   # :202  (0/None/NaN -> 0.5)
         type_filter = o.get("typeFilter") or o.get("type_filter")
         service_filter = o.get("serviceFilter") or o.get("service_filter")
         q = np.asarray(_emb.embed_texts(list(queries)) if len(queries) > 1 else [_emb.embed_text(queries[0])],
