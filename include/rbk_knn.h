@@ -55,7 +55,8 @@ typedef enum {
   RBK_ENOMEM = 2, /* host or device allocation failed */
   RBK_ECUDA = 3,  /* CUDA runtime/driver error, or no device */
   RBK_ENCCL = 4,  /* NCCL missing or failing (rbk_group_* with more than one GPU) */
-  RBK_EDIM = 5    /* "Vectors must have the same length" (embedder.ts:169-171) */
+  RBK_EDIM = 5,   /* "Vectors must have the same length" (embedder.ts:169-171) */
+  RBK_ENOTF32 = 6 /* a value is not exactly a float32 (only RBK_INDEX_KEEP_F32 indexes and groups return it) */
 } rbk_status;
 
 int rbk_abi_version(void);
@@ -84,7 +85,8 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * top-k search of the index takes the exhaustive kernel and every large-k search re-scores every live row: exact, at
  * the cost of the whole corpus per query. */
 #define RBK_INDEX_KEEP_F64 1u
-/* RBK_INDEX_F64_ON_HOST (only together with RBK_INDEX_KEEP_F64, else RBK_EINVAL): the [capacity][dim] float64 rows
+/* RBK_INDEX_F64_ON_HOST (only together with RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32, else RBK_EINVAL; also spelled
+ * RBK_INDEX_ROWS_ON_HOST): the [capacity][dim] exact rows (float64 below; float32 at half the bytes with KEEP_F32)
  * live in pinned, mapped host memory (cudaHostAlloc Mapped | Portable) instead of on the GPU; every other buffer stays
  * where it is.  Answers are bit-identical to a KEEP_F64 index on the device fed the same calls - slots, scores, counts,
  * exactness flags, fallback and retry decisions, compaction maps: the same values go through the same operations in
@@ -98,7 +100,28 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * or copy on the index stream, or the host after a synchronisation), so searches enqueued earlier never see a
  * half-written row.  The placement is fixed until rbk_index_set_tier. */
 #define RBK_INDEX_F64_ON_HOST 2u
-/* RBK_INDEX_SCAN_F16 (only together with RBK_INDEX_KEEP_F64, else RBK_EINVAL; combines with RBK_INDEX_F64_ON_HOST):
+/* RBK_INDEX_KEEP_F32 (exclusive with RBK_INDEX_KEEP_F64: both return RBK_EINVAL): keeps the exact rows as float32,
+ * [capacity][dim] at 4*dim bytes per row, instead of float64.  Only float32-exact values are stored: a double x is
+ * accepted iff it is NaN or (double)(float)x == x (so +-0, +-inf and float32 subnormals are; 0.1, 1e-300 and 1e39 are
+ * not).  rbk_index_append_f32 / _bf16 always qualify.  rbk_index_append_f64, rbk_index_append_f64_device,
+ * rbk_index_overwrite_f64 and rbk_index_overwrite_f64_batch check every value of the call on the device before anything
+ * is written (overwrite_f64_batch before its tombstoned-slot rule writes the live slots); a call holding any other value
+ * returns RBK_ENOTF32 and leaves the index exactly as it was - size, count, rows, norms, the corpus-side error bound,
+ * tombstone bits, and so the answers of every later search (a capacity grown during the call may stay grown).  NaN
+ * elements may lose their payload bits.  A group refuses the whole call before any member writes.
+ * The contract: a KEEP_F32 index fed the same calls answers exactly as a KEEP_F64 index with the same other flags -
+ * slots, fp64 scores and counts, -1 / NaN tails, exactness flags, retry and fallback decisions and the stats counters,
+ * debug scores, compaction maps, the corpus-side bound and the scan-band rule.  It holds because a float32 row widened to
+ * double IS the float64 row: every kernel widens each element on load and runs the same operations in the same order.
+ * What changes is the bytes: 9,228 instead of 15,372 device bytes per row at d = 1536 on the device tier (the row
+ * ceiling below uses them), 6,144 instead of 12,288 pinned host bytes with RBK_INDEX_ROWS_ON_HOST, and half the bytes
+ * read per row by the re-rank, the exhaustive fallback and rbk_index_exact_scores_f64. */
+#define RBK_INDEX_KEEP_F32 64u
+/* The placement flag under its general name: with either keep bit, the exact rows (float64 or float32) live in pinned,
+ * mapped host memory, as described for RBK_INDEX_F64_ON_HOST (host RAM then pays 8*dim or 4*dim bytes per row). */
+#define RBK_INDEX_ROWS_ON_HOST RBK_INDEX_F64_ON_HOST
+/* RBK_INDEX_SCAN_F16 (only together with RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32, else RBK_EINVAL; combines with
+ * RBK_INDEX_F64_ON_HOST):
  * the scan reads fp16 rows instead of bf16, at the same 2 bytes per element.  Each row x (and each query) is stored
  * scaled by its own power of two, h_i = RNE_f16(x_i * 2^e) with e = 15 - E, E the frexp exponent of max |x_i| over the
  * finite elements (so max|x| * 2^e is in [2^14, 2^15)); results that would be subnormal are stored as signed zeros.
@@ -111,15 +134,19 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
 #define RBK_INDEX_SCAN_F16 16u
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out);
 void rbk_index_destroy(rbk_index* idx); /* NULL is a no-op */
-/* The index's creation flags as they are now (RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16); 0 for
- * NULL. */
+/* The index's creation flags as they are now (RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32 | RBK_INDEX_F64_ON_HOST |
+ * RBK_INDEX_SCAN_F16); 0 for NULL. */
 uint32_t rbk_index_flags(const rbk_index* idx);
-/* Change the storage tier of a float64-backed index in place, from the float64 rows it holds: move them between the
- * device and pinned host memory (RBK_INDEX_F64_ON_HOST) and switch the scan between bf16 and fp16 (RBK_INDEX_SCAN_F16),
- * without reloading.
- *   - flags: a flag set rbk_index_create_ex accepts, with the index's own RBK_INDEX_KEEP_F64 bit (a float64 copy cannot
- *     be made from bf16 rows, and dropping it would change the answers); anything else returns RBK_EINVAL with the index
- *     untouched.  The current flags are a no-op (RBK_OK).  The member indexes of a group refuse the call (RBK_EINVAL):
+/* Change the storage tier of an index with exact rows in place, from the rows it holds: move them between the device
+ * and pinned host memory (RBK_INDEX_F64_ON_HOST), switch the scan between bf16 and fp16 (RBK_INDEX_SCAN_F16), and keep
+ * them as float64 or float32 (RBK_INDEX_KEEP_F64 / RBK_INDEX_KEEP_F32), in any combination, without reloading.
+ *   - flags: a flag set rbk_index_create_ex accepts with one of the keep bits (an exact copy cannot be made from bf16
+ *     rows, and dropping it would change the answers); anything else returns RBK_EINVAL with the index untouched.
+ *   - Widening (KEEP_F32 -> KEEP_F64) always succeeds given the memory.  Narrowing (KEEP_F64 -> KEEP_F32) succeeds only if
+ *     every stored slot [0, size()), live or tombstoned, holds float32-exact values (the rule of RBK_INDEX_KEEP_F32);
+ *     otherwise it returns RBK_ENOTF32, checked before anything changes.  Either way the new exact-row buffer is
+ *     allocated and filled before the old one is released: peak memory is the old plus the new exact rows.
+ *   - The current flags are a no-op (RBK_OK).  The member indexes of a group refuse the call (RBK_EINVAL):
  *     rbk_group_set_tier changes them together.
  *   - Every answer stays bit for bit: slots, fp64 scores, counts, -1 / NaN tails, exactness flags, compaction maps; so
  *     do size(), count(), slot_base, the capacity and the stats counters.
@@ -208,7 +235,7 @@ int64_t rbk_index_count(const rbk_index* idx); /* live rows  */
 int64_t rbk_index_size(const rbk_index* idx);  /* slots used, tombstones included */
 int32_t rbk_index_dim(const rbk_index* idx);
 /* Persistent corpus storage at the current capacity, in bytes: bf16 rows, inv_norm, norm2, tombstone bits and the
- * float64 rows (KEEP_F64), split by where they live.  Search and compaction scratch are not counted.  Either output
+ * exact rows (8*dim bytes per row with KEEP_F64, 4*dim with KEEP_F32), split by where they live.  Search and compaction scratch are not counted.  Either output
  * may be NULL. */
 rbk_status rbk_index_storage_bytes(const rbk_index* idx, int64_t* device_bytes, int64_t* pinned_host_bytes);
 /* Copy stored rows back (bf16 bits), for tests and for reload sidecars.  RBK_EINVAL on an RBK_INDEX_SCAN_F16 index. */
@@ -323,8 +350,8 @@ rbk_status rbk_merge_topk_packed_device(int32_t device, void* cuda_stream, int32
  * name. */
 typedef struct rbk_group rbk_group;
 rbk_status rbk_group_create(int32_t dim, const int32_t* device_ids, int32_t n_devices, int64_t capacity_hint,
-                            uint32_t flags /* RBK_INDEX_KEEP_F64 [| RBK_INDEX_F64_ON_HOST] [| RBK_INDEX_SCAN_F16]:
-                                              every member */,
+                            uint32_t flags /* RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32 [| RBK_INDEX_F64_ON_HOST]
+                                              [| RBK_INDEX_SCAN_F16]: every member */,
                             rbk_group** out);
 void rbk_group_destroy(rbk_group* grp); /* NULL is a no-op */
 rbk_status rbk_group_append_f64(rbk_group* grp, const double* rows, int64_t n_rows, int64_t* first_slot_out);
@@ -350,8 +377,8 @@ rbk_status rbk_group_compact(rbk_group* grp, int64_t* old_to_new, int64_t old_to
 /* rbk_index_trim on every member, and the group's own exchange buffers released. */
 rbk_status rbk_group_trim(rbk_group* grp);
 /* rbk_index_set_tier on every member together (read the flags of any member with rbk_index_flags): every member's
- * allocations happen before any member changes, so RBK_ENOMEM leaves the whole group as it was.  Synchronous; uses no
- * NCCL. */
+ * checks (RBK_ENOTF32 for a narrowing) and allocations happen before any member changes, so RBK_ENOMEM and RBK_ENOTF32
+ * leave the whole group as it was.  Synchronous; uses no NCCL. */
 rbk_status rbk_group_set_tier(rbk_group* grp, uint32_t flags);
 int64_t rbk_group_count(const rbk_group* grp); /* live rows */
 int64_t rbk_group_size(const rbk_group* grp);  /* slots used, tombstones included */

@@ -3,6 +3,7 @@
 
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <thread>
@@ -137,6 +138,22 @@ napi_status napi_get_value_bool(napi_env, napi_value value, bool* result) {
   Val* v = V(value);
   if (!v || v->kind != kBoolean) return napi_boolean_expected;
   *result = v->num != 0;
+  return napi_ok;
+}
+
+napi_status napi_get_value_string_utf8(napi_env, napi_value value, char* buf, size_t bufsize, size_t* result) {
+  Val* v = V(value);
+  if (!v || v->kind != kString) return napi_string_expected;
+  if (!buf) {
+    if (result) *result = v->str.size();
+    return napi_ok;
+  }
+  const size_t n = bufsize == 0 ? 0 : std::min(v->str.size(), bufsize - 1);   // Node truncates and terminates
+  if (bufsize) {
+    memcpy(buf, v->str.data(), n);
+    buf[n] = '\0';
+  }
+  if (result) *result = n;
   return napi_ok;
 }
 

@@ -102,6 +102,7 @@ napi_status napi_define_class(napi_env env, const char* utf8name, size_t length,
 // -- reading values
 napi_status napi_get_boolean(napi_env env, bool value, napi_value* result);
 napi_status napi_get_value_bool(napi_env env, napi_value value, bool* result);
+napi_status napi_get_value_string_utf8(napi_env env, napi_value value, char* buf, size_t bufsize, size_t* result);
 napi_status napi_has_named_property(napi_env env, napi_value object, const char* utf8name, bool* result);
 napi_status napi_get_named_property(napi_env env, napi_value object, const char* utf8name, napi_value* result);
 napi_status napi_get_value_int32(napi_env env, napi_value value, int32_t* result);

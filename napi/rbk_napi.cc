@@ -12,15 +12,20 @@
 //   const { RbkIndex } = require('./build/Release/rbk_knn.node')
 //   const ix = new RbkIndex(dim, device, capacityHint)          // one GPU  (rbk_index_*)
 //   const ix = new RbkIndex(dim, [0, 1, 2, 3], capacityHint)    // several GPUs behind one handle (rbk_group_*)
-//   const ix = new RbkIndex(dim, device, capacityHint, hostRows) // hostRows != 0: float64 rows in pinned host RAM
+//   const ix = new RbkIndex(dim, device, capacityHint, hostRows) // hostRows != 0: exact rows in pinned host RAM
+//   const ix = new RbkIndex(dim, device, capacityHint, hostRows, scanF16, exactRows)   // exactRows 'f64' | 'f32'
+//                                              // (absent: RUNBOOK_KNN_EXACT_ROWS, else 'f64')
 //   ix.appendF64(Float64Array rows)            -> firstSlot
 //   ix.appendBlobs(Buffer[] blobs)             -> firstSlot     // SQLite f64-LE BLOBs, packed in C++: no JS copies
 //   ix.overwriteF64(slot, Float64Array row); ix.overwriteF64Batch(BigInt64Array slots, Float64Array rows)
 //   ix.tombstone(BigInt64Array slots); ix.clear()
 //   ix.compact()                               -> BigInt64Array oldToNew   // reclaim tombstoned slots
 //   ix.trim()                                  // give unused device memory back (after compact / clear)
-//   ix.setTier({ f64OnHost, scanF16 })         // move the float64 rows / switch the scan in place (omitted: kept)
-//   ix.tier                                    -> { f64OnHost: boolean, scanF16: boolean }
+//   ix.setTier({ f64OnHost, scanF16, exactRows })   // move the exact rows / switch the scan / widen or narrow them in
+//                                              // place (omitted: kept)
+//   ix.tier                                    -> { f64OnHost: boolean, scanF16: boolean, exactRows: 'f64' | 'f32' }
+//   With exactRows 'f32', an append or overwrite holding a value no float32 can hold (RBK_ENOTF32, nothing written)
+//   widens the index to 'f64' in place and is repeated once, so the addon accepts every embedding a default index does.
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
 //   await ix.searchLarge(Float64Array queries, B, kFetch, minScore)   // kFetch up to 4096, same result object
@@ -31,6 +36,7 @@
 
 #include <cmath>
 #include <cstdint>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -81,11 +87,25 @@ struct Handle {
   rbk_index* ix = nullptr;
   rbk_group* grp = nullptr;
   int32_t dim = 0;
+  // A float32-row index refuses a value no float32 holds (RBK_ENOTF32) before writing anything: widen it to float64
+  // rows in place and repeat the call once.
+  template <typename F>
+  rbk_status widening(F&& call) {
+    rbk_status st = call();
+    if (st != RBK_ENOTF32 || !has_tier()) return st;
+    if ((st = set_tier((flags() & ~RBK_INDEX_KEEP_F32) | RBK_INDEX_KEEP_F64)) != RBK_OK) return st;
+    return call();
+  }
   rbk_status append_f64(const double* rows, int64_t n, int64_t* first) {
-    return grp ? rbk_group_append_f64(grp, rows, n, first) : rbk_index_append_f64(ix, rows, n, first);
+    return widening([&] {
+      return grp ? rbk_group_append_f64(grp, rows, n, first) : rbk_index_append_f64(ix, rows, n, first);
+    });
   }
   rbk_status overwrite_batch(const int64_t* slots, int64_t n, const double* rows) {
-    return grp ? rbk_group_overwrite_f64_batch(grp, slots, n, rows) : rbk_index_overwrite_f64_batch(ix, slots, n, rows);
+    return widening([&] {
+      return grp ? rbk_group_overwrite_f64_batch(grp, slots, n, rows)
+                 : rbk_index_overwrite_f64_batch(ix, slots, n, rows);
+    });
   }
   rbk_status tombstone(const int64_t* slots, int64_t n) {
     return grp ? rbk_group_tombstone(grp, slots, n) : rbk_index_tombstone(ix, slots, n);
@@ -137,9 +157,23 @@ void finalize_index(napi_env, void* data, void*) {
   delete h;
 }
 
+// 'f64' / 'f32' -> the keep bit; anything else -> 0.
+uint32_t keep_bit(const std::string& s) {
+  return s == "f64" ? RBK_INDEX_KEEP_F64 : (s == "f32" ? RBK_INDEX_KEEP_F32 : 0u);
+}
+
+// A JS string (at most 15 bytes are needed here); false if v is not a string.
+bool get_string(napi_env env, napi_value v, std::string* out) {
+  char buf[16];
+  size_t n = 0;
+  if (napi_get_value_string_utf8(env, v, buf, sizeof buf, &n) != napi_ok) return false;
+  out->assign(buf, n);
+  return true;
+}
+
 napi_value New(napi_env env, napi_callback_info info) {
-  size_t argc = 5;
-  napi_value argv[5], self;
+  size_t argc = 6;
+  napi_value argv[6], self;
   NAPI_OK(napi_get_cb_info(env, info, &argc, argv, &self, nullptr));
   int32_t dim = 0, device = 0, host_rows = 0, scan_f16 = 0;
   int64_t hint = 0;
@@ -147,14 +181,28 @@ napi_value New(napi_env env, napi_callback_info info) {
   if (argc > 2) napi_get_value_int64(env, argv[2], &hint);
   if (argc > 3) napi_get_value_int32(env, argv[3], &host_rows);
   if (argc > 4) napi_get_value_int32(env, argv[4], &scan_f16);
+  // exactRows (RUNBOOK_KNN_EXACT_ROWS when absent): 'f64' keeps the exact rows as float64, 'f32' as float32
+  std::string exact_rows;
+  if (argc > 5) {
+    if (!get_string(env, argv[5], &exact_rows)) exact_rows = "?";
+  } else {
+    const char* e = getenv("RUNBOOK_KNN_EXACT_ROWS");
+    exact_rows = e && *e ? e : "f64";
+  }
+  const uint32_t keep = keep_bit(exact_rows);
+  if (keep == 0) {
+    napi_throw_type_error(env, nullptr, "exactRows must be 'f64' or 'f32'");
+    return nullptr;
+  }
   Handle* h = new Handle();
   h->dim = dim;
   bool is_array = false;
   if (argc > 1) napi_is_array(env, argv[1], &is_array);
-  // KEEP_F64: the reference stores float64 embeddings; keep them so results are exact for any input.  hostRows
-  // (RUNBOOK_KNN_F64_ON_HOST in ts/gpu-embedding-index.ts): keep them in pinned host memory instead of on the GPU.
-  // scanF16 (RUNBOOK_KNN_SCAN_F16): the scan reads per-row scaled fp16 rows instead of bf16 (same answers).
-  const uint32_t flags = RBK_INDEX_KEEP_F64 | (host_rows != 0 ? RBK_INDEX_F64_ON_HOST : 0u) |
+  // KEEP_F64: the reference stores float64 embeddings; keep them so results are exact for any input (KEEP_F32: the
+  // same answers from float32 rows while every value is a float32).  hostRows (RUNBOOK_KNN_F64_ON_HOST in
+  // ts/gpu-embedding-index.ts): keep them in pinned host memory instead of on the GPU.  scanF16
+  // (RUNBOOK_KNN_SCAN_F16): the scan reads per-row scaled fp16 rows instead of bf16 (same answers).
+  const uint32_t flags = keep | (host_rows != 0 ? RBK_INDEX_F64_ON_HOST : 0u) |
                          (scan_f16 != 0 ? RBK_INDEX_SCAN_F16 : 0u);
   rbk_status st;
   if (is_array) {   // [0, 1, ...]: the corpus sharded over these GPUs, one call per search (rbk_group_*)
@@ -328,8 +376,8 @@ bool require_tier(napi_env env, Handle* h) {
   return false;
 }
 
-// setTier({ f64OnHost, scanF16 }): rbk_index_set_tier / rbk_group_set_tier.  A key that is absent keeps its setting;
-// one that is present must be a boolean.  Synchronous; answers do not change.
+// setTier({ f64OnHost, scanF16, exactRows }): rbk_index_set_tier / rbk_group_set_tier.  A key that is absent keeps its
+// setting; f64OnHost / scanF16 must be booleans, exactRows 'f64' or 'f32'.  Synchronous; answers do not change.
 napi_value SetTier(napi_env env, napi_callback_info info) {
   size_t argc = 1;
   napi_value argv[1] = {nullptr};
@@ -356,11 +404,25 @@ napi_value SetTier(napi_env env, napi_callback_info info) {
     }
     flags = on ? (flags | k.bit) : (flags & ~k.bit);
   }
+  bool has = false;
+  NAPI_OK(napi_has_named_property(env, argv[0], "exactRows", &has));
+  if (has) {
+    napi_value v;
+    std::string s;
+    NAPI_OK(napi_get_named_property(env, argv[0], "exactRows", &v));
+    const uint32_t keep = get_string(env, v, &s) ? keep_bit(s) : 0u;
+    if (keep == 0) {
+      napi_throw_type_error(env, nullptr, "setTier: exactRows must be 'f64' or 'f32'");
+      return nullptr;
+    }
+    flags = (flags & ~(RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)) | keep;
+  }
   if (h->set_tier(flags) != RBK_OK) return throw_rbk(env);
   return nullptr;
 }
 
-// tier -> { f64OnHost, scanF16 }: where the float64 rows live and which scan the index runs, as they are now.
+// tier -> { f64OnHost, scanF16, exactRows }: where the exact rows live, which scan the index runs and the exact rows'
+// width, as they are now.
 napi_value GetTier(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
@@ -372,6 +434,9 @@ napi_value GetTier(napi_env env, napi_callback_info info) {
   NAPI_OK(napi_get_boolean(env, (flags & RBK_INDEX_SCAN_F16) != 0, &f16));
   NAPI_OK(napi_set_named_property(env, out, "f64OnHost", host));
   NAPI_OK(napi_set_named_property(env, out, "scanF16", f16));
+  napi_value rows;
+  NAPI_OK(napi_create_string_utf8(env, (flags & RBK_INDEX_KEEP_F32) ? "f32" : "f64", NAPI_AUTO_LENGTH, &rows));
+  NAPI_OK(napi_set_named_property(env, out, "exactRows", rows));
   return out;
 }
 

@@ -12,11 +12,13 @@ import numpy as np
 
 LIB_PATH = Path(__file__).resolve().parent / "lib" / "librbk_knn.so"
 
-RBK_OK, RBK_EINVAL, RBK_ENOMEM, RBK_ECUDA, RBK_ENCCL, RBK_EDIM = range(6)
+RBK_OK, RBK_EINVAL, RBK_ENOMEM, RBK_ECUDA, RBK_ENCCL, RBK_EDIM, RBK_ENOTF32 = range(7)
 RBK_MAX_K_FETCH = 112
 RBK_MAX_K_FETCH_LARGE = 4096
 RBK_INDEX_KEEP_F64 = 1
 RBK_INDEX_F64_ON_HOST = 2
+RBK_INDEX_ROWS_ON_HOST = RBK_INDEX_F64_ON_HOST
+RBK_INDEX_KEEP_F32 = 64
 RBK_INDEX_SCAN_F16 = 16
 
 # every symbol include/rbk_knn.h declares (tests check the .so exports all of them)
@@ -45,6 +47,11 @@ class RbkError(RuntimeError):
 
 class DimensionError(RbkError, ValueError):
     """'Vectors must have the same length' (embedder.ts:169-171)."""
+
+
+class NotFloat32Error(RbkError, ValueError):
+    """RBK_ENOTF32: a keep_f32 index (or group) was given a float64 value that no float32 holds exactly; nothing was
+    written.  Widen the index (set_tier(exact_rows="f64")) and repeat the call to store it."""
 
 
 class RbkStats(C.Structure):
@@ -139,6 +146,8 @@ def check(status: int) -> None:
     msg = (lib.rbk_last_error() or b"").decode("utf-8", "replace")
     if status == RBK_EDIM:
         raise DimensionError(status, msg)
+    if status == RBK_ENOTF32:
+        raise NotFloat32Error(status, msg)
     raise RbkError(status, msg)
 
 
@@ -146,16 +155,30 @@ def ptr(a: np.ndarray | None):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
-def _index_flags(keep_f64: bool, f64_on_host: bool, scan_f16: bool = False) -> int:
-    """f64_on_host or scan_f16 without keep_f64 is passed through: the library rejects it with its own message."""
-    return ((RBK_INDEX_KEEP_F64 if keep_f64 else 0) | (RBK_INDEX_F64_ON_HOST if f64_on_host else 0)
-            | (RBK_INDEX_SCAN_F16 if scan_f16 else 0))
+def _index_flags(keep_f64: bool, f64_on_host: bool, scan_f16: bool = False, keep_f32: bool = False) -> int:
+    """f64_on_host or scan_f16 without a keep bit, or both keep bits, are passed through: the library rejects them
+    with its own message."""
+    return ((RBK_INDEX_KEEP_F64 if keep_f64 else 0) | (RBK_INDEX_KEEP_F32 if keep_f32 else 0)
+            | (RBK_INDEX_F64_ON_HOST if f64_on_host else 0) | (RBK_INDEX_SCAN_F16 if scan_f16 else 0))
 
 
-def _tier_flags(current: int, f64_on_host, scan_f16) -> int:
-    """The flag set of a tier change from the current one: None keeps a setting, RBK_INDEX_KEEP_F64 stays as it is
-    (an index without it is refused by the library with its own message)."""
+_EXACT_ROWS = {"f64": RBK_INDEX_KEEP_F64, "f32": RBK_INDEX_KEEP_F32}
+
+
+def exact_rows_of(flags: int) -> str | None:
+    """'f64' / 'f32' for an index keeping float64 / float32 exact rows, None for one without."""
+    flags = int(flags)
+    return "f64" if flags & RBK_INDEX_KEEP_F64 else ("f32" if flags & RBK_INDEX_KEEP_F32 else None)
+
+
+def _tier_flags(current: int, f64_on_host, scan_f16, exact_rows=None) -> int:
+    """The flag set of a tier change from the current one: None keeps a setting; exact_rows 'f64' / 'f32' sets the
+    keep bit even on an index without exact rows, which the library then refuses with its own message)."""
     flags = int(current)
+    if exact_rows is not None:
+        if exact_rows not in _EXACT_ROWS:
+            raise ValueError(f"exact_rows must be 'f64', 'f32' or None, not {exact_rows!r}")
+        flags = (flags & ~(RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)) | _EXACT_ROWS[exact_rows]
     for value, bit, name in ((f64_on_host, RBK_INDEX_F64_ON_HOST, "f64_on_host"),
                              (scan_f16, RBK_INDEX_SCAN_F16, "scan_f16")):
         if value is None:
@@ -213,16 +236,19 @@ class Index:
     """Thin object wrapper over rbk_index* (one GPU shard)."""
 
     def __init__(self, dim: int, device: int = 0, capacity_hint: int = 0, keep_f64: bool = False,
-                 f64_on_host: bool = False, scan_f16: bool = False):
+                 f64_on_host: bool = False, scan_f16: bool = False, keep_f32: bool = False):
         """keep_f64: RBK_INDEX_KEEP_F64 — exact for arbitrary float64 rows at 8*dim extra bytes per row.
-        f64_on_host: RBK_INDEX_F64_ON_HOST — those float64 rows live in pinned host memory instead of on the GPU (same
-        answers; the re-rank reads them over PCIe).  Requires keep_f64.
+        keep_f32: RBK_INDEX_KEEP_F32 — the same answers from float32 exact rows at 4*dim bytes per row, for rows whose
+        values are all float32-exact; append_f64 / overwrite of any other value raise NotFloat32Error with nothing
+        written.  Excludes keep_f64.
+        f64_on_host: RBK_INDEX_F64_ON_HOST (RBK_INDEX_ROWS_ON_HOST) — those exact rows live in pinned host memory
+        instead of on the GPU (same answers; the re-rank reads them over PCIe).  Requires keep_f64 or keep_f32.
         scan_f16: RBK_INDEX_SCAN_F16 — the scan reads per-row scaled fp16 rows instead of bf16 (same bytes, same
-        answers, a several times tighter error bound, so fewer wide retries).  Requires keep_f64."""
+        answers, a several times tighter error bound, so fewer wide retries).  Requires keep_f64 or keep_f32."""
         self._h = None
         h = C.c_void_p()
-        check(lib.rbk_index_create_ex(dim, device, capacity_hint, _index_flags(keep_f64, f64_on_host, scan_f16),
-                                      C.byref(h)))
+        check(lib.rbk_index_create_ex(dim, device, capacity_hint,
+                                      _index_flags(keep_f64, f64_on_host, scan_f16, keep_f32), C.byref(h)))
         self._h = h
         self.dim = dim
         self.device = device
@@ -249,14 +275,17 @@ class Index:
 
     @property
     def flags(self) -> int:
-        """The creation flags as they are now (RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16)."""
+        """The creation flags as they are now (RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32 | RBK_INDEX_F64_ON_HOST |
+        RBK_INDEX_SCAN_F16)."""
         return int(lib.rbk_index_flags(self._h))
 
-    def set_tier(self, *, f64_on_host: bool | None = None, scan_f16: bool | None = None) -> None:
-        """Change the storage tier in place (rbk_index_set_tier): move the float64 rows between the GPU and pinned host
-        memory, switch the scan between bf16 and fp16.  None keeps a setting.  Needs keep_f64; answers do not change.
-        Raises RbkError(RBK_ENOMEM) with the index unchanged when the new tier cannot be backed."""
-        check(lib.rbk_index_set_tier(self._h, _tier_flags(self.flags, f64_on_host, scan_f16)))
+    def set_tier(self, *, f64_on_host: bool | None = None, scan_f16: bool | None = None,
+                 exact_rows: str | None = None) -> None:
+        """Change the storage tier in place (rbk_index_set_tier): move the exact rows between the GPU and pinned host
+        memory, switch the scan between bf16 and fp16, keep the exact rows as 'f64' or 'f32'.  None keeps a setting.
+        Needs keep_f64 or keep_f32; answers do not change.  Raises RbkError(RBK_ENOMEM) with the index unchanged when
+        the new tier cannot be backed, NotFloat32Error when a stored value does not fit exact_rows='f32'."""
+        check(lib.rbk_index_set_tier(self._h, _tier_flags(self.flags, f64_on_host, scan_f16, exact_rows)))
 
     # -- mutation
     def _append(self, fn, rows: np.ndarray) -> int:
@@ -415,14 +444,15 @@ class Group:
     Every search is one C call: per-GPU scans, one NCCL all-gather, merge on devices[0], one synchronisation."""
 
     def __init__(self, dim: int, devices, capacity_hint: int = 0, keep_f64: bool = False, f64_on_host: bool = False,
-                 scan_f16: bool = False):
-        """f64_on_host: every member keeps its float64 rows in its own pinned host buffer (see Index).
-        scan_f16: every member scans fp16 rows (see Index)."""
+                 scan_f16: bool = False, keep_f32: bool = False):
+        """f64_on_host: every member keeps its exact rows in its own pinned host buffer (see Index).
+        scan_f16: every member scans fp16 rows (see Index).  keep_f32: every member keeps float32 exact rows (see
+        Index); a call with any non-float32 value is refused before any member writes."""
         self._h = None
         devs = np.ascontiguousarray(list(devices), dtype=np.int32)
         h = C.c_void_p()
         check(lib.rbk_group_create(dim, ptr(devs), devs.shape[0], capacity_hint,
-                                   _index_flags(keep_f64, f64_on_host, scan_f16), C.byref(h)))
+                                   _index_flags(keep_f64, f64_on_host, scan_f16, keep_f32), C.byref(h)))
         self._h = h
         self.dim = dim
         self.devices = [int(d) for d in devs]
@@ -490,10 +520,11 @@ class Group:
         """The members' creation flags as they are now (they share them)."""
         return int(lib.rbk_index_flags(C.c_void_p(lib.rbk_group_member(self._h, 0))))
 
-    def set_tier(self, *, f64_on_host: bool | None = None, scan_f16: bool | None = None) -> None:
+    def set_tier(self, *, f64_on_host: bool | None = None, scan_f16: bool | None = None,
+                 exact_rows: str | None = None) -> None:
         """Index.set_tier() on every member together: every member's allocations come first, so RBK_ENOMEM leaves the
         whole group as it was."""
-        check(lib.rbk_group_set_tier(self._h, _tier_flags(self.flags, f64_on_host, scan_f16)))
+        check(lib.rbk_group_set_tier(self._h, _tier_flags(self.flags, f64_on_host, scan_f16, exact_rows)))
 
     def count(self) -> int:
         return lib.rbk_group_count(self._h)

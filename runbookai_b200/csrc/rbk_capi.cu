@@ -239,23 +239,25 @@ rbk_status vm_map_to(const rbk_index* ix, VmRange* r, size_t bytes) {
   return RBK_OK;
 }
 
-// Bytes of each device corpus buffer at capacity `cap` (ix->vm order); 0 for the f64 rows unless they live on the device
-// (f64_dev: they would, -1: the index's own tier).
-void storage_at(const rbk_index* ix, int64_t cap, size_t out[rbk_index::kVmBuffers], int f64_dev = -1) {
-  if (f64_dev < 0) f64_dev = ix->keep_f64 && !ix->f64_on_host;
+// Bytes of each device corpus buffer at capacity `cap` (ix->vm order); 0 for the exact rows unless they live on the
+// device (f64_dev: they would, -1: the index's own tier), x_elem bytes per element (-1: the index's own width).
+void storage_at(const rbk_index* ix, int64_t cap, size_t out[rbk_index::kVmBuffers], int f64_dev = -1, int x_elem = -1) {
+  if (f64_dev < 0) f64_dev = ix->keep_rows() && !ix->rows_on_host;
+  if (x_elem < 0) x_elem = ix->x_elem;
   out[0] = static_cast<size_t>(cap) * ix->dpad * 2;
   out[1] = static_cast<size_t>(inv_norm_len(cap)) * 4;
   out[2] = static_cast<size_t>(cap) * 8;
   out[3] = static_cast<size_t>((cap + 31) / 32) * 4;
-  out[4] = f64_dev ? static_cast<size_t>(cap) * ix->dim * 8 : 0;
+  out[4] = f64_dev ? static_cast<size_t>(cap) * ix->dim * x_elem : 0;
 }
 
-// The most rows the device's memory could back with the f64 rows on the device (f64_dev) or not: the row ceiling of a
-// tier, min(2^31 - 512, total memory / device bytes per row) in whole tiles.
-int64_t tier_vm_rows(const rbk_index* ix, bool f64_dev) {
+// The most rows the device's memory could back with the exact rows (x_elem bytes per element, -1: the index's own) on
+// the device (f64_dev) or not: the row ceiling of a tier, min(2^31 - 512, total memory / device bytes per row) in whole
+// tiles.
+int64_t tier_vm_rows(const rbk_index* ix, bool f64_dev, int x_elem = -1) {
   // device bytes per row, the tombstone bit rounded up to a byte
   size_t per_row[rbk_index::kVmBuffers];
-  storage_at(ix, 1, per_row, f64_dev);
+  storage_at(ix, 1, per_row, f64_dev, x_elem);
   const int64_t row_bytes = static_cast<int64_t>(per_row[0] + 4 + per_row[2] + 1 + per_row[4]);
   return std::min<int64_t>((1ll << 31) - 2 * kBlockN, static_cast<int64_t>(ix->total_mem) / row_bytes / kBlockN * kBlockN);
 }
@@ -292,7 +294,7 @@ rbk_status vm_reserve(rbk_index* ix, size_t total_global_mem) {
   if ((res = api.MemGetAllocationGranularity(&ix->vm_gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM)) != CUDA_SUCCESS)
     return cu_fail(res, "cuMemGetAllocationGranularity");
   ix->total_mem = total_global_mem;
-  ix->vm_rows = tier_vm_rows(ix, ix->keep_f64 && !ix->f64_on_host);
+  ix->vm_rows = tier_vm_rows(ix, ix->keep_rows() && !ix->rows_on_host);
   size_t bytes[rbk_index::kVmBuffers];
   storage_at(ix, ix->vm_rows, bytes);
   for (int i = 0; i < rbk_index::kVmBuffers; ++i) {
@@ -306,7 +308,7 @@ rbk_status vm_reserve(rbk_index* ix, size_t total_global_mem) {
   ix->inv_norm = reinterpret_cast<float*>(ix->vm[1].base);
   ix->norm2 = reinterpret_cast<double*>(ix->vm[2].base);
   ix->dead_bits = reinterpret_cast<unsigned int*>(ix->vm[3].base);
-  if (ix->keep_f64 && !ix->f64_on_host) ix->rows_f64 = reinterpret_cast<double*>(ix->vm[4].base);
+  if (ix->keep_rows() && !ix->rows_on_host) ix->rows_x = reinterpret_cast<void*>(ix->vm[4].base);
   return RBK_OK;
 }
 
@@ -366,28 +368,37 @@ rbk_status vm_alias(const rbk_index* ix, const VmRange& src, size_t bytes, VmRan
   return RBK_OK;
 }
 
-// RBK_INDEX_F64_ON_HOST: a pinned buffer for `ncap` rows holding the first n_rows rows of the current one, which it
+// The pinned, mapped buffer of `bytes` that the exact rows of RBK_INDEX_ROWS_ON_HOST live in (one pointer under UVA).
+rbk_status alloc_host_rows(size_t bytes, void** out) {
+  void* r = nullptr;
+  // not write-combined: the host reads these rows when the index grows
+  cudaError_t e = cudaHostAlloc(&r, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaHostAlloc(exact rows on the host)");
+  void* dp = nullptr;
+  if ((e = cudaHostGetDevicePointer(&dp, r, 0)) != cudaSuccess || dp != r) {
+    cudaFreeHost(r);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaHostGetDevicePointer(exact rows on the host)");
+    return fail(RBK_ECUDA, "pinned host rows are mapped at another device address (no unified addressing)");
+  }
+  *out = r;
+  return RBK_OK;
+}
+
+// RBK_INDEX_ROWS_ON_HOST: a pinned buffer for `ncap` rows holding the first n_rows rows of the current one, which it
 // replaces (peak: old + new in host RAM).  Synchronises the index stream first, so that every kernel that wrote or read
 // the old rows has finished.
 rbk_status realloc_host_rows(rbk_index* ix, int64_t ncap) {
-  double* r64 = nullptr;
-  // not write-combined: the host reads these rows when the index grows
-  cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&r64), static_cast<size_t>(ncap) * ix->dim * 8,
-                                cudaHostAllocMapped | cudaHostAllocPortable);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaHostAlloc(f64 rows on the host)");
-  void* dp = nullptr;
-  if ((e = cudaHostGetDevicePointer(&dp, r64, 0)) != cudaSuccess || dp != r64) {
-    cudaFreeHost(r64);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaHostGetDevicePointer(f64 rows on the host)");
-    return fail(RBK_ECUDA, "pinned host rows are mapped at another device address (no unified addressing)");
-  }
-  if ((e = cudaStreamSynchronize(ix->stream)) != cudaSuccess) {
-    cudaFreeHost(r64);
+  void* r = nullptr;
+  rbk_status st = alloc_host_rows(static_cast<size_t>(ncap) * ix->x_row_bytes(), &r);
+  if (st != RBK_OK) return st;
+  cudaError_t e = cudaStreamSynchronize(ix->stream);
+  if (e != cudaSuccess) {
+    cudaFreeHost(r);
     return cuda_fail(e, "cudaStreamSynchronize");
   }
-  if (ix->n_rows > 0) memcpy(r64, ix->rows_f64, static_cast<size_t>(ix->n_rows) * ix->dim * 8);
-  if (ix->rows_f64) cudaFreeHost(ix->rows_f64);
-  ix->rows_f64 = r64;
+  if (ix->n_rows > 0) memcpy(r, ix->rows_x, static_cast<size_t>(ix->n_rows) * ix->x_row_bytes());
+  if (ix->rows_x) cudaFreeHost(ix->rows_x);
+  ix->rows_x = r;
   return RBK_OK;
 }
 
@@ -407,7 +418,7 @@ rbk_status ensure_capacity(rbk_index* ix, int64_t need) {
     st = vm_map_capacity(ix, ncap);
   }
   if (st != RBK_OK) return st;
-  if (ix->f64_on_host && (st = realloc_host_rows(ix, ncap)) != RBK_OK) {
+  if (ix->rows_on_host && (st = realloc_host_rows(ix, ncap)) != RBK_OK) {
     for (int i = 0; i < rbk_index::kVmBuffers; ++i) vm_unmap_from(&ix->vm[i], old[i]);
     return st;
   }
@@ -429,17 +440,24 @@ rbk_status append_rows(rbk_index* ix, const void* src, bool is_device, int elem,
   DeviceGuard dg(ix->device);
   if (first_out) *first_out = ix->n_rows;
   if (n == 0) return RBK_OK;
-  rbk_status st = ensure_capacity(ix, ix->n_rows + n);
+  // float32 exact rows take float64 sources only when every value fits: checked before anything is written
+  rbk_status st = elem == 8 && ix->x_elem == 4
+                      ? check_f32_exact(ix, static_cast<const double*>(src), is_device, n * ix->dim)
+                      : RBK_OK;
+  if (st != RBK_OK) return st;
+  st = ensure_capacity(ix, ix->n_rows + n);
   if (st != RBK_OK) return st;
   const int src_type = elem == 8 ? 0 : (elem == 4 ? 1 : 2);
   uint16_t* dst0 = ix->rows + static_cast<size_t>(ix->n_rows) * ix->dpad;
-  double* dst64 = ix->keep_f64 ? ix->rows_f64 + static_cast<size_t>(ix->n_rows) * ix->dim : nullptr;
+  unsigned char* dstx =
+      ix->keep_rows() ? static_cast<unsigned char*>(ix->rows_x) + static_cast<size_t>(ix->n_rows) * ix->x_row_bytes()
+                      : nullptr;
   if (is_device) {
-    if (elem == 2 && ix->dpad == ix->dim && !ix->keep_f64) {
+    if (elem == 2 && ix->dpad == ix->dim && !ix->keep_rows()) {
       CK(cudaMemcpyAsync(dst0, src, static_cast<size_t>(n) * ix->dim * 2, cudaMemcpyDeviceToDevice, ix->stream));
     } else {
-      CK(launch_convert_rows(src, src_type, n, ix->dim, ix->dpad, dst0, dst64, ix->stream, nullptr, nullptr, nullptr,
-                             ix->scan_f16));
+      CK(launch_convert_rows(src, src_type, n, ix->dim, ix->dpad, dst0, dstx, ix->x_elem, ix->stream, nullptr, nullptr,
+                             nullptr, ix->scan_f16));
       ix->stats.kernel_launches++;
     }
   } else {
@@ -451,16 +469,16 @@ rbk_status append_rows(rbk_index* ix, const void* src, bool is_device, int elem,
       const unsigned char* hp = static_cast<const unsigned char*>(src) + static_cast<size_t>(r0) * row_bytes;
       CK(cudaMemcpyAsync(ix->stage.p, hp, static_cast<size_t>(nr) * row_bytes, cudaMemcpyHostToDevice, ix->stream));
       CK(launch_convert_rows(ix->stage.p, src_type, nr, ix->dim, ix->dpad, dst0 + static_cast<size_t>(r0) * ix->dpad,
-                             dst64 ? dst64 + static_cast<size_t>(r0) * ix->dim : nullptr, ix->stream, nullptr, nullptr,
-                             nullptr, ix->scan_f16));
+                             dstx ? dstx + static_cast<size_t>(r0) * ix->x_row_bytes() : nullptr, ix->x_elem, ix->stream,
+                             nullptr, nullptr, nullptr, ix->scan_f16));
       ix->stats.kernel_launches++;
       // the staging buffer is reused by the next chunk; pageable H2D copies are already
       // synchronous with respect to the host buffer, the kernel is ordered by the stream
     }
   }
-  CK(launch_row_norms(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, ix->n_rows, n, ix->dim, ix->dpad, ix->inv_norm,
-                      ix->norm2, ix->d_counter + 1, ix->stream, nullptr, nullptr, ix->scan_f16));
-  ix->stats.kernel_launches += ix->keep_f64 ? 2 : 1;
+  CK(launch_row_norms(ix->rows, ix->rows_x, ix->x_elem, ix->n_rows, n, ix->dim, ix->dpad, ix->inv_norm, ix->norm2,
+                      ix->d_counter + 1, ix->stream, nullptr, nullptr, ix->scan_f16));
+  ix->stats.kernel_launches += ix->keep_rows() ? 2 : 1;
   // Host sources: pageable H2D copies have consumed the caller's buffer when cudaMemcpyAsync returns and everything
   // after is stream-ordered, so an append costs no host round trip.  Device sources are read by the copy/convert
   // kernel itself, and page-locked host sources by a copy that really is asynchronous: the caller may free or reuse
@@ -677,7 +695,7 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
       fp.block_m = kBlockM;
       fp.min_score = min_score;
       fp.rows = ix->rows;
-      fp.rows_f64 = ix->rows_f64;
+      fp.rows_x = ix->rows_x;
       fp.row_norm2 = ix->norm2;
       fp.n_rows = ix->n_rows;
       fp.slot = ix->slot;
@@ -686,7 +704,7 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
       fp.out_scores = d_scores + static_cast<size_t>(q0) * k_fetch;
       fp.out_counts = d_counts + q0;
       fp.flags = d_flags + q0;
-      CK(launch_finalize(fp, ix->f64_on_host, ix->stream));
+      CK(launch_finalize(fp, ix->rows_on_host, ix->x_elem, ix->stream));
       ix->stats.kernel_launches++;
     }
   }
@@ -710,7 +728,7 @@ rbk_status run_fallback(rbk_index* ix, const std::vector<int>& fails, int k_fetc
   ep.k_fetch = k_fetch;
   ep.min_score = min_score;
   ep.rows = ix->rows;
-  ep.rows_f64 = ix->rows_f64;
+  ep.rows_x = ix->rows_x;
   ep.row_norm2 = ix->norm2;
   ep.dead_bits = ix->dead_bits;
   ep.n_rows = ix->n_rows;
@@ -724,7 +742,7 @@ rbk_status run_fallback(rbk_index* ix, const std::vector<int>& fails, int k_fetc
   ep.out_slots = d_slots;
   ep.out_scores = d_scores;
   ep.out_counts = d_counts;
-  CK(launch_exact_fallback(ep, ix->stream));
+  CK(launch_exact_fallback(ep, ix->x_elem, ix->stream));
   // pageable source: the copy above has completed its host read before returning
   ix->stats.kernel_launches += 2;
   ix->stats.fallback_queries += nf;
@@ -867,7 +885,7 @@ rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, dou
     rp.k_fetch = k_eff;
     rp.min_score = min_score;
     rp.rows = ix->rows;
-    rp.rows_f64 = ix->rows_f64;
+    rp.rows_x = ix->rows_x;
     rp.row_norm2 = ix->norm2;
     rp.slot = ix->slot;
     rp.q_f64 = ix->q_f64.p + static_cast<size_t>(s0) * ix->dim;
@@ -892,7 +910,7 @@ rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, dou
       ss.max_tiles = static_cast<int>(sort_tiles(max_cap));
     }
     int launches = 0;
-    CK(launch_large_rerank(rp, sorted ? &ss : nullptr, max_cap, ix->f64_on_host, ix->stream, &launches));
+    CK(launch_large_rerank(rp, sorted ? &ss : nullptr, max_cap, ix->rows_on_host, ix->x_elem, ix->stream, &launches));
     ix->stats.kernel_launches += launches;
   }
   return RBK_OK;
@@ -970,7 +988,7 @@ rbk_status search_graph(rbk_index* ix, const void* q_host, int elem, int B, int 
   CK(ix->h_q.ensure(q_bytes));
   rbk_index::GraphKey key;
   memset(&key, 0, sizeof key);   // compared with memcmp: padding must be defined
-  const void* ptrs[20] = {ix->rows, ix->inv_norm, ix->norm2, ix->rows_f64, ix->dead_bits, ix->d_counter, ix->q_raw.p,
+  const void* ptrs[20] = {ix->rows, ix->inv_norm, ix->norm2, ix->rows_x, ix->dead_bits, ix->d_counter, ix->q_raw.p,
                           ix->q_bf16.p, ix->q_f64.p, ix->q_norm2.p, ix->q_eps.p, ix->q_inv_norm.p, ix->thr_init.p,
                           ix->cand.p, ix->cand_cnt.p, ix->hist.p, ix->o_block.p, ix->h_block.p, ix->h_q.p, nullptr};
   memcpy(key.ptr, ptrs, sizeof ptrs);
@@ -1169,7 +1187,7 @@ rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, 
 }
 
 int64_t compact_row_bytes(const rbk_index* ix) {
-  return static_cast<int64_t>(ix->dpad) * 2 + (ix->keep_f64 ? static_cast<int64_t>(ix->dim) * 8 : 0) + 12;
+  return static_cast<int64_t>(ix->dpad) * 2 + static_cast<int64_t>(ix->x_row_bytes()) + 12;
 }
 
 rbk_status compact_alloc(rbk_index* ix, int64_t C, int64_t chunk_rows, CompactStage* st) {
@@ -1180,7 +1198,7 @@ rbk_status compact_alloc(rbk_index* ix, int64_t C, int64_t chunk_rows, CompactSt
   CK(ix->cp_scan.ensure(static_cast<size_t>(n_words + n_blocks + n_chunks + 1)));
   unsigned char* p = ix->stage.p;
   st->rows = reinterpret_cast<uint16_t*>(p);
-  st->f64 = reinterpret_cast<double*>(p + C * ix->dpad * 2);
+  st->x = p + C * ix->dpad * 2;
   st->norm2 = reinterpret_cast<double*>(p + C * (row_bytes - 12));
   st->inv = reinterpret_cast<float*>(p + C * (row_bytes - 4));
   return RBK_OK;
@@ -1200,8 +1218,8 @@ rbk_status compact_map(rbk_index* ix, int64_t chunk_rows, int* h_chunk_pref, int
 }
 
 rbk_status compact_gather(rbk_index* ix, const CompactStage& st, int64_t s0, int64_t n, int64_t rank0) {
-  CK(launch_compact_gather(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, ix->norm2, ix->inv_norm, ix->cp_map.p, s0,
-                           n, rank0, ix->dim, ix->dpad, st.rows, st.f64, st.norm2, st.inv, ix->sm_count, ix->stream));
+  CK(launch_compact_gather(ix->rows, ix->rows_x, ix->x_elem, ix->norm2, ix->inv_norm, ix->cp_map.p, s0, n, rank0,
+                           ix->dim, ix->dpad, st.rows, st.x, st.norm2, st.inv, ix->sm_count, ix->stream));
   ix->stats.kernel_launches++;
   return RBK_OK;
 }
@@ -1226,16 +1244,20 @@ void compact_commit(rbk_index* ix, int64_t n_new) {
 }
 
 uint32_t index_flags(const rbk_index* ix) {
-  return (ix->keep_f64 ? RBK_INDEX_KEEP_F64 : 0u) | (ix->f64_on_host ? RBK_INDEX_F64_ON_HOST : 0u) |
-         (ix->scan_f16 ? RBK_INDEX_SCAN_F16 : 0u);
+  return (ix->x_elem == 8 ? RBK_INDEX_KEEP_F64 : 0u) | (ix->x_elem == 4 ? RBK_INDEX_KEEP_F32 : 0u) |
+         (ix->rows_on_host ? RBK_INDEX_ROWS_ON_HOST : 0u) | (ix->scan_f16 ? RBK_INDEX_SCAN_F16 : 0u);
 }
 
 rbk_status check_flags(uint32_t flags) {
-  if (flags & ~static_cast<uint32_t>(RBK_INDEX_KEEP_F64 | RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16))
+  constexpr uint32_t kKeep = RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32;
+  if (flags & ~static_cast<uint32_t>(kKeep | RBK_INDEX_ROWS_ON_HOST | RBK_INDEX_SCAN_F16))
     return fail(RBK_EINVAL, "unknown flag");
-  if ((flags & RBK_INDEX_F64_ON_HOST) && !(flags & RBK_INDEX_KEEP_F64))
+  if ((flags & kKeep) == kKeep)
+    return fail(RBK_EINVAL, "RBK_INDEX_KEEP_F64 and RBK_INDEX_KEEP_F32 exclude each other");
+  // (either keep bit satisfies these two; the messages name the float64 one, as they always have)
+  if ((flags & RBK_INDEX_ROWS_ON_HOST) && !(flags & kKeep))
     return fail(RBK_EINVAL, "RBK_INDEX_F64_ON_HOST requires RBK_INDEX_KEEP_F64");
-  if ((flags & RBK_INDEX_SCAN_F16) && !(flags & RBK_INDEX_KEEP_F64))
+  if ((flags & RBK_INDEX_SCAN_F16) && !(flags & kKeep))
     return fail(RBK_EINVAL, "RBK_INDEX_SCAN_F16 requires RBK_INDEX_KEEP_F64");
   return RBK_OK;
 }
@@ -1243,68 +1265,85 @@ rbk_status check_flags(uint32_t flags) {
 rbk_status tier_check(const rbk_index* ix, uint32_t flags) {
   rbk_status st = check_flags(flags);
   if (st != RBK_OK) return st;
-  if (((flags & RBK_INDEX_KEEP_F64) != 0) != ix->keep_f64)
-    return fail(RBK_EINVAL, ix->keep_f64 ? "a tier change keeps the float64 rows: RBK_INDEX_KEEP_F64 cannot be dropped"
-                                         : "a tier change cannot add RBK_INDEX_KEEP_F64: this index holds no float64 rows");
+  if (((flags & (RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)) != 0) != ix->keep_rows())
+    return fail(RBK_EINVAL, ix->keep_rows()
+                                ? "a tier change keeps the exact rows: RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32 must stay"
+                                : "a tier change cannot add RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32: this index holds no "
+                                  "exact rows");
   return RBK_OK;
+}
+
+rbk_status check_f32_exact(rbk_index* ix, const double* src, bool is_device, int64_t n) {
+  if (n <= 0) return RBK_OK;
+  CK(cudaMemsetAsync(ix->d_counter, 0, sizeof(int), ix->stream));
+  if (is_device) {
+    CK(launch_find_not_f32(src, n, ix->d_counter, ix->stream));
+    ix->stats.kernel_launches++;
+  } else {
+    const int64_t chunk = std::min<int64_t>(n, (64ll << 20) / 8);
+    CK(ix->stage.ensure(static_cast<size_t>(chunk) * 8));
+    for (int64_t i0 = 0; i0 < n; i0 += chunk) {
+      const int64_t nc = std::min<int64_t>(chunk, n - i0);
+      CK(cudaMemcpyAsync(ix->stage.p, src + i0, static_cast<size_t>(nc) * 8, cudaMemcpyHostToDevice, ix->stream));
+      CK(launch_find_not_f32(reinterpret_cast<const double*>(ix->stage.p), nc, ix->d_counter, ix->stream));
+      ix->stats.kernel_launches++;
+    }
+  }
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, ix->d_counter, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+  CK(cudaStreamSynchronize(ix->stream));
+  if (bad == 0) return RBK_OK;
+  return fail(RBK_ENOTF32, "a value is not exactly a float32, which an RBK_INDEX_KEEP_F32 index stores (nothing was "
+                           "written)");
 }
 
 rbk_status tier_prepare(rbk_index* ix, uint32_t flags, TierPlan* p) {
   *p = TierPlan();
   p->flags = flags;
-  const bool host = (flags & RBK_INDEX_F64_ON_HOST) != 0;
-  p->to_host = host && !ix->f64_on_host;
-  p->to_device = !host && ix->f64_on_host;
+  p->to_host = (flags & RBK_INDEX_ROWS_ON_HOST) != 0;
+  p->x_elem = (flags & RBK_INDEX_KEEP_F32) ? 4 : 8;
+  p->move = p->to_host != ix->rows_on_host || p->x_elem != ix->x_elem;
   p->rescan = ((flags & RBK_INDEX_SCAN_F16) != 0) != ix->scan_f16;
-  p->vm_rows = ix->vm_rows;
+  p->vm_rows = tier_vm_rows(ix, !p->to_host, p->x_elem);
   // searches enqueued earlier finish on the old tier; the corpus-side bound is read once they have
   CK(cudaMemcpyAsync(&p->eps_bits, ix->d_counter + 1, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
   CK(cudaStreamSynchronize(ix->stream));
-  if (p->to_host) {
-    // the pinned rows, as realloc_host_rows allocates them
-    cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&p->host_rows), static_cast<size_t>(ix->cap) * ix->dim * 8,
-                                  cudaHostAllocMapped | cudaHostAllocPortable);
-    if (e != cudaSuccess) {
-      p->host_rows = nullptr;
-      return cuda_fail(e, "cudaHostAlloc(f64 rows on the host)");
-    }
-    void* dp = nullptr;
-    if ((e = cudaHostGetDevicePointer(&dp, p->host_rows, 0)) != cudaSuccess || dp != p->host_rows) {
-      tier_abort(ix, p);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaHostGetDevicePointer(f64 rows on the host)");
-      return fail(RBK_ECUDA, "pinned host rows are mapped at another device address (no unified addressing)");
-    }
-    // The ceiling rises: buffers 0-3 get ranges sized for the host tier's vm_rows, and their chunks are mapped there
-    // too.  Nothing is copied, and no physical memory is added.
-    p->vm_rows = tier_vm_rows(ix, false);
+  if (ix->cap > p->vm_rows)   // the ceiling falls: exact rows moving to the device, or widened there
+    return fail(RBK_ENOMEM, "a capacity of " + std::to_string(ix->cap) + " rows exceeds the " +
+                                std::to_string(p->vm_rows) + " this device can hold with these exact rows on it");
+  // narrowing: every stored slot, live or tombstoned, must hold float32-exact values (read where the rows are)
+  if (p->x_elem < ix->x_elem) {
+    rbk_status st = check_f32_exact(ix, static_cast<const double*>(ix->rows_x), true, ix->n_rows * ix->dim);
+    if (st != RBK_OK) return st;
+  }
+  if (p->move && p->to_host) {
+    rbk_status st = alloc_host_rows(static_cast<size_t>(ix->cap) * ix->dim * p->x_elem, &p->host_rows);
+    if (st != RBK_OK) return st;
+  } else if (p->move) {
     size_t want[rbk_index::kVmBuffers];
-    storage_at(ix, p->vm_rows, want, 0);
-    for (int i = 0; i < 4; ++i) {
-      if (ix->vm[i].reserved >= static_cast<size_t>(round_up(static_cast<int64_t>(want[i]),
-                                                              static_cast<int64_t>(ix->vm_gran))))
-        continue;   // an index created on the host tier, or moved there before, has the larger range already
-      rbk_status st = vm_alias(ix, ix->vm[i], want[i], &p->vm[i]);
-      if (st != RBK_OK) {
-        tier_abort(ix, p);
-        return st;
-      }
-      p->alias[i] = true;
-    }
-  } else if (p->to_device) {
-    const int64_t dev_rows = tier_vm_rows(ix, true);
-    if (ix->cap > dev_rows)
-      return fail(RBK_ENOMEM, "a capacity of " + std::to_string(ix->cap) + " rows exceeds the " +
-                                  std::to_string(dev_rows) + " this device can hold with the float64 rows on it");
-    p->vm_rows = dev_rows;
-    size_t want[rbk_index::kVmBuffers];
-    storage_at(ix, dev_rows, want, 1);
+    storage_at(ix, p->vm_rows, want, 1, p->x_elem);
     rbk_status st = vm_reserve_range(ix, want[4], &p->vm[4]);
     if (st != RBK_OK) return st;
-    storage_at(ix, ix->cap, want, 1);
+    storage_at(ix, ix->cap, want, 1, p->x_elem);
     if ((st = vm_map_to(ix, &p->vm[4], want[4])) != RBK_OK) {
       tier_abort(ix, p);
       return st;
     }
+  }
+  // A ceiling that rises gives buffers 0-3 ranges sized for it, their chunks mapped there too.  Nothing is copied, and
+  // no physical memory is added.
+  size_t want[rbk_index::kVmBuffers];
+  storage_at(ix, p->vm_rows, want, 0);
+  for (int i = 0; i < 4; ++i) {
+    if (ix->vm[i].reserved >= static_cast<size_t>(round_up(static_cast<int64_t>(want[i]),
+                                                            static_cast<int64_t>(ix->vm_gran))))
+      continue;   // an index created on a tier with this ceiling or a higher one, or moved there before
+    rbk_status st = vm_alias(ix, ix->vm[i], want[i], &p->vm[i]);
+    if (st != RBK_OK) {
+      tier_abort(ix, p);
+      return st;
+    }
+    p->alias[i] = true;
   }
   return RBK_OK;
 }
@@ -1326,7 +1365,7 @@ void tier_abort(rbk_index* ix, TierPlan* p) {
 }
 
 namespace {
-// Re-derives the scan copy of rows [0, n_rows) - tombstoned ones too - from the float64 rows with the ingest kernels,
+// Re-derives the scan copy of rows [0, n_rows) - tombstoned ones too - from the exact rows with the ingest kernels,
 // and eps_c_max as the largest angle over them.  1/||c|| stays NaN for tombstoned rows.  A bound that proves nothing (an
 // off-band or non-finite row has been stored) stays so until rbk_index_clear, whatever rows the index holds now.
 rbk_status tier_rescan(rbk_index* ix, bool f16, int eps_bits) {
@@ -1334,9 +1373,9 @@ rbk_status tier_rescan(rbk_index* ix, bool f16, int eps_bits) {
   memcpy(&eps, &eps_bits, sizeof eps);
   const int eps0 = eps >= kEpsNone ? eps_bits : 0;
   CK(cudaMemcpyAsync(ix->d_counter + 1, &eps0, sizeof(int), cudaMemcpyHostToDevice, ix->stream));   // pageable: staged
-  CK(launch_convert_rows(ix->rows_f64, 0, ix->n_rows, ix->dim, ix->dpad, ix->rows, nullptr, ix->stream, nullptr, nullptr,
-                         nullptr, f16));
-  CK(launch_row_norms(ix->rows, ix->rows_f64, 0, ix->n_rows, ix->dim, ix->dpad, ix->inv_norm, ix->norm2,
+  CK(launch_convert_rows(ix->rows_x, ix->x_elem == 4 ? 1 : 0, ix->n_rows, ix->dim, ix->dpad, ix->rows, nullptr,
+                         ix->x_elem, ix->stream, nullptr, nullptr, nullptr, f16));
+  CK(launch_row_norms(ix->rows, ix->rows_x, ix->x_elem, 0, ix->n_rows, ix->dim, ix->dpad, ix->inv_norm, ix->norm2,
                       ix->d_counter + 1, ix->stream, nullptr, ix->dead_bits, f16));
   ix->scan_f16 = f16;
   return RBK_OK;
@@ -1345,42 +1384,48 @@ rbk_status tier_rescan(rbk_index* ix, bool f16, int eps_bits) {
 
 rbk_status tier_commit(rbk_index* ix, TierPlan* p) {
   const bool f16 = (p->flags & RBK_INDEX_SCAN_F16) != 0;
-  const size_t f64_bytes = static_cast<size_t>(ix->n_rows) * ix->dim * 8;
   rbk_status st = RBK_OK;
-  if (p->rescan && !ix->f64_on_host) {   // while the f64 rows are on the device: no PCIe reads
+  if (p->rescan && !ix->rows_on_host) {   // while the exact rows are on the device: no PCIe reads
     if ((st = tier_rescan(ix, f16, p->eps_bits)) != RBK_OK) return st;
     p->rescan = false;
   }
-  if (p->to_host) {
-    if (f64_bytes) CK(cudaMemcpyAsync(p->host_rows, ix->rows_f64, f64_bytes, cudaMemcpyDeviceToHost, ix->stream));
+  if (p->move) {
+    void* dst = p->to_host ? p->host_rows : reinterpret_cast<void*>(p->vm[4].base);
+    const int64_t n_el = ix->n_rows * ix->dim;
+    if (n_el > 0 && p->x_elem == ix->x_elem)   // a move between the device and the host: UVA picks the direction
+      CK(cudaMemcpyAsync(dst, ix->rows_x, static_cast<size_t>(n_el) * ix->x_elem, cudaMemcpyDefault, ix->stream));
+    else if (n_el > 0)                         // widen or narrow on the device, reading and writing where the rows are
+      CK(launch_convert_exact(ix->rows_x, ix->x_elem, dst, p->x_elem, n_el, ix->stream));
     CK(cudaStreamSynchronize(ix->stream));
-    for (int i = 0; i < 4; ++i) {
-      if (!p->alias[i]) continue;
-      vm_drop_mapping(&ix->vm[i]);   // the old addresses; the chunks now belong to the new range
-      ix->vm[i] = std::move(p->vm[i]);
-      p->vm[i] = VmRange();
-      p->alias[i] = false;
+    if (ix->rows_on_host) {
+      cudaFreeHost(ix->rows_x);
+    } else {
+      vm_unmap_from(&ix->vm[4], 0);
+      if (ix->vm[4].reserved) vmm_api().MemAddressFree(ix->vm[4].base, ix->vm[4].reserved);
+      ix->vm[4] = VmRange();
     }
-    vm_unmap_from(&ix->vm[4], 0);
-    if (ix->vm[4].reserved) vmm_api().MemAddressFree(ix->vm[4].base, ix->vm[4].reserved);
-    ix->vm[4] = VmRange();
-    ix->rows = reinterpret_cast<uint16_t*>(ix->vm[0].base);
-    ix->inv_norm = reinterpret_cast<float*>(ix->vm[1].base);
-    ix->norm2 = reinterpret_cast<double*>(ix->vm[2].base);
-    ix->dead_bits = reinterpret_cast<unsigned int*>(ix->vm[3].base);
-    ix->rows_f64 = p->host_rows;
-    p->host_rows = nullptr;
-    ix->f64_on_host = true;
-  } else if (p->to_device) {
-    double* dev = reinterpret_cast<double*>(p->vm[4].base);
-    if (f64_bytes) CK(cudaMemcpyAsync(dev, ix->rows_f64, f64_bytes, cudaMemcpyHostToDevice, ix->stream));
-    CK(cudaStreamSynchronize(ix->stream));
-    cudaFreeHost(ix->rows_f64);
-    ix->vm[4] = std::move(p->vm[4]);
-    p->vm[4] = VmRange();
-    ix->rows_f64 = dev;
-    ix->f64_on_host = false;
+    if (p->to_host) {
+      ix->rows_x = p->host_rows;
+      p->host_rows = nullptr;
+    } else {
+      ix->vm[4] = std::move(p->vm[4]);
+      p->vm[4] = VmRange();
+      ix->rows_x = reinterpret_cast<void*>(ix->vm[4].base);
+    }
+    ix->rows_on_host = p->to_host;
+    ix->x_elem = p->x_elem;
   }
+  for (int i = 0; i < 4; ++i) {
+    if (!p->alias[i]) continue;
+    vm_drop_mapping(&ix->vm[i]);   // the old addresses; the chunks now belong to the new range
+    ix->vm[i] = std::move(p->vm[i]);
+    p->vm[i] = VmRange();
+    p->alias[i] = false;
+  }
+  ix->rows = reinterpret_cast<uint16_t*>(ix->vm[0].base);
+  ix->inv_norm = reinterpret_cast<float*>(ix->vm[1].base);
+  ix->norm2 = reinterpret_cast<double*>(ix->vm[2].base);
+  ix->dead_bits = reinterpret_cast<unsigned int*>(ix->vm[3].base);
   ix->vm_rows = p->vm_rows;
   if (p->rescan && (st = tier_rescan(ix, f16, p->eps_bits)) != RBK_OK) return st;
   CK(cudaStreamSynchronize(ix->stream));
@@ -1426,8 +1471,8 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
   // row pitch = whole 128-byte lines (64-element k-blocks): no TMA box hangs over the end of a row
   ix->dpad = static_cast<int>(round_up(dim, kBlockK));
   ix->device = device;
-  ix->keep_f64 = (flags & RBK_INDEX_KEEP_F64) != 0;
-  ix->f64_on_host = (flags & RBK_INDEX_F64_ON_HOST) != 0;
+  ix->x_elem = (flags & RBK_INDEX_KEEP_F64) ? 8 : ((flags & RBK_INDEX_KEEP_F32) ? 4 : 0);
+  ix->rows_on_host = (flags & RBK_INDEX_ROWS_ON_HOST) != 0;
   ix->scan_f16 = (flags & RBK_INDEX_SCAN_F16) != 0;
   ix->sm_count = prop.multiProcessorCount;
   memset(&ix->stats, 0, sizeof ix->stats);
@@ -1464,7 +1509,7 @@ void rbk_index_destroy(rbk_index* ix) {
     DeviceGuard dg(ix->device);
     if (ix->stream) cudaStreamSynchronize(ix->stream);
     vm_free(ix);
-    if (ix->f64_on_host) cudaFreeHost(ix->rows_f64);
+    if (ix->rows_on_host) cudaFreeHost(ix->rows_x);
     cudaFree(ix->d_counter);
     release_scratch(ix);
     if (ix->ev_start) cudaEventDestroy(ix->ev_start);
@@ -1540,6 +1585,11 @@ rbk_status rbk_index_overwrite_f64_batch(rbk_index* ix, const int64_t* slots, in
       n = static_cast<int64_t>(u_slots.size());
     }
   }
+  // float32 exact rows: every value is checked before the first slot is written
+  if (ix->x_elem == 4) {
+    rbk_status st = check_f32_exact(ix, rows, false, n * ix->dim);
+    if (st != RBK_OK) return st;
+  }
   // one H2D of the slots, one of the rows (chunked through the staging buffer), two kernels per chunk that scatter
   // into the named slots and skip tombstoned ones on the device, ONE host round trip for the whole batch
   const size_t row_bytes = static_cast<size_t>(ix->dim) * 8;
@@ -1552,11 +1602,11 @@ rbk_status rbk_index_overwrite_f64_batch(rbk_index* ix, const int64_t* slots, in
     const int64_t nr = std::min<int64_t>(chunk_rows, n - r0);
     CK(cudaMemcpyAsync(ix->stage.p, reinterpret_cast<const unsigned char*>(rows) + static_cast<size_t>(r0) * row_bytes,
                        static_cast<size_t>(nr) * row_bytes, cudaMemcpyHostToDevice, ix->stream));
-    CK(launch_convert_rows(ix->stage.p, 0, nr, ix->dim, ix->dpad, ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr,
-                           ix->stream, ix->d_slots.p + r0, ix->dead_bits, ix->d_counter, ix->scan_f16));
-    CK(launch_row_norms(ix->rows, ix->keep_f64 ? ix->rows_f64 : nullptr, 0, nr, ix->dim, ix->dpad, ix->inv_norm,
-                        ix->norm2, ix->d_counter + 1, ix->stream, ix->d_slots.p + r0, ix->dead_bits, ix->scan_f16));
-    ix->stats.kernel_launches += ix->keep_f64 ? 3 : 2;
+    CK(launch_convert_rows(ix->stage.p, 0, nr, ix->dim, ix->dpad, ix->rows, ix->rows_x, ix->x_elem, ix->stream,
+                           ix->d_slots.p + r0, ix->dead_bits, ix->d_counter, ix->scan_f16));
+    CK(launch_row_norms(ix->rows, ix->rows_x, ix->x_elem, 0, nr, ix->dim, ix->dpad, ix->inv_norm, ix->norm2,
+                        ix->d_counter + 1, ix->stream, ix->d_slots.p + r0, ix->dead_bits, ix->scan_f16));
+    ix->stats.kernel_launches += ix->keep_rows() ? 3 : 2;
   }
   int dead = 0;
   CK(cudaMemcpyAsync(&dead, ix->d_counter, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
@@ -1645,9 +1695,9 @@ rbk_status rbk_index_compact(rbk_index* ix, int64_t* old_to_new, int64_t old_to_
     if (s != RBK_OK) return s;
     CK(cudaMemcpyAsync(ix->rows + d0 * ix->dpad, st.rows, static_cast<size_t>(L) * ix->dpad * 2,
                        cudaMemcpyDeviceToDevice, ix->stream));
-    if (ix->keep_f64)   // device or mapped host rows (RBK_INDEX_F64_ON_HOST): UVA picks the direction
-      CK(cudaMemcpyAsync(ix->rows_f64 + d0 * ix->dim, st.f64, static_cast<size_t>(L) * ix->dim * 8, cudaMemcpyDefault,
-                         ix->stream));
+    if (ix->keep_rows())   // device or mapped host rows (RBK_INDEX_ROWS_ON_HOST): UVA picks the direction
+      CK(cudaMemcpyAsync(static_cast<unsigned char*>(ix->rows_x) + d0 * ix->x_row_bytes(), st.x,
+                         static_cast<size_t>(L) * ix->x_row_bytes(), cudaMemcpyDefault, ix->stream));
     CK(cudaMemcpyAsync(ix->norm2 + d0, st.norm2, static_cast<size_t>(L) * 8, cudaMemcpyDeviceToDevice, ix->stream));
     CK(cudaMemcpyAsync(ix->inv_norm + d0, st.inv, static_cast<size_t>(L) * 4, cudaMemcpyDeviceToDevice, ix->stream));
   }
@@ -1667,7 +1717,7 @@ rbk_status rbk_index_trim(rbk_index* ix) {
   // never-appended rows already, so nothing below the new capacity changes
   const int64_t tcap = round_up(std::max<int64_t>(ix->n_rows, 1024), kBlockN);
   if (tcap < ix->cap) {
-    if (ix->f64_on_host) {
+    if (ix->rows_on_host) {
       rbk_status st = realloc_host_rows(ix, tcap);
       if (st != RBK_OK) return st;
     }
@@ -1709,7 +1759,7 @@ rbk_status rbk_index_storage_bytes(const rbk_index* ix, int64_t* device_bytes, i
   int64_t dev = 0;
   for (size_t b : bytes) dev += static_cast<int64_t>(b);
   if (device_bytes) *device_bytes = dev;
-  if (pinned_host_bytes) *pinned_host_bytes = ix->f64_on_host ? ix->cap * ix->dim * 8 : 0;
+  if (pinned_host_bytes) *pinned_host_bytes = ix->rows_on_host ? ix->cap * static_cast<int64_t>(ix->x_row_bytes()) : 0;
   return RBK_OK;
 }
 
@@ -1858,7 +1908,7 @@ rbk_status rbk_index_exact_scores_f64(rbk_index* ix, const double* queries, int3
   // the prep kernel gives the f64 copy and the reference's normA; its scan-side outputs are unused here
   CK(launch_prep_queries(ix->q_raw.p, 0, B, ix->dim, ix->dpad, -INFINITY, nullptr, query_buffers(ix, 0), ix->stream,
                          /*with_norm2=*/true, nullptr, 0, 0));
-  CK(launch_exact_scores(ix->rows, ix->rows_f64, ix->norm2, ix->dead_bits, ix->n_rows, ix->dim, ix->dpad, ix->q_f64.p,
+  CK(launch_exact_scores(ix->rows, ix->rows_x, ix->x_elem, ix->norm2, ix->dead_bits, ix->n_rows, ix->dim, ix->dpad, ix->q_f64.p,
                          ix->q_norm2.p, B, ix->o_scores.p, ix->stream));
   ix->stats.kernel_launches += 2;
   CK(cudaMemcpyAsync(out_scores, ix->o_scores.p, n * 8, cudaMemcpyDeviceToHost, ix->stream));

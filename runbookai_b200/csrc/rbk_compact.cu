@@ -3,6 +3,8 @@
 // 32-row words of dead_bits into old_to_new (an exclusive prefix count of live rows), and one gather kernel per
 // staging chunk copies the live rows of that chunk, packed, into the staging buffer; the host then places each staged
 // chunk with plain device-to-device copies (rbk_capi.cu).  All of it is an HBM stream with no reuse.
+#include <type_traits>
+
 #include "rbk_internal.h"
 
 namespace rbk {
@@ -91,15 +93,16 @@ __global__ void compact_map_kernel(const unsigned int* __restrict__ dead_bits, i
 }
 
 // Every live row of source rows [s0, s0 + n) goes to staging row old_to_new[s] - d0: its bf16 row (16-byte pieces),
-// its f64 row (when the index keeps one), norm2 and inv_norm.
+// its exact row (when the index keeps one; XT = double or float, moved as is), norm2 and inv_norm.
+template <typename XT>
 __global__ void __launch_bounds__(256) compact_gather_kernel(const uint16_t* __restrict__ rows,
-                                                             const double* __restrict__ rows_f64,
+                                                             const XT* __restrict__ rows_f64,
                                                              const double* __restrict__ norm2,
                                                              const float* __restrict__ inv_norm,
                                                              const long long* __restrict__ old_to_new, int64_t s0,
                                                              int64_t n, long long d0, int d, int dpad,
                                                              uint16_t* __restrict__ st_rows,
-                                                             double* __restrict__ st_f64,
+                                                             XT* __restrict__ st_f64,
                                                              double* __restrict__ st_norm2,
                                                              float* __restrict__ st_inv) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
@@ -113,16 +116,17 @@ __global__ void __launch_bounds__(256) compact_gather_kernel(const uint16_t* __r
     reinterpret_cast<uint4*>(st_rows + (j - d0) * dpad)[u] =
         __ldg(reinterpret_cast<const uint4*>(rows + (s0 + r) * dpad) + u);
   }
+  // two elements per move: 16 bytes (double2) or 8 (float2)
+  using X2 = typename std::conditional<sizeof(XT) == 8, double2, float2>::type;
   if (rows_f64 != nullptr) {
-    if ((d & 1) == 0) {   // rows start 16-byte aligned
+    if ((d & 1) == 0) {   // rows start aligned to two elements
       const int u2 = d >> 1;
       for (int64_t g = t0; g < n * u2; g += stride) {
         const int64_t r = g / u2;
         const int u = static_cast<int>(g - r * u2);
         const long long j = old_to_new[s0 + r];
         if (j < 0) continue;
-        reinterpret_cast<double2*>(st_f64 + (j - d0) * d)[u] =
-            __ldg(reinterpret_cast<const double2*>(rows_f64 + (s0 + r) * d) + u);
+        reinterpret_cast<X2*>(st_f64 + (j - d0) * d)[u] = __ldg(reinterpret_cast<const X2*>(rows_f64 + (s0 + r) * d) + u);
       }
     } else {
       for (int64_t g = t0; g < n * d; g += stride) {
@@ -157,16 +161,22 @@ cudaError_t launch_compact_map(const unsigned int* dead_bits, int64_t n_rows, in
   return cudaGetLastError();
 }
 
-cudaError_t launch_compact_gather(const uint16_t* rows, const double* rows_f64, const double* norm2,
+cudaError_t launch_compact_gather(const uint16_t* rows, const void* rows_x, int x_elem, const double* norm2,
                                   const float* inv_norm, const long long* old_to_new, int64_t s0, int64_t n,
-                                  long long d0, int d, int dpad, uint16_t* st_rows, double* st_f64, double* st_norm2,
+                                  long long d0, int d, int dpad, uint16_t* st_rows, void* st_x, double* st_norm2,
                                   float* st_inv, int sm_count, cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
   const int64_t work = n * (dpad >> 3);
   int64_t blocks = (work + 255) / 256;
   if (blocks > static_cast<int64_t>(sm_count) * 16) blocks = static_cast<int64_t>(sm_count) * 16;   // grid-stride
-  compact_gather_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-      rows, rows_f64, norm2, inv_norm, old_to_new, s0, n, d0, d, dpad, st_rows, st_f64, st_norm2, st_inv);
+  if (x_elem == 4)
+    compact_gather_kernel<float><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        rows, static_cast<const float*>(rows_x), norm2, inv_norm, old_to_new, s0, n, d0, d, dpad, st_rows,
+        static_cast<float*>(st_x), st_norm2, st_inv);
+  else
+    compact_gather_kernel<double><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        rows, static_cast<const double*>(rows_x), norm2, inv_norm, old_to_new, s0, n, d0, d, dpad, st_rows,
+        static_cast<double*>(st_x), st_norm2, st_inv);
   return cudaGetLastError();
 }
 

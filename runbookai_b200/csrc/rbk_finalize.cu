@@ -12,6 +12,8 @@
 #include <cuda_bf16.h>
 #include <limits.h>
 
+#include <type_traits>
+
 #include "rbk_f16.cuh"
 #include "rbk_internal.h"
 #include "rbk_ptx.cuh"
@@ -41,12 +43,18 @@ __device__ __forceinline__ double exact_dot(const double* __restrict__ q, const 
   for (; i < d; ++i) dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i), bf16_to_f64(row[i])));
   return dot;
 }
-// same, f64 sidecar row
-__device__ __forceinline__ double exact_dot_f64(const double* __restrict__ q, const double* __restrict__ row, int d) {
+// same, exact-source row of float64 or float32 elements (widened on load: the same operands either way)
+template <typename XT>
+__device__ __forceinline__ double exact_dot_f64(const double* __restrict__ q, const XT* __restrict__ row, int d) {
   double dot = 0.0;
-  for (int i = 0; i < d; ++i) dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i), __ldg(row + i)));
+  for (int i = 0; i < d; ++i) dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i), static_cast<double>(__ldg(row + i))));
   return dot;
 }
+// two exact-row elements per load: 16 bytes of float64, 8 of float32
+template <typename XT>
+using Pair = typename std::conditional<sizeof(XT) == 8, double2, float2>::type;
+__device__ __forceinline__ double2 widen2(double2 v) { return v; }
+__device__ __forceinline__ double2 widen2(float2 v) { return make_double2(v.x, v.y); }
 // embedder.ts:183  dotProduct / (Math.sqrt(normA) * Math.sqrt(normB))
 __device__ __forceinline__ double exact_cosine(double dot, double na, double nb) {
   return __ddiv_rn(dot, __dmul_rn(__dsqrt_rn(na), __dsqrt_rn(nb)));
@@ -275,10 +283,11 @@ __device__ __forceinline__ void for_each_key(const unsigned long long* __restric
 // so a block needs many bytes in flight to stream: 256 threads x 8 x 16 B = 32 KB.
 constexpr int kHostLoads = 8;
 
-// kHostRows: rows_f64 is mapped host memory (RBK_INDEX_F64_ON_HOST).  Only the f64 staging differs; the device-tier
-// instantiation compiles to the same code as before the host tier existed.
-template <bool kHostRows>
-__global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p) {
+// kHostRows: rows_x is mapped host memory (RBK_INDEX_ROWS_ON_HOST).  Only the exact-row staging differs; the device-tier
+// instantiation compiles to the same code as before the host tier existed.  XT: the exact rows' element type (float
+// for RBK_INDEX_KEEP_F32), widened to double as it is staged, so the chains below see the same operands.
+template <bool kHostRows, typename XT>
+__device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
   const int ql = blockIdx.x;  // query index inside this launch
   const int tid = threadIdx.x;
   const int qb = ql / p.block_m, qrow = ql % p.block_m;
@@ -458,7 +467,7 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
   int my_row = 0;
   double dot = 0.0;
   if (tid < nsel) my_row = static_cast<int>(key_row(s_sel[tid]));
-  if (p.rows_f64 == nullptr) {
+  if (p.rows_x == nullptr) {
     int chunk = nsel > 0 ? ((p.key_cap * 8 / nsel - 16) / 2) & ~7 : kQChunk;
     chunk = chunk < kQChunk ? chunk : kQChunk;
     const int chunk16 = chunk >> 3;                                   // 16-byte units per row chunk
@@ -512,6 +521,7 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
     // exact source = f64 rows in mapped host memory: the same chunks walked in the same order, but staged with
     // 16-byte loads, kHostLoads of them in flight per thread (8-byte ones for odd d, whose rows are not all 16-byte
     // aligned).  The chunk is even so that every 16-byte piece of an even-d row starts aligned.
+    const XT* rows_x = static_cast<const XT*>(p.rows_x);
     double* s_rows64 = reinterpret_cast<double*>(s_keys);
     int chunk = nsel > 0 ? (p.key_cap / nsel - 1) : kQChunk;
     chunk = (chunk < kQChunk ? chunk : kQChunk) & ~1;
@@ -530,7 +540,7 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
             if (i < nsel * len2) {
               const int rr = i / len2, u = i - rr * len2;
               const int row = static_cast<int>(key_row(s_sel[rr]));
-              v[b] = __ldg(reinterpret_cast<const double2*>(p.rows_f64 + static_cast<size_t>(row) * p.d + c0) + u);
+              v[b] = widen2(__ldg(reinterpret_cast<const Pair<XT>*>(rows_x + static_cast<size_t>(row) * p.d + c0) + u));
             }
           }
 #pragma unroll
@@ -552,7 +562,7 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
             if (i < nsel * len) {
               const int rr = i / len, u = i - rr * len;
               const int row = static_cast<int>(key_row(s_sel[rr]));
-              v[b] = __ldg(p.rows_f64 + static_cast<size_t>(row) * p.d + c0 + u);
+              v[b] = static_cast<double>(__ldg(rows_x + static_cast<size_t>(row) * p.d + c0 + u));
             }
           }
 #pragma unroll
@@ -576,6 +586,7 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
     }
   } else {
     // exact source = the f64 sidecar: same staging, 8-byte elements (odd stride in doubles: conflict-free)
+    const XT* rows_x = static_cast<const XT*>(p.rows_x);
     double* s_rows64 = reinterpret_cast<double*>(s_keys);
     int chunk = nsel > 0 ? (p.key_cap / nsel - 1) : kQChunk;          // doubles per row chunk
     chunk = chunk < kQChunk ? chunk : kQChunk;
@@ -586,7 +597,7 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
       for (int i = tid; i < nsel * len; i += kFinThreads) {
         const int rr = i / len, u = i - rr * len;
         const int row = static_cast<int>(key_row(s_sel[rr]));
-        s_rows64[rr * row_stride + u] = __ldg(p.rows_f64 + static_cast<size_t>(row) * p.d + c0 + u);
+        s_rows64[rr * row_stride + u] = static_cast<double>(__ldg(rows_x + static_cast<size_t>(row) * p.d + c0 + u));
       }
       for (int i = tid; i < len; i += kFinThreads) s_q[i] = __ldg(qv + c0 + i);
       __syncthreads();
@@ -651,6 +662,16 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
     }
     p.flags[ql] = ok ? 0 : 1;
   }
+}
+
+// One kernel per exact-row type: float64 rows (finalize_kernel) and float32 rows (finalize_f32_kernel).
+template <bool kHostRows>
+__global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p) {
+  finalize_rows<kHostRows, double>(p);
+}
+template <bool kHostRows>
+__global__ void __launch_bounds__(kFinThreads) finalize_f32_kernel(FinalizeParams p) {
+  finalize_rows<kHostRows, float>(p);
 }
 
 // --------------------------------------------------------------------------- exact fallback (K0)
@@ -719,6 +740,7 @@ __device__ __forceinline__ void exact_push(ExactTopK& t, double sc, int row) {
   t.row[pos] = row;
 }
 
+template <typename XT>
 __global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
   __shared__ ExactTopK t;
   const int tid = threadIdx.x;
@@ -740,9 +762,9 @@ __global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
     if (row < r1) {
       const bool dead = (p.dead_bits[row >> 5] >> (row & 31)) & 1u;
       if (!dead) {   // zero-norm rows give NaN and fail the compare below, like in the reference (S3)
-        const double dot = p.rows_f64 != nullptr
-                               ? exact_dot_f64(qv, p.rows_f64 + static_cast<size_t>(row) * p.d, p.d)
-                               : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
+        const XT* rows_x = static_cast<const XT*>(p.rows_x);
+        const double dot = rows_x != nullptr ? exact_dot_f64(qv, rows_x + static_cast<size_t>(row) * p.d, p.d)
+                                             : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
         const double sc = exact_cosine(dot, na, p.row_norm2[row]);
         if (sc >= p.min_score) exact_push(t, sc, static_cast<int>(row));
       }
@@ -884,8 +906,9 @@ __global__ void __launch_bounds__(256) large_emit_all_kernel(const double* __res
 // thread then walks its own chain from there, in the same order as exact_dot_f64.
 constexpr int kLsChunk = 16;   // doubles per staged row piece (128 bytes)
 
-template <bool kHostRows>
-__global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
+template <bool kHostRows, typename XT>
+__device__ __forceinline__ void large_score_rows(const LargeRerankParams& p) {
+  const XT* rows_x = static_cast<const XT*>(p.rows_x);
   const int q = blockIdx.y;
   const int i = blockIdx.x * 256 + threadIdx.x;
   const int n = min(p.emit_cnt[q], p.emit_cap[q]);
@@ -894,8 +917,8 @@ __global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
     const size_t o = static_cast<size_t>(p.emit_off[q]) + i;
     const int row = p.emit_rows[o];
     const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
-    const double dot = p.rows_f64 != nullptr ? exact_dot_f64(qv, p.rows_f64 + static_cast<size_t>(row) * p.d, p.d)
-                                             : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
+    const double dot = rows_x != nullptr ? exact_dot_f64(qv, rows_x + static_cast<size_t>(row) * p.d, p.d)
+                                         : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
     p.cand_scores[o] = exact_cosine(dot, p.q_norm2[q], p.row_norm2[row]);
   } else {
     __shared__ double s_x[256 * (kLsChunk + 1)];   // odd pitch in doubles: conflict-free walks
@@ -922,7 +945,8 @@ __global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
             const int e = i0 + b * 256;
             if (e < m * len2) {
               const int rr = e / len2, u = e - rr * len2;
-              v[b] = __ldg(reinterpret_cast<const double2*>(p.rows_f64 + static_cast<size_t>(s_row[rr]) * p.d + c0) + u);
+              v[b] = widen2(
+                  __ldg(reinterpret_cast<const Pair<XT>*>(rows_x + static_cast<size_t>(s_row[rr]) * p.d + c0) + u));
             }
           }
 #pragma unroll
@@ -943,7 +967,7 @@ __global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
             const int e = i0 + b * 256;
             if (e < m * len) {
               const int rr = e / len, u = e - rr * len;
-              v[b] = __ldg(p.rows_f64 + static_cast<size_t>(s_row[rr]) * p.d + c0 + u);
+              v[b] = static_cast<double>(__ldg(rows_x + static_cast<size_t>(s_row[rr]) * p.d + c0 + u));
             }
           }
 #pragma unroll
@@ -965,6 +989,15 @@ __global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
     }
     if (tid < m) p.cand_scores[o] = exact_cosine(dot, p.q_norm2[q], p.row_norm2[s_row[tid]]);
   }
+}
+
+template <bool kHostRows>
+__global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
+  large_score_rows<kHostRows, double>(p);
+}
+template <bool kHostRows>
+__global__ void __launch_bounds__(256) large_score_f32_kernel(LargeRerankParams p) {
+  large_score_rows<kHostRows, float>(p);
 }
 
 // re-rank, part 2: one block per query keeps the best k_fetch of its candidates by (score desc, row asc) in a
@@ -1206,8 +1239,9 @@ __global__ void __launch_bounds__(256) seg_write_kernel(LargeRerankParams p, Seg
 // that applies `>= minScore`, the stable sort and the cut itself (vector-store.ts:212-221).  Searches for any number of
 // hits do not need it: rbk_index_search_unbounded_f64 sorts on the device and copies back only the answer, which is far
 // faster than this route's 8 bytes per row and query over PCIe plus a host sort.  Kept simple: one fp64 pass per query.
+template <typename XT>
 __global__ void __launch_bounds__(256) exact_scores_kernel(const uint16_t* __restrict__ rows,
-                                                           const double* __restrict__ rows_f64,
+                                                           const XT* __restrict__ rows_f64,
                                                            const double* __restrict__ row_norm2,
                                                            const unsigned int* __restrict__ dead_bits, int64_t n_rows,
                                                            int d, int dpad, const double* __restrict__ q_f64,
@@ -1324,36 +1358,42 @@ cudaError_t launch_prep_queries(const void* src, int src_type, int B, int d, int
   return cudaGetLastError();
 }
 
-cudaError_t launch_finalize(const FinalizeParams& p_in, bool rows_on_host, cudaStream_t stream) {
+cudaError_t launch_finalize(const FinalizeParams& p_in, bool rows_on_host, int x_elem, cudaStream_t stream) {
   if (p_in.B <= 0) return cudaSuccess;
   FinalizeParams p = p_in;
   // >= 2048 keys (16 KB: room for 128 candidate rows x 56 elements per re-rank chunk)
   p.key_cap = p.B <= 160 ? 16384 : (p.B <= 320 ? 8192 : 2048);
   const size_t smem = static_cast<size_t>(p.key_cap) * 8;
-  auto kernel = rows_on_host ? finalize_kernel<true> : finalize_kernel<false>;
+  auto kernel = x_elem == 4 ? (rows_on_host ? finalize_f32_kernel<true> : finalize_f32_kernel<false>)
+                            : (rows_on_host ? finalize_kernel<true> : finalize_kernel<false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
   if (e != cudaSuccess) return e;
   kernel<<<p.B, kFinThreads, smem, stream>>>(p);
   return cudaGetLastError();
 }
 
-cudaError_t launch_exact_fallback(const ExactParams& p, cudaStream_t stream) {
+cudaError_t launch_exact_fallback(const ExactParams& p, int x_elem, cudaStream_t stream) {
   if (p.n_fail <= 0) return cudaSuccess;
   dim3 grid(p.n_blocks, p.n_fail);
-  exact_scan_kernel<<<grid, kExThreads, 0, stream>>>(p);
+  if (x_elem == 4) exact_scan_kernel<float><<<grid, kExThreads, 0, stream>>>(p);
+  else exact_scan_kernel<double><<<grid, kExThreads, 0, stream>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   exact_merge_kernel<<<p.n_fail, kExThreads, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
-cudaError_t launch_exact_scores(const uint16_t* rows, const double* rows_f64, const double* row_norm2,
+cudaError_t launch_exact_scores(const uint16_t* rows, const void* rows_x, int x_elem, const double* row_norm2,
                                 const unsigned int* dead_bits, int64_t n_rows, int d, int dpad, const double* q_f64,
                                 const double* q_norm2, int B, double* out, cudaStream_t stream) {
   if (B <= 0 || n_rows <= 0) return cudaSuccess;
   dim3 grid(static_cast<unsigned>((n_rows + 255) / 256), static_cast<unsigned>(B));
-  exact_scores_kernel<<<grid, 256, 0, stream>>>(rows, rows_f64, row_norm2, dead_bits, n_rows, d, dpad, q_f64, q_norm2,
-                                                out);
+  if (x_elem == 4)
+    exact_scores_kernel<float><<<grid, 256, 0, stream>>>(rows, static_cast<const float*>(rows_x), row_norm2, dead_bits,
+                                                         n_rows, d, dpad, q_f64, q_norm2, out);
+  else
+    exact_scores_kernel<double><<<grid, 256, 0, stream>>>(rows, static_cast<const double*>(rows_x), row_norm2,
+                                                          dead_bits, n_rows, d, dpad, q_f64, q_norm2, out);
   return cudaGetLastError();
 }
 
@@ -1374,14 +1414,19 @@ cudaError_t launch_large_emit_all(const double* q_eps, const unsigned int* dead_
 }
 
 cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
-                                bool rows_on_host, cudaStream_t stream, int* launches) {
+                                bool rows_on_host, int x_elem, cudaStream_t stream, int* launches) {
   *launches = 0;
   if (p.B <= 0) return cudaSuccess;
   cudaError_t e;
   if (max_cap > 0) {
     dim3 grid(static_cast<unsigned>((max_cap + 255) / 256), static_cast<unsigned>(p.B));
-    if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
-    else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);
+    if (x_elem == 4) {
+      if (rows_on_host) large_score_f32_kernel<true><<<grid, 256, 0, stream>>>(p);
+      else large_score_f32_kernel<false><<<grid, 256, 0, stream>>>(p);
+    } else {
+      if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
+      else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);
+    }
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
   }

@@ -105,11 +105,24 @@ inline void locate(const rbk_group* g, int64_t slot, int* dev, int64_t* local) {
   *local = (blk / g->G) * g->block + slot % g->block;
 }
 
+// RBK_ENOTF32 if the group keeps float32 rows and any of the n rows is not float32-exact (checked on member 0).
+rbk_status group_check_f32(rbk_group* g, const double* rows, int64_t n) {
+  rbk_index* ix = g->parts[0];
+  if (ix->x_elem != 4) return RBK_OK;
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  return check_f32_exact(ix, rows, false, n * g->dim);
+}
+
 rbk_status group_append(rbk_group* g, const void* rows, int elem, int64_t n, int64_t* first_out) {
   if (!g) return fail(RBK_EINVAL, "null group");
   if (n < 0 || (n > 0 && !rows)) return fail(RBK_EINVAL, "bad rows argument");
   std::lock_guard<std::mutex> lk(g->mu);
   if (first_out) *first_out = g->n_slots;
+  if (elem == 8) {   // every row of the call, whichever member it would go to, before any member writes
+    rbk_status st = group_check_f32(g, static_cast<const double*>(rows), n);
+    if (st != RBK_OK) return st;
+  }
   const size_t row_bytes = static_cast<size_t>(g->dim) * elem;
   int64_t done = 0;
   while (done < n) {
@@ -508,9 +521,10 @@ rbk_status group_compact(rbk_group* g, int64_t* old_to_new, int64_t old_to_new_l
         // device, peer or mapped host rows (RBK_INDEX_F64_ON_HOST): UVA picks the direction
         CK(cudaMemcpyAsync(ix->rows + s.dst_row * ix->dpad, ss.rows + s.src_off * ix->dpad,
                            static_cast<size_t>(s.len) * ix->dpad * 2, cudaMemcpyDefault, ix->stream));
-        if (ix->keep_f64)
-          CK(cudaMemcpyAsync(ix->rows_f64 + s.dst_row * ix->dim, ss.f64 + s.src_off * ix->dim,
-                             static_cast<size_t>(s.len) * ix->dim * 8, cudaMemcpyDefault, ix->stream));
+        if (ix->keep_rows())   // moved as bytes, x_row_bytes() per row
+          CK(cudaMemcpyAsync(static_cast<unsigned char*>(ix->rows_x) + s.dst_row * ix->x_row_bytes(),
+                             static_cast<const unsigned char*>(ss.x) + s.src_off * ix->x_row_bytes(),
+                             static_cast<size_t>(s.len) * ix->x_row_bytes(), cudaMemcpyDefault, ix->stream));
         CK(cudaMemcpyAsync(ix->norm2 + s.dst_row, ss.norm2 + s.src_off, static_cast<size_t>(s.len) * 8,
                            cudaMemcpyDefault, ix->stream));
         CK(cudaMemcpyAsync(ix->inv_norm + s.dst_row, ss.inv + s.src_off, static_cast<size_t>(s.len) * 4,
@@ -650,9 +664,10 @@ rbk_status rbk_group_overwrite_f64_batch(rbk_group* g, const int64_t* slots, int
   std::lock_guard<std::mutex> lk(g->mu);
   for (int64_t i = 0; i < n; ++i)
     if (slots[i] < 0 || slots[i] >= g->n_slots) return fail(RBK_EINVAL, "slot out of range");
+  rbk_status worst = group_check_f32(g, rows, n);   // no member writes if any row is refused
+  if (worst != RBK_OK) return worst;
   std::vector<std::vector<int64_t>> local, order;
   split_slots(g, slots, n, &local, &order);
-  rbk_status worst = RBK_OK;
   std::string msg;
   for (int d = 0; d < g->G; ++d) {
     if (local[d].empty()) continue;

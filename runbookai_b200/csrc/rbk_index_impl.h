@@ -154,14 +154,19 @@ struct rbk_index {
   uint16_t* rows = nullptr;
   float* inv_norm = nullptr;  // padded to a multiple of kBlockN (+ one tile), NaN-filled
   double* norm2 = nullptr;
-  double* rows_f64 = nullptr;   // optional exact-source sidecar [cap][dim] (RBK_INDEX_KEEP_F64)
-  bool keep_f64 = false;
-  // RBK_INDEX_F64_ON_HOST: rows_f64 is pinned, mapped host memory (one pointer under UVA).  Every write to it is
+  // optional exact-source rows [cap][dim] of x_elem bytes each: float64 (RBK_INDEX_KEEP_F64, x_elem 8) or float32
+  // (RBK_INDEX_KEEP_F32, x_elem 4; every stored value is float32-exact, so its widening is the float64 row); x_elem 0:
+  // none
+  void* rows_x = nullptr;
+  int x_elem = 0;
+  bool keep_rows() const { return x_elem != 0; }
+  size_t x_row_bytes() const { return static_cast<size_t>(dim) * x_elem; }
+  // RBK_INDEX_ROWS_ON_HOST: rows_x is pinned, mapped host memory (one pointer under UVA).  Every write to it is
   // stream-ordered: a kernel or copy on `stream`, or the host after a synchronisation of `stream`.
-  bool f64_on_host = false;
+  bool rows_on_host = false;
   // RBK_INDEX_SCAN_F16: `rows` (and the queries' scan copies) hold per-row scaled fp16 instead of bf16, and the scan
-  // runs its fp16 instantiation (rbk_scan_f16.cu).  Requires keep_f64, so nothing ever decodes these rows as values
-  // except the norm kernels: the re-rank, the fallback and the exact scores read rows_f64.
+  // runs its fp16 instantiation (rbk_scan_f16.cu).  Requires exact rows, so nothing ever decodes these rows as values
+  // except the norm kernels: the re-rank, the fallback and the exact scores read rows_x.
   bool scan_f16 = false;
   unsigned int* dead_bits = nullptr;
   int* d_counter = nullptr;   // [0] tombstone counter, [1] eps_c_max (float bits)
@@ -273,11 +278,11 @@ rbk_status large_finish(rbk_index* ix);
 rbk_status large_check(rbk_index* ix);
 
 // The steps of a compaction, shared by rbk_index_compact and rbk_group_compact (caller holds ix->mu and has the index's
-// device current).  Staging of C rows, packed: bf16 (or fp16) rows [C][dpad] | f64 rows [C][dim] (KEEP_F64) | norm2 [C]
-// | inv_norm [C].
+// device current).  Staging of C rows, packed: bf16 (or fp16) rows [C][dpad] | exact rows [C][dim] (x_elem bytes each,
+// when kept) | norm2 [C] | inv_norm [C].
 struct CompactStage {
   uint16_t* rows;
-  double* f64;
+  void* x;
   double* norm2;
   float* inv;
 };
@@ -298,29 +303,36 @@ void compact_commit(rbk_index* ix, int64_t n_new);
 
 // The steps of a storage tier change, shared by rbk_index_set_tier and rbk_group_set_tier (caller holds ix->mu and has
 // the index's device current).  tier_prepare makes every allocation the change needs and changes nothing the index
-// shows: the pinned rows and the larger address ranges, their physical chunks mapped there a second time (device to
-// host), or the device f64 range, mapped for cap rows (host to device).  Then exactly one of tier_abort, which releases
-// what tier_prepare made, or tier_commit, which moves the rows, re-derives the scan copy when its type changes, and drops
-// every cache keyed on the old tier or the old pointers.  A tier_commit that fails (a CUDA error only) leaves what it
-// has not yet taken over in the plan, for tier_abort; the index itself may then be part-way changed.
+// shows, and checks that a narrowing (float64 to float32 exact rows) changes no stored value (RBK_ENOTF32 otherwise): the
+// new exact-row buffer when the rows move or change width - pinned [cap][dim], or a device range mapped for cap rows -
+// and, when the row ceiling rises, larger address ranges for buffers 0-3 with their physical chunks mapped there a
+// second time.  Then exactly one of tier_abort, which releases what tier_prepare made, or tier_commit, which moves (or
+// widens / narrows) the rows, re-derives the scan copy when its type changes, and drops every cache keyed on the old
+// tier or the old pointers.  A tier_commit that fails (a CUDA error only) leaves what it has not yet taken over in the
+// plan, for tier_abort; the index itself may then be part-way changed.
 struct TierPlan {
   uint32_t flags = 0;
-  bool to_host = false, to_device = false, rescan = false;
+  bool move = false, to_host = false, rescan = false;   // move: the exact rows go to a new buffer (to_host: pinned)
+  int x_elem = 0;                       // the new exact-row width
   int64_t vm_rows = 0;                  // the ceiling of the new tier
-  double* host_rows = nullptr;          // to_host: the pinned [cap][dim] buffer
+  void* host_rows = nullptr;            // move && to_host: the pinned [cap][dim] buffer
   bool alias[rbk_index::kVmBuffers] = {};
-  VmRange vm[rbk_index::kVmBuffers];    // to_host: buffers 0-3 re-reserved (where alias[i]); to_device: buffer 4
+  VmRange vm[rbk_index::kVmBuffers];    // buffers 0-3 re-reserved (where alias[i]); move to the device: buffer 4
   int eps_bits = 0;                     // eps_c_max before the change (float bits)
 };
 uint32_t index_flags(const rbk_index* ix);
 // RBK_EINVAL for a flag set rbk_index_create_ex refuses (check_flags, which it shares), or one the index cannot move to
-// (the KEEP_F64 bit must stay; group membership is the caller's).
+// (an index with exact rows keeps one of the keep bits, one without gets none; group membership is the caller's).
 rbk_status check_flags(uint32_t flags);
 rbk_status tier_check(const rbk_index* ix, uint32_t flags);
 rbk_status tier_prepare(rbk_index* ix, uint32_t flags, TierPlan* p);
 void tier_abort(rbk_index* ix, TierPlan* p);
 rbk_status tier_commit(rbk_index* ix, TierPlan* p);
 const char* last_error();
+// RBK_ENOTF32 (with its message) if any of the n doubles at src - host memory (staged through ix->stage) or, with
+// is_device, device memory - is not float32-exact (launch_find_not_f32); changes nothing in the index.  Caller holds
+// ix->mu and has the index's device current.
+rbk_status check_f32_exact(rbk_index* ix, const double* src, bool is_device, int64_t n);
 
 }  // namespace impl
 }  // namespace rbk

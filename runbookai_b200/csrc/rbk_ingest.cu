@@ -25,11 +25,13 @@ __device__ __forceinline__ uint16_t f32_to_bf16_bits(float x) {
   return __bfloat16_as_ushort(__float2bfloat16_rn(x));
 }
 
-// One thread produces 8 consecutive output elements (one 16-byte store).
-template <typename SrcT>
+// One thread produces 8 consecutive output elements (one 16-byte store).  XT: element type of the exact rows (double,
+// or float for RBK_INDEX_KEEP_F32, whose sources hold float32-exact values: the scan copy is derived from the source
+// value, which equals the stored one).
+template <typename SrcT, typename XT>
 __global__ void __launch_bounds__(256) convert_rows_kernel(const SrcT* __restrict__ src, int64_t n_rows, int d,
                                                            int dpad, uint16_t* __restrict__ dst,
-                                                           double* __restrict__ dst_f64, bool aligned,
+                                                           XT* __restrict__ dst_f64, bool aligned,
                                                            const int64_t* __restrict__ slot_map,
                                                            const unsigned int* __restrict__ dead_bits,
                                                            int* __restrict__ n_dead) {
@@ -99,7 +101,7 @@ __global__ void __launch_bounds__(256) convert_rows_kernel(const SrcT* __restric
           if constexpr (sizeof(SrcT) == 8) x = static_cast<double>(s[j]);
           else if constexpr (sizeof(SrcT) == 4) x = static_cast<double>(static_cast<float>(s[j]));
           else x = static_cast<double>(__uint_as_float(static_cast<uint32_t>(s[j]) << 16));
-          dst_f64[row * d + c0 + j] = x;
+          dst_f64[row * d + c0 + j] = static_cast<XT>(x);
         }
       }
     }
@@ -125,10 +127,10 @@ __device__ __forceinline__ double src_to_f64(SrcT v) {   // exact widening of ev
 // (dst_f64 null: the source IS the sidecar, when a tier change re-derives the scan copy from it).
 // Same slot_map / dead_bits / n_dead contract as convert_rows_kernel.
 constexpr int kF16ConvThreads = 256;
-template <typename SrcT>
+template <typename SrcT, typename XT>
 __global__ void __launch_bounds__(kF16ConvThreads) convert_rows_f16_kernel(
     const SrcT* __restrict__ src, int64_t n_rows, int d, int dpad, uint16_t* __restrict__ dst,
-    double* __restrict__ dst_f64, const int64_t* __restrict__ slot_map, const unsigned int* __restrict__ dead_bits,
+    XT* __restrict__ dst_f64, const int64_t* __restrict__ slot_map, const unsigned int* __restrict__ dead_bits,
     int* __restrict__ n_dead) {
   const int lane = threadIdx.x & 31;
   const int64_t warps = static_cast<int64_t>(gridDim.x) * (kF16ConvThreads / 32);
@@ -158,7 +160,7 @@ __global__ void __launch_bounds__(kF16ConvThreads) convert_rows_f16_kernel(
         o[j] = 0;
         if (c0 + j < d) {
           const double x = src_to_f64(s[c0 + j]);
-          if (dst_f64 != nullptr) dst_f64[row * d + c0 + j] = x;
+          if (dst_f64 != nullptr) dst_f64[row * d + c0 + j] = static_cast<XT>(x);
           o[j] = f16_bits_flush(scale_pow2(x, e));
         }
       }
@@ -284,6 +286,7 @@ __global__ void __launch_bounds__(kNormRows) row_norms_kernel(const uint16_t* __
 // (x * 2^e - h: the same angle).  The row's liveness in the scan must stay what a bf16 index gives it, so that both
 // tiers answer alike: a row whose bf16 rounding has a zero or non-finite norm (elements past float32's range, or all of
 // them below bf16's) gets the NaN inv_norm and the corpus angle such a row gets in a bf16 index.
+// XT: element type of the exact rows (float for RBK_INDEX_KEEP_F32), widened to double as it is staged.
 constexpr int kNorm64Chunk = 32;        // doubles per staged chunk (256 B per row)
 constexpr int kNorm64Pitch = kNorm64Chunk + 1;
 
@@ -297,9 +300,9 @@ __device__ __forceinline__ float angle_bound(double diff2, double n2) {
   return eps;
 }
 
-template <bool kF16>
+template <bool kF16, typename XT>
 __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t* __restrict__ rows_base,
-                                                                  const double* __restrict__ rows_f64_base,
+                                                                  const XT* __restrict__ rows_f64_base,
                                                                   const int64_t* __restrict__ slot_map,
                                                                   const unsigned int* __restrict__ dead_bits,
                                                                   int64_t first_row, int64_t n_items, int d, int dpad,
@@ -330,7 +333,7 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
       for (int i = tid; i < kNormRows * len; i += kNormRows) {
         const int rr = i / len, el = i - rr * len;
         const long long row = s_row[rr];
-        s_x[rr * kNorm64Pitch + el] = row >= 0 ? __ldg(rows_f64_base + row * d + c0 + el) : 0.0;
+        s_x[rr * kNorm64Pitch + el] = row >= 0 ? static_cast<double>(__ldg(rows_f64_base + row * d + c0 + el)) : 0.0;
       }
       __syncthreads();
       if (my_row >= 0)
@@ -354,7 +357,7 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
       double x = 0.0;
       uint16_t bq = 0;
       if (row >= 0) {
-        x = __ldg(rows_f64_base + row * d + c0 + el);
+        x = static_cast<double>(__ldg(rows_f64_base + row * d + c0 + el));
         bq = __ldg(rows_base + row * dpad + c0 + el);
       }
       s_x[rr * kNorm64Pitch + el] = x;
@@ -417,6 +420,25 @@ __global__ void tombstone_kernel(const int64_t* __restrict__ slots, int64_t n, i
   }
 }
 
+__global__ void __launch_bounds__(256) find_not_f32_kernel(const double* __restrict__ src, int64_t n,
+                                                           int* __restrict__ found) {
+  bool bad = false;
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const double x = src[i];
+    bad |= x == x && static_cast<double>(__double2float_rn(x)) != x;
+  }
+  if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) *found = 1;
+}
+
+template <typename SrcT, typename DstT>
+__global__ void __launch_bounds__(256) convert_exact_kernel(const SrcT* __restrict__ src, DstT* __restrict__ dst,
+                                                            int64_t n) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    dst[i] = static_cast<DstT>(src[i]);
+}
+
 int grid_for(int64_t items, int threads, int max_blocks) {
   int64_t b = (items + threads - 1) / threads;
   if (b < 1) b = 1;
@@ -426,10 +448,11 @@ int grid_for(int64_t items, int threads, int max_blocks) {
 
 }  // namespace
 
-cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, int d, int dpad, uint16_t* dst_rows,
-                                double* dst_f64, cudaStream_t stream, const int64_t* slot_map,
-                                const unsigned int* dead_bits, int* n_dead, bool f16) {
-  if (n_rows <= 0) return cudaSuccess;
+namespace {
+template <typename XT>
+cudaError_t convert_rows_typed(const void* src, int src_type, int64_t n_rows, int d, int dpad, uint16_t* dst_rows,
+                               XT* dst_x, cudaStream_t stream, const int64_t* slot_map, const unsigned int* dead_bits,
+                               int* n_dead, bool f16) {
   if (f16) {
     constexpr int rows_per_block = kF16ConvThreads / 32;
     int dev = 0, sms = 0;
@@ -438,14 +461,14 @@ cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, i
     if (e != cudaSuccess) return e;
     const int grid = grid_for(n_rows, rows_per_block, sms * 8);
     if (src_type == 0)
-      convert_rows_f16_kernel<double><<<grid, kF16ConvThreads, 0, stream>>>(
-          static_cast<const double*>(src), n_rows, d, dpad, dst_rows, dst_f64, slot_map, dead_bits, n_dead);
+      convert_rows_f16_kernel<double, XT><<<grid, kF16ConvThreads, 0, stream>>>(
+          static_cast<const double*>(src), n_rows, d, dpad, dst_rows, dst_x, slot_map, dead_bits, n_dead);
     else if (src_type == 1)
-      convert_rows_f16_kernel<float><<<grid, kF16ConvThreads, 0, stream>>>(
-          static_cast<const float*>(src), n_rows, d, dpad, dst_rows, dst_f64, slot_map, dead_bits, n_dead);
+      convert_rows_f16_kernel<float, XT><<<grid, kF16ConvThreads, 0, stream>>>(
+          static_cast<const float*>(src), n_rows, d, dpad, dst_rows, dst_x, slot_map, dead_bits, n_dead);
     else
-      convert_rows_f16_kernel<uint16_t><<<grid, kF16ConvThreads, 0, stream>>>(
-          static_cast<const uint16_t*>(src), n_rows, d, dpad, dst_rows, dst_f64, slot_map, dead_bits, n_dead);
+      convert_rows_f16_kernel<uint16_t, XT><<<grid, kF16ConvThreads, 0, stream>>>(
+          static_cast<const uint16_t*>(src), n_rows, d, dpad, dst_rows, dst_x, slot_map, dead_bits, n_dead);
     return cudaGetLastError();
   }
   const int64_t total = n_rows * (dpad >> 3);
@@ -457,25 +480,39 @@ cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, i
   // vector loads need d % 8 == 0 (every 8-group starts 16-byte aligned) and an aligned base
   const bool aligned = (d & 7) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
   if (src_type == 0)
-    convert_rows_kernel<double><<<grid, 256, 0, stream>>>(static_cast<const double*>(src), n_rows, d, dpad, dst_rows,
-                                                          dst_f64, aligned, slot_map, dead_bits, n_dead);
+    convert_rows_kernel<double, XT><<<grid, 256, 0, stream>>>(static_cast<const double*>(src), n_rows, d, dpad,
+                                                              dst_rows, dst_x, aligned, slot_map, dead_bits, n_dead);
   else if (src_type == 1)
-    convert_rows_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const float*>(src), n_rows, d, dpad, dst_rows,
-                                                         dst_f64, aligned, slot_map, dead_bits, n_dead);
+    convert_rows_kernel<float, XT><<<grid, 256, 0, stream>>>(static_cast<const float*>(src), n_rows, d, dpad,
+                                                             dst_rows, dst_x, aligned, slot_map, dead_bits, n_dead);
   else
-    convert_rows_kernel<uint16_t><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(src), n_rows, d, dpad,
-                                                            dst_rows, dst_f64, aligned, slot_map, dead_bits, n_dead);
+    convert_rows_kernel<uint16_t, XT><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(src), n_rows, d, dpad,
+                                                                dst_rows, dst_x, aligned, slot_map, dead_bits, n_dead);
   return cudaGetLastError();
 }
+}  // namespace
 
-cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_base, int64_t first_row, int64_t n_items,
-                             int d, int dpad, float* inv_norm_base, double* norm2_base, int* eps_c_max,
+cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, int d, int dpad, uint16_t* dst_rows,
+                                void* dst_x, int x_elem, cudaStream_t stream, const int64_t* slot_map,
+                                const unsigned int* dead_bits, int* n_dead, bool f16) {
+  if (n_rows <= 0) return cudaSuccess;
+  if (x_elem == 4)
+    return convert_rows_typed(src, src_type, n_rows, d, dpad, dst_rows, static_cast<float*>(dst_x), stream, slot_map,
+                              dead_bits, n_dead, f16);
+  return convert_rows_typed(src, src_type, n_rows, d, dpad, dst_rows, static_cast<double*>(dst_x), stream, slot_map,
+                            dead_bits, n_dead, f16);
+}
+
+cudaError_t launch_row_norms(const uint16_t* rows_base, const void* rows_x_base, int x_elem, int64_t first_row,
+                             int64_t n_items, int d, int dpad, float* inv_norm_base, double* norm2_base, int* eps_c_max,
                              cudaStream_t stream, const int64_t* slot_map, const unsigned int* dead_bits, bool f16) {
   if (n_items <= 0) return cudaSuccess;
-  if (f16 && rows_f64_base == nullptr) return cudaErrorInvalidValue;   // the fp16 tier always keeps the f64 rows
-  // dead_bits without slot_map (a tier change): the f64 kernel folds every row's angle in, tombstoned or not
-  if (!slot_map && dead_bits && rows_f64_base == nullptr) return cudaErrorInvalidValue;
+  if (f16 && rows_x_base == nullptr) return cudaErrorInvalidValue;   // the fp16 tier always keeps the exact rows
+  // dead_bits without slot_map (a tier change): the exact-row kernel folds every row's angle in, tombstoned or not
+  if (!slot_map && dead_bits && rows_x_base == nullptr) return cudaErrorInvalidValue;
   const unsigned blocks = static_cast<unsigned>((n_items + kNormRows - 1) / kNormRows);
+  // the bf16 kernel only tests rows_f64_base for null
+  const double* rows_f64_base = static_cast<const double*>(rows_x_base);
   if (f16)
     row_norms_kernel<true><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits, first_row,
                                                              n_items, d, dpad, inv_norm_base, norm2_base, eps_c_max);
@@ -483,15 +520,53 @@ cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_b
     row_norms_kernel<false><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits, first_row,
                                                               n_items, d, dpad, inv_norm_base, norm2_base, eps_c_max);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess || rows_f64_base == nullptr) return e;
-  if (f16)
-    row_norms_f64_kernel<true><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits,
-                                                                 first_row, n_items, d, dpad, norm2_base, inv_norm_base,
-                                                                 eps_c_max);
+  if (e != cudaSuccess || rows_x_base == nullptr) return e;
+  const float* rows_f32_base = static_cast<const float*>(rows_x_base);
+  if (f16 && x_elem == 4)
+    row_norms_f64_kernel<true, float><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f32_base, slot_map, dead_bits,
+                                                                        first_row, n_items, d, dpad, norm2_base,
+                                                                        inv_norm_base, eps_c_max);
+  else if (f16)
+    row_norms_f64_kernel<true, double><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits,
+                                                                         first_row, n_items, d, dpad, norm2_base,
+                                                                         inv_norm_base, eps_c_max);
+  else if (x_elem == 4)
+    row_norms_f64_kernel<false, float><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f32_base, slot_map, dead_bits,
+                                                                         first_row, n_items, d, dpad, norm2_base,
+                                                                         inv_norm_base, eps_c_max);
   else
-    row_norms_f64_kernel<false><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map, dead_bits,
-                                                                  first_row, n_items, d, dpad, norm2_base,
-                                                                  inv_norm_base, eps_c_max);
+    row_norms_f64_kernel<false, double><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f64_base, slot_map,
+                                                                          dead_bits, first_row, n_items, d, dpad,
+                                                                          norm2_base, inv_norm_base, eps_c_max);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_find_not_f32(const double* src, int64_t n, int* found, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  int dev = 0, sms = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) return e;
+  find_not_f32_kernel<<<grid_for(n, 256, sms * 16), 256, 0, stream>>>(src, n, found);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_convert_exact(const void* src, int src_elem, void* dst, int dst_elem, int64_t n,
+                                 cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  int dev = 0, sms = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) return e;
+  const int grid = grid_for(n, 256, sms * 16);
+  if (src_elem == 8 && dst_elem == 4)
+    convert_exact_kernel<double, float><<<grid, 256, 0, stream>>>(static_cast<const double*>(src),
+                                                                  static_cast<float*>(dst), n);
+  else if (src_elem == 4 && dst_elem == 8)
+    convert_exact_kernel<float, double><<<grid, 256, 0, stream>>>(static_cast<const float*>(src),
+                                                                  static_cast<double*>(dst), n);
+  else
+    return cudaErrorInvalidValue;
   return cudaGetLastError();
 }
 

@@ -65,28 +65,42 @@ cudaError_t launch_scan_large_f16(const CUtensorMap& tmap_q, const CUtensorMap& 
                                   LargeScanMode mode, cudaStream_t stream);
 
 // ---- ingest (rbk_ingest.cu) ----
+// The exact-source rows of an index that keeps them (RBK_INDEX_KEEP_F64 / RBK_INDEX_KEEP_F32) are [cap][d] elements of
+// x_elem bytes: 8 = float64, 4 = float32.  Every kernel that reads them widens each element to float64 on load and
+// then runs the same operations in the same order, so a float32 row of float32-exact values gives the same bits as
+// the float64 row.
 // src element type: 0 = f64, 1 = f32, 2 = bf16 bits.  src is device memory, row pitch = d.
-// dst_f64 (nullable): exact-source sidecar rows, pitch d.
-// slot_map (nullable, bulk overwrite): dst_rows / dst_f64 are the index's row 0 and source row r lands in row
+// dst_x (nullable): exact-source rows (x_elem bytes per element, pitch d); a float32 destination takes only sources
+// whose values are float32-exact (launch_find_not_f32 checks that first).
+// slot_map (nullable, bulk overwrite): dst_rows / dst_x are the index's row 0 and source row r lands in row
 // slot_map[r]; rows whose slot is tombstoned (dead_bits) are skipped and counted in *n_dead.
-// f16: store the rows by the RBK_INDEX_SCAN_F16 rule (rbk_f16.cuh) instead of as bf16.  dst_f64 null with f16 only
-// when src is the index's own f64 rows (a tier change re-deriving the scan copy).
+// f16: store the rows by the RBK_INDEX_SCAN_F16 rule (rbk_f16.cuh) instead of as bf16.  dst_x null with f16 only
+// when src is the index's own exact rows (a tier change re-deriving the scan copy).
 cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, int d, int dpad,
-                                uint16_t* dst_rows, double* dst_f64, cudaStream_t stream,
+                                uint16_t* dst_rows, void* dst_x, int x_elem, cudaStream_t stream,
                                 const int64_t* slot_map = nullptr, const unsigned int* dead_bits = nullptr,
                                 int* n_dead = nullptr, bool f16 = false);
 // Norms of rows [first_row, first_row + n_items) of the index (or, with slot_map, of rows slot_map[i]; tombstoned
-// ones skipped).  All array arguments are the index's BASE pointers.  rows_f64_base (nullable): when given,
-// norm2 comes from it and the bf16-vs-f64 angle bound is max-ed into *eps_c_max (float bits in an int).
-// f16: the rows are RBK_INDEX_SCAN_F16 fp16 rows (rows_f64_base required); the angle is that of their rounding.
-// dead_bits without slot_map (rows_f64_base required; a tier change re-deriving every stored row): every row's norm2
+// ones skipped).  All array arguments are the index's BASE pointers.  rows_x_base (nullable, x_elem bytes per
+// element): when given, norm2 comes from it and the bf16-vs-exact angle bound is max-ed into *eps_c_max (float bits
+// in an int).
+// f16: the rows are RBK_INDEX_SCAN_F16 fp16 rows (rows_x_base required); the angle is that of their rounding.
+// dead_bits without slot_map (rows_x_base required; a tier change re-deriving every stored row): every row's norm2
 // and angle are computed, but a tombstoned row's inv_norm stays NaN.
-cudaError_t launch_row_norms(const uint16_t* rows_base, const double* rows_f64_base, int64_t first_row,
+cudaError_t launch_row_norms(const uint16_t* rows_base, const void* rows_x_base, int x_elem, int64_t first_row,
                              int64_t n_items, int d, int dpad, float* inv_norm_base, double* norm2_base,
                              int* eps_c_max, cudaStream_t stream, const int64_t* slot_map = nullptr,
                              const unsigned int* dead_bits = nullptr, bool f16 = false);
 cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows, float* inv_norm,
                              unsigned int* dead_bits, int* n_killed, cudaStream_t stream);
+// *found = 1 if any of the n doubles at src (device or mapped host memory) is one a float32 cannot hold (else *found is
+// left as it is): x is accepted iff it is NaN or (double)(float)x == x (so +-0, +-inf and float32 subnormals are, 0.1
+// and 1e-300 are not).
+cudaError_t launch_find_not_f32(const double* src, int64_t n, int* found, cudaStream_t stream);
+// dst[i] = src[i] for n elements, from src_elem to dst_elem bytes (8 <-> 4; a float64 -> float32 copy only of values
+// launch_find_not_f32 accepted): a tier change that widens or narrows the exact rows.
+cudaError_t launch_convert_exact(const void* src, int src_elem, void* dst, int dst_elem, int64_t n,
+                                 cudaStream_t stream);
 
 // ---- compaction (rbk_compact.cu) ----
 // old_to_new [n_rows] (new local slot, -1 = tombstoned) from dead_bits by a two-level exclusive scan over the 32-row
@@ -95,10 +109,10 @@ cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows
 cudaError_t launch_compact_map(const unsigned int* dead_bits, int64_t n_rows, int64_t chunk_rows, int* word_pref,
                                int* block_sum, long long* old_to_new, int* chunk_pref, cudaStream_t stream);
 // Packs the live rows among source rows [s0, s0 + n) into staging row old_to_new[s] - d0: bf16 row (pitch dpad),
-// f64 row (pitch d; skipped when rows_f64 is null), norm2, inv_norm.
-cudaError_t launch_compact_gather(const uint16_t* rows, const double* rows_f64, const double* norm2,
+// exact row (x_elem bytes per element, pitch d; skipped when rows_x is null), norm2, inv_norm.
+cudaError_t launch_compact_gather(const uint16_t* rows, const void* rows_x, int x_elem, const double* norm2,
                                   const float* inv_norm, const long long* old_to_new, int64_t s0, int64_t n,
-                                  long long d0, int d, int dpad, uint16_t* st_rows, double* st_f64, double* st_norm2,
+                                  long long d0, int d, int dpad, uint16_t* st_rows, void* st_x, double* st_norm2,
                                   float* st_inv, int sm_count, cudaStream_t stream);
 
 // ---- query preparation + finalize + exhaustive fallback + shard merge (rbk_finalize.cu) ----
@@ -142,7 +156,7 @@ struct FinalizeParams {
   int q0;  // global index of the first query of this launch (sub-batch offset)
   double min_score;
   const uint16_t* rows;
-  const double* rows_f64;   // nullable: exact-source sidecar (pitch d); the re-rank reads it instead of `rows`
+  const void* rows_x;       // nullable: exact-source rows (pitch d, x_elem of the launch); the re-rank reads them
   const double* row_norm2;
   int64_t n_rows;
   SlotLayout slot;
@@ -152,9 +166,10 @@ struct FinalizeParams {
   int* out_counts;        // [B]
   int* flags;             // [B] 1 = not provably exact -> exhaustive fallback
 };
-// rows_on_host: rows_f64 is mapped host memory (RBK_INDEX_F64_ON_HOST); the re-rank stages it with wide loads, more
-// of them in flight, to cover the PCIe round trip.  Same scores either way.
-cudaError_t launch_finalize(const FinalizeParams& p, bool rows_on_host, cudaStream_t stream);
+// rows_on_host: rows_x is mapped host memory (RBK_INDEX_ROWS_ON_HOST); the re-rank stages it with wide loads, more
+// of them in flight, to cover the PCIe round trip.  Same scores either way.  x_elem: bytes per exact-row element (8 or
+// 4; ignored when rows_x is null), here and in every launcher below that takes it.
+cudaError_t launch_finalize(const FinalizeParams& p, bool rows_on_host, int x_elem, cudaStream_t stream);
 
 struct ExactParams {
   const int* fail_list;  // [n_fail] query indices
@@ -162,7 +177,7 @@ struct ExactParams {
   int d, dpad, k_fetch;
   double min_score;
   const uint16_t* rows;
-  const double* rows_f64;   // nullable: exact-source sidecar
+  const void* rows_x;       // nullable: exact-source rows
   const double* row_norm2;
   const unsigned int* dead_bits;  // tombstones
   int64_t n_rows;
@@ -177,7 +192,7 @@ struct ExactParams {
   double* out_scores;
   int* out_counts;
 };
-cudaError_t launch_exact_fallback(const ExactParams& p, cudaStream_t stream);
+cudaError_t launch_exact_fallback(const ExactParams& p, int x_elem, cudaStream_t stream);
 
 // ---- large-k search (rbk_finalize.cu): select between the two scan passes, exact re-rank after them ----
 // theta [B] (raw domain) and cap [B] (C_q) from the count pass's histograms hist [B][kHistBins].
@@ -192,7 +207,7 @@ struct LargeRerankParams {
   int B, d, dpad, k_fetch;
   double min_score;
   const uint16_t* rows;
-  const double* rows_f64;   // nullable: exact-source sidecar
+  const void* rows_x;       // nullable: exact-source rows
   const double* row_norm2;
   SlotLayout slot;
   const double* q_f64;      // offset to the sub-batch, like every per-query array below
@@ -227,10 +242,10 @@ struct SegSortScratch {
 // launch_finalize; the scoring kernel then stages its candidates' rows in shared memory with coalesced loads.
 // *launches: kernels enqueued.
 cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
-                                bool rows_on_host, cudaStream_t stream, int* launches);
+                                bool rows_on_host, int x_elem, cudaStream_t stream, int* launches);
 
 // Exact fp64 cosine of every row for B prepared queries: out [B][n_rows], NaN = tombstoned / zero row.
-cudaError_t launch_exact_scores(const uint16_t* rows, const double* rows_f64, const double* row_norm2,
+cudaError_t launch_exact_scores(const uint16_t* rows, const void* rows_x, int x_elem, const double* row_norm2,
                                 const unsigned int* dead_bits, int64_t n_rows, int d, int dpad, const double* q_f64,
                                 const double* q_norm2, int B, double* out, cudaStream_t stream);
 

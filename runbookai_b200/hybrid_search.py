@@ -33,7 +33,8 @@ def reciprocal_rank_fusion(fts_results: Sequence[RetrievedChunk], vector_results
 
 
 class HybridRetriever:
-    def __init__(self, config: dict, fts_store=None, device: int | None = None, scan_f16: bool | None = None):
+    def __init__(self, config: dict, fts_store=None, device: int | None = None, scan_f16: bool | None = None,
+                 exact_rows: str | None = None):
         """hybrid-search.ts:27-42."""
         self.config = {"ftsWeight": 0.4, "vectorWeight": 0.6, "rrf_k": 60}
         self.config.update({k: v for k, v in config.items() if v is not None})
@@ -45,7 +46,7 @@ class HybridRetriever:
         if _emb.is_embedder_configured():
             vector_path = config.get("vectorStorePath") or config["storePath"].replace(".db", "_vectors.db", 1)
             self.vector_store = create_vector_store(vector_path.replace("/vectors.db", "", 1), device,
-                                                    scan_f16=scan_f16)  # :39-40 quirk
+                                                    scan_f16=scan_f16, exact_rows=exact_rows)  # :39-40 quirk
 
     def has_vector_search(self) -> bool:
         return self.vector_store is not None and _emb.is_embedder_configured()   # :47-49

@@ -37,10 +37,12 @@ def _bucket(chunks) -> dict:
 
 
 class KnowledgeRetriever:
-    def __init__(self, config: dict, device: int | None = None, vector_store=None, scan_f16: bool | None = None):
+    def __init__(self, config: dict, device: int | None = None, vector_store=None, scan_f16: bool | None = None,
+                 exact_rows: str | None = None):
         """config: {storePath, sources: [callable(since) -> iterable of documents], vectorStorePath?}
         (retriever/index.ts:19-39).  scan_f16: the vector store's scan precision (see VectorStore; None:
-        RUNBOOK_KNN_SCAN_F16)."""
+        RUNBOOK_KNN_SCAN_F16).  exact_rows: the vector store's exact-row width (see VectorStore; None:
+        RUNBOOK_KNN_EXACT_ROWS)."""
         self.config = config
         d = os.path.dirname(config["storePath"])
         if d:
@@ -52,7 +54,8 @@ class KnowledgeRetriever:
             self._hybrid = HybridRetriever({"storePath": config["storePath"],
                                             "vectorStorePath": config.get("vectorStorePath")
                                             or os.path.join(d or ".", "vectors.db")},
-                                           fts_store=self.store, device=device, scan_f16=scan_f16)
+                                           fts_store=self.store, device=device, scan_f16=scan_f16,
+                                           exact_rows=exact_rows)
             if vector_store is not None:       # tests inject a store built on the CPU stand-in index
                 if self._hybrid.vector_store is not None:
                     self._hybrid.vector_store.close()

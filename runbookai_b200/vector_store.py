@@ -42,7 +42,8 @@ from typing import Sequence
 import numpy as np
 
 from . import embedder as _emb
-from ._native import RBK_EDIM, RBK_INDEX_F64_ON_HOST, RBK_INDEX_SCAN_F16, RBK_MAX_K_FETCH, DimensionError, Index
+from ._native import (RBK_EDIM, RBK_ENOTF32, RBK_INDEX_F64_ON_HOST, RBK_INDEX_SCAN_F16, RBK_MAX_K_FETCH, DimensionError,
+                      Index, RbkError, exact_rows_of)
 
 SCHEMA = """
       CREATE TABLE IF NOT EXISTS vector_embeddings (
@@ -135,7 +136,7 @@ def shared_index_count() -> int:
 
 class VectorStore:
     def __init__(self, db_path: str, device: int | None = None, index_factory=None, shared: bool = False,
-                 f64_on_host: bool | None = None, scan_f16: bool | None = None):
+                 f64_on_host: bool | None = None, scan_f16: bool | None = None, exact_rows: str | None = None):
         # index_factory(dim, device) -> object with the _native.Index surface; tests inject a
         # CPU stand-in to exercise the host logic where there is no GPU
         # keep_f64: the reference stores float64 embeddings; keep them so the re-rank is exact for any input.
@@ -145,6 +146,14 @@ class VectorStore:
         # scan_f16 (None: RUNBOOK_KNN_SCAN_F16=1 enables): the scan reads per-row scaled fp16 rows instead of bf16 - the
         # same answers and bytes, a tighter error bound, so fewer batches need the wide retry.  A shared index keeps the
         # setting of the instance that created it, until set_tier().
+        # exact_rows (None: RUNBOOK_KNN_EXACT_ROWS, default "f64"): "f32" keeps the exact rows as float32 - the same
+        # answers at half their bytes, for embeddings whose values are all float32-exact.  An append or overwrite the
+        # index refuses (a value no float32 holds) widens the index to float64 in place and is repeated once, so this
+        # store accepts every embedding a default one does; exact_rows then reports "f64".
+        if exact_rows is None:
+            exact_rows = os.environ.get("RUNBOOK_KNN_EXACT_ROWS", "f64")
+        if exact_rows not in ("f64", "f32"):
+            raise ValueError(f"exact_rows must be 'f64' or 'f32', not {exact_rows!r}")
         if f64_on_host is None:
             f64_on_host = os.environ.get("RUNBOOK_KNN_F64_ON_HOST", "0") == "1"
         if scan_f16 is None:
@@ -152,9 +161,11 @@ class VectorStore:
         # what this instance asks for; the index, once there is one, reports its own tier (f64_on_host / scan_f16)
         self._want_f64_on_host = bool(f64_on_host)
         self._want_scan_f16 = bool(scan_f16)
+        self._want_exact_rows = exact_rows
         self._index_factory = index_factory or (
-            lambda dim, dev: Index(dim, device=dev, keep_f64=True, f64_on_host=self._want_f64_on_host,
-                                   scan_f16=self._want_scan_f16))
+            lambda dim, dev: Index(dim, device=dev, **({"keep_f64": True} if self._want_exact_rows == "f64"
+                                                       else {"keep_f32": True}),
+                                   f64_on_host=self._want_f64_on_host, scan_f16=self._want_scan_f16))
         # one connection, usable from the micro-batcher's worker thread too; serialised by a lock
         self.db = sqlite3.connect(db_path, check_same_thread=False)
         self.db.row_factory = sqlite3.Row
@@ -235,6 +246,26 @@ class VectorStore:
         """Whether the scan reads fp16 rows: the index's tier once there is one, else what this instance asked for."""
         flags = self._index_flags()
         return self._want_scan_f16 if flags is None else bool(flags & RBK_INDEX_SCAN_F16)
+
+    @property
+    def exact_rows(self) -> str:
+        """'f64' or 'f32': what the index keeps its exact rows as once there is one (an "f32" store that met a
+        non-float32 embedding has widened to "f64"), else what this instance asked for."""
+        flags = self._index_flags()
+        kept = None if flags is None else exact_rows_of(flags)
+        return self._want_exact_rows if kept is None else kept
+
+    def _exact_call(self, fn, *args):
+        """fn(*args) on the index; a float32 index that refuses a value (RBK_ENOTF32, nothing written) is widened to
+        float64 in place and the call repeated once.  The caller holds the state lock."""
+        try:
+            return fn(*args)
+        except RbkError as e:
+            if e.status != RBK_ENOTF32:
+                raise
+        self._index.set_tier(exact_rows="f64")
+        self._want_exact_rows = "f64"
+        return fn(*args)
 
     def set_tier(self, f64_on_host: bool | None = None, scan_f16: bool | None = None) -> None:
         """Change the storage tier of the index in place, from the float64 rows it already holds (no reload from
@@ -324,7 +355,7 @@ class VectorStore:
             ix = self._ensure_index(dim)
             step = max(1, (64 << 20) // (dim * 8))
             for r0 in range(0, n, step):
-                first = ix.append_f64(mm[r0:r0 + step])          # straight from the page cache to the device
+                first = self._exact_call(ix.append_f64, mm[r0:r0 + step])   # straight from the page cache to the device
                 if first != r0:
                     raise RuntimeError("slot numbering out of step while loading the sidecar")
             for i, vid in enumerate(ids):
@@ -405,7 +436,7 @@ class VectorStore:
         step = max(1, (32 << 20) // (dim * 8))
         for r0 in range(0, len(good), step):
             blob = b"".join(r["embedding"] for r in good[r0:r0 + step])
-            first = ix.append_f64(np.frombuffer(blob, dtype="<f8").reshape(-1, dim))
+            first = self._exact_call(ix.append_f64, np.frombuffer(blob, dtype="<f8").reshape(-1, dim))
             for i, r in enumerate(good[r0:r0 + step]):   # the slot the ENGINE assigned, not a private count
                 while len(self._ids) < first + i:
                     self._ids.append(None)
@@ -430,9 +461,9 @@ class VectorStore:
             return
         self._st.bad_ids.discard(vid)
         if slot is not None:
-            ix.overwrite_f64(slot, e)     # existing key keeps its Map position (S9b)
+            self._exact_call(ix.overwrite_f64, slot, e)     # existing key keeps its Map position (S9b)
         else:
-            self._slot_of[vid] = ix.append_f64(e[None, :])
+            self._slot_of[vid] = self._exact_call(ix.append_f64, e[None, :])
             self._ids.append(vid)
 
     _INSERT = """
@@ -501,9 +532,10 @@ class VectorStore:
             last[v] = e
         again = [v for v in last if v in self._slot_of]
         if again:
-            ix.overwrite_f64_batch([self._slot_of[v] for v in again], np.stack([last[v] for v in again]))
+            self._exact_call(ix.overwrite_f64_batch, [self._slot_of[v] for v in again],
+                             np.stack([last[v] for v in again]))
         if fresh:
-            first = ix.append_f64(np.stack([last[v] for v in fresh]))
+            first = self._exact_call(ix.append_f64, np.stack([last[v] for v in fresh]))
             for i, v in enumerate(fresh):
                 self._slot_of[v] = first + i
                 while len(self._ids) < first + i:
@@ -677,13 +709,15 @@ class VectorStore:
 
 
 def create_vector_store(base_dir: str = ".runbook", device: int | None = None, index_factory=None,
-                        shared: bool | None = None, scan_f16: bool | None = None) -> VectorStore:
+                        shared: bool | None = None, scan_f16: bool | None = None,
+                        exact_rows: str | None = None) -> VectorStore:
     """vector-store.ts:338-341.  shared (default on; RUNBOOK_KNN_SHARED_INDEX=0 turns it off): call sites
     that build and close a store per use attach to the process-wide index of that db instead of re-uploading.
-    scan_f16: see VectorStore (None: RUNBOOK_KNN_SCAN_F16)."""
+    scan_f16, exact_rows: see VectorStore (None: RUNBOOK_KNN_SCAN_F16, RUNBOOK_KNN_EXACT_ROWS)."""
     if shared is None:
         shared = os.environ.get("RUNBOOK_KNN_SHARED_INDEX", "1") != "0"
-    return VectorStore(f"{base_dir}/vectors.db", device, index_factory, shared=shared, scan_f16=scan_f16)
+    return VectorStore(f"{base_dir}/vectors.db", device, index_factory, shared=shared, scan_f16=scan_f16,
+                       exact_rows=exact_rows)
 
 
 createVectorStore = create_vector_store

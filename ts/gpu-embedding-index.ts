@@ -43,6 +43,14 @@ function scanF16FromEnv(): number {
   return process.env.RUNBOOK_KNN_SCAN_F16 === '1' ? 1 : 0;
 }
 
+/**
+ * RUNBOOK_KNN_EXACT_ROWS="f32" keeps the exact rows as float32 instead of float64 (RBK_INDEX_KEEP_F32): the same answers
+ * at half the exact-row bytes while every embedding value is a float32.  The addon reads the variable itself when its
+ * constructor gets no `exactRows` argument, and widens the index to float64 in place (repeating the call) the first
+ * time an append or overwrite holds a value no float32 can hold, so no embedding is ever refused.
+ */
+export type ExactRows = 'f64' | 'f32';
+
 export class GpuEmbeddingIndex {
   private index: any | null = null;
   private idOfSlot: (string | null)[] = [];
@@ -247,17 +255,19 @@ export class GpuEmbeddingIndex {
   /**
    * Change the storage tier of the loaded index in place (rbk_index_set_tier / rbk_group_set_tier): `f64OnHost` moves
    * the float64 rows between the GPU and pinned host memory, `scanF16` switches the scan between bf16 and fp16.  An
-   * omitted key keeps its setting.  Answers and slots do not change, so nothing is remapped; the native call waits
+   * omitted key keeps its setting; `exactRows` widens ('f64') or narrows ('f32', refused unless every stored value is a
+   * float32) the exact rows.  Answers and slots do not change, so nothing is remapped; the native call waits
    * for the index's queued device work itself.  Nothing is automatic: an append that throws for lack of device memory
    * is the caller's to retry after `setTier({ f64OnHost: true })`.  Throws (with the index unchanged) if the new tier
    * cannot be backed, and against a library built before tier changes.
    */
-  setTier(tier: { f64OnHost?: boolean; scanF16?: boolean }): void {
+  setTier(tier: { f64OnHost?: boolean; scanF16?: boolean; exactRows?: ExactRows }): void {
     this.index?.setTier(tier);
   }
 
-  /** Where the float64 rows live and which scan runs, as they are now; null before the first row is loaded. */
-  get tier(): { f64OnHost: boolean; scanF16: boolean } | null {
+  /** Where the exact rows live, which scan runs and the exact rows' width, as they are now; null before the first row
+   * is loaded. */
+  get tier(): { f64OnHost: boolean; scanF16: boolean; exactRows: ExactRows } | null {
     return this.index ? this.index.tier : null;
   }
 
