@@ -56,7 +56,7 @@ typedef enum {
   RBK_ECUDA = 3,  /* CUDA runtime/driver error, or no device */
   RBK_ENCCL = 4,  /* NCCL missing or failing (rbk_group_* with more than one GPU) */
   RBK_EDIM = 5,   /* "Vectors must have the same length" (embedder.ts:169-171) */
-  RBK_ENOTF32 = 6 /* a value is not exactly a float32 (only RBK_INDEX_KEEP_F32 indexes and groups return it) */
+  RBK_ENOTF32 = 6 /* a value is not exactly a float32 (only RBK_INDEX_KEEP_F32 and RBK_INDEX_KEEP_F32_SPLIT indexes and groups return it) */
 } rbk_status;
 
 int rbk_abi_version(void);
@@ -132,10 +132,27 @@ rbk_status rbk_index_create(int32_t dim, int32_t device, int64_t capacity_hint, 
  * not on the scaled copy).  The placement is fixed until rbk_index_set_tier; read the stored bits with
  * rbk_index_read_rows_f16. */
 #define RBK_INDEX_SCAN_F16 16u
+/* RBK_INDEX_KEEP_F32_SPLIT (a keep bit: exclusive with RBK_INDEX_KEEP_F64, RBK_INDEX_KEEP_F32 and RBK_INDEX_SCAN_F16, all
+ * RBK_EINVAL; combines with RBK_INDEX_ROWS_ON_HOST): keeps float32 exact rows like RBK_INDEX_KEEP_F32, with the same
+ * accepted values, the same checks and the same RBK_ENOTF32 contract, but stores each float32 only once.  Its high 16
+ * bits live in the bf16 scan copy, which is rounded for that purpose, and only the low 16 bits are kept beside it: the
+ * exact rows cost 2*dim bytes per row instead of 4*dim.  For a float32 with bits u the scan copy is (u + 0x8000) >> 16
+ * (bf16 rounded to nearest with ties away from zero, on the magnitude; a NaN becomes the bf16 NaN 0x7FFF), the low half
+ * is u & 0xFFFF, and u = ((s - (r >> 15)) << 16) | r rebuilds the value exactly (a NaN stays a NaN, its payload may be
+ * lost).  With RBK_INDEX_ROWS_ON_HOST only the low halves move to pinned, mapped host memory (2*dim bytes per row); the
+ * scan copy stays on the device.
+ * The contract: fed the same calls, a split index gives the answers of a KEEP_F32 index with the same placement - slots,
+ * fp64 scores, counts, -1 / NaN tails, compaction maps, RBK_ENOTF32 refusals with the index untouched, and the scan-band
+ * rule.  Where no stored value has a low half of exactly 0x8000 (a tie, where ties-away and ties-to-even round apart) it
+ * also has the same stored scan bits, corpus-side bound, debug scores, exactness flags, retry and fallback decisions and
+ * stats counters; otherwise only those decision-side outputs may differ.  rbk_index_read_rows_bf16 returns the scan
+ * copy.  At d = 1536: 6,156 device bytes per row on the device tier (9,228 with KEEP_F32), and 3,072 pinned host bytes
+ * per row with RBK_INDEX_ROWS_ON_HOST (6,144 with KEEP_F32); the row ceiling and rbk_index_storage_bytes count them. */
+#define RBK_INDEX_KEEP_F32_SPLIT 128u
 rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hint, uint32_t flags, rbk_index** out);
 void rbk_index_destroy(rbk_index* idx); /* NULL is a no-op */
-/* The index's creation flags as they are now (RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32 | RBK_INDEX_F64_ON_HOST |
- * RBK_INDEX_SCAN_F16); 0 for NULL. */
+/* The index's creation flags as they are now (RBK_INDEX_KEEP_F64, RBK_INDEX_KEEP_F32 or RBK_INDEX_KEEP_F32_SPLIT |
+ * RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16); 0 for NULL. */
 uint32_t rbk_index_flags(const rbk_index* idx);
 /* Change the storage tier of an index with exact rows in place, from the rows it holds: move them between the device
  * and pinned host memory (RBK_INDEX_F64_ON_HOST), switch the scan between bf16 and fp16 (RBK_INDEX_SCAN_F16), and keep
@@ -146,6 +163,9 @@ uint32_t rbk_index_flags(const rbk_index* idx);
  *     every stored slot [0, size()), live or tombstoned, holds float32-exact values (the rule of RBK_INDEX_KEEP_F32);
  *     otherwise it returns RBK_ENOTF32, checked before anything changes.  Either way the new exact-row buffer is
  *     allocated and filled before the old one is released: peak memory is the old plus the new exact rows.
+ *     RBK_INDEX_KEEP_F32_SPLIT takes part in every such change, in and out, the same way (narrowing from KEEP_F64 is
+ *     checked the same way); entering or leaving it also rewrites the scan copy under the target's rounding and
+ *     recomputes the norms and the corpus-side bound, like a change of scan type.
  *   - The current flags are a no-op (RBK_OK).  The member indexes of a group refuse the call (RBK_EINVAL):
  *     rbk_group_set_tier changes them together.
  *   - Every answer stays bit for bit: slots, fp64 scores, counts, -1 / NaN tails, exactness flags, compaction maps; so

@@ -13,7 +13,7 @@
 //   const ix = new RbkIndex(dim, device, capacityHint)          // one GPU  (rbk_index_*)
 //   const ix = new RbkIndex(dim, [0, 1, 2, 3], capacityHint)    // several GPUs behind one handle (rbk_group_*)
 //   const ix = new RbkIndex(dim, device, capacityHint, hostRows) // hostRows != 0: exact rows in pinned host RAM
-//   const ix = new RbkIndex(dim, device, capacityHint, hostRows, scanF16, exactRows)   // exactRows 'f64' | 'f32'
+//   const ix = new RbkIndex(dim, device, capacityHint, hostRows, scanF16, exactRows)   // exactRows 'f64' | 'f32' | 'f32_split'
 //                                              // (absent: RUNBOOK_KNN_EXACT_ROWS, else 'f64')
 //   ix.appendF64(Float64Array rows)            -> firstSlot
 //   ix.appendBlobs(Buffer[] blobs)             -> firstSlot     // SQLite f64-LE BLOBs, packed in C++: no JS copies
@@ -23,8 +23,9 @@
 //   ix.trim()                                  // give unused device memory back (after compact / clear)
 //   ix.setTier({ f64OnHost, scanF16, exactRows })   // move the exact rows / switch the scan / widen or narrow them in
 //                                              // place (omitted: kept)
-//   ix.tier                                    -> { f64OnHost: boolean, scanF16: boolean, exactRows: 'f64' | 'f32' }
-//   With exactRows 'f32', an append or overwrite holding a value no float32 can hold (RBK_ENOTF32, nothing written)
+//   ix.tier                                    -> { f64OnHost: boolean, scanF16: boolean, exactRows: 'f64' | 'f32' | 'f32_split' }
+//   With exactRows 'f32' or 'f32_split', an append or overwrite holding a value no float32 can hold (RBK_ENOTF32,
+//   nothing written)
 //   widens the index to 'f64' in place and is repeated once, so the addon accepts every embedding a default index does.
 //   await ix.search(Float64Array queries, B, kFetch, minScore)
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
@@ -93,7 +94,8 @@ struct Handle {
   rbk_status widening(F&& call) {
     rbk_status st = call();
     if (st != RBK_ENOTF32 || !has_tier()) return st;
-    if ((st = set_tier((flags() & ~RBK_INDEX_KEEP_F32) | RBK_INDEX_KEEP_F64)) != RBK_OK) return st;
+    if ((st = set_tier((flags() & ~(RBK_INDEX_KEEP_F32 | RBK_INDEX_KEEP_F32_SPLIT)) | RBK_INDEX_KEEP_F64)) != RBK_OK)
+      return st;
     return call();
   }
   rbk_status append_f64(const double* rows, int64_t n, int64_t* first) {
@@ -157,9 +159,10 @@ void finalize_index(napi_env, void* data, void*) {
   delete h;
 }
 
-// 'f64' / 'f32' -> the keep bit; anything else -> 0.
+// 'f64' / 'f32' / 'f32_split' -> the keep bit; anything else -> 0.
 uint32_t keep_bit(const std::string& s) {
-  return s == "f64" ? RBK_INDEX_KEEP_F64 : (s == "f32" ? RBK_INDEX_KEEP_F32 : 0u);
+  return s == "f64" ? RBK_INDEX_KEEP_F64
+                    : (s == "f32" ? RBK_INDEX_KEEP_F32 : (s == "f32_split" ? RBK_INDEX_KEEP_F32_SPLIT : 0u));
 }
 
 // A JS string (at most 15 bytes are needed here); false if v is not a string.
@@ -181,7 +184,8 @@ napi_value New(napi_env env, napi_callback_info info) {
   if (argc > 2) napi_get_value_int64(env, argv[2], &hint);
   if (argc > 3) napi_get_value_int32(env, argv[3], &host_rows);
   if (argc > 4) napi_get_value_int32(env, argv[4], &scan_f16);
-  // exactRows (RUNBOOK_KNN_EXACT_ROWS when absent): 'f64' keeps the exact rows as float64, 'f32' as float32
+  // exactRows (RUNBOOK_KNN_EXACT_ROWS when absent): 'f64' keeps the exact rows as float64, 'f32' as float32,
+  // 'f32_split' as float32 split into the scan copy and low halves (the refusal names the two plain widths)
   std::string exact_rows;
   if (argc > 5) {
     if (!get_string(env, argv[5], &exact_rows)) exact_rows = "?";
@@ -377,7 +381,7 @@ bool require_tier(napi_env env, Handle* h) {
 }
 
 // setTier({ f64OnHost, scanF16, exactRows }): rbk_index_set_tier / rbk_group_set_tier.  A key that is absent keeps its
-// setting; f64OnHost / scanF16 must be booleans, exactRows 'f64' or 'f32'.  Synchronous; answers do not change.
+// setting; f64OnHost / scanF16 must be booleans, exactRows 'f64', 'f32' or 'f32_split'.  Synchronous; answers do not change.
 napi_value SetTier(napi_env env, napi_callback_info info) {
   size_t argc = 1;
   napi_value argv[1] = {nullptr};
@@ -415,7 +419,7 @@ napi_value SetTier(napi_env env, napi_callback_info info) {
       napi_throw_type_error(env, nullptr, "setTier: exactRows must be 'f64' or 'f32'");
       return nullptr;
     }
-    flags = (flags & ~(RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)) | keep;
+    flags = (flags & ~(RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32 | RBK_INDEX_KEEP_F32_SPLIT)) | keep;
   }
   if (h->set_tier(flags) != RBK_OK) return throw_rbk(env);
   return nullptr;
@@ -435,7 +439,8 @@ napi_value GetTier(napi_env env, napi_callback_info info) {
   NAPI_OK(napi_set_named_property(env, out, "f64OnHost", host));
   NAPI_OK(napi_set_named_property(env, out, "scanF16", f16));
   napi_value rows;
-  NAPI_OK(napi_create_string_utf8(env, (flags & RBK_INDEX_KEEP_F32) ? "f32" : "f64", NAPI_AUTO_LENGTH, &rows));
+  const char* kept = (flags & RBK_INDEX_KEEP_F32) ? "f32" : ((flags & RBK_INDEX_KEEP_F32_SPLIT) ? "f32_split" : "f64");
+  NAPI_OK(napi_create_string_utf8(env, kept, NAPI_AUTO_LENGTH, &rows));
   NAPI_OK(napi_set_named_property(env, out, "exactRows", rows));
   return out;
 }

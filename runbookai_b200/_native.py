@@ -19,6 +19,7 @@ RBK_INDEX_KEEP_F64 = 1
 RBK_INDEX_F64_ON_HOST = 2
 RBK_INDEX_ROWS_ON_HOST = RBK_INDEX_F64_ON_HOST
 RBK_INDEX_KEEP_F32 = 64
+RBK_INDEX_KEEP_F32_SPLIT = 128
 RBK_INDEX_SCAN_F16 = 16
 
 # every symbol include/rbk_knn.h declares (tests check the .so exports all of them)
@@ -155,20 +156,27 @@ def ptr(a: np.ndarray | None):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
-def _index_flags(keep_f64: bool, f64_on_host: bool, scan_f16: bool = False, keep_f32: bool = False) -> int:
-    """f64_on_host or scan_f16 without a keep bit, or both keep bits, are passed through: the library rejects them
+def _index_flags(keep_f64: bool, f64_on_host: bool, scan_f16: bool = False, keep_f32: bool = False,
+                 keep_f32_split: bool = False) -> int:
+    """f64_on_host or scan_f16 without a keep bit, or several keep bits, are passed through: the library rejects them
     with its own message."""
     return ((RBK_INDEX_KEEP_F64 if keep_f64 else 0) | (RBK_INDEX_KEEP_F32 if keep_f32 else 0)
+            | (RBK_INDEX_KEEP_F32_SPLIT if keep_f32_split else 0)
             | (RBK_INDEX_F64_ON_HOST if f64_on_host else 0) | (RBK_INDEX_SCAN_F16 if scan_f16 else 0))
 
 
-_EXACT_ROWS = {"f64": RBK_INDEX_KEEP_F64, "f32": RBK_INDEX_KEEP_F32}
+_EXACT_ROWS = {"f64": RBK_INDEX_KEEP_F64, "f32": RBK_INDEX_KEEP_F32, "f32_split": RBK_INDEX_KEEP_F32_SPLIT}
+_KEEP_BITS = RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32 | RBK_INDEX_KEEP_F32_SPLIT
 
 
 def exact_rows_of(flags: int) -> str | None:
-    """'f64' / 'f32' for an index keeping float64 / float32 exact rows, None for one without."""
+    """'f64' / 'f32' / 'f32_split' for an index keeping float64 / float32 / split float32 exact rows, None for one
+    without."""
     flags = int(flags)
-    return "f64" if flags & RBK_INDEX_KEEP_F64 else ("f32" if flags & RBK_INDEX_KEEP_F32 else None)
+    for name, bit in _EXACT_ROWS.items():
+        if flags & bit:
+            return name
+    return None
 
 
 def _tier_flags(current: int, f64_on_host, scan_f16, exact_rows=None) -> int:
@@ -177,8 +185,8 @@ def _tier_flags(current: int, f64_on_host, scan_f16, exact_rows=None) -> int:
     flags = int(current)
     if exact_rows is not None:
         if exact_rows not in _EXACT_ROWS:
-            raise ValueError(f"exact_rows must be 'f64', 'f32' or None, not {exact_rows!r}")
-        flags = (flags & ~(RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)) | _EXACT_ROWS[exact_rows]
+            raise ValueError(f"exact_rows must be 'f64', 'f32', 'f32_split' or None, not {exact_rows!r}")
+        flags = (flags & ~_KEEP_BITS) | _EXACT_ROWS[exact_rows]
     for value, bit, name in ((f64_on_host, RBK_INDEX_F64_ON_HOST, "f64_on_host"),
                              (scan_f16, RBK_INDEX_SCAN_F16, "scan_f16")):
         if value is None:
@@ -236,11 +244,15 @@ class Index:
     """Thin object wrapper over rbk_index* (one GPU shard)."""
 
     def __init__(self, dim: int, device: int = 0, capacity_hint: int = 0, keep_f64: bool = False,
-                 f64_on_host: bool = False, scan_f16: bool = False, keep_f32: bool = False):
+                 f64_on_host: bool = False, scan_f16: bool = False, keep_f32: bool = False,
+                 keep_f32_split: bool = False):
         """keep_f64: RBK_INDEX_KEEP_F64 — exact for arbitrary float64 rows at 8*dim extra bytes per row.
         keep_f32: RBK_INDEX_KEEP_F32 — the same answers from float32 exact rows at 4*dim bytes per row, for rows whose
         values are all float32-exact; append_f64 / overwrite of any other value raise NotFloat32Error with nothing
         written.  Excludes keep_f64.
+        keep_f32_split: RBK_INDEX_KEEP_F32_SPLIT — the answers of keep_f32 at 2*dim bytes per row: the bf16 scan copy
+        holds each float32's high half and only the low halves are kept beside it.  Same values accepted, same
+        NotFloat32Error.  Excludes keep_f64, keep_f32 and scan_f16.
         f64_on_host: RBK_INDEX_F64_ON_HOST (RBK_INDEX_ROWS_ON_HOST) — those exact rows live in pinned host memory
         instead of on the GPU (same answers; the re-rank reads them over PCIe).  Requires keep_f64 or keep_f32.
         scan_f16: RBK_INDEX_SCAN_F16 — the scan reads per-row scaled fp16 rows instead of bf16 (same bytes, same
@@ -248,7 +260,8 @@ class Index:
         self._h = None
         h = C.c_void_p()
         check(lib.rbk_index_create_ex(dim, device, capacity_hint,
-                                      _index_flags(keep_f64, f64_on_host, scan_f16, keep_f32), C.byref(h)))
+                                      _index_flags(keep_f64, f64_on_host, scan_f16, keep_f32, keep_f32_split),
+                                      C.byref(h)))
         self._h = h
         self.dim = dim
         self.device = device
@@ -275,16 +288,17 @@ class Index:
 
     @property
     def flags(self) -> int:
-        """The creation flags as they are now (RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32 | RBK_INDEX_F64_ON_HOST |
-        RBK_INDEX_SCAN_F16)."""
+        """The creation flags as they are now (RBK_INDEX_KEEP_F64, RBK_INDEX_KEEP_F32 or RBK_INDEX_KEEP_F32_SPLIT |
+        RBK_INDEX_F64_ON_HOST | RBK_INDEX_SCAN_F16)."""
         return int(lib.rbk_index_flags(self._h))
 
     def set_tier(self, *, f64_on_host: bool | None = None, scan_f16: bool | None = None,
                  exact_rows: str | None = None) -> None:
         """Change the storage tier in place (rbk_index_set_tier): move the exact rows between the GPU and pinned host
-        memory, switch the scan between bf16 and fp16, keep the exact rows as 'f64' or 'f32'.  None keeps a setting.
-        Needs keep_f64 or keep_f32; answers do not change.  Raises RbkError(RBK_ENOMEM) with the index unchanged when
-        the new tier cannot be backed, NotFloat32Error when a stored value does not fit exact_rows='f32'."""
+        memory, switch the scan between bf16 and fp16, keep the exact rows as 'f64', 'f32' or 'f32_split'.  None keeps
+        a setting.  Needs exact rows; answers do not change.  Raises RbkError(RBK_ENOMEM) with the index unchanged when
+        the new tier cannot be backed, NotFloat32Error when a stored value does not fit exact_rows='f32' or
+        'f32_split'."""
         check(lib.rbk_index_set_tier(self._h, _tier_flags(self.flags, f64_on_host, scan_f16, exact_rows)))
 
     # -- mutation
@@ -444,15 +458,17 @@ class Group:
     Every search is one C call: per-GPU scans, one NCCL all-gather, merge on devices[0], one synchronisation."""
 
     def __init__(self, dim: int, devices, capacity_hint: int = 0, keep_f64: bool = False, f64_on_host: bool = False,
-                 scan_f16: bool = False, keep_f32: bool = False):
+                 scan_f16: bool = False, keep_f32: bool = False, keep_f32_split: bool = False):
         """f64_on_host: every member keeps its exact rows in its own pinned host buffer (see Index).
-        scan_f16: every member scans fp16 rows (see Index).  keep_f32: every member keeps float32 exact rows (see
-        Index); a call with any non-float32 value is refused before any member writes."""
+        scan_f16: every member scans fp16 rows (see Index).  keep_f32 / keep_f32_split: every member keeps float32
+        exact rows, whole or split (see Index); a call with any non-float32 value is refused before any member
+        writes."""
         self._h = None
         devs = np.ascontiguousarray(list(devices), dtype=np.int32)
         h = C.c_void_p()
         check(lib.rbk_group_create(dim, ptr(devs), devs.shape[0], capacity_hint,
-                                   _index_flags(keep_f64, f64_on_host, scan_f16, keep_f32), C.byref(h)))
+                                   _index_flags(keep_f64, f64_on_host, scan_f16, keep_f32, keep_f32_split),
+                                   C.byref(h)))
         self._h = h
         self.dim = dim
         self.devices = [int(d) for d in devs]

@@ -441,7 +441,7 @@ rbk_status append_rows(rbk_index* ix, const void* src, bool is_device, int elem,
   if (first_out) *first_out = ix->n_rows;
   if (n == 0) return RBK_OK;
   // float32 exact rows take float64 sources only when every value fits: checked before anything is written
-  rbk_status st = elem == 8 && ix->x_elem == 4
+  rbk_status st = elem == 8 && ix->f32_rows()
                       ? check_f32_exact(ix, static_cast<const double*>(src), is_device, n * ix->dim)
                       : RBK_OK;
   if (st != RBK_OK) return st;
@@ -1245,15 +1245,20 @@ void compact_commit(rbk_index* ix, int64_t n_new) {
 
 uint32_t index_flags(const rbk_index* ix) {
   return (ix->x_elem == 8 ? RBK_INDEX_KEEP_F64 : 0u) | (ix->x_elem == 4 ? RBK_INDEX_KEEP_F32 : 0u) |
+         (ix->x_elem == 2 ? RBK_INDEX_KEEP_F32_SPLIT : 0u) |
          (ix->rows_on_host ? RBK_INDEX_ROWS_ON_HOST : 0u) | (ix->scan_f16 ? RBK_INDEX_SCAN_F16 : 0u);
 }
 
 rbk_status check_flags(uint32_t flags) {
-  constexpr uint32_t kKeep = RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32;
+  constexpr uint32_t kKeep = RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32 | RBK_INDEX_KEEP_F32_SPLIT;
   if (flags & ~static_cast<uint32_t>(kKeep | RBK_INDEX_ROWS_ON_HOST | RBK_INDEX_SCAN_F16))
     return fail(RBK_EINVAL, "unknown flag");
-  if ((flags & kKeep) == kKeep)
+  if ((flags & (RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)) == (RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32))
     return fail(RBK_EINVAL, "RBK_INDEX_KEEP_F64 and RBK_INDEX_KEEP_F32 exclude each other");
+  if ((flags & RBK_INDEX_KEEP_F32_SPLIT) && (flags & (RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)))
+    return fail(RBK_EINVAL, "RBK_INDEX_KEEP_F32_SPLIT excludes RBK_INDEX_KEEP_F64 and RBK_INDEX_KEEP_F32");
+  if ((flags & RBK_INDEX_KEEP_F32_SPLIT) && (flags & RBK_INDEX_SCAN_F16))
+    return fail(RBK_EINVAL, "RBK_INDEX_KEEP_F32_SPLIT excludes RBK_INDEX_SCAN_F16: its scan copy holds the high halves");
   // (either keep bit satisfies these two; the messages name the float64 one, as they always have)
   if ((flags & RBK_INDEX_ROWS_ON_HOST) && !(flags & kKeep))
     return fail(RBK_EINVAL, "RBK_INDEX_F64_ON_HOST requires RBK_INDEX_KEEP_F64");
@@ -1265,7 +1270,7 @@ rbk_status check_flags(uint32_t flags) {
 rbk_status tier_check(const rbk_index* ix, uint32_t flags) {
   rbk_status st = check_flags(flags);
   if (st != RBK_OK) return st;
-  if (((flags & (RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32)) != 0) != ix->keep_rows())
+  if (((flags & (RBK_INDEX_KEEP_F64 | RBK_INDEX_KEEP_F32 | RBK_INDEX_KEEP_F32_SPLIT)) != 0) != ix->keep_rows())
     return fail(RBK_EINVAL, ix->keep_rows()
                                 ? "a tier change keeps the exact rows: RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32 must stay"
                                 : "a tier change cannot add RBK_INDEX_KEEP_F64 or RBK_INDEX_KEEP_F32: this index holds no "
@@ -1293,15 +1298,15 @@ rbk_status check_f32_exact(rbk_index* ix, const double* src, bool is_device, int
   CK(cudaMemcpyAsync(&bad, ix->d_counter, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
   CK(cudaStreamSynchronize(ix->stream));
   if (bad == 0) return RBK_OK;
-  return fail(RBK_ENOTF32, "a value is not exactly a float32, which an RBK_INDEX_KEEP_F32 index stores (nothing was "
-                           "written)");
+  return fail(RBK_ENOTF32, "a value is not exactly a float32, which an RBK_INDEX_KEEP_F32 or KEEP_F32_SPLIT index "
+                           "stores (nothing was written)");
 }
 
 rbk_status tier_prepare(rbk_index* ix, uint32_t flags, TierPlan* p) {
   *p = TierPlan();
   p->flags = flags;
   p->to_host = (flags & RBK_INDEX_ROWS_ON_HOST) != 0;
-  p->x_elem = (flags & RBK_INDEX_KEEP_F32) ? 4 : 8;
+  p->x_elem = (flags & RBK_INDEX_KEEP_F32) ? 4 : ((flags & RBK_INDEX_KEEP_F32_SPLIT) ? 2 : 8);
   p->move = p->to_host != ix->rows_on_host || p->x_elem != ix->x_elem;
   p->rescan = ((flags & RBK_INDEX_SCAN_F16) != 0) != ix->scan_f16;
   p->vm_rows = tier_vm_rows(ix, !p->to_host, p->x_elem);
@@ -1312,7 +1317,7 @@ rbk_status tier_prepare(rbk_index* ix, uint32_t flags, TierPlan* p) {
     return fail(RBK_ENOMEM, "a capacity of " + std::to_string(ix->cap) + " rows exceeds the " +
                                 std::to_string(p->vm_rows) + " this device can hold with these exact rows on it");
   // narrowing: every stored slot, live or tombstoned, must hold float32-exact values (read where the rows are)
-  if (p->x_elem < ix->x_elem) {
+  if (ix->x_elem == 8 && p->x_elem != 8) {
     rbk_status st = check_f32_exact(ix, static_cast<const double*>(ix->rows_x), true, ix->n_rows * ix->dim);
     if (st != RBK_OK) return st;
   }
@@ -1373,8 +1378,9 @@ rbk_status tier_rescan(rbk_index* ix, bool f16, int eps_bits) {
   memcpy(&eps, &eps_bits, sizeof eps);
   const int eps0 = eps >= kEpsNone ? eps_bits : 0;
   CK(cudaMemcpyAsync(ix->d_counter + 1, &eps0, sizeof(int), cudaMemcpyHostToDevice, ix->stream));   // pageable: staged
-  CK(launch_convert_rows(ix->rows_x, ix->x_elem == 4 ? 1 : 0, ix->n_rows, ix->dim, ix->dpad, ix->rows, nullptr,
-                         ix->x_elem, ix->stream, nullptr, nullptr, nullptr, f16));
+  if (ix->x_elem != 2)   // a split index's scan copy was written with its low halves (tier_commit)
+    CK(launch_convert_rows(ix->rows_x, ix->x_elem == 4 ? 1 : 0, ix->n_rows, ix->dim, ix->dpad, ix->rows, nullptr,
+                           ix->x_elem, ix->stream, nullptr, nullptr, nullptr, f16));
   CK(launch_row_norms(ix->rows, ix->rows_x, ix->x_elem, 0, ix->n_rows, ix->dim, ix->dpad, ix->inv_norm, ix->norm2,
                       ix->d_counter + 1, ix->stream, nullptr, ix->dead_bits, f16));
   ix->scan_f16 = f16;
@@ -1385,7 +1391,11 @@ rbk_status tier_rescan(rbk_index* ix, bool f16, int eps_bits) {
 rbk_status tier_commit(rbk_index* ix, TierPlan* p) {
   const bool f16 = (p->flags & RBK_INDEX_SCAN_F16) != 0;
   rbk_status st = RBK_OK;
-  if (p->rescan && !ix->rows_on_host) {   // while the exact rows are on the device: no PCIe reads
+  // Into or out of the split, the scan copy changes with the exact rows (it holds their high halves): it is rewritten
+  // from the new rows, and the norms and the bound with it, once they are in place.
+  const bool resplit = p->move && (p->x_elem == 2) != (ix->x_elem == 2);
+  if (resplit) p->rescan = true;
+  if (p->rescan && !ix->rows_on_host && !resplit) {   // while the exact rows are on the device: no PCIe reads
     if ((st = tier_rescan(ix, f16, p->eps_bits)) != RBK_OK) return st;
     p->rescan = false;
   }
@@ -1394,8 +1404,11 @@ rbk_status tier_commit(rbk_index* ix, TierPlan* p) {
     const int64_t n_el = ix->n_rows * ix->dim;
     if (n_el > 0 && p->x_elem == ix->x_elem)   // a move between the device and the host: UVA picks the direction
       CK(cudaMemcpyAsync(dst, ix->rows_x, static_cast<size_t>(n_el) * ix->x_elem, cudaMemcpyDefault, ix->stream));
+    else if (n_el > 0 && p->x_elem == 2)       // into the split: both halves from the float32-exact rows
+      CK(launch_convert_rows(ix->rows_x, ix->x_elem == 4 ? 1 : 0, ix->n_rows, ix->dim, ix->dpad, ix->rows, dst, 2,
+                             ix->stream));
     else if (n_el > 0)                         // widen or narrow on the device, reading and writing where the rows are
-      CK(launch_convert_exact(ix->rows_x, ix->x_elem, dst, p->x_elem, n_el, ix->stream));
+      CK(launch_convert_exact(ix->rows_x, ix->x_elem, dst, p->x_elem, n_el, ix->stream, ix->rows, ix->dim, ix->dpad));
     CK(cudaStreamSynchronize(ix->stream));
     if (ix->rows_on_host) {
       cudaFreeHost(ix->rows_x);
@@ -1471,7 +1484,10 @@ rbk_status rbk_index_create_ex(int32_t dim, int32_t device, int64_t capacity_hin
   // row pitch = whole 128-byte lines (64-element k-blocks): no TMA box hangs over the end of a row
   ix->dpad = static_cast<int>(round_up(dim, kBlockK));
   ix->device = device;
-  ix->x_elem = (flags & RBK_INDEX_KEEP_F64) ? 8 : ((flags & RBK_INDEX_KEEP_F32) ? 4 : 0);
+  ix->x_elem = (flags & RBK_INDEX_KEEP_F64)         ? 8
+               : (flags & RBK_INDEX_KEEP_F32)       ? 4
+               : (flags & RBK_INDEX_KEEP_F32_SPLIT) ? 2
+                                                    : 0;
   ix->rows_on_host = (flags & RBK_INDEX_ROWS_ON_HOST) != 0;
   ix->scan_f16 = (flags & RBK_INDEX_SCAN_F16) != 0;
   ix->sm_count = prop.multiProcessorCount;
@@ -1586,7 +1602,7 @@ rbk_status rbk_index_overwrite_f64_batch(rbk_index* ix, const int64_t* slots, in
     }
   }
   // float32 exact rows: every value is checked before the first slot is written
-  if (ix->x_elem == 4) {
+  if (ix->f32_rows()) {
     rbk_status st = check_f32_exact(ix, rows, false, n * ix->dim);
     if (st != RBK_OK) return st;
   }

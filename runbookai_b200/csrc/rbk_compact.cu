@@ -116,8 +116,10 @@ __global__ void __launch_bounds__(256) compact_gather_kernel(const uint16_t* __r
     reinterpret_cast<uint4*>(st_rows + (j - d0) * dpad)[u] =
         __ldg(reinterpret_cast<const uint4*>(rows + (s0 + r) * dpad) + u);
   }
-  // two elements per move: 16 bytes (double2) or 8 (float2)
-  using X2 = typename std::conditional<sizeof(XT) == 8, double2, float2>::type;
+  // two elements per move: 16 bytes (double2), 8 (float2) or 4 (the split's low halves, ushort2; their high halves
+  // moved with the scan copy above)
+  using X2 = typename std::conditional<sizeof(XT) == 8, double2,
+                                       typename std::conditional<sizeof(XT) == 4, float2, ushort2>::type>::type;
   if (rows_f64 != nullptr) {
     if ((d & 1) == 0) {   // rows start aligned to two elements
       const int u2 = d >> 1;
@@ -134,7 +136,8 @@ __global__ void __launch_bounds__(256) compact_gather_kernel(const uint16_t* __r
         const int u = static_cast<int>(g - r * d);
         const long long j = old_to_new[s0 + r];
         if (j < 0) continue;
-        st_f64[(j - d0) * d + u] = __ldg(rows_f64 + (s0 + r) * d + u);
+        if constexpr (kIsSplit<XT>) st_f64[(j - d0) * d + u].bits = __ldg(&rows_f64[(s0 + r) * d + u].bits);
+        else st_f64[(j - d0) * d + u] = __ldg(rows_f64 + (s0 + r) * d + u);
       }
     }
   }
@@ -173,6 +176,10 @@ cudaError_t launch_compact_gather(const uint16_t* rows, const void* rows_x, int 
     compact_gather_kernel<float><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
         rows, static_cast<const float*>(rows_x), norm2, inv_norm, old_to_new, s0, n, d0, d, dpad, st_rows,
         static_cast<float*>(st_x), st_norm2, st_inv);
+  else if (x_elem == 2)
+    compact_gather_kernel<F32Lo><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        rows, static_cast<const F32Lo*>(rows_x), norm2, inv_norm, old_to_new, s0, n, d0, d, dpad, st_rows,
+        static_cast<F32Lo*>(st_x), st_norm2, st_inv);
   else
     compact_gather_kernel<double><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
         rows, static_cast<const double*>(rows_x), norm2, inv_norm, old_to_new, s0, n, d0, d, dpad, st_rows,

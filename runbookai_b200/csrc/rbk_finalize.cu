@@ -43,18 +43,58 @@ __device__ __forceinline__ double exact_dot(const double* __restrict__ q, const 
   for (; i < d; ++i) dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i), bf16_to_f64(row[i])));
   return dot;
 }
-// same, exact-source row of float64 or float32 elements (widened on load: the same operands either way)
+// One exact-row element widened to double.  x: the element; hi: the same element of the scan copy, which only the split
+// (F32Lo, x_elem 2) reads - it holds the high half of the float32.
 template <typename XT>
-__device__ __forceinline__ double exact_dot_f64(const double* __restrict__ q, const XT* __restrict__ row, int d) {
+__device__ __forceinline__ double ldx(const XT* x, const uint16_t* hi) {
+  return static_cast<double>(__ldg(x));
+}
+__device__ __forceinline__ double ldx(const F32Lo* x, const uint16_t* hi) {
+  return split_f64(__ldg(hi), __ldg(&x->bits));
+}
+// same, exact-source row of float64, float32 or split float32 elements (widened on load: the same operands either way);
+// hi: the row of the scan copy
+template <typename XT>
+__device__ __forceinline__ double exact_dot_f64(const double* __restrict__ q, const XT* __restrict__ row, int d,
+                                                const uint16_t* __restrict__ hi) {
   double dot = 0.0;
-  for (int i = 0; i < d; ++i) dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i), static_cast<double>(__ldg(row + i))));
+  for (int i = 0; i < d; ++i) dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i), ldx(row + i, hi + i)));
   return dot;
 }
-// two exact-row elements per load: 16 bytes of float64, 8 of float32
+// The split's rows are read eight elements at a time, one 16-byte load from each half (the rows start 16-byte aligned
+// when d % 8 == 0; the scan copy's always do): a thread walking its own row issues an eighth of the loads.  Same chain.
+__device__ __forceinline__ double exact_dot_f64(const double* __restrict__ q, const F32Lo* __restrict__ row, int d,
+                                                const uint16_t* __restrict__ hi) {
+  double dot = 0.0;
+  int i = 0;
+  if ((d & 7) == 0) {
+    const uint4* lp = reinterpret_cast<const uint4*>(row);
+    const uint4* hp = reinterpret_cast<const uint4*>(hi);
+    for (; i < d; i += 8) {
+      const uint4 l = __ldg(lp + (i >> 3)), h = __ldg(hp + (i >> 3));
+      const uint32_t lw[4] = {l.x, l.y, l.z, l.w}, hw[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i + 2 * j), split_f64(hw[j] & 0xFFFFu, lw[j] & 0xFFFFu)));
+        dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i + 2 * j + 1), split_f64(hw[j] >> 16, lw[j] >> 16)));
+      }
+    }
+  }
+  for (; i < d; ++i) dot = __dadd_rn(dot, __dmul_rn(__ldg(q + i), ldx(row + i, hi + i)));
+  return dot;
+}
+// two exact-row elements per load: 16 bytes of float64, 8 of float32, 4 of low halves (plus 4 of the scan copy)
 template <typename XT>
-using Pair = typename std::conditional<sizeof(XT) == 8, double2, float2>::type;
+using Pair = typename std::conditional<sizeof(XT) == 8, double2,
+                                       typename std::conditional<sizeof(XT) == 4, float2, ushort2>::type>::type;
 __device__ __forceinline__ double2 widen2(double2 v) { return v; }
 __device__ __forceinline__ double2 widen2(float2 v) { return make_double2(v.x, v.y); }
+__device__ __forceinline__ double2 ldx2(const double2* x, const uint16_t*) { return widen2(__ldg(x)); }
+__device__ __forceinline__ double2 ldx2(const float2* x, const uint16_t*) { return widen2(__ldg(x)); }
+__device__ __forceinline__ double2 ldx2(const ushort2* x, const uint16_t* hi) {
+  const ushort2 r = __ldg(x), s = __ldg(reinterpret_cast<const ushort2*>(hi));
+  return make_double2(split_f64(s.x, r.x), split_f64(s.y, r.y));
+}
 // embedder.ts:183  dotProduct / (Math.sqrt(normA) * Math.sqrt(normB))
 __device__ __forceinline__ double exact_cosine(double dot, double na, double nb) {
   return __ddiv_rn(dot, __dmul_rn(__dsqrt_rn(na), __dsqrt_rn(nb)));
@@ -540,7 +580,8 @@ __device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
             if (i < nsel * len2) {
               const int rr = i / len2, u = i - rr * len2;
               const int row = static_cast<int>(key_row(s_sel[rr]));
-              v[b] = widen2(__ldg(reinterpret_cast<const Pair<XT>*>(rows_x + static_cast<size_t>(row) * p.d + c0) + u));
+              v[b] = ldx2(reinterpret_cast<const Pair<XT>*>(rows_x + static_cast<size_t>(row) * p.d + c0) + u,
+                          p.rows + static_cast<size_t>(row) * p.dpad + c0 + 2 * u);
             }
           }
 #pragma unroll
@@ -562,7 +603,7 @@ __device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
             if (i < nsel * len) {
               const int rr = i / len, u = i - rr * len;
               const int row = static_cast<int>(key_row(s_sel[rr]));
-              v[b] = static_cast<double>(__ldg(rows_x + static_cast<size_t>(row) * p.d + c0 + u));
+              v[b] = ldx(rows_x + static_cast<size_t>(row) * p.d + c0 + u, p.rows + static_cast<size_t>(row) * p.dpad + c0 + u);
             }
           }
 #pragma unroll
@@ -597,7 +638,8 @@ __device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
       for (int i = tid; i < nsel * len; i += kFinThreads) {
         const int rr = i / len, u = i - rr * len;
         const int row = static_cast<int>(key_row(s_sel[rr]));
-        s_rows64[rr * row_stride + u] = static_cast<double>(__ldg(rows_x + static_cast<size_t>(row) * p.d + c0 + u));
+        s_rows64[rr * row_stride + u] =
+            ldx(rows_x + static_cast<size_t>(row) * p.d + c0 + u, p.rows + static_cast<size_t>(row) * p.dpad + c0 + u);
       }
       for (int i = tid; i < len; i += kFinThreads) s_q[i] = __ldg(qv + c0 + i);
       __syncthreads();
@@ -672,6 +714,11 @@ __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p)
 template <bool kHostRows>
 __global__ void __launch_bounds__(kFinThreads) finalize_f32_kernel(FinalizeParams p) {
   finalize_rows<kHostRows, float>(p);
+}
+// and split float32 rows (finalize_split_kernel): low halves in rows_x, high halves in rows
+template <bool kHostRows>
+__global__ void __launch_bounds__(kFinThreads) finalize_split_kernel(FinalizeParams p) {
+  finalize_rows<kHostRows, F32Lo>(p);
 }
 
 // --------------------------------------------------------------------------- exact fallback (K0)
@@ -763,7 +810,8 @@ __global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
       const bool dead = (p.dead_bits[row >> 5] >> (row & 31)) & 1u;
       if (!dead) {   // zero-norm rows give NaN and fail the compare below, like in the reference (S3)
         const XT* rows_x = static_cast<const XT*>(p.rows_x);
-        const double dot = rows_x != nullptr ? exact_dot_f64(qv, rows_x + static_cast<size_t>(row) * p.d, p.d)
+        const double dot = rows_x != nullptr ? exact_dot_f64(qv, rows_x + static_cast<size_t>(row) * p.d, p.d,
+                                                             p.rows + static_cast<size_t>(row) * p.dpad)
                                              : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
         const double sc = exact_cosine(dot, na, p.row_norm2[row]);
         if (sc >= p.min_score) exact_push(t, sc, static_cast<int>(row));
@@ -917,7 +965,8 @@ __device__ __forceinline__ void large_score_rows(const LargeRerankParams& p) {
     const size_t o = static_cast<size_t>(p.emit_off[q]) + i;
     const int row = p.emit_rows[o];
     const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
-    const double dot = rows_x != nullptr ? exact_dot_f64(qv, rows_x + static_cast<size_t>(row) * p.d, p.d)
+    const double dot = rows_x != nullptr ? exact_dot_f64(qv, rows_x + static_cast<size_t>(row) * p.d, p.d,
+                                                         p.rows + static_cast<size_t>(row) * p.dpad)
                                          : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
     p.cand_scores[o] = exact_cosine(dot, p.q_norm2[q], p.row_norm2[row]);
   } else {
@@ -945,8 +994,8 @@ __device__ __forceinline__ void large_score_rows(const LargeRerankParams& p) {
             const int e = i0 + b * 256;
             if (e < m * len2) {
               const int rr = e / len2, u = e - rr * len2;
-              v[b] = widen2(
-                  __ldg(reinterpret_cast<const Pair<XT>*>(rows_x + static_cast<size_t>(s_row[rr]) * p.d + c0) + u));
+              v[b] = ldx2(reinterpret_cast<const Pair<XT>*>(rows_x + static_cast<size_t>(s_row[rr]) * p.d + c0) + u,
+                          p.rows + static_cast<size_t>(s_row[rr]) * p.dpad + c0 + 2 * u);
             }
           }
 #pragma unroll
@@ -967,7 +1016,8 @@ __device__ __forceinline__ void large_score_rows(const LargeRerankParams& p) {
             const int e = i0 + b * 256;
             if (e < m * len) {
               const int rr = e / len, u = e - rr * len;
-              v[b] = static_cast<double>(__ldg(rows_x + static_cast<size_t>(s_row[rr]) * p.d + c0 + u));
+              v[b] = ldx(rows_x + static_cast<size_t>(s_row[rr]) * p.d + c0 + u,
+                         p.rows + static_cast<size_t>(s_row[rr]) * p.dpad + c0 + u);
             }
           }
 #pragma unroll
@@ -998,6 +1048,10 @@ __global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
 template <bool kHostRows>
 __global__ void __launch_bounds__(256) large_score_f32_kernel(LargeRerankParams p) {
   large_score_rows<kHostRows, float>(p);
+}
+template <bool kHostRows>
+__global__ void __launch_bounds__(256) large_score_split_kernel(LargeRerankParams p) {
+  large_score_rows<kHostRows, F32Lo>(p);
 }
 
 // re-rank, part 2: one block per query keeps the best k_fetch of its candidates by (score desc, row asc) in a
@@ -1253,7 +1307,8 @@ __global__ void __launch_bounds__(256) exact_scores_kernel(const uint16_t* __res
   double sc = __longlong_as_double(0x7FF8000000000000ll);
   if (!((dead_bits[row >> 5] >> (row & 31)) & 1u)) {
     const double* qv = q_f64 + static_cast<size_t>(q) * d;
-    const double dot = rows_f64 != nullptr ? exact_dot_f64(qv, rows_f64 + static_cast<size_t>(row) * d, d)
+    const double dot = rows_f64 != nullptr ? exact_dot_f64(qv, rows_f64 + static_cast<size_t>(row) * d, d,
+                                                           rows + static_cast<size_t>(row) * dpad)
                                            : exact_dot(qv, rows + static_cast<size_t>(row) * dpad, d);
     sc = exact_cosine(dot, q_norm2[q], row_norm2[row]);
   }
@@ -1364,8 +1419,9 @@ cudaError_t launch_finalize(const FinalizeParams& p_in, bool rows_on_host, int x
   // >= 2048 keys (16 KB: room for 128 candidate rows x 56 elements per re-rank chunk)
   p.key_cap = p.B <= 160 ? 16384 : (p.B <= 320 ? 8192 : 2048);
   const size_t smem = static_cast<size_t>(p.key_cap) * 8;
-  auto kernel = x_elem == 4 ? (rows_on_host ? finalize_f32_kernel<true> : finalize_f32_kernel<false>)
-                            : (rows_on_host ? finalize_kernel<true> : finalize_kernel<false>);
+  auto kernel = x_elem == 4   ? (rows_on_host ? finalize_f32_kernel<true> : finalize_f32_kernel<false>)
+                : x_elem == 2 ? (rows_on_host ? finalize_split_kernel<true> : finalize_split_kernel<false>)
+                              : (rows_on_host ? finalize_kernel<true> : finalize_kernel<false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
   if (e != cudaSuccess) return e;
   kernel<<<p.B, kFinThreads, smem, stream>>>(p);
@@ -1376,6 +1432,7 @@ cudaError_t launch_exact_fallback(const ExactParams& p, int x_elem, cudaStream_t
   if (p.n_fail <= 0) return cudaSuccess;
   dim3 grid(p.n_blocks, p.n_fail);
   if (x_elem == 4) exact_scan_kernel<float><<<grid, kExThreads, 0, stream>>>(p);
+  else if (x_elem == 2) exact_scan_kernel<F32Lo><<<grid, kExThreads, 0, stream>>>(p);
   else exact_scan_kernel<double><<<grid, kExThreads, 0, stream>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
@@ -1390,6 +1447,9 @@ cudaError_t launch_exact_scores(const uint16_t* rows, const void* rows_x, int x_
   dim3 grid(static_cast<unsigned>((n_rows + 255) / 256), static_cast<unsigned>(B));
   if (x_elem == 4)
     exact_scores_kernel<float><<<grid, 256, 0, stream>>>(rows, static_cast<const float*>(rows_x), row_norm2, dead_bits,
+                                                         n_rows, d, dpad, q_f64, q_norm2, out);
+  else if (x_elem == 2)
+    exact_scores_kernel<F32Lo><<<grid, 256, 0, stream>>>(rows, static_cast<const F32Lo*>(rows_x), row_norm2, dead_bits,
                                                          n_rows, d, dpad, q_f64, q_norm2, out);
   else
     exact_scores_kernel<double><<<grid, 256, 0, stream>>>(rows, static_cast<const double*>(rows_x), row_norm2,
@@ -1423,6 +1483,9 @@ cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch
     if (x_elem == 4) {
       if (rows_on_host) large_score_f32_kernel<true><<<grid, 256, 0, stream>>>(p);
       else large_score_f32_kernel<false><<<grid, 256, 0, stream>>>(p);
+    } else if (x_elem == 2) {
+      if (rows_on_host) large_score_split_kernel<true><<<grid, 256, 0, stream>>>(p);
+      else large_score_split_kernel<false><<<grid, 256, 0, stream>>>(p);
     } else {
       if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
       else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);

@@ -108,7 +108,7 @@ inline void locate(const rbk_group* g, int64_t slot, int* dev, int64_t* local) {
 // RBK_ENOTF32 if the group keeps float32 rows and any of the n rows is not float32-exact (checked on member 0).
 rbk_status group_check_f32(rbk_group* g, const double* rows, int64_t n) {
   rbk_index* ix = g->parts[0];
-  if (ix->x_elem != 4) return RBK_OK;
+  if (!ix->f32_rows()) return RBK_OK;
   std::lock_guard<std::mutex> lk(ix->mu);
   DeviceGuard dg(ix->device);
   return check_f32_exact(ix, rows, false, n * g->dim);

@@ -155,11 +155,13 @@ struct rbk_index {
   float* inv_norm = nullptr;  // padded to a multiple of kBlockN (+ one tile), NaN-filled
   double* norm2 = nullptr;
   // optional exact-source rows [cap][dim] of x_elem bytes each: float64 (RBK_INDEX_KEEP_F64, x_elem 8) or float32
-  // (RBK_INDEX_KEEP_F32, x_elem 4; every stored value is float32-exact, so its widening is the float64 row); x_elem 0:
+  // (RBK_INDEX_KEEP_F32, x_elem 4; every stored value is float32-exact, so its widening is the float64 row) or the low
+  // halves of float32 rows whose high halves are `rows` (RBK_INDEX_KEEP_F32_SPLIT, x_elem 2; rbk_internal.h); x_elem 0:
   // none
   void* rows_x = nullptr;
   int x_elem = 0;
   bool keep_rows() const { return x_elem != 0; }
+  bool f32_rows() const { return x_elem == 4 || x_elem == 2; }   // only float32-exact values may be stored
   size_t x_row_bytes() const { return static_cast<size_t>(dim) * x_elem; }
   // RBK_INDEX_ROWS_ON_HOST: rows_x is pinned, mapped host memory (one pointer under UVA).  Every write to it is
   // stream-ordered: a kernel or copy on `stream`, or the host after a synchronisation of `stream`.

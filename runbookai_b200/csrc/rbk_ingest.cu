@@ -58,6 +58,22 @@ __global__ void __launch_bounds__(256) convert_rows_kernel(const SrcT* __restric
       // pad columns (the row pitch is a whole number of 128-byte lines): zeros, and nothing to read
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = 0;
+    } else if constexpr (kIsSplit<XT>) {
+      // RBK_INDEX_KEEP_F32_SPLIT: the scan copy by the split rule (rbk_internal.h) and the low half beside it; a bf16
+      // source is its own scan copy, with a zero low half.  dst_f64 null: only the scan copy (a tier change into the
+      // split re-derives it from float32-exact rows).
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        o[j] = 0;
+        if (c0 + j < d) {
+          uint32_t u;
+          if constexpr (sizeof(SrcT) == 8) u = __float_as_uint(__double2float_rn(static_cast<double>(s[j])));
+          else if constexpr (sizeof(SrcT) == 4) u = __float_as_uint(static_cast<float>(s[j]));
+          else u = static_cast<uint32_t>(s[j]) << 16;
+          o[j] = sizeof(SrcT) == 2 ? static_cast<uint16_t>(s[j]) : split_hi(u);
+          if (dst_f64 != nullptr) dst_f64[row * d + c0 + j].bits = static_cast<uint16_t>(u & 0xFFFFu);
+        }
+      }
     } else if (aligned) {
       if constexpr (sizeof(SrcT) == 8) {
         const double2* s2 = reinterpret_cast<const double2*>(s);
@@ -93,15 +109,17 @@ __global__ void __launch_bounds__(256) convert_rows_kernel(const SrcT* __restric
         o[j] = b;
       }
     }
-    if (dst_f64 != nullptr) {   // exact-source sidecar: the original values, widened to f64 (pitch d)
+    if constexpr (!kIsSplit<XT>) {
+      if (dst_f64 != nullptr) {   // exact-source sidecar: the original values, widened to f64 (pitch d)
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        if (c0 + j < d) {
-          double x;
-          if constexpr (sizeof(SrcT) == 8) x = static_cast<double>(s[j]);
-          else if constexpr (sizeof(SrcT) == 4) x = static_cast<double>(static_cast<float>(s[j]));
-          else x = static_cast<double>(__uint_as_float(static_cast<uint32_t>(s[j]) << 16));
-          dst_f64[row * d + c0 + j] = static_cast<XT>(x);
+        for (int j = 0; j < 8; ++j) {
+          if (c0 + j < d) {
+            double x;
+            if constexpr (sizeof(SrcT) == 8) x = static_cast<double>(s[j]);
+            else if constexpr (sizeof(SrcT) == 4) x = static_cast<double>(static_cast<float>(s[j]));
+            else x = static_cast<double>(__uint_as_float(static_cast<uint32_t>(s[j]) << 16));
+            dst_f64[row * d + c0 + j] = static_cast<XT>(x);
+          }
         }
       }
     }
@@ -357,8 +375,13 @@ __global__ void __launch_bounds__(kNormRows) row_norms_f64_kernel(const uint16_t
       double x = 0.0;
       uint16_t bq = 0;
       if (row >= 0) {
-        x = static_cast<double>(__ldg(rows_f64_base + row * d + c0 + el));
-        bq = __ldg(rows_base + row * dpad + c0 + el);
+        if constexpr (kIsSplit<XT>) {   // the float32 row joined from its scan copy and its low half
+          bq = __ldg(rows_base + row * dpad + c0 + el);
+          x = split_f64(bq, __ldg(&rows_f64_base[row * d + c0 + el].bits));
+        } else {
+          x = static_cast<double>(__ldg(rows_f64_base + row * d + c0 + el));
+          bq = __ldg(rows_base + row * dpad + c0 + el);
+        }
       }
       s_x[rr * kNorm64Pitch + el] = x;
       s_b[rr * (kNorm64Chunk + 2) + el] = bq;
@@ -439,6 +462,19 @@ __global__ void __launch_bounds__(256) convert_exact_kernel(const SrcT* __restri
     dst[i] = static_cast<DstT>(src[i]);
 }
 
+// Out of the split: element i of row i / d is the float32 joined from its scan copy (pitch dpad) and its low half.
+template <typename DstT>
+__global__ void __launch_bounds__(256) join_exact_kernel(const F32Lo* __restrict__ src,
+                                                         const uint16_t* __restrict__ rows, int d, int dpad,
+                                                         DstT* __restrict__ dst, int64_t n) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t row = i / d;
+    const float x = __uint_as_float(split_join(__ldg(rows + row * dpad + (i - row * d)), __ldg(&src[i].bits)));
+    dst[i] = static_cast<DstT>(x);
+  }
+}
+
 int grid_for(int64_t items, int threads, int max_blocks) {
   int64_t b = (items + threads - 1) / threads;
   if (b < 1) b = 1;
@@ -453,7 +489,9 @@ template <typename XT>
 cudaError_t convert_rows_typed(const void* src, int src_type, int64_t n_rows, int d, int dpad, uint16_t* dst_rows,
                                XT* dst_x, cudaStream_t stream, const int64_t* slot_map, const unsigned int* dead_bits,
                                int* n_dead, bool f16) {
-  if (f16) {
+  if constexpr (kIsSplit<XT>) {
+    if (f16) return cudaErrorInvalidValue;   // the split's scan copy is bf16 by construction
+  } else if (f16) {
     constexpr int rows_per_block = kF16ConvThreads / 32;
     int dev = 0, sms = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -499,6 +537,9 @@ cudaError_t launch_convert_rows(const void* src, int src_type, int64_t n_rows, i
   if (x_elem == 4)
     return convert_rows_typed(src, src_type, n_rows, d, dpad, dst_rows, static_cast<float*>(dst_x), stream, slot_map,
                               dead_bits, n_dead, f16);
+  if (x_elem == 2)
+    return convert_rows_typed(src, src_type, n_rows, d, dpad, dst_rows, static_cast<F32Lo*>(dst_x), stream, slot_map,
+                              dead_bits, n_dead, f16);
   return convert_rows_typed(src, src_type, n_rows, d, dpad, dst_rows, static_cast<double*>(dst_x), stream, slot_map,
                             dead_bits, n_dead, f16);
 }
@@ -522,7 +563,12 @@ cudaError_t launch_row_norms(const uint16_t* rows_base, const void* rows_x_base,
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || rows_x_base == nullptr) return e;
   const float* rows_f32_base = static_cast<const float*>(rows_x_base);
-  if (f16 && x_elem == 4)
+  if (x_elem == 2) {
+    if (f16) return cudaErrorInvalidValue;
+    row_norms_f64_kernel<false, F32Lo><<<blocks, kNormRows, 0, stream>>>(
+        rows_base, static_cast<const F32Lo*>(rows_x_base), slot_map, dead_bits, first_row, n_items, d, dpad,
+        norm2_base, inv_norm_base, eps_c_max);
+  } else if (f16 && x_elem == 4)
     row_norms_f64_kernel<true, float><<<blocks, kNormRows, 0, stream>>>(rows_base, rows_f32_base, slot_map, dead_bits,
                                                                         first_row, n_items, d, dpad, norm2_base,
                                                                         inv_norm_base, eps_c_max);
@@ -552,14 +598,22 @@ cudaError_t launch_find_not_f32(const double* src, int64_t n, int* found, cudaSt
 }
 
 cudaError_t launch_convert_exact(const void* src, int src_elem, void* dst, int dst_elem, int64_t n,
-                                 cudaStream_t stream) {
+                                 cudaStream_t stream, const uint16_t* rows, int d, int dpad) {
   if (n <= 0) return cudaSuccess;
   int dev = 0, sms = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   if (e != cudaSuccess) return e;
   const int grid = grid_for(n, 256, sms * 16);
-  if (src_elem == 8 && dst_elem == 4)
+  if (src_elem == 2 && (rows == nullptr || d <= 0))
+    return cudaErrorInvalidValue;
+  else if (src_elem == 2 && dst_elem == 4)
+    join_exact_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const F32Lo*>(src), rows, d, dpad,
+                                                       static_cast<float*>(dst), n);
+  else if (src_elem == 2 && dst_elem == 8)
+    join_exact_kernel<double><<<grid, 256, 0, stream>>>(static_cast<const F32Lo*>(src), rows, d, dpad,
+                                                        static_cast<double*>(dst), n);
+  else if (src_elem == 8 && dst_elem == 4)
     convert_exact_kernel<double, float><<<grid, 256, 0, stream>>>(static_cast<const double*>(src),
                                                                   static_cast<float*>(dst), n);
   else if (src_elem == 4 && dst_elem == 8)

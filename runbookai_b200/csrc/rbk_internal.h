@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace rbk {
 
 // ---- tiling of the fused scan (rbk_scan.cu) ----
@@ -65,10 +67,30 @@ cudaError_t launch_scan_large_f16(const CUtensorMap& tmap_q, const CUtensorMap& 
                                   LargeScanMode mode, cudaStream_t stream);
 
 // ---- ingest (rbk_ingest.cu) ----
-// The exact-source rows of an index that keeps them (RBK_INDEX_KEEP_F64 / RBK_INDEX_KEEP_F32) are [cap][d] elements of
-// x_elem bytes: 8 = float64, 4 = float32.  Every kernel that reads them widens each element to float64 on load and
-// then runs the same operations in the same order, so a float32 row of float32-exact values gives the same bits as
-// the float64 row.
+// The exact-source rows of an index that keeps them (RBK_INDEX_KEEP_F64 / RBK_INDEX_KEEP_F32 /
+// RBK_INDEX_KEEP_F32_SPLIT) are [cap][d] elements of x_elem bytes: 8 = float64, 4 = float32, 2 = the low halves of
+// float32 values whose high halves are the scan copy `rows` (pitch dpad).  Every kernel that reads them widens each
+// element to float64 on load and then runs the same operations in the same order, so a float32 row of float32-exact
+// values gives the same bits as the float64 row.
+//
+// The split rule (x_elem 2), for a float32 with bits u: the scan copy is s = (u + 0x8000) >> 16 - bf16 rounded to
+// nearest, ties away from zero, on the magnitude - and the low half is r = u & 0xFFFF.  Then u = ((s - (r >> 15)) << 16)
+// | r exactly: r >= 0x8000 is exactly when the rounding carried into s.  Round-to-nearest-even cannot be undone so (a tie
+// r == 0x8000 gives one s for two u).  A NaN's scan copy is the canonical bf16 NaN 0x7FFF, which still joins to a NaN.
+struct F32Lo {
+  uint16_t bits;
+};
+__host__ __device__ __forceinline__ uint16_t split_hi(uint32_t u) {
+  return (u & 0x7FFFFFFFu) > 0x7F800000u ? static_cast<uint16_t>(0x7FFFu) : static_cast<uint16_t>((u + 0x8000u) >> 16);
+}
+__host__ __device__ __forceinline__ uint32_t split_join(uint32_t s, uint32_t r) { return ((s - (r >> 15)) << 16) | r; }
+template <typename XT>
+constexpr bool kIsSplit = std::is_same<XT, F32Lo>::value;
+#ifdef __CUDACC__
+__device__ __forceinline__ double split_f64(uint16_t s, uint16_t r) {
+  return static_cast<double>(__uint_as_float(split_join(s, r)));
+}
+#endif
 // src element type: 0 = f64, 1 = f32, 2 = bf16 bits.  src is device memory, row pitch = d.
 // dst_x (nullable): exact-source rows (x_elem bytes per element, pitch d); a float32 destination takes only sources
 // whose values are float32-exact (launch_find_not_f32 checks that first).
@@ -98,9 +120,11 @@ cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows
 // and 1e-300 are not).
 cudaError_t launch_find_not_f32(const double* src, int64_t n, int* found, cudaStream_t stream);
 // dst[i] = src[i] for n elements, from src_elem to dst_elem bytes (8 <-> 4; a float64 -> float32 copy only of values
-// launch_find_not_f32 accepted): a tier change that widens or narrows the exact rows.
+// launch_find_not_f32 accepted): a tier change that widens or narrows the exact rows.  src_elem 2 (out of the split):
+// n = n_rows * d elements, each joined with its high half in rows (pitch dpad).  A change INTO the split writes both
+// halves with launch_convert_rows (x_elem 2) instead.
 cudaError_t launch_convert_exact(const void* src, int src_elem, void* dst, int dst_elem, int64_t n,
-                                 cudaStream_t stream);
+                                 cudaStream_t stream, const uint16_t* rows = nullptr, int d = 0, int dpad = 0);
 
 // ---- compaction (rbk_compact.cu) ----
 // old_to_new [n_rows] (new local slot, -1 = tombstoned) from dead_bits by a two-level exclusive scan over the 32-row
@@ -167,8 +191,8 @@ struct FinalizeParams {
   int* flags;             // [B] 1 = not provably exact -> exhaustive fallback
 };
 // rows_on_host: rows_x is mapped host memory (RBK_INDEX_ROWS_ON_HOST); the re-rank stages it with wide loads, more
-// of them in flight, to cover the PCIe round trip.  Same scores either way.  x_elem: bytes per exact-row element (8 or
-// 4; ignored when rows_x is null), here and in every launcher below that takes it.
+// of them in flight, to cover the PCIe round trip.  Same scores either way.  x_elem: bytes per exact-row element (8, 4
+// or 2; ignored when rows_x is null), here and in every launcher below that takes it.
 cudaError_t launch_finalize(const FinalizeParams& p, bool rows_on_host, int x_elem, cudaStream_t stream);
 
 struct ExactParams {

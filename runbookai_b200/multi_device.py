@@ -25,11 +25,13 @@ from ._native import RBK_EDIM, DimensionError, Index
 
 class MultiDeviceIndex:
     def __init__(self, dim: int, devices: Sequence[int], capacity_hint: int = 0, keep_f64: bool = False,
-                 block: int = 4096, index_factory: Callable | None = None, keep_f32: bool = False):
+                 block: int = 4096, index_factory: Callable | None = None, keep_f32: bool = False,
+                 keep_f32_split: bool = False):
         if not devices:
             raise ValueError("devices must name at least one GPU")
         make = index_factory or (lambda d, dev: Index(d, device=dev, capacity_hint=-(-capacity_hint // len(devices)),
-                                                      keep_f64=keep_f64, keep_f32=keep_f32))
+                                                      keep_f64=keep_f64, keep_f32=keep_f32,
+                                                      keep_f32_split=keep_f32_split))
         self.dim = dim
         self.devices = list(devices)
         self.block = int(block)

@@ -149,11 +149,12 @@ class VectorStore:
         # exact_rows (None: RUNBOOK_KNN_EXACT_ROWS, default "f64"): "f32" keeps the exact rows as float32 - the same
         # answers at half their bytes, for embeddings whose values are all float32-exact.  An append or overwrite the
         # index refuses (a value no float32 holds) widens the index to float64 in place and is repeated once, so this
-        # store accepts every embedding a default one does; exact_rows then reports "f64".
+        # store accepts every embedding a default one does; exact_rows then reports "f64".  "f32_split" keeps the same
+        # float32 values at half the bytes again (the scan copy holds their high halves), and widens the same way.
         if exact_rows is None:
             exact_rows = os.environ.get("RUNBOOK_KNN_EXACT_ROWS", "f64")
-        if exact_rows not in ("f64", "f32"):
-            raise ValueError(f"exact_rows must be 'f64' or 'f32', not {exact_rows!r}")
+        if exact_rows not in ("f64", "f32", "f32_split"):
+            raise ValueError(f"exact_rows must be 'f64', 'f32' or 'f32_split', not {exact_rows!r}")
         if f64_on_host is None:
             f64_on_host = os.environ.get("RUNBOOK_KNN_F64_ON_HOST", "0") == "1"
         if scan_f16 is None:
@@ -163,8 +164,7 @@ class VectorStore:
         self._want_scan_f16 = bool(scan_f16)
         self._want_exact_rows = exact_rows
         self._index_factory = index_factory or (
-            lambda dim, dev: Index(dim, device=dev, **({"keep_f64": True} if self._want_exact_rows == "f64"
-                                                       else {"keep_f32": True}),
+            lambda dim, dev: Index(dim, device=dev, **{"keep_" + self._want_exact_rows: True},
                                    f64_on_host=self._want_f64_on_host, scan_f16=self._want_scan_f16))
         # one connection, usable from the micro-batcher's worker thread too; serialised by a lock
         self.db = sqlite3.connect(db_path, check_same_thread=False)
@@ -249,8 +249,8 @@ class VectorStore:
 
     @property
     def exact_rows(self) -> str:
-        """'f64' or 'f32': what the index keeps its exact rows as once there is one (an "f32" store that met a
-        non-float32 embedding has widened to "f64"), else what this instance asked for."""
+        """'f64', 'f32' or 'f32_split': what the index keeps its exact rows as once there is one (a float32 store that
+        met a non-float32 embedding has widened to "f64"), else what this instance asked for."""
         flags = self._index_flags()
         kept = None if flags is None else exact_rows_of(flags)
         return self._want_exact_rows if kept is None else kept

@@ -1,18 +1,21 @@
 #!/usr/bin/env python
-"""Float32 exact rows (RBK_INDEX_KEEP_F32) against float64 ones (RBK_INDEX_KEEP_F64): what the narrower rows save.
+"""Float32 exact rows (RBK_INDEX_KEEP_F32) and split float32 rows (RBK_INDEX_KEEP_F32_SPLIT) against float64 ones
+(RBK_INDEX_KEEP_F64): what the narrower rows save.
 
     python scripts/f32_rows_bench.py [--rows 1000000] [--dim 1536] [--steps 5] [--warmup 2]
 
-Four indexes receive the same float32-exact rows (N(0,1) drawn as float32, widened to float64; about 18 GB of pinned
-host memory at the defaults): KEEP_F64 and KEEP_F32, each with its exact rows on the device and in pinned host memory
-(RBK_INDEX_F64_ON_HOST).  A tie group of 150 copies of one row is planted so that one query must take the exhaustive
-fallback.  Reports, as one JSON line:
+Six indexes receive the same float32-exact rows (N(0,1) drawn as float32, widened to float64; about 21 GB of pinned
+host memory at the defaults): KEEP_F64, KEEP_F32 and KEEP_F32_SPLIT, each with its exact rows on the device and in
+pinned host memory (RBK_INDEX_F64_ON_HOST).  A tie group of 150 copies of one row is planted so that one query must take
+the exhaustive fallback.  Reports, as one JSON line:
   * the card name, power limit and PCIe link (read-only nvidia-smi queries);
-  * storage_bytes() of all four indexes;
-  * the append time of each from a host float64 source (KEEP_F32: with the float32-exactness check);
-  * search device time, F64 and F32 alternated call by call, on each tier: B in {1, 32, 256} x k_fetch in {20, 1000};
+  * storage_bytes() of all six indexes;
+  * the append time of each from a host float64 source (the float32 widths: with the float32-exactness check);
+  * search device time, the three widths alternated call by call, on each tier: B in {1, 32, 256} x k_fetch in
+    {20, 1000};
   * the forced exhaustive-fallback query and one exact_scores query on each index;
-  * the wall time of an in-place F64 -> F32 and F32 -> F64 set_tier of the device-tier KEEP_F64 index;
+  * the wall time of in-place set_tier changes of the device-tier KEEP_F64 index: F64 -> F32, F32 -> split,
+    split -> F32, F32 -> F64 and F64 -> split;
   * bit-equality of every answer between the widths, and oracle parity (ids and fp64 scores) of 64 queries.
 Writes nothing to the tree.
 """
@@ -91,8 +94,10 @@ def main():
     q = corpus[rng.choice(n, 256, replace=False)] + 0.5 * rng.standard_normal((256, d))
     q_tie = corpus[tie_rows[0]][None, :] * 1.5
 
-    names = [("device", "f64"), ("device", "f32"), ("host", "f64"), ("host", "f32")]
-    ix = {(t, w): nat.Index(d, 0, n, keep_f64=w == "f64", keep_f32=w == "f32", f64_on_host=t == "host")
+    widths = ("f64", "f32", "f32_split")
+    names = [(t, w) for t in ("device", "host") for w in widths]
+    ix = {(t, w): nat.Index(d, 0, n, keep_f64=w == "f64", keep_f32=w == "f32", keep_f32_split=w == "f32_split",
+                            f64_on_host=t == "host")
           for t, w in names}
     append_s = {}
     for key in names:
@@ -108,18 +113,19 @@ def main():
             def call(x, B=B, k=k):
                 return x.search(q[:B], k, None) if k <= nat.RBK_MAX_K_FETCH else x.search_large(q[:B], k, None)
             for _ in range(args.warmup):
-                for w in ("f64", "f32"):
+                for w in widths:
                     call(ix[(tier, w)])
-            ms = {"f64": [], "f32": []}
+            ms = {w: [] for w in widths}
             for _ in range(args.steps):
-                for w in ("f64", "f32"):                   # alternated call by call: same clocks for both
+                for w in widths:                           # alternated call by call: same clocks for all three
                     r = call(ix[(tier, w)])
                     ms[w].append(r[3])
                     results[(tier, w, B, k)] = r[:3]
             med = {w: float(np.median(v)) for w, v in ms.items()}
-            timing[f"{tier}_B{B}_k{k}"] = {"f64_ms": med["f64"], "f32_ms": med["f32"], "f64_over_f32": med["f64"] / med["f32"],
-                                          "bit_equal": bool(same(results[(tier, "f64", B, k)],
-                                                                 results[(tier, "f32", B, k)]))}
+            timing[f"{tier}_B{B}_k{k}"] = {
+                "f64_ms": med["f64"], "f32_ms": med["f32"], "f32_split_ms": med["f32_split"],
+                "f64_over_f32": med["f64"] / med["f32"], "f32_over_split": med["f32"] / med["f32_split"],
+                "bit_equal": bool(all(same(results[(tier, "f64", B, k)], results[(tier, w, B, k)]) for w in widths))}
 
     fallback, exact = {}, {}
     for key in names:
@@ -144,24 +150,23 @@ def main():
         parity[f"{key[0]}_{key[1]}"] = bool(ok)
     parity["queries"] = CHECKED + 1
     parity["oracle_seconds"] = oracle_s
-    parity["fallback_widths_bit_equal"] = {t: bool(same(fallback[(t, "f64")]["result"], fallback[(t, "f32")]["result"]))
-                                           for t in ("device", "host")}
-    parity["exact_scores_widths_bit_equal"] = {t: bool(exact[(t, "f64")].tobytes() == exact[(t, "f32")].tobytes())
-                                               for t in ("device", "host")}
+    parity["fallback_widths_bit_equal"] = {t: bool(all(same(fallback[(t, "f64")]["result"], fallback[(t, w)]["result"])
+                                                       for w in widths)) for t in ("device", "host")}
+    parity["exact_scores_widths_bit_equal"] = {t: bool(all(exact[(t, "f64")].tobytes() == exact[(t, w)].tobytes()
+                                                           for w in widths)) for t in ("device", "host")}
 
-    # in place, on the device tier: narrow the KEEP_F64 index, then widen it back
+    # in place, on the device tier: the KEEP_F64 index through every width and back
     x = ix[("device", "f64")]
     for k in list(ix):
         if k != ("device", "f64"):
             ix.pop(k).close()                                     # room for old + new exact rows
     before = x.search(q[:32], 20, None)[:3]
-    _, narrow_s = timed(torch, lambda: x.set_tier(exact_rows="f32"))
-    narrowed = x.flags, x.storage_bytes(), x.search(q[:32], 20, None)[:3]
-    _, widen_s = timed(torch, lambda: x.set_tier(exact_rows="f64"))
-    widened = x.flags, x.storage_bytes(), x.search(q[:32], 20, None)[:3]
-    set_tier = {"narrow_f64_to_f32_s": narrow_s, "widen_f32_to_f64_s": widen_s,
-                "flags_after": [narrowed[0], widened[0]], "storage_after": [narrowed[1], widened[1]],
-                "answers_bit_equal": bool(same(before, narrowed[2]) and same(before, widened[2]))}
+    set_tier = {"flags_after": [], "storage_after": [], "answers_bit_equal": True}
+    for src, dst in (("f64", "f32"), ("f32", "f32_split"), ("f32_split", "f32"), ("f32", "f64"), ("f64", "f32_split")):
+        _, set_tier[f"{src}_to_{dst}_s"] = timed(torch, lambda dst=dst: x.set_tier(exact_rows=dst))
+        set_tier["flags_after"].append(x.flags)
+        set_tier["storage_after"].append(x.storage_bytes())
+        set_tier["answers_bit_equal"] &= bool(same(before, x.search(q[:32], 20, None)[:3]))
     x.close()
 
     print(json.dumps({

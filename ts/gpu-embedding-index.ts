@@ -45,11 +45,12 @@ function scanF16FromEnv(): number {
 
 /**
  * RUNBOOK_KNN_EXACT_ROWS="f32" keeps the exact rows as float32 instead of float64 (RBK_INDEX_KEEP_F32): the same answers
- * at half the exact-row bytes while every embedding value is a float32.  The addon reads the variable itself when its
+ * at half the exact-row bytes while every embedding value is a float32.  "f32_split" (RBK_INDEX_KEEP_F32_SPLIT) halves
+ * them again: the scan's bf16 copy holds each float32's high half, and only the low halves are kept beside it.  The addon reads the variable itself when its
  * constructor gets no `exactRows` argument, and widens the index to float64 in place (repeating the call) the first
  * time an append or overwrite holds a value no float32 can hold, so no embedding is ever refused.
  */
-export type ExactRows = 'f64' | 'f32';
+export type ExactRows = 'f64' | 'f32' | 'f32_split';
 
 export class GpuEmbeddingIndex {
   private index: any | null = null;
@@ -255,8 +256,8 @@ export class GpuEmbeddingIndex {
   /**
    * Change the storage tier of the loaded index in place (rbk_index_set_tier / rbk_group_set_tier): `f64OnHost` moves
    * the float64 rows between the GPU and pinned host memory, `scanF16` switches the scan between bf16 and fp16.  An
-   * omitted key keeps its setting; `exactRows` widens ('f64') or narrows ('f32', refused unless every stored value is a
-   * float32) the exact rows.  Answers and slots do not change, so nothing is remapped; the native call waits
+   * omitted key keeps its setting; `exactRows` widens ('f64') or narrows ('f32' or 'f32_split', refused unless every
+   * stored value is a float32) the exact rows.  Answers and slots do not change, so nothing is remapped; the native call waits
    * for the index's queued device work itself.  Nothing is automatic: an append that throws for lack of device memory
    * is the caller's to retry after `setTier({ f64OnHost: true })`.  Throws (with the index unchanged) if the new tier
    * cannot be backed, and against a library built before tier changes.
