@@ -804,7 +804,11 @@ __global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
   const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
   const double na = p.q_norm2[q];
   for (int64_t base = r0; base < r1; base += kExThreads) {
-    if (t.n > kExBuf - kExThreads) exact_compact(t, p.k_fetch);  // uniform: t.n read after a barrier
+    // Every thread reads t.n before any push of this iteration moves it: read after the last barrier alone, a fast
+    // thread's push could send a slow one into exact_compact's barriers without the others.
+    const int n_now = t.n;
+    __syncthreads();
+    if (n_now > kExBuf - kExThreads) exact_compact(t, p.k_fetch);
     const int64_t row = base + tid;
     if (row < r1) {
       const bool dead = (p.dead_bits[row >> 5] >> (row & 31)) & 1u;
@@ -840,7 +844,9 @@ __global__ void __launch_bounds__(kExThreads) exact_merge_kernel(ExactParams p) 
   __syncthreads();
   const int total = p.n_blocks * p.k_fetch;
   for (int base = 0; base < total; base += kExThreads) {
-    if (t.n > kExBuf - kExThreads) exact_compact(t, p.k_fetch);
+    const int n_now = t.n;   // read by every thread before any push moves it (as in exact_scan_kernel)
+    __syncthreads();
+    if (n_now > kExBuf - kExThreads) exact_compact(t, p.k_fetch);
     const int i = base + tid;
     if (i < total) {
       const int b = i / p.k_fetch, e = i % p.k_fetch;
