@@ -316,6 +316,24 @@ rbk_status rbk_index_search_unbounded_f64(rbk_index* idx, const double* queries,
                                           int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                           int32_t* out_counts, float* kernel_ms_out);
 
+/* Each query of a batch at its own k_fetch[b] (>= 1) and min_score[b] (any value but NaN; -INFINITY = none), in one
+ * call: row b of the result is exactly what rbk_index_search_unbounded_f64 returns for query b alone with B = 1 at
+ * k_fetch[b] and min_score[b] - the same slots, the same fp64 score bits, the same count - and so, where those accept
+ * the k, what rbk_index_search_large_f64 and rbk_index_search_f64 return.  The rows of out_slots / out_scores are
+ * K = max_b k_fetch[b] entries long ([B][K]); entries [out_counts[b], K) are slot -1 / the quiet NaN
+ * 0x7FF8000000000000.  Argument checks, before any device work and in the order of the other searches: a null array
+ * with B > 0 or a k_fetch[b] < 1 is RBK_EINVAL, the wrong query_dim RBK_EDIM, a NaN min_score[b] RBK_EINVAL; B = 0 is
+ * RBK_OK.  One call adds 1 to the searches counter and B to the queries counter.
+ * The whole batch takes one route, picked by K: up to RBK_MAX_K_FETCH the fused top-k' scan at k' = k'(K), every query
+ * cut, counted and proven at its own k and threshold (a query whose proof fails is re-answered, at its own parameters,
+ * by the wide rescan and then the exhaustive kernel); above it the two-scan large-k pipeline for every query, each one
+ * cut at its own k_eff (min(k_fetch[b], count()) when K > RBK_MAX_K_FETCH_LARGE, else k_fetch[b]).  So callers that want
+ * different k and thresholds share one pass over the corpus (two for the large-k route), where one search per distinct
+ * (k, min_score) would cost a pass each.  Host queries in, host results out; synchronous. */
+rbk_status rbk_index_search_each_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
+                                     const int32_t* k_fetch, const double* min_score, int64_t* out_slots,
+                                     double* out_scores, int32_t* out_counts, float* kernel_ms_out);
+
 /* The exact fp64 cosine of EVERY row, out_scores[b * size() + slot], NaN for tombstoned / zero rows (which the
  * reference's `>= minScore` drops too, S3), for a host that applies the threshold, the stable sort and the cut itself
  * (vector-store.ts:212-221).  One fp64 pass over the corpus per query and 8 * size() bytes per query to the host; a
@@ -424,6 +442,12 @@ rbk_status rbk_group_search_large_f64(rbk_group* grp, const double* queries, int
 rbk_status rbk_group_search_unbounded_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
                                           int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                           int32_t* out_counts, float* device_ms_out);
+/* rbk_index_search_each_f64 over the group: every member takes the route of the batch's largest k, the merge cuts
+ * query b at its own k_fetch[b] (k_eff on the large-k route), and a batch re-answered after a member's proof failed is
+ * re-answered at the same per-query parameters.  Same arguments, checks, layout and answers as the index call. */
+rbk_status rbk_group_search_each_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
+                                     const int32_t* k_fetch, const double* min_score, int64_t* out_slots,
+                                     double* out_scores, int32_t* out_counts, float* device_ms_out);
 
 /* ---- introspection ---- */
 typedef struct {

@@ -283,6 +283,70 @@ int main(int argc, char** argv) {
     }
   }
 
+  // searchEach(): optional each.txt holds one "kFetch minScore" pair per query (minScore may be -inf); results land in
+  // each_* with rows of K = max kFetch entries.  has_search_each.txt gets the hasSearchEach getter first.  Then one call
+  // with a kFetch of 0 must reject with the library's message (err_each), and one with a short kFetch must throw
+  // (err_each_len).
+  {
+    std::ifstream ef(g_dir + "/each.txt");
+    std::vector<int32_t> ke;
+    std::vector<double> me;
+    std::string ks, ms;
+    while (ef >> ks >> ms) {
+      ke.push_back(static_cast<int32_t>(strtol(ks.c_str(), nullptr, 10)));
+      me.push_back(strtod(ms.c_str(), nullptr));
+    }
+    if (!ke.empty()) {
+      if (ke.size() != static_cast<size_t>(n_q)) die("each.txt needs one pair per query");
+      napi_value has = nullptr;
+      if (!mock::get_accessor(env, ix, "hasSearchEach", &has, &err)) die("hasSearchEach threw: " + err);
+      write_text("has_search_each.txt", mock::as_bool(has) ? "1" : "0");
+      int K = 0;
+      for (int32_t v : ke) K = v > K ? v : K;
+      auto call_each = [&](const std::vector<int32_t>& kv, Result* out) {
+        napi_value promise = nullptr, settled = nullptr;
+        if (!mock::call_method(env, ix, "searchEach",
+                               {mock::typed_array(env, napi_float64_array, queries.data(), queries.size()),
+                                mock::number(env, n_q), mock::typed_array(env, napi_int32_array, kv.data(), kv.size()),
+                                mock::typed_array(env, napi_float64_array, me.data(), me.size())},
+                               &promise, &err))
+          return false;
+        mock::run_event_loop(env);
+        const int state = mock::promise_state(promise, &settled);
+        if (state == 2) {
+          err = mock::error_message(settled);
+          return false;
+        }
+        if (state != 1) die("searchEach() left its promise pending");
+        napi_typedarray_type t;
+        size_t n;
+        const void* p = mock::typed_data(mock::get_property(env, settled, "slots"), &t, &n);
+        if (!p || t != napi_bigint64_array || n != static_cast<size_t>(n_q) * K) die("searchEach slots are not [B*K]");
+        out->slots.assign(static_cast<const int64_t*>(p), static_cast<const int64_t*>(p) + n);
+        p = mock::typed_data(mock::get_property(env, settled, "scores"), &t, &n);
+        if (!p || t != napi_float64_array || n != static_cast<size_t>(n_q) * K) die("searchEach scores are not [B*K]");
+        out->scores.assign(static_cast<const double*>(p), static_cast<const double*>(p) + n);
+        p = mock::typed_data(mock::get_property(env, settled, "counts"), &t, &n);
+        if (!p || t != napi_int32_array || n != static_cast<size_t>(n_q)) die("searchEach counts are not [B]");
+        out->counts.assign(static_cast<const int32_t*>(p), static_cast<const int32_t*>(p) + n);
+        return true;
+      };
+      Result er;
+      if (!call_each(ke, &er)) die("searchEach rejected: " + err);
+      write_bin("each_slots.i64", er.slots.data(), er.slots.size() * 8);
+      write_bin("each_scores.f64", er.scores.data(), er.scores.size() * 8);
+      write_bin("each_counts.i32", er.counts.data(), er.counts.size() * 4);
+      std::vector<int32_t> bad = ke;
+      bad[0] = 0;
+      Result none;
+      if (call_each(bad, &none)) die("searchEach with a kFetch of 0 did not reject");
+      log << "err_each " << err << "\n";
+      bad.pop_back();
+      if (call_each(bad, &none)) die("searchEach with a short kFetch did not throw");
+      log << "err_each_len " << err << "\n";
+    }
+  }
+
   // ---- error paths: each must surface as a JS exception / rejection with the reference's wording
   {
     std::vector<double> odd(static_cast<size_t>(dim) + 1, 1.0);

@@ -31,10 +31,14 @@
 //        -> { slots: BigInt64Array, scores: Float64Array, counts: Int32Array }
 //   await ix.searchLarge(Float64Array queries, B, kFetch, minScore)   // kFetch up to 4096, same result object
 //   await ix.searchUnbounded(Float64Array queries, B, kFetch, minScore)   // any kFetch >= 1, same result object
+//   await ix.searchEach(Float64Array queries, B, Int32Array kFetch, Float64Array minScore)   // each query at its own
+//        kFetch[b] and minScore[b]: the same result object with rows of K = max(kFetch) entries
+//   ix.hasSearchEach                           -> boolean: the library has searchEach (else it throws)
 //
 // Build (where Node headers exist):  node-gyp with  libraries: ["-lrbk_knn"], include_dirs: ["../include"].
 #include <node_api.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstdlib>
@@ -68,6 +72,9 @@
 #pragma weak rbk_index_set_tier
 #pragma weak rbk_group_set_tier
 #pragma weak rbk_group_member
+// The same for the per-query search; `searchEach` throws where it is missing.
+#pragma weak rbk_index_search_each_f64
+#pragma weak rbk_group_search_each_f64
 
 namespace {
 
@@ -141,6 +148,14 @@ struct Handle {
                               int32_t* c) {
     return grp ? rbk_group_search_unbounded_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
                : rbk_index_search_unbounded_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
+  }
+  bool has_search_each() const {
+    return grp ? rbk_group_search_each_f64 != nullptr : rbk_index_search_each_f64 != nullptr;
+  }
+  rbk_status search_each(const double* q, int32_t B, int32_t qdim, const int32_t* k, const double* ms, int64_t* s,
+                         double* v, int32_t* c) {
+    return grp ? rbk_group_search_each_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
+               : rbk_index_search_each_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
   }
 };
 
@@ -454,7 +469,7 @@ napi_value Count(napi_env env, napi_callback_info info) {
 }
 
 // ---- search: runs on a libuv worker so the JS thread never blocks on the GPU ----
-enum class SearchKind { kScan, kLarge, kUnbounded };   // search / searchLarge / searchUnbounded
+enum class SearchKind { kScan, kLarge, kUnbounded, kEach };   // search / searchLarge / searchUnbounded / searchEach
 
 struct SearchJob {
   Handle* ix;
@@ -462,6 +477,8 @@ struct SearchJob {
   int32_t B, dim, k;
   SearchKind kind;
   double min_score;
+  std::vector<int32_t> k_each;      // searchEach: kFetch[B] and minScore[B]; k is then their largest k
+  std::vector<double> min_each;
   std::vector<int64_t> slots;
   std::vector<double> scores;
   std::vector<int32_t> counts;
@@ -473,6 +490,12 @@ struct SearchJob {
 
 void search_execute(napi_env, void* data) {
   SearchJob* j = static_cast<SearchJob*>(data);
+  if (j->kind == SearchKind::kEach) {
+    j->st = j->ix->search_each(j->queries.data(), j->B, j->dim, j->k_each.data(), j->min_each.data(), j->slots.data(),
+                               j->scores.data(), j->counts.data());
+    if (j->st != RBK_OK) j->err = rbk_last_error();
+    return;
+  }
   auto fn = j->kind == SearchKind::kLarge       ? &Handle::search_large
             : j->kind == SearchKind::kUnbounded ? &Handle::search_unbounded
                                                 : &Handle::search;
@@ -523,16 +546,49 @@ napi_value QueueSearch(napi_env env, napi_callback_info info, SearchKind kind) {
                      "searchUnbounded: this librbk_knn.so has no unbounded search (rbk_*_search_unbounded_f64)");
     return nullptr;
   }
+  if (kind == SearchKind::kEach && !ix->has_search_each()) {
+    napi_throw_error(env, nullptr, "searchEach: this librbk_knn.so has no per-query search (rbk_*_search_each_f64)");
+    return nullptr;
+  }
   napi_typedarray_type t;
   size_t len;
   void* data;
   NAPI_OK(napi_get_typedarray_info(env, argv[0], &t, &len, &data, nullptr, nullptr));
+  int32_t B = 0;
+  napi_get_value_int32(env, argv[1], &B);
+  std::vector<int32_t> k_each;
+  std::vector<double> min_each;
+  if (kind == SearchKind::kEach) {   // kFetch: Int32Array[B], minScore: Float64Array[B] (-Infinity: no threshold)
+    napi_typedarray_type tk, tm;
+    size_t nk, nm;
+    void *pk, *pm;
+    if (napi_get_typedarray_info(env, argv[2], &tk, &nk, &pk, nullptr, nullptr) != napi_ok ||
+        napi_get_typedarray_info(env, argv[3], &tm, &nm, &pm, nullptr, nullptr) != napi_ok ||
+        tk != napi_int32_array || tm != napi_float64_array) {
+      napi_throw_type_error(env, nullptr, "searchEach: kFetch must be an Int32Array and minScore a Float64Array");
+      return nullptr;
+    }
+    if (B < 0 || nk != static_cast<size_t>(B) || nm != static_cast<size_t>(B)) {
+      napi_throw_error(env, nullptr, "searchEach: kFetch and minScore need one entry per query");
+      return nullptr;
+    }
+    k_each.assign(static_cast<int32_t*>(pk), static_cast<int32_t*>(pk) + nk);
+    min_each.assign(static_cast<double*>(pm), static_cast<double*>(pm) + nm);
+  }
   auto* j = new SearchJob();
   j->ix = ix;
   j->kind = kind;
-  napi_get_value_int32(env, argv[1], &j->B);
-  napi_get_value_int32(env, argv[2], &j->k);
-  napi_get_value_double(env, argv[3], &j->min_score);   // pass -Infinity for "no threshold"
+  j->B = B;
+  if (kind == SearchKind::kEach) {
+    // the row stride; a kFetch[b] < 1 leaves it at 0 or 1, and the library refuses the call with its own message
+    j->k = 0;
+    for (int32_t v : k_each) j->k = std::max(j->k, v);
+    j->k_each = std::move(k_each);
+    j->min_each = std::move(min_each);
+  } else {
+    napi_get_value_int32(env, argv[2], &j->k);
+    napi_get_value_double(env, argv[3], &j->min_score);   // pass -Infinity for "no threshold"
+  }
   j->dim = j->B > 0 ? (int32_t)(len / (size_t)j->B) : 0;   // a wrong length surfaces as RBK_EDIM
   j->queries.assign(static_cast<double*>(data), static_cast<double*>(data) + len);
   j->slots.resize((size_t)j->B * j->k);
@@ -551,6 +607,15 @@ napi_value SearchLarge(napi_env env, napi_callback_info info) { return QueueSear
 napi_value SearchUnbounded(napi_env env, napi_callback_info info) {
   return QueueSearch(env, info, SearchKind::kUnbounded);
 }
+napi_value SearchEach(napi_env env, napi_callback_info info) { return QueueSearch(env, info, SearchKind::kEach); }
+
+napi_value HasSearchEach(napi_env env, napi_callback_info info) {
+  size_t argc = 0;
+  Handle* h = unwrap(env, info, &argc, nullptr);
+  napi_value out;
+  NAPI_OK(napi_get_boolean(env, h->has_search_each(), &out));
+  return out;
+}
 
 napi_value Init(napi_env env, napi_value exports) {
   napi_property_descriptor props[] = {
@@ -568,6 +633,8 @@ napi_value Init(napi_env env, napi_value exports) {
       {"search", nullptr, Search, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"searchLarge", nullptr, SearchLarge, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"searchUnbounded", nullptr, SearchUnbounded, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"searchEach", nullptr, SearchEach, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"hasSearchEach", nullptr, nullptr, HasSearchEach, nullptr, nullptr, napi_default, nullptr},
   };
   napi_value cls;
   NAPI_OK(napi_define_class(env, "RbkIndex", NAPI_AUTO_LENGTH, New, nullptr, sizeof props / sizeof props[0], props, &cls));

@@ -37,6 +37,7 @@ SYMBOLS = [
     "rbk_group_devices", "rbk_group_member", "rbk_group_redone_batches", "rbk_group_search_f32", "rbk_group_search_f64",
     "rbk_group_search_large_f64", "rbk_group_search_unbounded_f64",
     "rbk_index_flags", "rbk_index_set_tier", "rbk_group_set_tier",
+    "rbk_index_search_each_f64", "rbk_group_search_each_f64",
 ]
 
 
@@ -130,6 +131,8 @@ def _load() -> C.CDLL:
     for n in ("rbk_group_search_f32", "rbk_group_search_f64", "rbk_group_search_large_f64",
               "rbk_group_search_unbounded_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
+    for n in ("rbk_index_search_each_f64", "rbk_group_search_each_f64"):
+        getattr(lib, n).argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_debug_scores_f32.argtypes = [vp, vp, i32, vp]
     lib.rbk_index_flags.argtypes = [vp]
     lib.rbk_index_flags.restype = C.c_uint32
@@ -206,6 +209,29 @@ def _search_large(fn, h, queries, k_fetch: int, min_score):
     ms = C.c_float(0)
     ms_arg = -np.inf if min_score is None else float(min_score)
     check(fn(h, ptr(q), B, q.shape[1], k_fetch, ms_arg, ptr(slots), ptr(scores), ptr(counts), C.byref(ms)))
+    return slots, scores, counts, ms.value
+
+
+def _search_each(fn, h, queries, k_fetch, min_score):
+    """rbk_*_search_each_f64: k_fetch [B] ints >= 1, min_score [B] floats or None (-inf, as in search()).  Returns
+    (slots int64 [B, K], scores float64 [B, K], counts int32 [B], device_ms) with K = max(k_fetch); row b is what
+    search_unbounded(queries[b], k_fetch[b], min_score[b]) returns, padded with -1 / NaN to K entries."""
+    q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
+    B = q.shape[0]
+    k = np.ascontiguousarray(np.asarray(k_fetch, dtype=np.int64).reshape(-1))
+    ms_list = list(min_score) if np.ndim(min_score) else [min_score] * B
+    m = np.ascontiguousarray([-np.inf if v is None else float(v) for v in ms_list], dtype=np.float64)
+    if k.shape[0] != B or m.shape[0] != B:
+        raise ValueError(f"k_fetch and min_score need one entry per query ({B}), not {k.shape[0]} and {m.shape[0]}")
+    if (k < 1).any() or (k > np.iinfo(np.int32).max).any():
+        raise RbkError(RBK_EINVAL, "every k_fetch must be in [1, 2^31 - 1]")
+    k32 = k.astype(np.int32)
+    K = int(k32.max()) if B else 0
+    slots = np.empty((B, K), dtype=np.int64)
+    scores = np.empty((B, K), dtype=np.float64)
+    counts = np.empty((B,), dtype=np.int32)
+    ms = C.c_float(0)
+    check(fn(h, ptr(q), B, q.shape[1], ptr(k32), ptr(m), ptr(slots), ptr(scores), ptr(counts), C.byref(ms)))
     return slots, scores, counts, ms.value
 
 
@@ -415,6 +441,12 @@ class Index:
         two scans, then the candidates sorted on the device, at most count() hits per query."""
         return _search_large(lib.rbk_index_search_unbounded_f64, self._h, queries, k_fetch, min_score)
 
+    def search_each(self, queries, k_fetch, min_score):
+        """Each query at its own k_fetch[b] and min_score[b] (None = -inf) in one call (f64 queries): (slots [B, K],
+        scores [B, K], counts [B], device_ms), K = max(k_fetch).  Row b equals search_unbounded(queries[b], k_fetch[b],
+        min_score[b]); one scan for the batch when K <= RBK_MAX_K_FETCH, else the two scans of the large-k search."""
+        return _search_each(lib.rbk_index_search_each_f64, self._h, queries, k_fetch, min_score)
+
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: the reference's cosine of every row, NaN for tombstoned / zero rows."""
         q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
@@ -572,6 +604,10 @@ class Group:
 
     def search_unbounded(self, queries, k_fetch: int, min_score: float | None = 0.5):
         return _search_large(lib.rbk_group_search_unbounded_f64, self._h, queries, k_fetch, min_score)
+
+    def search_each(self, queries, k_fetch, min_score):
+        """Index.search_each() over the group: one call, every member on the route of the largest k."""
+        return _search_each(lib.rbk_group_search_each_f64, self._h, queries, k_fetch, min_score)
 
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: every device's exact scores, put back in global slot order (4096-row blocks dealt

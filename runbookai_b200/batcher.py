@@ -6,8 +6,13 @@ The reference issues knowledge queries one at a time (`InvestigationOrchestrator
 One GPU pass over the corpus costs the same for 1 query as for 128, so concurrent callers
 (several investigations in one process, the Slack gateway, hypothesis branches) should share a
 pass: this class coalesces `search()` calls that arrive within a short window into ONE
-`VectorStore.search_batch`, and hands every caller exactly what its own `search()` would have
-returned (per-query topK / minScore / filters are applied after the shared device call).
+device call, and hands every caller exactly what its own `search()` would have returned.  On an
+index with `search_each` that call is ONE search at every caller's own k_fetch = 2*topK and minScore,
+large callers included (a caller whose 2*topK is not an integer in [1, 4096] still goes through
+`VectorStore.search` alone: its own error, or a result that would make every row of the shared one
+that wide); on any other index object the shared pass fetches for the most demanding
+caller at the lowest minScore and each caller's own cut is re-applied on the host, while callers
+whose 2*topK exceeds the scan's candidate lists take `VectorStore.search` on their own.
 
     batcher = MicroBatcher(store, window_ms=2.0, max_batch=256)
     fut = batcher.submit("redis pool exhausted", {"topK": 5})     # concurrent.futures.Future
@@ -23,8 +28,14 @@ from concurrent.futures import Future
 import numpy as np
 
 from . import embedder as _emb
-from ._native import RBK_EDIM, RBK_MAX_K_FETCH, DimensionError
+from ._native import RBK_EDIM, RBK_MAX_K_FETCH, RBK_MAX_K_FETCH_LARGE, DimensionError
 from .vector_store import NOT_CONFIGURED, VectorStore, js_or
+
+
+def _shareable(k_fetch) -> bool:
+    """A k_fetch one search_each call can carry for everybody: an integer in [1, RBK_MAX_K_FETCH_LARGE]."""
+    return isinstance(k_fetch, (int, np.integer)) and not isinstance(k_fetch, bool) and \
+        1 <= k_fetch <= RBK_MAX_K_FETCH_LARGE
 
 
 class MicroBatcher:
@@ -93,6 +104,18 @@ class MicroBatcher:
             if not _emb.is_embedder_configured():
                 raise RuntimeError(NOT_CONFIGURED)
             st = self.store
+            if getattr(st._index, "search_each", None) is not None:
+                alone = [b for b in batch if not _shareable(2 * js_or(b[1].get("topK"), b[1].get("top_k"), 10))]
+                for q_, o_, f_ in alone:
+                    try:
+                        f_.set_result(st.search(q_, o_))
+                    except Exception as exc:
+                        f_.set_exception(exc)
+                    self.served += 1
+                batch = [b for b in batch if b not in alone]
+                if batch:
+                    self._serve_each(batch)
+                return
             # callers that want more than the scan's candidate lists hold (topK > 56) take the large-k path of
             # VectorStore.search on their own; everybody else shares one device pass
             big = [b for b in batch if 2 * js_or(b[1].get("topK"), b[1].get("top_k"), 10) > RBK_MAX_K_FETCH]
@@ -135,3 +158,26 @@ class MicroBatcher:
             for _, _, f in batch:
                 if not f.done():
                     f.set_exception(exc)
+
+    def _serve_each(self, batch) -> None:
+        """The whole window in one index.search_each: caller i at its own k_fetch = 2*topK and minScore, so its row is
+        exactly its own search()'s device answer (vector-store.ts:207-221) and only the hydration is left."""
+        st = self.store
+        qvec = np.asarray(_emb.embed_texts([b[0] for b in batch]), dtype=np.float64)
+        top_ks = [js_or(o.get("topK"), o.get("top_k"), 10) for _, o, _ in batch]
+        mins = [js_or(o.get("minScore"), o.get("min_score"), 0.5) for _, o, _ in batch]
+        with st._st.lock:   # state checks, scan and slot -> id lookup against the same table (the index may be shared)
+            if st._index is None or not st._ids:
+                for _, _, f in batch:
+                    f.set_result([])
+                return
+            if st._ragged or qvec.shape[1] != st._index.dim:
+                raise DimensionError(RBK_EDIM, "Vectors must have the same length")
+            slots, scores, counts, _ = st._index.search_each(qvec, [2 * k for k in top_ks], mins)
+            picked = [([st._ids[int(s)] for s in slots[i, :counts[i]]], scores[i, :counts[i]]) for i in range(len(batch))]
+        self.batches += 1
+        for i, (_, o, fut) in enumerate(batch):
+            ids_i, v_i = picked[i]
+            fut.set_result(st._hydrate(ids_i, v_i, top_ks[i], o.get("typeFilter") or o.get("type_filter"),
+                                       o.get("serviceFilter") or o.get("service_filter")))
+            self.served += 1

@@ -557,11 +557,13 @@ cudaError_t zero_scan_scratch(rbk_index* ix, int Bs) {
 }
 
 // The prep kernel for all B queries; it also zeroes the first sub-batch's scan scratch.
-rbk_status prep_queries(rbk_index* ix, const void* d_q, int src_type, int B, double min_score, bool with_norm2) {
+// min_each (nullable): each query's own min_score.
+rbk_status prep_queries(rbk_index* ix, const void* d_q, int src_type, int B, double min_score, bool with_norm2,
+                        const double* min_each = nullptr) {
   CK(launch_prep_queries(d_q, src_type, B, ix->dim, ix->dpad, min_score,
                          reinterpret_cast<const float*>(ix->d_counter + 1),
                          query_buffers(ix, 0), ix->stream, with_norm2, ix->hist.p, std::min(kMaxSubBatch, B),
-                         progress_slots(ix), ix->scan_f16));
+                         progress_slots(ix), ix->scan_f16, min_each));
   ix->stats.kernel_launches++;
   return RBK_OK;
 }
@@ -646,18 +648,47 @@ rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, i
   return RBK_OK;
 }
 
+rbk_status check_each_args(rbk_index* ix, int B, bool have_q, int query_dim, const int32_t* k, const double* min_score,
+                           int* K) {
+  *K = 0;
+  if (!ix) return fail(RBK_EINVAL, "null index");
+  if (B < 0 || (B > 0 && !have_q)) return fail(RBK_EINVAL, "bad queries argument");
+  if (B > 0 && (!k || !min_score)) return fail(RBK_EINVAL, "null k_fetch or min_score array");
+  for (int b = 0; b < B; ++b) {
+    if (k[b] < 1) return fail(RBK_EINVAL, "k_fetch[" + std::to_string(b) + "] must be >= 1");
+    *K = std::max(*K, static_cast<int>(k[b]));
+  }
+  if (query_dim != ix->dim) return fail(RBK_EDIM, "Vectors must have the same length");  // embedder.ts:170
+  for (int b = 0; b < B; ++b)
+    if (min_score[b] != min_score[b]) return fail(RBK_EINVAL, "min_score[" + std::to_string(b) + "] is NaN");
+  return RBK_OK;
+}
+
+rbk_status upload_cuts(rbk_index* ix, int B, const int32_t* k, const double* min_score, QueryCuts* out) {
+  CK(ix->e_k.ensure(B));
+  CK(ix->e_min.ensure(B));
+  // pageable sources: both copies have read the caller's arrays when they return
+  CK(cudaMemcpyAsync(ix->e_k.p, k, sizeof(int) * B, cudaMemcpyHostToDevice, ix->stream));
+  CK(cudaMemcpyAsync(ix->e_min.p, min_score, sizeof(double) * B, cudaMemcpyHostToDevice, ix->stream));
+  out->k = ix->e_k.p;
+  out->min_score = ix->e_min.p;
+  return RBK_OK;
+}
+
 }  // namespace impl
 }  // namespace rbk
 
 namespace {
 
-// Launch the scan (+ optionally finalize) for every sub-batch.  d_q: device queries.
+// Launch the scan (+ optionally finalize) for every sub-batch.  d_q: device queries.  each: per-query cuts (k_fetch is
+// then the largest k: it sets k' for the whole batch, and the row stride).
 rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_fetch, double min_score,
-                    long long* d_slots, double* d_scores, int* d_counts, int* d_flags, float* dbg) {
+                    long long* d_slots, double* d_scores, int* d_counts, int* d_flags, float* dbg,
+                    const QueryCuts& each = QueryCuts()) {
   const int kprime = pick_kprime(ix, k_fetch);
   ix->stats.last_kprime = kprime;
   // normA is left to the finalize kernel
-  rbk_status st = prep_queries(ix, d_q, src_type, B, min_score, /*with_norm2=*/d_counts == nullptr);
+  rbk_status st = prep_queries(ix, d_q, src_type, B, min_score, /*with_norm2=*/d_counts == nullptr, each.min_score);
   if (st != RBK_OK) return st;
   if (ix->n_rows == 0) {
     // nothing to scan: finalize would read unwritten lists; emit empty results directly
@@ -704,6 +735,8 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
       fp.out_scores = d_scores + static_cast<size_t>(q0) * k_fetch;
       fp.out_counts = d_counts + q0;
       fp.flags = d_flags + q0;
+      fp.k_each = each.k ? each.k + q0 : nullptr;
+      fp.min_each = each.min_score ? each.min_score + q0 : nullptr;
       CK(launch_finalize(fp, ix->rows_on_host, ix->x_elem, ix->stream));
       ix->stats.kernel_launches++;
     }
@@ -712,7 +745,7 @@ rbk_status run_scan(rbk_index* ix, const void* d_q, int src_type, int B, int k_f
 }
 
 rbk_status run_fallback(rbk_index* ix, const std::vector<int>& fails, int k_fetch, double min_score,
-                        long long* d_slots, double* d_scores, int* d_counts) {
+                        long long* d_slots, double* d_scores, int* d_counts, const QueryCuts& each = QueryCuts()) {
   const int nf = static_cast<int>(fails.size());
   const int nb = std::max(1, std::min<int>(ix->sm_count * 2, static_cast<int>((ix->n_rows + 255) / 256)));
   CK(ix->fail_list.ensure(nf));
@@ -742,6 +775,8 @@ rbk_status run_fallback(rbk_index* ix, const std::vector<int>& fails, int k_fetc
   ep.out_slots = d_slots;
   ep.out_scores = d_scores;
   ep.out_counts = d_counts;
+  ep.k_each = each.k;
+  ep.min_each = each.min_score;
   CK(launch_exact_fallback(ep, ix->x_elem, ix->stream));
   // pageable source: the copy above has completed its host read before returning
   ix->stats.kernel_launches += 2;
@@ -756,13 +791,13 @@ namespace impl {
 // Enqueue-only search of device-resident queries (caller holds the lock).  No host synchronisation: the
 // exactness flags land in d_flags and are the caller's to check (rbk_index_search_device_async, rbk_group.cu).
 rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, int k_fetch, double min_score,
-                          long long* d_slots, double* d_scores, int* d_counts, int* d_flags) {
+                          long long* d_slots, double* d_scores, int* d_counts, int* d_flags, const QueryCuts& each) {
   ix->stats.searches++;
   ix->stats.queries += B;
-  return run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr);
+  return run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr, each);
 }
 
-rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double min_score) {
+rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double min_score, const QueryCuts& each) {
   ix->stats.searches++;
   ix->stats.queries += B;
   ix->stats.last_kprime = k_eff;
@@ -775,7 +810,7 @@ rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double 
   CK(ix->h_loff.ensure(B));
   CK(ix->h_lerr.ensure(1));
   // normA is computed here: the re-rank has no spare thread to walk the chain beside its candidates
-  rbk_status st = prep_queries(ix, d_q, 0, B, min_score, /*with_norm2=*/true);
+  rbk_status st = prep_queries(ix, d_q, 0, B, min_score, /*with_norm2=*/true, each.min_score);
   if (st != RBK_OK) return st;
   if (ix->n_rows == 0) {
     memset(ix->h_lcap.p, 0, sizeof(int) * B);
@@ -790,7 +825,7 @@ rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double 
     st = launch_sub_batch<kScanCount>(ix, q0, sp);
     if (st != RBK_OK) return st;
     CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Bs, k_eff, static_cast<int>(ix->n_rows),
-                           ix->lg_theta.p + q0, ix->lg_cap.p + q0, ix->stream));
+                           ix->lg_theta.p + q0, ix->lg_cap.p + q0, ix->stream, each.k ? each.k + q0 : nullptr));
     ix->stats.kernel_launches++;
   }
   CK(cudaMemcpyAsync(ix->h_lcap.p, ix->lg_cap.p, sizeof(int) * B, cudaMemcpyDeviceToHost, ix->stream));
@@ -856,7 +891,7 @@ rbk_status large_prepare(rbk_index* ix, int B, bool sorted, const std::vector<st
 }
 
 rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, double min_score, long long* d_slots,
-                      double* d_scores, int* d_counts) {
+                      double* d_scores, int* d_counts, const QueryCuts& each) {
   if (ix->n_rows == 0) return fill_empty_results(ix, q1 - q0, k_eff, d_slots, d_scores, d_counts);
   int64_t group_tiles = 0;
   if (sorted)
@@ -899,6 +934,8 @@ rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, dou
     rp.out_scores = d_scores + static_cast<size_t>(s0 - q0) * k_eff;
     rp.out_counts = d_counts + (s0 - q0);
     rp.overflow = ix->lg_err.p;
+    rp.k_each = each.k ? each.k + s0 : nullptr;
+    rp.min_each = each.min_score ? each.min_score + s0 : nullptr;
     const int max_cap = *std::max_element(ix->h_lcap.p + s0, ix->h_lcap.p + s0 + Bs);
     SegSortScratch ss;
     if (sorted) {
@@ -974,6 +1011,8 @@ void release_scratch(rbk_index* ix) {
   ix->o_block.release();
   ix->h_block.release();
   ix->h_flags.release();
+  ix->e_k.release();
+  ix->e_min.release();
   ix->h_q.release();
 }
 
@@ -1083,10 +1122,13 @@ struct TimedSearch {
 };
 
 // Whole search, synchronous.  q_host/q_dev: exactly one is non-null.  Host outputs (out_*) may be null
-// (device-output variant); device outputs may be null (host variant uses index scratch).
+// (device-output variant); device outputs may be null (host variant uses index scratch).  k_each / min_each (host [B],
+// nullable; checked by the caller): a search_each call's cut and threshold per query, k_fetch their largest k; such a
+// call never replays the captured graph.
 rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int elem, int B, int query_dim,
                        int k_fetch, double min_score, long long* d_slots, double* d_scores, int* d_counts,
-                       int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out) {
+                       int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out,
+                       const int32_t* k_each = nullptr, const double* min_each = nullptr) {
   rbk_status st = check_search_args(ix, B, q_host || q_dev, query_dim, k_fetch, min_score);
   if (st != RBK_OK) return st;
   std::lock_guard<std::mutex> lk(ix->mu);
@@ -1116,7 +1158,12 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
     CK(ix->h_flags.ensure(B));
     h_flags = ix->h_flags.p;
   }
-  if (packed && q_host && B <= kBlockM && ix->n_rows > 0 && ix->use_graph) {
+  QueryCuts each;
+  if (k_each) {
+    st = upload_cuts(ix, B, k_each, min_each, &each);
+    if (st != RBK_OK) return st;
+  }
+  if (packed && q_host && B <= kBlockM && ix->n_rows > 0 && ix->use_graph && !k_each) {
     bool done = false;
     st = search_graph(ix, q_host, elem, B, k_fetch, min_score, L, &done);
     if (st != RBK_OK) return st;
@@ -1136,7 +1183,7 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
     d_q = ix->q_raw.p;
   }
   const int src_type = elem == 8 ? 0 : 1;
-  st = enqueue_search(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags);
+  st = enqueue_search(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, each);
   if (st != RBK_OK) return st;
   auto copy_back = [&]() -> cudaError_t {
     if (packed) return cudaMemcpyAsync(ix->h_block.p, ix->o_block.p, L.bytes, cudaMemcpyDeviceToHost, ix->stream);
@@ -1157,13 +1204,13 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
     // near-ties then fit among the candidates and the proof goes through.  Results of the queries that had
     // already passed are recomputed to the same values (both passes are exact).
     ix->kprime_override = kMaxKPrime;
-    st = run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr);
+    st = run_scan(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, nullptr, each);
     ix->kprime_override = 0;
     if (st != RBK_OK) return st;
     ix->stats.retry_batches++;
   }
   if (!fails.empty()) {
-    st = run_fallback(ix, fails, k_fetch, min_score, d_slots, d_scores, d_counts);
+    st = run_fallback(ix, fails, k_fetch, min_score, d_slots, d_scores, d_counts, each);
     if (st != RBK_OK) return st;
     // the exhaustive answers are exact by construction: clear the flags the caller may forward
     CK(cudaMemsetAsync(d_flags, 0, sizeof(int) * B, ix->stream));
@@ -1181,9 +1228,10 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
 namespace rbk {
 namespace impl {
 rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, int k_fetch, double min_score,
-                               long long* d_slots, double* d_scores, int* d_counts) {
+                               long long* d_slots, double* d_scores, int* d_counts, const int32_t* k_each,
+                               const double* min_each) {
   return search_core(ix, nullptr, d_q, elem, B, ix ? ix->dim : 0, k_fetch, min_score, d_slots, d_scores, d_counts,
-                     nullptr, nullptr, nullptr, nullptr);
+                     nullptr, nullptr, nullptr, nullptr, k_each, min_each);
 }
 
 int64_t compact_row_bytes(const rbk_index* ix) {
@@ -1831,10 +1879,11 @@ rbk_status rbk_index_search_device(rbk_index* ix, const void* dev_queries_f32, i
 namespace {
 // The large-k search for k_fetch in [1, max_k] (rbk_index_impl.h): the count scan, one wait, then per query group
 // the emit scan and the cut into o_block, its D2H into the pinned h_block, a wait, and the copy into the caller's rows
-// of k_fetch entries.
+// of k_fetch entries.  k_each / min_each (host [B], nullable; checked by the caller): a search_each call's own cut and
+// threshold per query, k_fetch their largest k; each query is then cut at its own k_eff.
 rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
                         double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
-                        float* kernel_ms_out) {
+                        float* kernel_ms_out, const int32_t* k_each = nullptr, const double* min_each = nullptr) {
   if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
   rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
   if (st != RBK_OK) return st;
@@ -1848,6 +1897,10 @@ rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t
   const bool sorted = k_fetch > RBK_MAX_K_FETCH_LARGE;
   // the sort's buffers are sized by k_eff: no query can have more hits than there are live rows
   const int k_eff = sorted ? static_cast<int>(std::min<int64_t>(k_fetch, ix->n_live)) : k_fetch;
+  std::vector<int32_t> k_eff_each;   // search_each: every query's own k_eff, by the same rule
+  if (k_each)
+    for (int b = 0; b < B; ++b)
+      k_eff_each.push_back(sorted ? static_cast<int32_t>(std::min<int64_t>(k_each[b], ix->n_live)) : k_each[b]);
   if (k_eff == 0) {
     fill_result_tail(out_slots, out_scores, B, k_fetch, 0);
     memset(out_counts, 0, sizeof(int32_t) * B);
@@ -1860,8 +1913,10 @@ rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t
   TimedSearch ts{ix};
   st = ts.begin();
   if (st != RBK_OK) return st;
+  QueryCuts each;
+  if (k_each && (st = upload_cuts(ix, B, k_eff_each.data(), min_each, &each)) != RBK_OK) return st;
   CK(cudaMemcpyAsync(ix->q_raw.p, queries, static_cast<size_t>(B) * ix->dim * 8, cudaMemcpyHostToDevice, ix->stream));
-  st = large_count(ix, ix->q_raw.p, B, k_eff, min_score);
+  st = large_count(ix, ix->q_raw.p, B, k_eff, min_score, each);
   if (st != RBK_OK) return st;
   CK(cudaStreamSynchronize(ix->stream));   // C_q sizes the candidate buffers and the query groups
   std::vector<int64_t> cost(B);
@@ -1878,7 +1933,8 @@ rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t
   for (const auto& gr : groups) {
     const ResultBlock R(gr.second - gr.first, k_eff);
     unsigned char* base = ix->o_block.p;
-    st = large_emit(ix, gr.first, gr.second, sorted, k_eff, min_score, R.slots(base), R.scores(base), R.counts(base));
+    st = large_emit(ix, gr.first, gr.second, sorted, k_eff, min_score, R.slots(base), R.scores(base), R.counts(base),
+                    each);
     if (st == RBK_OK && gr.second == B) st = large_finish(ix);   // the overflow count rides the last round trip
     if (st != RBK_OK) return st;
     CK(cudaMemcpyAsync(ix->h_block.p, base, R.off_counts + sizeof(int32_t) * R.B, cudaMemcpyDeviceToHost, ix->stream));
@@ -1906,6 +1962,29 @@ rbk_status rbk_index_search_unbounded_f64(rbk_index* ix, const double* queries, 
                                           int32_t* out_counts, float* kernel_ms_out) {
   return search_large(ix, queries, B, query_dim, k_fetch, min_score, INT32_MAX, out_slots, out_scores, out_counts,
                       kernel_ms_out);
+}
+
+rbk_status rbk_index_search_each_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
+                                     const int32_t* k_fetch, const double* min_score, int64_t* out_slots,
+                                     double* out_scores, int32_t* out_counts, float* kernel_ms_out) {
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  int K = 0;
+  rbk_status st = check_each_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, &K);
+  if (st != RBK_OK) return st;
+  if (B == 0) {
+    if (kernel_ms_out) *kernel_ms_out = 0.f;
+    std::lock_guard<std::mutex> lk(ix->mu);
+    ix->stats.searches++;
+    return RBK_OK;
+  }
+  // One route for the whole batch, picked by its largest k: the scan's top-k' with every query cut at its own k, or
+  // the two-scan large-k pipeline for every query (exact on either route, so a small k loses nothing there).  The
+  // scalar min_score of both is unused: every kernel that applies one reads the query's own.
+  if (K <= RBK_MAX_K_FETCH)
+    return search_core(ix, queries, nullptr, 8, B, query_dim, K, -INFINITY, nullptr, nullptr, nullptr, out_slots,
+                       out_scores, out_counts, kernel_ms_out, k_fetch, min_score);
+  return search_large(ix, queries, B, query_dim, K, -INFINITY, INT32_MAX, out_slots, out_scores, out_counts,
+                      kernel_ms_out, k_fetch, min_score);
 }
 
 rbk_status rbk_index_exact_scores_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,

@@ -111,11 +111,13 @@ __device__ __forceinline__ double exact_cosine(double dot, double na, double nb)
 // of rbk_f16.cuh, applied to the f64 query, or to the f32 one widened exactly); q_inv_norm = 1/||h|| (so it carries
 // the scale) and the angle in q_eps is that of h.  The query stays live or dead (q_inv_norm NaN, thr_init +inf) exactly
 // as in a bf16 index, so that the two tiers take the same decisions on zero, tiny or huge queries.
-template <typename SrcT, bool kNorm2, bool kF16>
+// kEach: the start threshold comes from the query's own min_each[q] (rbk_index_search_each_f64) instead of min_score.
+template <typename SrcT, bool kNorm2, bool kF16, bool kEach = false>
 __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restrict__ src, int d, int dpad,
                                                            double min_score, double acc_eps,
                                                            const float* __restrict__ eps_c, QueryBuffers qb,
-                                                           unsigned int* __restrict__ scratch, int Bs, int n_progress) {
+                                                           unsigned int* __restrict__ scratch, int Bs, int n_progress,
+                                                           const double* __restrict__ min_each) {
   const int q = blockIdx.x;
   const int tid = threadIdx.x;
   if (scratch != nullptr && q < Bs) {
@@ -274,17 +276,18 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const SrcT* __restric
     qb.q_eps[q] = eps;
     const float invf = ok ? static_cast<float>(inv) : __uint_as_float(0x7FC00000u);
     qb.q_inv_norm[q] = invf;
+    const double min_q = kEach ? min_each[q] : min_score;
     float thr;
     if (!ok || !(eps < kEpsNone)) {
       // zero / non-finite query: cosine is NaN for every row (S3) -> nothing matches; or a bound that proves
       // nothing: the scan is skipped and the query is answered exactly (finalize flags it, large_select emits all)
       thr = INFINITY;
-    } else if (min_score == -INFINITY) {
+    } else if (min_q == -INFINITY) {
       thr = -INFINITY;
     } else {
       // a row can only reach min_score if approx > min_score - eps; go to the raw domain
       // (divide by inv_norm_q) and step two ulps down so rounding never hides a row.
-      const double raw = (min_score - eps) / static_cast<double>(invf);
+      const double raw = (min_q - eps) / static_cast<double>(invf);
       float t = static_cast<float>(raw);
       t = nextafterf(nextafterf(t, -INFINITY), -INFINITY);
       thr = t;
@@ -326,7 +329,9 @@ constexpr int kHostLoads = 8;
 // kHostRows: rows_x is mapped host memory (RBK_INDEX_ROWS_ON_HOST).  Only the exact-row staging differs; the device-tier
 // instantiation compiles to the same code as before the host tier existed.  XT: the exact rows' element type (float
 // for RBK_INDEX_KEEP_F32), widened to double as it is staged, so the chains below see the same operands.
-template <bool kHostRows, typename XT>
+// kEach: the query's cut and threshold come from p.k_each / p.min_each (rbk_index_search_each_f64); p.k_fetch is the
+// row stride.  The scalar instantiations read neither array.
+template <bool kHostRows, typename XT, bool kEach>
 __device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
   const int ql = blockIdx.x;  // query index inside this launch
   const int tid = threadIdx.x;
@@ -657,17 +662,19 @@ __device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
   }
   __syncthreads();
   const double na = s_na;
+  const int k_q = kEach ? p.k_each[ql] : p.k_fetch;             // this query's cut (<= k_fetch, the row stride)
+  const double min_q = kEach ? p.min_each[ql] : p.min_score;    // and threshold
   if (tid < nsel) {
     const double sc = exact_cosine(dot, na, p.row_norm2[my_row]);
     s_score[tid] = sc;
     s_row[tid] = my_row;
-    const int ok = sc >= p.min_score ? 1 : 0;  // vector-store.ts:212 (NaN fails; -inf = no threshold)
+    const int ok = sc >= min_q ? 1 : 0;  // vector-store.ts:212 (NaN fails; -inf = no threshold)
     s_valid[tid] = ok;
     if (ok) atomicAdd(&s_nvalid, 1);
   }
   __syncthreads();
   const int nvalid = s_nvalid;
-  const int count = nvalid < p.k_fetch ? nvalid : p.k_fetch;
+  const int count = nvalid < k_q ? nvalid : k_q;
   // ---- final order: score desc, ties -> lower slot (stable sort over insertion order) ----
   if (tid < nsel && s_valid[tid]) {
     const double sc = s_score[tid];
@@ -678,11 +685,11 @@ __device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
       const double sj = s_score[j];
       rank += (sj > sc || (sj == sc && s_row[j] < row)) ? 1 : 0;
     }
-    if (rank < p.k_fetch) {
+    if (rank < k_q) {
       p.out_slots[static_cast<size_t>(ql) * p.k_fetch + rank] = p.slot.global(row);
       p.out_scores[static_cast<size_t>(ql) * p.k_fetch + rank] = sc;
     }
-    if (rank == p.k_fetch - 1) s_ekth = sc;
+    if (rank == k_q - 1) s_ekth = sc;
   }
   for (int i = count + tid; i < p.k_fetch; i += kFinThreads) {
     p.out_slots[static_cast<size_t>(ql) * p.k_fetch + i] = -1;
@@ -699,26 +706,51 @@ __device__ __forceinline__ void finalize_rows(const FinalizeParams& p) {
       ok = true;  // nothing was ever dropped except by thr_init (provably below min_score)
     } else {
       const double bound = static_cast<double>(tau_raw) * static_cast<double>(p.q.q_inv_norm[ql]) + p.q.q_eps[ql];
-      if (count == p.k_fetch) ok = s_ekth > bound;       // every outsider scores strictly below the k-th hit
-      else ok = bound < p.min_score;                      // no outsider can pass the threshold
+      if (count == k_q) ok = s_ekth > bound;             // every outsider scores strictly below the k-th hit
+      else ok = bound < min_q;                            // no outsider can pass the threshold
     }
     p.flags[ql] = ok ? 0 : 1;
   }
 }
 
+}  // namespace
+// The entry points of the three exact-row types (float64, float32, split float32) sit in a named namespace, so that
+// their symbols, which the build tests pair up by name across the row types, carry no hash of this file.
+namespace entry {
 // One kernel per exact-row type: float64 rows (finalize_kernel) and float32 rows (finalize_f32_kernel).
 template <bool kHostRows>
 __global__ void __launch_bounds__(kFinThreads) finalize_kernel(FinalizeParams p) {
-  finalize_rows<kHostRows, double>(p);
+  finalize_rows<kHostRows, double, false>(p);
 }
 template <bool kHostRows>
 __global__ void __launch_bounds__(kFinThreads) finalize_f32_kernel(FinalizeParams p) {
-  finalize_rows<kHostRows, float>(p);
+  finalize_rows<kHostRows, float, false>(p);
 }
 // and split float32 rows (finalize_split_kernel): low halves in rows_x, high halves in rows
 template <bool kHostRows>
 __global__ void __launch_bounds__(kFinThreads) finalize_split_kernel(FinalizeParams p) {
-  finalize_rows<kHostRows, F32Lo>(p);
+  finalize_rows<kHostRows, F32Lo, false>(p);
+}
+}  // namespace entry
+namespace {
+// The exact-row type of x_elem bytes per element, for the per-query kernels below (named by width, so that their
+// symbols stay apart from the scalar kernels' per-type ones).
+template <int kXElem>
+struct XOf {
+  using T = double;
+};
+template <>
+struct XOf<4> {
+  using T = float;
+};
+template <>
+struct XOf<2> {
+  using T = F32Lo;
+};
+// rbk_index_search_each_f64: every exact-row type and placement, each query at its own cut and threshold.
+template <bool kHostRows, int kXElem>
+__global__ void __launch_bounds__(kFinThreads) finalize_each_kernel(FinalizeParams p) {
+  finalize_rows<kHostRows, typename XOf<kXElem>::T, true>(p);
 }
 
 // --------------------------------------------------------------------------- exact fallback (K0)
@@ -787,8 +819,9 @@ __device__ __forceinline__ void exact_push(ExactTopK& t, double sc, int row) {
   t.row[pos] = row;
 }
 
-template <typename XT>
-__global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
+// kEach: each failing query is cut at its own p.k_each[q] and filtered at p.min_each[q]; p.k_fetch stays the stride.
+template <typename XT, bool kEach>
+__device__ __forceinline__ void exact_scan_rows(const ExactParams& p) {
   __shared__ ExactTopK t;
   const int tid = threadIdx.x;
   const int f = blockIdx.y;
@@ -803,12 +836,15 @@ __global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
   const int64_t r1 = r0 + chunk < p.n_rows ? r0 + chunk : p.n_rows;
   const double* qv = p.q_f64 + static_cast<size_t>(q) * p.d;
   const double na = p.q_norm2[q];
+  const double min_q = kEach ? p.min_each[q] : p.min_score;
+  // the cut is read where a compaction needs it, not held in a register across the scan
+  auto k_q = [&]() { return kEach ? __ldg(p.k_each + q) : p.k_fetch; };
   for (int64_t base = r0; base < r1; base += kExThreads) {
     // Every thread reads t.n before any push of this iteration moves it: read after the last barrier alone, a fast
     // thread's push could send a slow one into exact_compact's barriers without the others.
     const int n_now = t.n;
     __syncthreads();
-    if (n_now > kExBuf - kExThreads) exact_compact(t, p.k_fetch);
+    if (n_now > kExBuf - kExThreads) exact_compact(t, k_q());
     const int64_t row = base + tid;
     if (row < r1) {
       const bool dead = (p.dead_bits[row >> 5] >> (row & 31)) & 1u;
@@ -818,18 +854,26 @@ __global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
                                                              p.rows + static_cast<size_t>(row) * p.dpad)
                                              : exact_dot(qv, p.rows + static_cast<size_t>(row) * p.dpad, p.d);
         const double sc = exact_cosine(dot, na, p.row_norm2[row]);
-        if (sc >= p.min_score) exact_push(t, sc, static_cast<int>(row));
+        if (sc >= min_q) exact_push(t, sc, static_cast<int>(row));
       }
     }
     __syncthreads();
   }
-  exact_compact(t, p.k_fetch);
+  exact_compact(t, k_q());
   const size_t o = (static_cast<size_t>(f) * p.n_blocks + blockIdx.x) * p.k_fetch;
   for (int i = tid; i < t.n; i += kExThreads) {
     p.part_scores[o + i] = t.score[i];
     p.part_rows[o + i] = t.row[i];
   }
   if (tid == 0) p.part_cnt[f * p.n_blocks + blockIdx.x] = t.n;
+}
+template <typename XT>
+__global__ void __launch_bounds__(kExThreads) exact_scan_kernel(ExactParams p) {
+  exact_scan_rows<XT, false>(p);
+}
+template <int kXElem>
+__global__ void __launch_bounds__(kExThreads) exact_scan_each_kernel(ExactParams p) {
+  exact_scan_rows<typename XOf<kXElem>::T, true>(p);
 }
 
 __global__ void __launch_bounds__(kExThreads) exact_merge_kernel(ExactParams p) {
@@ -843,10 +887,11 @@ __global__ void __launch_bounds__(kExThreads) exact_merge_kernel(ExactParams p) 
   }
   __syncthreads();
   const int total = p.n_blocks * p.k_fetch;
+  const int k_q = p.k_each != nullptr ? p.k_each[q] : p.k_fetch;
   for (int base = 0; base < total; base += kExThreads) {
     const int n_now = t.n;   // read by every thread before any push moves it (as in exact_scan_kernel)
     __syncthreads();
-    if (n_now > kExBuf - kExThreads) exact_compact(t, p.k_fetch);
+    if (n_now > kExBuf - kExThreads) exact_compact(t, k_q);
     const int i = base + tid;
     if (i < total) {
       const int b = i / p.k_fetch, e = i % p.k_fetch;
@@ -857,7 +902,7 @@ __global__ void __launch_bounds__(kExThreads) exact_merge_kernel(ExactParams p) 
     }
     __syncthreads();
   }
-  exact_compact(t, p.k_fetch);
+  exact_compact(t, k_q);
   const int n = t.n;
   for (int i = tid; i < p.k_fetch; i += kExThreads) {
     const size_t o = static_cast<size_t>(q) * p.k_fetch + i;
@@ -881,9 +926,10 @@ __global__ void __launch_bounds__(256) large_select_kernel(const unsigned int* _
                                                            const float* __restrict__ inv_norm_q,
                                                            const double* __restrict__ q_eps, int k_fetch,
                                                            int n_rows, float* __restrict__ theta,
-                                                           int* __restrict__ cap) {
+                                                           int* __restrict__ cap, const int* __restrict__ k_each) {
   const int q = blockIdx.x;
   const int tid = threadIdx.x;
+  const unsigned int k_q = static_cast<unsigned int>(k_each != nullptr ? k_each[q] : k_fetch);
   __shared__ unsigned int s_grp[256];          // suffix sums over groups of 4 bins
   __shared__ unsigned int s_suf[kHistBins];    // rows counted in bins >= b
   __shared__ int s_top;
@@ -903,7 +949,7 @@ __global__ void __launch_bounds__(256) large_select_kernel(const unsigned int* _
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     s_suf[4 * tid + j] = suf;
-    if (suf >= static_cast<unsigned int>(k_fetch)) best = 4 * tid + j;
+    if (suf >= k_q) best = 4 * tid + j;
     suf -= c[j];
   }
   if (best >= 0) atomicMax(&s_top, best);
@@ -1047,6 +1093,8 @@ __device__ __forceinline__ void large_score_rows(const LargeRerankParams& p) {
   }
 }
 
+}  // namespace
+namespace entry {   // (see finalize_kernel)
 template <bool kHostRows>
 __global__ void __launch_bounds__(256) large_score_kernel(LargeRerankParams p) {
   large_score_rows<kHostRows, double>(p);
@@ -1059,6 +1107,8 @@ template <bool kHostRows>
 __global__ void __launch_bounds__(256) large_score_split_kernel(LargeRerankParams p) {
   large_score_rows<kHostRows, F32Lo>(p);
 }
+}  // namespace entry
+namespace {
 
 // re-rank, part 2: one block per query keeps the best k_fetch of its candidates by (score desc, row asc) in a
 // shared-memory buffer of S >= k_fetch + blockDim entries, compacted (bitonic sort, cut at k_fetch) whenever the next
@@ -1121,14 +1171,16 @@ __global__ void __launch_bounds__(kTopThreads) large_topk_kernel(LargeRerankPara
   const int emitted = p.emit_cnt[q];
   const int n_cand = min(emitted, p.emit_cap[q]);
   const size_t off = static_cast<size_t>(p.emit_off[q]);
+  const int k_q = p.k_each != nullptr ? p.k_each[q] : p.k_fetch;   // the query's cut; p.k_fetch is the row stride
+  const double min_q = p.min_each != nullptr ? p.min_each[q] : p.min_score;
   for (int base = 0; base < n_cand; base += kTopThreads) {
-    if (s_n > S - kTopThreads) large_compact(s_sc, s_rw, S, &s_n, p.k_fetch, &s_have, &s_ts, &s_tr);  // uniform
+    if (s_n > S - kTopThreads) large_compact(s_sc, s_rw, S, &s_n, k_q, &s_have, &s_ts, &s_tr);  // uniform
     const int i = base + tid;
     if (i < n_cand) {
       const double sc = p.cand_scores[off + i];
       const int row = p.emit_rows[off + i];
       // vector-store.ts:212 (NaN fails; -inf = no threshold), then only what can still make the cut
-      if (sc >= p.min_score && (!s_have || hit_before(sc, row, s_ts, s_tr))) {
+      if (sc >= min_q && (!s_have || hit_before(sc, row, s_ts, s_tr))) {
         const int pos = atomicAdd(&s_n, 1);
         s_sc[pos] = sc;
         s_rw[pos] = row;
@@ -1136,7 +1188,7 @@ __global__ void __launch_bounds__(kTopThreads) large_topk_kernel(LargeRerankPara
     }
     __syncthreads();
   }
-  large_compact(s_sc, s_rw, S, &s_n, p.k_fetch, &s_have, &s_ts, &s_tr);
+  large_compact(s_sc, s_rw, S, &s_n, k_q, &s_have, &s_ts, &s_tr);
   const int n = s_n;
   for (int i = tid; i < p.k_fetch; i += kTopThreads) {
     const size_t o = static_cast<size_t>(q) * p.k_fetch + i;
@@ -1179,6 +1231,7 @@ __global__ void __launch_bounds__(kSortThreads) seg_tile_sort_kernel(LargeRerank
   int S = 2;             // the bitonic network's width: a power of two >= m
   while (S < m) S <<= 1;
   const size_t base = static_cast<size_t>(p.emit_off[q]) + i0;
+  const double min_q = p.min_each != nullptr ? p.min_each[q] : p.min_score;
   if (tid == 0) s_pass = 0;
   __syncthreads();
   int mine = 0;
@@ -1187,7 +1240,7 @@ __global__ void __launch_bounds__(kSortThreads) seg_tile_sort_kernel(LargeRerank
     int rw = INT_MAX;    // after every real row, even one scoring -inf
     if (i < m) {
       const double v = p.cand_scores[base + i];
-      if (v >= p.min_score) {   // vector-store.ts:212 (NaN fails; -inf = no threshold)
+      if (v >= min_q) {   // vector-store.ts:212 (NaN fails; -inf = no threshold)
         sc = v;
         rw = p.emit_rows[base + i];
         ++mine;
@@ -1218,7 +1271,7 @@ __global__ void __launch_bounds__(kSortThreads) seg_tile_sort_kernel(LargeRerank
       __syncthreads();
     }
   }
-  const int L = min(s_pass, p.k_fetch);
+  const int L = min(s_pass, p.k_each != nullptr ? p.k_each[q] : p.k_fetch);   // truncated at the query's own cut
   for (int i = tid; i < L; i += kSortThreads) {
     p.cand_scores[base + i] = s_sc[i];
     p.emit_rows[base + i] = s_rw[i];
@@ -1226,7 +1279,9 @@ __global__ void __launch_bounds__(kSortThreads) seg_tile_sort_kernel(LargeRerank
   if (tid == 0) s.len[0][s.tile_off[q] + t] = L;
 }
 
-// Merge pass `pass` (0-based): runs of 2^pass tiles -> runs of 2^(pass+1) tiles.  One block per input tile.
+// Merge pass `pass` (0-based): runs of 2^pass tiles -> runs of 2^(pass+1) tiles.  One block per input tile.  kEach:
+// every run is truncated at its query's own p.k_each[q].
+template <bool kEach = false>
 __global__ void __launch_bounds__(kMergeThreads) seg_merge_kernel(LargeRerankParams p, SegSortScratch s, int pass) {
   const int q = blockIdx.y, t = blockIdx.x, tid = threadIdx.x;
   const int n = min(p.emit_cnt[q], p.emit_cap[q]);
@@ -1245,7 +1300,7 @@ __global__ void __launch_bounds__(kMergeThreads) seg_merge_kernel(LargeRerankPar
   int* len_out = (dst ? s.len[1] : s.len[0]) + s.tile_off[q];
   const int La = len_in[r * w];
   const int Lb = partner * w < nt ? len_in[partner * w] : 0;   // the last run of an odd count has no partner: copied
-  const int L = min(La + Lb, p.k_fetch);
+  const int L = min(La + Lb, kEach ? p.k_each[q] : p.k_fetch);
   if (local == 0 && (r & 1) == 0 && tid == 0) len_out[r * w] = L;
   const size_t seg = static_cast<size_t>(p.emit_off[q]);
   const size_t mine = seg + static_cast<size_t>(r) * w * kSortTile;
@@ -1331,7 +1386,8 @@ __global__ void __launch_bounds__(128) merge_shards_kernel(int G, int B, int k, 
                                                            const char* __restrict__ flags_base, size_t slots_stride,
                                                            size_t scores_stride, size_t counts_stride,
                                                            size_t flags_stride, long long* out_slots,
-                                                           double* out_scores, int* out_counts, int* out_flags) {
+                                                           double* out_scores, int* out_counts, int* out_flags,
+                                                           const int* __restrict__ k_each) {
   // shard g's arrays start g * stride bytes after shard 0's (dense [G][...] arrays: stride = array size;
   // packed per-rank blocks, e.g. straight out of ONE all-gather: the same block stride for all three)
   auto slots_of = [&](int g) { return reinterpret_cast<const long long*>(slots_base + g * slots_stride); };
@@ -1340,7 +1396,8 @@ __global__ void __launch_bounds__(128) merge_shards_kernel(int G, int B, int k, 
   const int b = blockIdx.x;
   int total = 0;
   for (int g = 0; g < G; ++g) total += count_of(g, b);
-  const int n_out = total < k ? total : k;
+  const int k_b = k_each != nullptr ? k_each[b] : k;   // query b's cut; k is the row stride of every list
+  const int n_out = total < k_b ? total : k_b;
   for (int i = threadIdx.x; i < G * k; i += blockDim.x) {
     const int g = i / k, e = i % k;
     if (e >= count_of(g, b)) continue;
@@ -1362,7 +1419,7 @@ __global__ void __launch_bounds__(128) merge_shards_kernel(int G, int B, int k, 
       }
       rank += lo;
     }
-    if (rank < k) {
+    if (rank < k_b) {
       out_slots[o + rank] = sl;
       out_scores[o + rank] = sc;
     }
@@ -1386,35 +1443,47 @@ __global__ void __launch_bounds__(128) merge_shards_kernel(int G, int B, int k, 
 
 }  // namespace
 
-template <typename SrcT, bool kNorm2>
+template <typename SrcT, bool kNorm2, bool kEach = false>
 void launch_prep_typed(const SrcT* src, bool f16, int B, int d, int dpad, double min_score, double acc_eps,
                        const float* eps_c, const QueryBuffers& qb, cudaStream_t stream, unsigned int* scratch, int Bs,
-                       int n_progress) {
+                       int n_progress, const double* min_each) {
   if (f16)
-    prep_queries_kernel<SrcT, kNorm2, true><<<B, 128, 0, stream>>>(src, d, dpad, min_score, acc_eps, eps_c, qb, scratch,
-                                                                   Bs, n_progress);
+    prep_queries_kernel<SrcT, kNorm2, true, kEach><<<B, 128, 0, stream>>>(src, d, dpad, min_score, acc_eps, eps_c, qb,
+                                                                          scratch, Bs, n_progress, min_each);
   else
-    prep_queries_kernel<SrcT, kNorm2, false><<<B, 128, 0, stream>>>(src, d, dpad, min_score, acc_eps, eps_c, qb,
-                                                                    scratch, Bs, n_progress);
+    prep_queries_kernel<SrcT, kNorm2, false, kEach><<<B, 128, 0, stream>>>(src, d, dpad, min_score, acc_eps, eps_c, qb,
+                                                                           scratch, Bs, n_progress, min_each);
 }
 
 cudaError_t launch_prep_queries(const void* src, int src_type, int B, int d, int dpad, double min_score,
                                 const float* eps_c, const QueryBuffers& qb, cudaStream_t stream, bool with_norm2,
-                                unsigned int* scratch, int Bs, int n_progress, bool f16) {
+                                unsigned int* scratch, int Bs, int n_progress, bool f16, const double* min_each) {
   if (B <= 0) return cudaSuccess;
   const double acc_eps = accumulation_eps(d);
   const double* sd = static_cast<const double*>(src);
   const float* sf = static_cast<const float*>(src);
-  if (src_type == 0) {
+  if (min_each != nullptr) {   // rbk_index_search_each_f64 takes float64 queries only
+    if (src_type != 0) return cudaErrorInvalidValue;
     if (with_norm2)
-      launch_prep_typed<double, true>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
+      launch_prep_typed<double, true, true>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs,
+                                            n_progress, min_each);
     else
-      launch_prep_typed<double, false>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
+      launch_prep_typed<double, false, true>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs,
+                                             n_progress, min_each);
+  } else if (src_type == 0) {
+    if (with_norm2)
+      launch_prep_typed<double, true>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress,
+                                      nullptr);
+    else
+      launch_prep_typed<double, false>(sd, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs,
+                                       n_progress, nullptr);
   } else {
     if (with_norm2)
-      launch_prep_typed<float, true>(sf, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
+      launch_prep_typed<float, true>(sf, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress,
+                                     nullptr);
     else
-      launch_prep_typed<float, false>(sf, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs, n_progress);
+      launch_prep_typed<float, false>(sf, f16, B, d, dpad, min_score, acc_eps, eps_c, qb, stream, scratch, Bs,
+                                      n_progress, nullptr);
   }
   return cudaGetLastError();
 }
@@ -1425,9 +1494,14 @@ cudaError_t launch_finalize(const FinalizeParams& p_in, bool rows_on_host, int x
   // >= 2048 keys (16 KB: room for 128 candidate rows x 56 elements per re-rank chunk)
   p.key_cap = p.B <= 160 ? 16384 : (p.B <= 320 ? 8192 : 2048);
   const size_t smem = static_cast<size_t>(p.key_cap) * 8;
+  using namespace entry;
   auto kernel = x_elem == 4   ? (rows_on_host ? finalize_f32_kernel<true> : finalize_f32_kernel<false>)
                 : x_elem == 2 ? (rows_on_host ? finalize_split_kernel<true> : finalize_split_kernel<false>)
                               : (rows_on_host ? finalize_kernel<true> : finalize_kernel<false>);
+  if (p.k_each != nullptr)   // rbk_index_search_each_f64 sets both arrays or neither
+    kernel = x_elem == 4   ? (rows_on_host ? finalize_each_kernel<true, 4> : finalize_each_kernel<false, 4>)
+             : x_elem == 2 ? (rows_on_host ? finalize_each_kernel<true, 2> : finalize_each_kernel<false, 2>)
+                           : (rows_on_host ? finalize_each_kernel<true, 8> : finalize_each_kernel<false, 8>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
   if (e != cudaSuccess) return e;
   kernel<<<p.B, kFinThreads, smem, stream>>>(p);
@@ -1437,9 +1511,17 @@ cudaError_t launch_finalize(const FinalizeParams& p_in, bool rows_on_host, int x
 cudaError_t launch_exact_fallback(const ExactParams& p, int x_elem, cudaStream_t stream) {
   if (p.n_fail <= 0) return cudaSuccess;
   dim3 grid(p.n_blocks, p.n_fail);
-  if (x_elem == 4) exact_scan_kernel<float><<<grid, kExThreads, 0, stream>>>(p);
-  else if (x_elem == 2) exact_scan_kernel<F32Lo><<<grid, kExThreads, 0, stream>>>(p);
-  else exact_scan_kernel<double><<<grid, kExThreads, 0, stream>>>(p);
+  if (p.k_each != nullptr) {   // rbk_index_search_each_f64 sets both arrays or neither
+    if (x_elem == 4) exact_scan_each_kernel<4><<<grid, kExThreads, 0, stream>>>(p);
+    else if (x_elem == 2) exact_scan_each_kernel<2><<<grid, kExThreads, 0, stream>>>(p);
+    else exact_scan_each_kernel<8><<<grid, kExThreads, 0, stream>>>(p);
+  } else if (x_elem == 4) {
+    exact_scan_kernel<float><<<grid, kExThreads, 0, stream>>>(p);
+  } else if (x_elem == 2) {
+    exact_scan_kernel<F32Lo><<<grid, kExThreads, 0, stream>>>(p);
+  } else {
+    exact_scan_kernel<double><<<grid, kExThreads, 0, stream>>>(p);
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   exact_merge_kernel<<<p.n_fail, kExThreads, 0, stream>>>(p);
@@ -1465,9 +1547,9 @@ cudaError_t launch_exact_scores(const uint16_t* rows, const void* rows_x, int x_
 
 cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init, const float* inv_norm_q,
                                 const double* q_eps, int B, int k_fetch, int n_rows, float* theta, int* cap,
-                                cudaStream_t stream) {
+                                cudaStream_t stream, const int* k_each) {
   if (B <= 0) return cudaSuccess;
-  large_select_kernel<<<B, 256, 0, stream>>>(hist, thr_init, inv_norm_q, q_eps, k_fetch, n_rows, theta, cap);
+  large_select_kernel<<<B, 256, 0, stream>>>(hist, thr_init, inv_norm_q, q_eps, k_fetch, n_rows, theta, cap, k_each);
   return cudaGetLastError();
 }
 
@@ -1481,6 +1563,7 @@ cudaError_t launch_large_emit_all(const double* q_eps, const unsigned int* dead_
 
 cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
                                 bool rows_on_host, int x_elem, cudaStream_t stream, int* launches) {
+  using namespace entry;
   *launches = 0;
   if (p.B <= 0) return cudaSuccess;
   cudaError_t e;
@@ -1520,7 +1603,8 @@ cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
     for (; (1 << passes) < s.max_tiles; ++passes) {
-      seg_merge_kernel<<<grid, kMergeThreads, 0, stream>>>(p, s, passes);
+      if (p.k_each != nullptr) seg_merge_kernel<true><<<grid, kMergeThreads, 0, stream>>>(p, s, passes);
+      else seg_merge_kernel<<<grid, kMergeThreads, 0, stream>>>(p, s, passes);
       if ((e = cudaGetLastError()) != cudaSuccess) return e;
       ++*launches;
     }
@@ -1536,13 +1620,13 @@ cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch
 cudaError_t launch_merge_shards(int G, int B, int k_fetch, const void* slots, const void* scores, const void* counts,
                                 const void* flags, size_t slots_stride, size_t scores_stride, size_t counts_stride,
                                 size_t flags_stride, long long* out_slots, double* out_scores, int* out_counts,
-                                int* out_flags, cudaStream_t stream) {
+                                int* out_flags, cudaStream_t stream, const int* k_each) {
   if (B <= 0) return cudaSuccess;
   merge_shards_kernel<<<B, 128, 0, stream>>>(G, B, k_fetch, static_cast<const char*>(slots),
                                              static_cast<const char*>(scores), static_cast<const char*>(counts),
                                              static_cast<const char*>(flags), slots_stride, scores_stride,
                                              counts_stride, flags_stride, out_slots, out_scores, out_counts,
-                                             flags ? out_flags : nullptr);
+                                             flags ? out_flags : nullptr, k_each);
   return cudaGetLastError();
 }
 

@@ -204,8 +204,8 @@ rbk_status stage_and_enqueue(rbk_group* g, const void* queries, int elem, const 
 
 // all-gather of the packed blocks (G > 1) + merge on device 0 into g->out; enqueue only.  Co-located members (a device
 // list with a repeat, no communicator): member 0's stream waits for every member's block and copies it into its own
-// `all` buffer.
-rbk_status exchange_and_merge(rbk_group* g, const ResultBlock& L, int k_fetch) {
+// `all` buffer.  k_each (nullable, on device 0): query b is cut at k_each[b], k_fetch being the row stride.
+rbk_status exchange_and_merge(rbk_group* g, const ResultBlock& L, int k_fetch, const int* k_each = nullptr) {
   if (g->G > 1 && g->comms.empty()) {
     for (int d = 1; d < g->G; ++d) {
       DeviceGuard dg(g->devices[d]);
@@ -238,7 +238,7 @@ rbk_status exchange_and_merge(rbk_group* g, const ResultBlock& L, int k_fetch) {
   unsigned char* o = g->out.p;
   CK(launch_merge_shards(g->G, static_cast<int>(L.B), k_fetch, base, base + L.off_scores, base + L.off_counts,
                          base + L.off_flags, L.bytes, L.bytes, L.bytes, L.bytes, L.slots(o), L.scores(o), L.counts(o),
-                         L.flags(o), g->parts[0]->stream));
+                         L.flags(o), g->parts[0]->stream, k_each));
   return RBK_OK;
 }
 
@@ -252,8 +252,11 @@ rbk_status collect(rbk_group* g, const ResultBlock& L) {
   return RBK_OK;
 }
 
+// k_each / min_each (host [B], nullable; checked by the caller): a search_each call's cut and threshold per query,
+// k_fetch their largest k.  Every member gets them on its own device; the merge reads member 0's copy.
 rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, int32_t query_dim, int32_t k_fetch,
-                        double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out) {
+                        double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out,
+                        const int32_t* k_each = nullptr, const double* min_each = nullptr) {
   if (!g) return fail(RBK_EINVAL, "null group");
   if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
   rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score);
@@ -263,13 +266,20 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
   std::lock_guard<std::mutex> lk(g->mu);
   const ResultBlock L(B, k_fetch);
   const int src_type = elem == 8 ? 0 : 1;
+  const int* merge_k = nullptr;
   st = stage_and_enqueue(g, queries, elem, L, /*zero_dirty=*/true, [&](int d, rbk_index* ix) {
     unsigned char* l = g->dev[d].local.p;
+    QueryCuts each;
+    if (k_each) {
+      rbk_status s2 = upload_cuts(ix, B, k_each, min_each, &each);
+      if (s2 != RBK_OK) return s2;
+      if (d == 0) merge_k = each.k;
+    }
     return enqueue_search(ix, g->dev[d].q.p, src_type, B, k_fetch, min_score, L.slots(l), L.scores(l), L.counts(l),
-                          L.flags(l));
+                          L.flags(l), each);
   });
   if (st != RBK_OK) return st;
-  st = exchange_and_merge(g, L, k_fetch);
+  st = exchange_and_merge(g, L, k_fetch, merge_k);
   if (st != RBK_OK) return st;
   st = collect(g, L);   // the ONE host round trip of an exact batch
   if (st != RBK_OK) return st;
@@ -283,12 +293,12 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
       unsigned char* l = g->dev[d].local.p;
       // the staged queries keep the caller's type: f64 ones must not be read as f32
       st = search_device_exact(g->parts[d], g->dev[d].q.p, elem, B, k_fetch, min_score, L.slots(l), L.scores(l),
-                               L.counts(l));
+                               L.counts(l), k_each, min_each);
       if (st != RBK_OK) return st;
       DeviceGuard dg(g->parts[d]->device);
       CK(cudaMemsetAsync(L.flags(l), 0, static_cast<size_t>(B) * 4, g->parts[d]->stream));   // exact by construction
     }
-    st = exchange_and_merge(g, L, k_fetch);
+    st = exchange_and_merge(g, L, k_fetch, merge_k);   // (the re-answer re-uploaded the same cuts in place)
     if (st != RBK_OK) return st;
     st = collect(g, L);
     if (st != RBK_OK) return st;
@@ -304,9 +314,10 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
 // re-score and cut on every device into its packed block of k_eff entries per query (flags zero: the answers are
 // exact by construction), the all-gather and merge of group_search, and the copy into the caller's rows of k_fetch
 // entries.
+// k_each / min_each: as for group_search; each query is cut at its own k_eff (by the same rule, from the group's count).
 rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
                               double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
-                              float* ms_out) {
+                              float* ms_out, const int32_t* k_each = nullptr, const double* min_each = nullptr) {
   if (!g) return fail(RBK_EINVAL, "null group");
   if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
   rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
@@ -321,8 +332,17 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
     memset(out_counts, 0, sizeof(int32_t) * B);
     return RBK_OK;
   }
+  std::vector<int32_t> k_eff_each;
+  if (k_each)
+    for (int b = 0; b < B; ++b)
+      k_eff_each.push_back(sorted ? static_cast<int32_t>(std::min<int64_t>(k_each[b], rbk_group_count(g))) : k_each[b]);
+  std::vector<QueryCuts> each(g->G);   // every member's copy of the cuts, on its own device
   st = stage_and_enqueue(g, queries, 8, ResultBlock(B, 1), /*zero_dirty=*/false, [&](int d, rbk_index* ix) {
-    return large_count(ix, g->dev[d].q.p, B, k_eff, min_score);
+    if (k_each) {
+      rbk_status s2 = upload_cuts(ix, B, k_eff_each.data(), min_each, &each[d]);
+      if (s2 != RBK_OK) return s2;
+    }
+    return large_count(ix, g->dev[d].q.p, B, k_eff, min_score, each[d]);
   });
   if (st != RBK_OK) return st;
   for (int d = 0; d < g->G; ++d) {
@@ -362,12 +382,13 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
       std::lock_guard<std::mutex> il(ix->mu);
       DeviceGuard dg(ix->device);
       unsigned char* l = g->dev[d].local.p;
-      st = large_emit(ix, gr.first, gr.second, sorted, k_eff, min_score, L.slots(l), L.scores(l), L.counts(l));
+      st = large_emit(ix, gr.first, gr.second, sorted, k_eff, min_score, L.slots(l), L.scores(l), L.counts(l),
+                      each[d]);
       if (st == RBK_OK && gr.second == B) st = large_finish(ix);   // the overflow count rides the last round trip
       if (st != RBK_OK) return st;
       CK(cudaMemsetAsync(L.flags(l), 0, static_cast<size_t>(Bg) * 4, ix->stream));
     }
-    st = exchange_and_merge(g, L, k_eff);
+    st = exchange_and_merge(g, L, k_eff, each[0].k ? each[0].k + gr.first : nullptr);   // the group's own rows
     if (st != RBK_OK) return st;
     st = collect(g, L);
     if (st != RBK_OK) return st;
@@ -801,6 +822,26 @@ rbk_status rbk_group_search_large_f64(rbk_group* g, const double* queries, int32
   return group_search_large(g, queries, B, query_dim, k_fetch, min_score, RBK_MAX_K_FETCH_LARGE, out_slots, out_scores,
                             out_counts, device_ms_out);
 }
+rbk_status rbk_group_search_each_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,
+                                     const int32_t* k_fetch, const double* min_score, int64_t* out_slots,
+                                     double* out_scores, int32_t* out_counts, float* device_ms_out) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  int K = 0;
+  rbk_status st = check_each_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score, &K);
+  if (st != RBK_OK) return st;
+  if (B == 0) {
+    if (device_ms_out) *device_ms_out = 0.f;
+    return RBK_OK;
+  }
+  // every member runs the route rbk_index_search_each_f64 picks for the batch's largest k
+  if (K <= RBK_MAX_K_FETCH)
+    return group_search(g, queries, 8, B, query_dim, K, -INFINITY, out_slots, out_scores, out_counts, device_ms_out,
+                        k_fetch, min_score);
+  return group_search_large(g, queries, B, query_dim, K, -INFINITY, INT32_MAX, out_slots, out_scores, out_counts,
+                            device_ms_out, k_fetch, min_score);
+}
+
 rbk_status rbk_group_search_unbounded_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,
                                           int32_t k_fetch, double min_score, int64_t* out_slots, double* out_scores,
                                           int32_t* out_counts, float* device_ms_out) {

@@ -205,6 +205,9 @@ struct rbk_index {
   rbk::impl::DevBuf<unsigned char> o_block;
   rbk::impl::PinBuf<unsigned char> h_block;
   rbk::impl::PinBuf<int> h_flags;
+  // rbk_index_search_each_f64: each query's k_fetch (or k_eff) and min_score on the device
+  rbk::impl::DevBuf<int> e_k;
+  rbk::impl::DevBuf<double> e_min;
   CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
@@ -238,6 +241,18 @@ struct rbk_index {
 namespace rbk {
 namespace impl {
 
+// The per-query cut and threshold of a search_each call, on one index's device (its e_k / e_min, [B]).  Both null in
+// every other search, which applies its scalar k_fetch and min_score to every query.
+struct QueryCuts {
+  const int* k = nullptr;
+  const double* min_score = nullptr;
+};
+// Copies k [B] and min_score [B] from the host into ix->e_k / ix->e_min (caller holds the lock, device current).
+rbk_status upload_cuts(rbk_index* ix, int B, const int32_t* k, const double* min_score, QueryCuts* out);
+// The argument checks of a search_each call, in check_search_args' order; *K = the largest k (0 when B == 0).
+rbk_status check_each_args(rbk_index* ix, int B, bool have_q, int query_dim, const int32_t* k, const double* min_score,
+                           int* K);
+
 // caller holds ix->mu and has the index's device current.  The scan's query buffer keeps kBlockM zeroed rows beyond
 // the last whole query block, so that a scan launch may start at any query (a large-k search's query groups): such a
 // launch's query map covers round_up(Bs, kBlockM) rows from its first query.
@@ -246,12 +261,16 @@ rbk_status ensure_query_scratch(rbk_index* ix, int B, int elem);
 rbk_status check_search_args(rbk_index* ix, int B, bool have_q, int query_dim, int k_fetch, double min_score,
                              int max_k = RBK_MAX_K_FETCH);
 // Enqueue-only search of device-resident queries: no host synchronisation, exactness flags land in d_flags.
+// each: a search_each call's per-query cut and threshold (k_fetch is then the row stride, their largest k).
 rbk_status enqueue_search(rbk_index* ix, const void* d_q, int src_type, int B, int k_fetch, double min_score,
-                          long long* d_slots, double* d_scores, int* d_counts, int* d_flags);
+                          long long* d_slots, double* d_scores, int* d_counts, int* d_flags,
+                          const QueryCuts& each = QueryCuts());
 // Synchronous exact search of device-resident queries of `elem` bytes (8 = f64, 4 = f32), retry and exhaustive
-// fallback included: rbk_index_search_device for either query type.  Takes the index lock itself.
+// fallback included: rbk_index_search_device for either query type.  Takes the index lock itself.  k_each / min_each
+// (host [B], nullable): a search_each call's own cut and threshold per query, k_fetch their largest k.
 rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, int k_fetch, double min_score,
-                               long long* d_slots, double* d_scores, int* d_counts);
+                               long long* d_slots, double* d_scores, int* d_counts, const int32_t* k_each = nullptr,
+                               const double* min_each = nullptr);
 // Large-k search of B device-resident f64 queries (caller holds the lock, scratch for B queries is allocated), for
 // any k_fetch above the scan's: the count scan, one host synchronisation, then the queries in contiguous groups whose
 // device storage fits kLargeBudget, each group costing one emit scan.  `sorted` (the caller's k_fetch is above
@@ -266,7 +285,10 @@ rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, 
 //                   ([q1 - q0][k_eff]); enqueue only;
 //   large_finish  : the D2H of the overflow counter (enqueue only);
 //   large_check   : (after the next synchronisation) RBK_ECUDA if any query emitted more rows than its bound.
-rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double min_score);
+// A search_each call passes its cuts (each.k: every query's own k_eff) to large_count and large_emit; k_eff is then the
+// largest of them: the count scan's running threshold and the row stride of the results.
+rbk_status large_count(rbk_index* ix, const void* d_q, int B, int k_eff, double min_score,
+                       const QueryCuts& each = QueryCuts());
 constexpr int64_t kLargeBudget = 256ll << 20;
 // device bytes per candidate: emit row + exact score (sorted in place), and the sort's second buffer
 inline int64_t large_cand_bytes(bool sorted) { return sorted ? 4 + 8 + 12 : 4 + 8; }
@@ -275,7 +297,7 @@ inline int64_t large_result_bytes(int k_eff) { return 16ll * k_eff + 8; }
 std::vector<std::pair<int, int>> split_by_budget(const std::vector<int64_t>& cost);
 rbk_status large_prepare(rbk_index* ix, int B, bool sorted, const std::vector<std::pair<int, int>>& groups);
 rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, double min_score, long long* d_slots,
-                      double* d_scores, int* d_counts);
+                      double* d_scores, int* d_counts, const QueryCuts& each = QueryCuts());
 rbk_status large_finish(rbk_index* ix);
 rbk_status large_check(rbk_index* ix);
 

@@ -155,9 +155,11 @@ struct QueryBuffers {
 // queries, n_progress pacing slots), zeroed by the kernel.
 // f16: the scan's copy follows the RBK_INDEX_SCAN_F16 rule (rbk_f16.cuh) and q_eps holds the angle of that rounding;
 // a query is live (finite q_inv_norm) exactly when it would be for a bf16 index.
+// min_each (nullable): each query's own min_score [B], in place of min_score.
 cudaError_t launch_prep_queries(const void* src, int src_type, int B, int d, int dpad, double min_score,
                                 const float* eps_c, const QueryBuffers& qb, cudaStream_t stream, bool with_norm2,
-                                unsigned int* scratch, int Bs, int n_progress, bool f16 = false);
+                                unsigned int* scratch, int Bs, int n_progress, bool f16 = false,
+                                const double* min_each = nullptr);
 
 // local row -> global slot.  Contiguous shards: slot_base + row.  A group that deals rows out block-cyclically over
 // G devices (rbk_group.cu): device g's local row r is global slot ((r / block) * G + g) * block + r % block - still
@@ -189,6 +191,10 @@ struct FinalizeParams {
   double* out_scores;     // [B][k_fetch]
   int* out_counts;        // [B]
   int* flags;             // [B] 1 = not provably exact -> exhaustive fallback
+  // rbk_index_search_each_f64: each query's own cut and threshold, [B] offset to the sub-batch like q (nullable: k_fetch
+  // and min_score for every query).  Then k_fetch is the row stride of the outputs, the largest k_each.
+  const int* k_each;
+  const double* min_each;
 };
 // rows_on_host: rows_x is mapped host memory (RBK_INDEX_ROWS_ON_HOST); the re-rank stages it with wide loads, more
 // of them in flight, to cover the PCIe round trip.  Same scores either way.  x_elem: bytes per exact-row element (8, 4
@@ -215,6 +221,8 @@ struct ExactParams {
   long long* out_slots;
   double* out_scores;
   int* out_counts;
+  const int* k_each;         // nullable: per-query cut and threshold, indexed like q_f64 (k_fetch is then the stride)
+  const double* min_each;
 };
 cudaError_t launch_exact_fallback(const ExactParams& p, int x_elem, cudaStream_t stream);
 
@@ -222,9 +230,10 @@ cudaError_t launch_exact_fallback(const ExactParams& p, int x_elem, cudaStream_t
 // theta [B] (raw domain) and cap [B] (C_q) from the count pass's histograms hist [B][kHistBins].
 // A query whose q_eps is not below kEpsNone gets theta = +inf (the emit scan skips it) and C_q = n_rows; then
 // launch_large_emit_all writes every live row into its segment.
+// k_each (nullable): each query's own k_fetch [B], in place of k_fetch.
 cudaError_t launch_large_select(const unsigned int* hist, const float* thr_init, const float* inv_norm_q,
                                 const double* q_eps, int B, int k_fetch, int n_rows, float* theta, int* cap,
-                                cudaStream_t stream);
+                                cudaStream_t stream, const int* k_each = nullptr);
 cudaError_t launch_large_emit_all(const double* q_eps, const unsigned int* dead_bits, int64_t n_rows, int B,
                                   const long long* emit_off, int* emit_cnt, int* emit_rows, cudaStream_t stream);
 struct LargeRerankParams {
@@ -245,6 +254,8 @@ struct LargeRerankParams {
   double* out_scores;       // [B][k_fetch]
   int* out_counts;          // [B]
   int* overflow;            // += queries whose emit pass found more rows than C_q (a broken count)
+  const int* k_each;        // nullable: per-query cut and threshold, offset to the sub-batch (k_fetch is then the
+  const double* min_each;   // row stride, the largest k_each)
 };
 
 // The cut of k_fetch > RBK_MAX_K_FETCH_LARGE: a segmented sort in global memory.  Each query's segment of emit_rows /
@@ -275,10 +286,11 @@ cudaError_t launch_exact_scores(const uint16_t* rows, const void* rows_x, int x_
 
 // slots/scores/counts/flags point at shard 0's arrays; shard g's arrays start g * <stride> bytes later.
 // flags (nullable): per-shard exactness flags i32[B]; out_flags: i32[B+1] ([b] = OR over shards, [B] += dirty queries).
+// k_each (nullable, device i32[B]): query b is cut at k_each[b]; k_fetch stays the row stride of every list.
 cudaError_t launch_merge_shards(int G, int B, int k_fetch, const void* slots, const void* scores, const void* counts,
                                 const void* flags, size_t slots_stride, size_t scores_stride, size_t counts_stride,
                                 size_t flags_stride, long long* out_slots, double* out_scores, int* out_counts,
-                                int* out_flags, cudaStream_t stream);
+                                int* out_flags, cudaStream_t stream, const int* k_each = nullptr);
 
 // Bound on the fp32 tensor-core accumulation + scaling error of an approximate cosine.
 inline double accumulation_eps(int d) { return (double)(d + 8) * (1.0 / 4194304.0); }  // (d+8) * 2^-22

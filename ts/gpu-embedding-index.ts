@@ -214,6 +214,43 @@ export class GpuEmbeddingIndex {
     }
   }
 
+  /** Whether bestEach is available: the loaded addon's library has the per-query search (rbk_*_search_each_f64). */
+  get hasBestEach(): boolean {
+    return this.index !== null && this.index.hasSearchEach === true;
+  }
+
+  /**
+   * bestBatch with each query at its own limit and minScore, in ONE native call (rbk_*_search_each_f64): one scan when
+   * every limit is <= 112, else the two scans of the large-k search for all of them.  Result b is exactly what
+   * best(queries[b], limits[b], minScores[b]) returns.  Throws against a library without the per-query search
+   * (hasBestEach false).
+   */
+  async bestEach(queries: number[][], limits: number[], minScores: number[]): Promise<ScoredId[][]> {
+    while (this.compacting) await this.compacting; // never search against a table that is being renumbered
+    if (!this.index || this.slotOfId.size === 0) return queries.map(() => []);
+    if (this.badIds.size > 0 || queries.some((q) => q.length !== this.dim)) {
+      throw new Error('Vectors must have the same length');
+    }
+    const B = queries.length;
+    const packed = new Float64Array(B * this.dim);
+    queries.forEach((q, b) => packed.set(q, b * this.dim));
+    const K = Math.max(1, ...limits);
+    this.inFlight++;
+    try {
+      const { slots, scores, counts } = await this.index.searchEach(
+        packed, B, Int32Array.from(limits), Float64Array.from(minScores));
+      return queries.map((_, b) => {
+        const out: ScoredId[] = [];
+        for (let i = 0; i < counts[b]; i++) {
+          out.push({ id: this.idOfSlot[Number(slots[b * K + i])]!, score: scores[b * K + i] });
+        }
+        return out;
+      });
+    } finally {
+      if (--this.inFlight === 0) this.drained.splice(0).forEach((wake) => wake());
+    }
+  }
+
   /**
    * Give the slots of deleted ids back (the reference's Map.delete frees its entry; a tombstone alone does not): the
    * device index moves its live rows down in Map order and returns oldToNew, through which slotOfId and idOfSlot are
@@ -280,10 +317,13 @@ export class GpuEmbeddingIndex {
 
 /**
  * Query micro-batcher (SURVEY 8f-3): concurrent `best()` calls that arrive within `windowMs` share ONE device pass
- * (`bestBatch`), and every caller gets exactly what its own `best()` would have returned - the pass fetches for the
- * most demanding caller (largest limit, lowest minScore) and each caller's own `>= minScore` and cut are re-applied.
- * runbookai_b200/batcher.py is the tested mirror of this class (same coalescing, same per-caller cut, same
- * behaviour on close).  Callers whose limit exceeds one scan (112) go through on their own, to the large-k search.
+ * and every caller gets exactly what its own `best()` would have returned.  With a library that has the per-query
+ * search (`hasBestEach`) the window is ONE `bestEach` at every caller's own limit and minScore, callers above one
+ * scan's limit (112) included; only a limit that is not an integer in [1, 4096] goes through on its own (its own error,
+ * or a result that would make every row of the shared one that wide).  Without it the pass (`bestBatch`) fetches for
+ * the most demanding caller (largest limit, lowest minScore), each caller's own `>= minScore` and cut are re-applied,
+ * and callers above 112 go through on their own, to the large-k search.  runbookai_b200/batcher.py is the tested
+ * mirror of this class (same coalescing, same per-caller answers, same behaviour on close).
  */
 export class SearchBatcher {
   private queue: Array<{
@@ -301,7 +341,8 @@ export class SearchBatcher {
 
   best(query: number[], limit: number, minScore: number): Promise<ScoredId[]> {
     if (this.closed) return Promise.reject(new Error('batcher closed'));
-    if (limit > 112) return this.index.best(query, limit, minScore);
+    const alone = this.index.hasBestEach ? !(Number.isInteger(limit) && limit >= 1 && limit <= 4096) : limit > 112;
+    if (alone) return this.index.best(query, limit, minScore);
     return new Promise((resolve, reject) => {
       this.queue.push({ query, limit, minScore, resolve, reject });
       if (this.queue.length >= this.maxBatch) this.flush();
@@ -322,9 +363,16 @@ export class SearchBatcher {
     const batch = this.queue.splice(0, this.maxBatch);
     if (batch.length === 0) return;
     if (this.queue.length > 0) this.timer = setTimeout(() => this.flush(), 0);
+    this.batches++;
+    if (this.index.hasBestEach) {
+      this.index
+        .bestEach(batch.map((w) => w.query), batch.map((w) => w.limit), batch.map((w) => w.minScore))
+        .then((all) => batch.forEach((w, i) => w.resolve(all[i])))
+        .catch((e) => batch.forEach((w) => w.reject(e)));
+      return;
+    }
     const limit = Math.max(...batch.map((w) => w.limit));
     const minScore = Math.min(...batch.map((w) => w.minScore));
-    this.batches++;
     this.index
       .bestBatch(batch.map((w) => w.query), limit, minScore)
       .then((all) =>
