@@ -341,6 +341,24 @@ rbk_status rbk_index_search_each_f64(rbk_index* idx, const double* queries, int3
 rbk_status rbk_index_exact_scores_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
                                       double* out_scores);
 
+/* Stored rows as queries ("the chunks most like this stored chunk"): row b of the result is exactly what
+ * rbk_index_search_each_f64 returns for one host query - the stored values of global slot query_slots[b] - at
+ * k_fetch[b] and min_score[b]: the same slots, fp64 score bits, count and -1 / quiet-NaN tail in the [B][K] layout,
+ * K = max_b k_fetch[b].  The stored values are the float64 row (RBK_INDEX_KEEP_F64), the float32 row widened
+ * (RBK_INDEX_KEEP_F32), the float32 joined from the scan copy's high half and the kept low half, widened
+ * (RBK_INDEX_KEEP_F32_SPLIT), or the bf16 row widened (no exact rows), on either placement and scan type; a NaN element
+ * may lose its payload bits.  The query's own slot is part of its answer.  Slots are global: an index answers only for
+ * [slot_base, slot_base + size()).  Argument checks, before any device work and in the order of
+ * rbk_index_search_each_f64: a null array with B > 0, a k_fetch[b] < 1, a NaN min_score[b] or a slot the index does
+ * not hold is RBK_EINVAL.  A tombstoned slot is RBK_EINVAL too, found on the device by the gather and reported after the
+ * round trip the search makes anyway; the outputs are then unspecified and nothing else changes.  B = 0 is RBK_OK.  One
+ * call adds 1 to the searches counter and B to the queries counter.  The slots are answered in chunks of 1024 queries,
+ * each taking the route of its own largest k, so device memory does not grow with B (a pass over every row of the
+ * index needs one chunk's scratch).  Synchronous. */
+rbk_status rbk_index_search_slots_f64(rbk_index* idx, const int64_t* query_slots, int32_t B, const int32_t* k_fetch,
+                                      const double* min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* kernel_ms_out);
+
 /* Enqueue-only variant: nothing is synchronised, the call returns as soon as the kernels are queued on the index
  * stream, so batches pipeline back to back and an exchange step (all-gather + rbk_merge_topk_packed_device) can be
  * queued behind it without a host round trip in between.  dev_out_flags_i32[B]: 0 = the answer of query b is
@@ -448,6 +466,13 @@ rbk_status rbk_group_search_unbounded_f64(rbk_group* grp, const double* queries,
 rbk_status rbk_group_search_each_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
                                      const int32_t* k_fetch, const double* min_score, int64_t* out_slots,
                                      double* out_scores, int32_t* out_counts, float* device_ms_out);
+/* rbk_index_search_slots_f64 over the group: the member that holds each global slot gathers its stored values into the
+ * group's pinned query staging (one round trip per chunk of 1024 queries, which also reports a tombstoned slot), then
+ * rbk_group_search_each_f64 runs from there.  A slot the group does not hold (>= rbk_group_size()) is RBK_EINVAL.  Same
+ * arguments, checks, layout and answers as the index call on a single index holding the same rows. */
+rbk_status rbk_group_search_slots_f64(rbk_group* grp, const int64_t* query_slots, int32_t B, const int32_t* k_fetch,
+                                      const double* min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* device_ms_out);
 
 /* ---- introspection ---- */
 typedef struct {

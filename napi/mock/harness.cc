@@ -347,6 +347,73 @@ int main(int argc, char** argv) {
     }
   }
 
+  // searchSlots(): optional slots.txt holds "slot kFetch minScore" triples (minScore may be -inf); results land in
+  // slots_* with rows of K = max kFetch entries.  has_search_slots.txt gets the hasSearchSlots getter first.  Then one
+  // call with a kFetch of 0 must reject with the library's message (err_slots), and one naming a slot past the end
+  // too (err_slots_range).
+  {
+    std::ifstream sf(g_dir + "/slots.txt");
+    std::vector<int64_t> qs;
+    std::vector<int32_t> ks_v;
+    std::vector<double> ms_v;
+    std::string ss, ks, ms;
+    while (sf >> ss >> ks >> ms) {
+      qs.push_back(strtoll(ss.c_str(), nullptr, 10));
+      ks_v.push_back(static_cast<int32_t>(strtol(ks.c_str(), nullptr, 10)));
+      ms_v.push_back(strtod(ms.c_str(), nullptr));
+    }
+    if (!qs.empty()) {
+      napi_value has = nullptr;
+      if (!mock::get_accessor(env, ix, "hasSearchSlots", &has, &err)) die("hasSearchSlots threw: " + err);
+      write_text("has_search_slots.txt", mock::as_bool(has) ? "1" : "0");
+      const int nb = static_cast<int>(qs.size());
+      int K = 0;
+      for (int32_t v : ks_v) K = v > K ? v : K;
+      auto call_slots = [&](const std::vector<int64_t>& sv, const std::vector<int32_t>& kv, Result* out) {
+        napi_value promise = nullptr, settled = nullptr;
+        if (!mock::call_method(env, ix, "searchSlots",
+                               {mock::typed_array(env, napi_bigint64_array, sv.data(), sv.size()), mock::number(env, nb),
+                                mock::typed_array(env, napi_int32_array, kv.data(), kv.size()),
+                                mock::typed_array(env, napi_float64_array, ms_v.data(), ms_v.size())},
+                               &promise, &err))
+          return false;
+        mock::run_event_loop(env);
+        const int state = mock::promise_state(promise, &settled);
+        if (state == 2) {
+          err = mock::error_message(settled);
+          return false;
+        }
+        if (state != 1) die("searchSlots() left its promise pending");
+        napi_typedarray_type t;
+        size_t n;
+        const void* p = mock::typed_data(mock::get_property(env, settled, "slots"), &t, &n);
+        if (!p || t != napi_bigint64_array || n != static_cast<size_t>(nb) * K) die("searchSlots slots are not [B*K]");
+        out->slots.assign(static_cast<const int64_t*>(p), static_cast<const int64_t*>(p) + n);
+        p = mock::typed_data(mock::get_property(env, settled, "scores"), &t, &n);
+        if (!p || t != napi_float64_array || n != static_cast<size_t>(nb) * K) die("searchSlots scores are not [B*K]");
+        out->scores.assign(static_cast<const double*>(p), static_cast<const double*>(p) + n);
+        p = mock::typed_data(mock::get_property(env, settled, "counts"), &t, &n);
+        if (!p || t != napi_int32_array || n != static_cast<size_t>(nb)) die("searchSlots counts are not [B]");
+        out->counts.assign(static_cast<const int32_t*>(p), static_cast<const int32_t*>(p) + n);
+        return true;
+      };
+      Result sr;
+      if (!call_slots(qs, ks_v, &sr)) die("searchSlots rejected: " + err);
+      write_bin("slots_slots.i64", sr.slots.data(), sr.slots.size() * 8);
+      write_bin("slots_scores.f64", sr.scores.data(), sr.scores.size() * 8);
+      write_bin("slots_counts.i32", sr.counts.data(), sr.counts.size() * 4);
+      std::vector<int32_t> bad = ks_v;
+      bad[0] = 0;
+      Result none;
+      if (call_slots(qs, bad, &none)) die("searchSlots with a kFetch of 0 did not reject");
+      log << "err_slots " << err << "\n";
+      std::vector<int64_t> far = qs;
+      far[0] = int64_t{1} << 40;
+      if (call_slots(far, ks_v, &none)) die("searchSlots past the last slot did not reject");
+      log << "err_slots_range " << err << "\n";
+    }
+  }
+
   // ---- error paths: each must surface as a JS exception / rejection with the reference's wording
   {
     std::vector<double> odd(static_cast<size_t>(dim) + 1, 1.0);

@@ -34,6 +34,9 @@
 //   await ix.searchEach(Float64Array queries, B, Int32Array kFetch, Float64Array minScore)   // each query at its own
 //        kFetch[b] and minScore[b]: the same result object with rows of K = max(kFetch) entries
 //   ix.hasSearchEach                           -> boolean: the library has searchEach (else it throws)
+//   await ix.searchSlots(BigInt64Array slots, B, Int32Array kFetch, Float64Array minScore)   // searchEach whose
+//        queries are the stored rows of those global slots, read where the index keeps them: the same result object
+//   ix.hasSearchSlots                          -> boolean: the library has searchSlots (else it throws)
 //
 // Build (where Node headers exist):  node-gyp with  libraries: ["-lrbk_knn"], include_dirs: ["../include"].
 #include <node_api.h>
@@ -75,6 +78,9 @@
 // The same for the per-query search; `searchEach` throws where it is missing.
 #pragma weak rbk_index_search_each_f64
 #pragma weak rbk_group_search_each_f64
+// The same for stored rows as queries; `searchSlots` throws where it is missing.
+#pragma weak rbk_index_search_slots_f64
+#pragma weak rbk_group_search_slots_f64
 
 namespace {
 
@@ -156,6 +162,14 @@ struct Handle {
                          double* v, int32_t* c) {
     return grp ? rbk_group_search_each_f64(grp, q, B, qdim, k, ms, s, v, c, nullptr)
                : rbk_index_search_each_f64(ix, q, B, qdim, k, ms, s, v, c, nullptr);
+  }
+  bool has_search_slots() const {
+    return grp ? rbk_group_search_slots_f64 != nullptr : rbk_index_search_slots_f64 != nullptr;
+  }
+  rbk_status search_slots(const int64_t* q, int32_t B, const int32_t* k, const double* ms, int64_t* s, double* v,
+                          int32_t* c) {
+    return grp ? rbk_group_search_slots_f64(grp, q, B, k, ms, s, v, c, nullptr)
+               : rbk_index_search_slots_f64(ix, q, B, k, ms, s, v, c, nullptr);
   }
 };
 
@@ -469,7 +483,8 @@ napi_value Count(napi_env env, napi_callback_info info) {
 }
 
 // ---- search: runs on a libuv worker so the JS thread never blocks on the GPU ----
-enum class SearchKind { kScan, kLarge, kUnbounded, kEach };   // search / searchLarge / searchUnbounded / searchEach
+// search / searchLarge / searchUnbounded / searchEach / searchSlots
+enum class SearchKind { kScan, kLarge, kUnbounded, kEach, kSlots };
 
 struct SearchJob {
   Handle* ix;
@@ -477,7 +492,8 @@ struct SearchJob {
   int32_t B, dim, k;
   SearchKind kind;
   double min_score;
-  std::vector<int32_t> k_each;      // searchEach: kFetch[B] and minScore[B]; k is then their largest k
+  std::vector<int64_t> query_slots;  // searchSlots: the queries' global slots [B]
+  std::vector<int32_t> k_each;      // searchEach, searchSlots: kFetch[B] and minScore[B]; k is then their largest k
   std::vector<double> min_each;
   std::vector<int64_t> slots;
   std::vector<double> scores;
@@ -490,6 +506,12 @@ struct SearchJob {
 
 void search_execute(napi_env, void* data) {
   SearchJob* j = static_cast<SearchJob*>(data);
+  if (j->kind == SearchKind::kSlots) {
+    j->st = j->ix->search_slots(j->query_slots.data(), j->B, j->k_each.data(), j->min_each.data(), j->slots.data(),
+                                j->scores.data(), j->counts.data());
+    if (j->st != RBK_OK) j->err = rbk_last_error();
+    return;
+  }
   if (j->kind == SearchKind::kEach) {
     j->st = j->ix->search_each(j->queries.data(), j->B, j->dim, j->k_each.data(), j->min_each.data(), j->slots.data(),
                                j->scores.data(), j->counts.data());
@@ -550,26 +572,38 @@ napi_value QueueSearch(napi_env env, napi_callback_info info, SearchKind kind) {
     napi_throw_error(env, nullptr, "searchEach: this librbk_knn.so has no per-query search (rbk_*_search_each_f64)");
     return nullptr;
   }
+  if (kind == SearchKind::kSlots && !ix->has_search_slots()) {
+    napi_throw_error(env, nullptr, "searchSlots: this librbk_knn.so has no search by slot (rbk_*_search_slots_f64)");
+    return nullptr;
+  }
+  const bool each = kind == SearchKind::kEach || kind == SearchKind::kSlots;
+  const char* what = kind == SearchKind::kSlots ? "searchSlots" : "searchEach";
   napi_typedarray_type t;
   size_t len;
   void* data;
   NAPI_OK(napi_get_typedarray_info(env, argv[0], &t, &len, &data, nullptr, nullptr));
+  if (kind == SearchKind::kSlots && t != napi_bigint64_array) {
+    napi_throw_type_error(env, nullptr, "searchSlots: slots must be a BigInt64Array");
+    return nullptr;
+  }
   int32_t B = 0;
   napi_get_value_int32(env, argv[1], &B);
   std::vector<int32_t> k_each;
   std::vector<double> min_each;
-  if (kind == SearchKind::kEach) {   // kFetch: Int32Array[B], minScore: Float64Array[B] (-Infinity: no threshold)
+  if (each) {   // kFetch: Int32Array[B], minScore: Float64Array[B] (-Infinity: no threshold)
     napi_typedarray_type tk, tm;
     size_t nk, nm;
     void *pk, *pm;
     if (napi_get_typedarray_info(env, argv[2], &tk, &nk, &pk, nullptr, nullptr) != napi_ok ||
         napi_get_typedarray_info(env, argv[3], &tm, &nm, &pm, nullptr, nullptr) != napi_ok ||
         tk != napi_int32_array || tm != napi_float64_array) {
-      napi_throw_type_error(env, nullptr, "searchEach: kFetch must be an Int32Array and minScore a Float64Array");
+      napi_throw_type_error(env, nullptr, (std::string(what) + ": kFetch must be an Int32Array and minScore a "
+                                                          "Float64Array").c_str());
       return nullptr;
     }
-    if (B < 0 || nk != static_cast<size_t>(B) || nm != static_cast<size_t>(B)) {
-      napi_throw_error(env, nullptr, "searchEach: kFetch and minScore need one entry per query");
+    if (B < 0 || nk != static_cast<size_t>(B) || nm != static_cast<size_t>(B) ||
+        (kind == SearchKind::kSlots && len != static_cast<size_t>(B))) {
+      napi_throw_error(env, nullptr, (std::string(what) + ": kFetch and minScore need one entry per query").c_str());
       return nullptr;
     }
     k_each.assign(static_cast<int32_t*>(pk), static_cast<int32_t*>(pk) + nk);
@@ -579,7 +613,7 @@ napi_value QueueSearch(napi_env env, napi_callback_info info, SearchKind kind) {
   j->ix = ix;
   j->kind = kind;
   j->B = B;
-  if (kind == SearchKind::kEach) {
+  if (each) {
     // the row stride; a kFetch[b] < 1 leaves it at 0 or 1, and the library refuses the call with its own message
     j->k = 0;
     for (int32_t v : k_each) j->k = std::max(j->k, v);
@@ -589,8 +623,12 @@ napi_value QueueSearch(napi_env env, napi_callback_info info, SearchKind kind) {
     napi_get_value_int32(env, argv[2], &j->k);
     napi_get_value_double(env, argv[3], &j->min_score);   // pass -Infinity for "no threshold"
   }
-  j->dim = j->B > 0 ? (int32_t)(len / (size_t)j->B) : 0;   // a wrong length surfaces as RBK_EDIM
-  j->queries.assign(static_cast<double*>(data), static_cast<double*>(data) + len);
+  if (kind == SearchKind::kSlots) {
+    j->query_slots.assign(static_cast<int64_t*>(data), static_cast<int64_t*>(data) + len);
+  } else {
+    j->dim = j->B > 0 ? (int32_t)(len / (size_t)j->B) : 0;   // a wrong length surfaces as RBK_EDIM
+    j->queries.assign(static_cast<double*>(data), static_cast<double*>(data) + len);
+  }
   j->slots.resize((size_t)j->B * j->k);
   j->scores.resize((size_t)j->B * j->k);
   j->counts.resize((size_t)j->B);
@@ -609,11 +647,21 @@ napi_value SearchUnbounded(napi_env env, napi_callback_info info) {
 }
 napi_value SearchEach(napi_env env, napi_callback_info info) { return QueueSearch(env, info, SearchKind::kEach); }
 
+napi_value SearchSlots(napi_env env, napi_callback_info info) { return QueueSearch(env, info, SearchKind::kSlots); }
+
 napi_value HasSearchEach(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
   napi_value out;
   NAPI_OK(napi_get_boolean(env, h->has_search_each(), &out));
+  return out;
+}
+
+napi_value HasSearchSlots(napi_env env, napi_callback_info info) {
+  size_t argc = 0;
+  Handle* h = unwrap(env, info, &argc, nullptr);
+  napi_value out;
+  NAPI_OK(napi_get_boolean(env, h->has_search_slots(), &out));
   return out;
 }
 
@@ -635,6 +683,8 @@ napi_value Init(napi_env env, napi_value exports) {
       {"searchUnbounded", nullptr, SearchUnbounded, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"searchEach", nullptr, SearchEach, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"hasSearchEach", nullptr, nullptr, HasSearchEach, nullptr, nullptr, napi_default, nullptr},
+      {"searchSlots", nullptr, SearchSlots, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"hasSearchSlots", nullptr, nullptr, HasSearchSlots, nullptr, nullptr, napi_default, nullptr},
   };
   napi_value cls;
   NAPI_OK(napi_define_class(env, "RbkIndex", NAPI_AUTO_LENGTH, New, nullptr, sizeof props / sizeof props[0], props, &cls));

@@ -38,6 +38,7 @@ SYMBOLS = [
     "rbk_group_search_large_f64", "rbk_group_search_unbounded_f64",
     "rbk_index_flags", "rbk_index_set_tier", "rbk_group_set_tier",
     "rbk_index_search_each_f64", "rbk_group_search_each_f64",
+    "rbk_index_search_slots_f64", "rbk_group_search_slots_f64",
 ]
 
 
@@ -133,6 +134,8 @@ def _load() -> C.CDLL:
         getattr(lib, n).argtypes = [vp, vp, i32, i32, i32, f64, vp, vp, vp, C.POINTER(C.c_float)]
     for n in ("rbk_index_search_each_f64", "rbk_group_search_each_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp, C.POINTER(C.c_float)]
+    for n in ("rbk_index_search_slots_f64", "rbk_group_search_slots_f64"):
+        getattr(lib, n).argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_debug_scores_f32.argtypes = [vp, vp, i32, vp]
     lib.rbk_index_flags.argtypes = [vp]
     lib.rbk_index_flags.restype = C.c_uint32
@@ -218,6 +221,17 @@ def _search_each(fn, h, queries, k_fetch, min_score):
     search_unbounded(queries[b], k_fetch[b], min_score[b]) returns, padded with -1 / NaN to K entries."""
     q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
     B = q.shape[0]
+    k32, m, K = _cuts(B, k_fetch, min_score)
+    slots = np.empty((B, K), dtype=np.int64)
+    scores = np.empty((B, K), dtype=np.float64)
+    counts = np.empty((B,), dtype=np.int32)
+    ms = C.c_float(0)
+    check(fn(h, ptr(q), B, q.shape[1], ptr(k32), ptr(m), ptr(slots), ptr(scores), ptr(counts), C.byref(ms)))
+    return slots, scores, counts, ms.value
+
+
+def _cuts(B: int, k_fetch, min_score):
+    """The int32 k_fetch [B], float64 min_score [B] and largest k of a search_each or search_slots call."""
     k = np.ascontiguousarray(np.asarray(k_fetch, dtype=np.int64).reshape(-1))
     ms_list = list(min_score) if np.ndim(min_score) else [min_score] * B
     m = np.ascontiguousarray([-np.inf if v is None else float(v) for v in ms_list], dtype=np.float64)
@@ -226,13 +240,21 @@ def _search_each(fn, h, queries, k_fetch, min_score):
     if (k < 1).any() or (k > np.iinfo(np.int32).max).any():
         raise RbkError(RBK_EINVAL, "every k_fetch must be in [1, 2^31 - 1]")
     k32 = k.astype(np.int32)
-    K = int(k32.max()) if B else 0
-    slots = np.empty((B, K), dtype=np.int64)
+    return k32, m, (int(k32.max()) if B else 0)
+
+
+def _search_slots(fn, h, slots, k_fetch, min_score):
+    """rbk_*_search_slots_f64: the stored rows of global slots [B] as the queries; k_fetch and min_score (None = -inf)
+    one per query or one for all.  Returns what _search_each returns for the host copies of those rows."""
+    sl = np.ascontiguousarray(np.asarray(slots, dtype=np.int64).reshape(-1))
+    B = sl.shape[0]
+    k32, m, K = _cuts(B, np.full(B, k_fetch) if np.ndim(k_fetch) == 0 else k_fetch, min_score)
+    out_slots = np.empty((B, K), dtype=np.int64)
     scores = np.empty((B, K), dtype=np.float64)
     counts = np.empty((B,), dtype=np.int32)
     ms = C.c_float(0)
-    check(fn(h, ptr(q), B, q.shape[1], ptr(k32), ptr(m), ptr(slots), ptr(scores), ptr(counts), C.byref(ms)))
-    return slots, scores, counts, ms.value
+    check(fn(h, ptr(sl), B, ptr(k32), ptr(m), ptr(out_slots), ptr(scores), ptr(counts), C.byref(ms)))
+    return out_slots, scores, counts, ms.value
 
 
 def _search_any_k(ix, queries, k_fetch: int, min_score):
@@ -447,6 +469,13 @@ class Index:
         min_score[b]); one scan for the batch when K <= RBK_MAX_K_FETCH, else the two scans of the large-k search."""
         return _search_each(lib.rbk_index_search_each_f64, self._h, queries, k_fetch, min_score)
 
+    def search_slots(self, slots, k_fetch, min_score):
+        """search_each() whose queries are the stored rows of global slots [B] (the exact rows widened to float64, or
+        the bf16 rows without them), read on the device: (slots [B, K], scores [B, K], counts [B], device_ms).  k_fetch
+        and min_score (None = -inf): one per query or one for all.  A query's own slot is among its hits; a slot this
+        index does not hold, or a tombstoned one, raises RbkError (RBK_EINVAL)."""
+        return _search_slots(lib.rbk_index_search_slots_f64, self._h, slots, k_fetch, min_score)
+
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: the reference's cosine of every row, NaN for tombstoned / zero rows."""
         q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
@@ -608,6 +637,10 @@ class Group:
     def search_each(self, queries, k_fetch, min_score):
         """Index.search_each() over the group: one call, every member on the route of the largest k."""
         return _search_each(lib.rbk_group_search_each_f64, self._h, queries, k_fetch, min_score)
+
+    def search_slots(self, slots, k_fetch, min_score):
+        """Index.search_slots() over the group: each slot's member gathers its row, then one search_each."""
+        return _search_slots(lib.rbk_group_search_slots_f64, self._h, slots, k_fetch, min_score)
 
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: every device's exact scores, put back in global slot order (4096-row blocks dealt

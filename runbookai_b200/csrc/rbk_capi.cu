@@ -675,6 +675,26 @@ rbk_status upload_cuts(rbk_index* ix, int B, const int32_t* k, const double* min
   return RBK_OK;
 }
 
+rbk_status gather_queries(rbk_index* ix, const int64_t* rows, int B) {
+  CK(ix->q_raw.ensure(static_cast<size_t>(B) * ix->dim * 8));
+  CK(ix->sq_rows.ensure(B));
+  CK(ix->sq_dead.ensure(1));
+  CK(ix->h_sq_dead.ensure(1));
+  // pageable source: the copy has read the caller's rows when it returns
+  CK(cudaMemcpyAsync(ix->sq_rows.p, rows, sizeof(int64_t) * B, cudaMemcpyHostToDevice, ix->stream));
+  CK(cudaMemsetAsync(ix->sq_dead.p, 0, sizeof(int), ix->stream));
+  CK(launch_gather_rows(ix->rows, ix->rows_x, ix->x_elem, ix->dead_bits, ix->sq_rows.p, B, ix->dim, ix->dpad,
+                        reinterpret_cast<double*>(ix->q_raw.p), ix->sq_dead.p, ix->stream));
+  ix->stats.kernel_launches++;
+  CK(cudaMemcpyAsync(ix->h_sq_dead.p, ix->sq_dead.p, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+  return RBK_OK;
+}
+
+rbk_status check_gathered(const rbk_index* ix) {
+  if (ix->h_sq_dead.p[0] == 0) return RBK_OK;
+  return fail(RBK_EINVAL, "query slot is tombstoned (" + std::to_string(ix->h_sq_dead.p[0]) + " of the batch)");
+}
+
 }  // namespace impl
 }  // namespace rbk
 
@@ -1013,6 +1033,9 @@ void release_scratch(rbk_index* ix) {
   ix->h_flags.release();
   ix->e_k.release();
   ix->e_min.release();
+  ix->sq_rows.release();
+  ix->sq_dead.release();
+  ix->h_sq_dead.release();
   ix->h_q.release();
 }
 
@@ -1121,18 +1144,38 @@ struct TimedSearch {
   }
 };
 
-// Whole search, synchronous.  q_host/q_dev: exactly one is non-null.  Host outputs (out_*) may be null
-// (device-output variant); device outputs may be null (host variant uses index scratch).  k_each / min_each (host [B],
-// nullable; checked by the caller): a search_each call's cut and threshold per query, k_fetch their largest k; such a
-// call never replays the captured graph.
-rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int elem, int B, int query_dim,
-                       int k_fetch, double min_score, long long* d_slots, double* d_scores, int* d_counts,
-                       int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out,
-                       const int32_t* k_each = nullptr, const double* min_each = nullptr) {
-  rbk_status st = check_search_args(ix, B, q_host || q_dev, query_dim, k_fetch, min_score);
-  if (st != RBK_OK) return st;
-  std::lock_guard<std::mutex> lk(ix->mu);
-  DeviceGuard dg(ix->device);
+// Where a synchronous search's queries come from, exactly one of: a host array (`host`, of the search's elem bytes
+// per element), queries already on the device (`dev`), or local rows of the index whose stored values are the queries
+// (`rows`, host [B]: rbk_index_search_slots_f64).  The H2D or the gather into q_raw is the search's first timed work.
+struct QuerySource {
+  const void* host = nullptr;
+  const void* dev = nullptr;
+  const int64_t* rows = nullptr;
+};
+
+rbk_status load_queries(rbk_index* ix, const QuerySource& q, int B, int elem, const void** d_q) {
+  *d_q = q.dev;
+  if (q.rows) {
+    rbk_status st = gather_queries(ix, q.rows, B);
+    if (st != RBK_OK) return st;
+    *d_q = ix->q_raw.p;
+  } else if (q.host) {
+    CK(cudaMemcpyAsync(ix->q_raw.p, q.host, static_cast<size_t>(B) * ix->dim * elem, cudaMemcpyHostToDevice,
+                       ix->stream));
+    *d_q = ix->q_raw.p;
+  }
+  return RBK_OK;
+}
+
+// Whole search, synchronous (caller holds the lock, device current, arguments checked).  Host outputs (out_*) may be
+// null (device-output variant); device outputs may be null (host variant uses index scratch).  k_each / min_each (host
+// [B], nullable; checked by the caller): a search_each call's cut and threshold per query, k_fetch their largest k; such
+// a call never replays the captured graph, nor does a search of gathered rows.
+rbk_status search_locked(rbk_index* ix, const QuerySource& q, int elem, int B, int k_fetch, double min_score,
+                         long long* d_slots, double* d_scores, int* d_counts, int64_t* out_slots, double* out_scores,
+                         int32_t* out_counts, float* ms_out, const int32_t* k_each = nullptr,
+                         const double* min_each = nullptr) {
+  rbk_status st;
   if (ms_out) *ms_out = 0.f;
   if (B == 0) {
     ix->stats.searches++;
@@ -1163,9 +1206,9 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
     st = upload_cuts(ix, B, k_each, min_each, &each);
     if (st != RBK_OK) return st;
   }
-  if (packed && q_host && B <= kBlockM && ix->n_rows > 0 && ix->use_graph && !k_each) {
+  if (packed && q.host && B <= kBlockM && ix->n_rows > 0 && ix->use_graph && !k_each) {
     bool done = false;
-    st = search_graph(ix, q_host, elem, B, k_fetch, min_score, L, &done);
+    st = search_graph(ix, q.host, elem, B, k_fetch, min_score, L, &done);
     if (st != RBK_OK) return st;
     if (done) {
       if (ms_out) *ms_out = ix->stats.last_total_ms;
@@ -1176,12 +1219,8 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
   TimedSearch ts{ix};
   st = ts.begin();
   if (st != RBK_OK) return st;
-  const void* d_q = q_dev;
-  if (q_host) {
-    CK(cudaMemcpyAsync(ix->q_raw.p, q_host, static_cast<size_t>(B) * ix->dim * elem, cudaMemcpyHostToDevice,
-                       ix->stream));
-    d_q = ix->q_raw.p;
-  }
+  const void* d_q = nullptr;
+  if ((st = load_queries(ix, q, B, elem, &d_q)) != RBK_OK) return st;
   const int src_type = elem == 8 ? 0 : 1;
   st = enqueue_search(ix, d_q, src_type, B, k_fetch, min_score, d_slots, d_scores, d_counts, d_flags, each);
   if (st != RBK_OK) return st;
@@ -1194,6 +1233,7 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
     CK(copy_back());
     st = ts.round_trip();   // the ONE host round trip of an exact batch
     if (st != RBK_OK) return st;
+    if (q.rows && (st = check_gathered(ix)) != RBK_OK) return st;
     fails.clear();
     for (int b = 0; b < B; ++b)
       if (h_flags[b]) fails.push_back(b);
@@ -1221,6 +1261,22 @@ rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int
   ts.finish(ms_out);
   if (out_slots) L.unpack(ix->h_block.p, out_slots, out_scores, out_counts);
   return RBK_OK;
+}
+
+// search_locked of host (q_host) or device (q_dev) queries, exactly one non-null: checks the arguments, takes the lock.
+rbk_status search_core(rbk_index* ix, const void* q_host, const void* q_dev, int elem, int B, int query_dim,
+                       int k_fetch, double min_score, long long* d_slots, double* d_scores, int* d_counts,
+                       int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out,
+                       const int32_t* k_each = nullptr, const double* min_each = nullptr) {
+  rbk_status st = check_search_args(ix, B, q_host || q_dev, query_dim, k_fetch, min_score);
+  if (st != RBK_OK) return st;
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  QuerySource q;
+  q.host = q_host;
+  q.dev = q_dev;
+  return search_locked(ix, q, elem, B, k_fetch, min_score, d_slots, d_scores, d_counts, out_slots, out_scores,
+                       out_counts, ms_out, k_each, min_each);
 }
 
 }  // namespace
@@ -1881,14 +1937,12 @@ namespace {
 // the emit scan and the cut into o_block, its D2H into the pinned h_block, a wait, and the copy into the caller's rows
 // of k_fetch entries.  k_each / min_each (host [B], nullable; checked by the caller): a search_each call's own cut and
 // threshold per query, k_fetch their largest k; each query is then cut at its own k_eff.
-rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
-                        double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
-                        float* kernel_ms_out, const int32_t* k_each = nullptr, const double* min_each = nullptr) {
-  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
-  rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
-  if (st != RBK_OK) return st;
-  std::lock_guard<std::mutex> lk(ix->mu);
-  DeviceGuard dg(ix->device);
+// large_locked: the caller holds the lock, has the device current and has checked the arguments; the queries come from
+// q (float64 ones).
+rbk_status large_locked(rbk_index* ix, const QuerySource& q, int32_t B, int32_t k_fetch, double min_score,
+                        int64_t* out_slots, double* out_scores, int32_t* out_counts, float* kernel_ms_out,
+                        const int32_t* k_each = nullptr, const double* min_each = nullptr) {
+  rbk_status st;
   if (kernel_ms_out) *kernel_ms_out = 0.f;
   if (B == 0) {
     ix->stats.searches++;
@@ -1915,10 +1969,12 @@ rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t
   if (st != RBK_OK) return st;
   QueryCuts each;
   if (k_each && (st = upload_cuts(ix, B, k_eff_each.data(), min_each, &each)) != RBK_OK) return st;
-  CK(cudaMemcpyAsync(ix->q_raw.p, queries, static_cast<size_t>(B) * ix->dim * 8, cudaMemcpyHostToDevice, ix->stream));
-  st = large_count(ix, ix->q_raw.p, B, k_eff, min_score, each);
+  const void* d_q = nullptr;
+  if ((st = load_queries(ix, q, B, 8, &d_q)) != RBK_OK) return st;
+  st = large_count(ix, d_q, B, k_eff, min_score, each);
   if (st != RBK_OK) return st;
   CK(cudaStreamSynchronize(ix->stream));   // C_q sizes the candidate buffers and the query groups
+  if (q.rows && (st = check_gathered(ix)) != RBK_OK) return st;
   std::vector<int64_t> cost(B);
   for (int b = 0; b < B; ++b) cost[b] = ix->h_lcap.p[b] * large_cand_bytes(sorted) + large_result_bytes(k_eff);
   const std::vector<std::pair<int, int>> groups = split_by_budget(cost);
@@ -1947,6 +2003,20 @@ rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t
   if (st != RBK_OK) return st;
   ts.finish(kernel_ms_out);
   return RBK_OK;
+}
+
+rbk_status search_large(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
+                        double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
+                        float* kernel_ms_out, const int32_t* k_each = nullptr, const double* min_each = nullptr) {
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  rbk_status st = check_search_args(ix, B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
+  if (st != RBK_OK) return st;
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  QuerySource q;
+  q.host = queries;
+  return large_locked(ix, q, B, k_fetch, min_score, out_slots, out_scores, out_counts, kernel_ms_out, k_each,
+                      min_each);
 }
 }  // namespace
 
@@ -1985,6 +2055,61 @@ rbk_status rbk_index_search_each_f64(rbk_index* ix, const double* queries, int32
                        out_scores, out_counts, kernel_ms_out, k_fetch, min_score);
   return search_large(ix, queries, B, query_dim, K, -INFINITY, INT32_MAX, out_slots, out_scores, out_counts,
                       kernel_ms_out, k_fetch, min_score);
+}
+
+rbk_status rbk_index_search_slots_f64(rbk_index* ix, const int64_t* query_slots, int32_t B, const int32_t* k_fetch,
+                                      const double* min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* kernel_ms_out) {
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  int K = 0;
+  rbk_status st = check_each_args(ix, B, query_slots != nullptr, ix ? ix->dim : 0, k_fetch, min_score, &K);
+  if (st != RBK_OK) return st;
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  if (kernel_ms_out) *kernel_ms_out = 0.f;
+  std::vector<int64_t> rows(B);
+  for (int b = 0; b < B; ++b) {
+    rows[b] = ix->slot.local(query_slots[b]);
+    if (rows[b] < 0 || rows[b] >= ix->n_rows)
+      return fail(RBK_EINVAL, "query_slots[" + std::to_string(b) + "] is not a slot of this index");
+  }
+  // every slot is held, so none is live: the large-k route would answer before its gather could say so
+  if (B > 0 && ix->n_live == 0) return fail(RBK_EINVAL, "query slot is tombstoned (the index has no live row)");
+  // one call is one search, however many chunks it takes
+  const int64_t searches = ix->stats.searches + 1;
+  std::vector<int64_t> c_slots;
+  std::vector<double> c_scores;
+  for (int c0 = 0; c0 < B; c0 += kSlotChunk) {
+    const int Bc = std::min(kSlotChunk, B - c0);
+    const int Kc = *std::max_element(k_fetch + c0, k_fetch + c0 + Bc);
+    const size_t o = static_cast<size_t>(c0) * K;
+    // a chunk's rows are Kc entries long: straight into the caller's rows when that is K, else through c_*
+    if (Kc < K) {
+      c_slots.resize(static_cast<size_t>(Bc) * Kc);
+      c_scores.resize(static_cast<size_t>(Bc) * Kc);
+    }
+    int64_t* cs = Kc < K ? c_slots.data() : out_slots + o;
+    double* cd = Kc < K ? c_scores.data() : out_scores + o;
+    QuerySource q;
+    q.rows = rows.data() + c0;
+    float ms = 0.f;
+    // the route rbk_index_search_each_f64 takes for the chunk's largest k
+    st = Kc <= RBK_MAX_K_FETCH
+             ? search_locked(ix, q, 8, Bc, Kc, -INFINITY, nullptr, nullptr, nullptr, cs, cd, out_counts + c0, &ms,
+                             k_fetch + c0, min_score + c0)
+             : large_locked(ix, q, Bc, Kc, -INFINITY, cs, cd, out_counts + c0, &ms, k_fetch + c0, min_score + c0);
+    if (st != RBK_OK) return st;
+    if (Kc < K) {
+      for (int b = 0; b < Bc; ++b) {
+        memcpy(out_slots + o + static_cast<size_t>(b) * K, cs + static_cast<size_t>(b) * Kc, sizeof(int64_t) * Kc);
+        memcpy(out_scores + o + static_cast<size_t>(b) * K, cd + static_cast<size_t>(b) * Kc, sizeof(double) * Kc);
+      }
+      fill_result_tail(out_slots + o, out_scores + o, Bc, K, Kc);
+    }
+    if (kernel_ms_out) *kernel_ms_out += ms;
+  }
+  ix->stats.searches = searches;
+  return RBK_OK;
 }
 
 rbk_status rbk_index_exact_scores_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,

@@ -92,6 +92,7 @@ struct rbk_group {
   std::vector<Dev> dev;
   DevBuf<unsigned char> out;     // device 0: the merged block (dirty_word)
   PinBuf<unsigned char> h_out, h_q;
+  PinBuf<double> h_sq;           // rbk_group_search_slots_f64: the members' gathered query rows
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int64_t redone_batches = 0;
 };
@@ -254,16 +255,11 @@ rbk_status collect(rbk_group* g, const ResultBlock& L) {
 
 // k_each / min_each (host [B], nullable; checked by the caller): a search_each call's cut and threshold per query,
 // k_fetch their largest k.  Every member gets them on its own device; the merge reads member 0's copy.
-rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, int32_t query_dim, int32_t k_fetch,
-                        double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out,
-                        const int32_t* k_each = nullptr, const double* min_each = nullptr) {
-  if (!g) return fail(RBK_EINVAL, "null group");
-  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
-  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score);
-  if (st != RBK_OK) return st;
-  if (ms_out) *ms_out = 0.f;
-  if (B == 0) return RBK_OK;
-  std::lock_guard<std::mutex> lk(g->mu);
+// group_search_locked: the caller holds g->mu and has checked the arguments (B > 0).
+rbk_status group_search_locked(rbk_group* g, const void* queries, int elem, int32_t B, int32_t k_fetch,
+                               double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts,
+                               float* ms_out, const int32_t* k_each = nullptr, const double* min_each = nullptr) {
+  rbk_status st;
   const ResultBlock L(B, k_fetch);
   const int src_type = elem == 8 ? 0 : 1;
   const int* merge_k = nullptr;
@@ -308,6 +304,20 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
   return RBK_OK;
 }
 
+rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, int32_t query_dim, int32_t k_fetch,
+                        double min_score, int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out,
+                        const int32_t* k_each = nullptr, const double* min_each = nullptr) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score);
+  if (st != RBK_OK) return st;
+  if (ms_out) *ms_out = 0.f;
+  if (B == 0) return RBK_OK;
+  std::lock_guard<std::mutex> lk(g->mu);
+  return group_search_locked(g, queries, elem, B, k_fetch, min_score, out_slots, out_scores, out_counts, ms_out, k_each,
+                             min_each);
+}
+
 // Large-k search over the group, k_fetch in [1, max_k] (the pipeline and the k_eff / cut rule of rbk_index_impl.h):
 // the count scan on every device and ONE wait for all of them, then the queries in contiguous groups whose candidates
 // on all devices together, plus the result blocks they move, fit kLargeBudget.  Per query group: emit scan, exact
@@ -315,16 +325,11 @@ rbk_status group_search(rbk_group* g, const void* queries, int elem, int32_t B, 
 // exact by construction), the all-gather and merge of group_search, and the copy into the caller's rows of k_fetch
 // entries.
 // k_each / min_each: as for group_search; each query is cut at its own k_eff (by the same rule, from the group's count).
-rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
-                              double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
-                              float* ms_out, const int32_t* k_each = nullptr, const double* min_each = nullptr) {
-  if (!g) return fail(RBK_EINVAL, "null group");
-  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
-  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
-  if (st != RBK_OK) return st;
-  if (ms_out) *ms_out = 0.f;
-  if (B == 0) return RBK_OK;
-  std::lock_guard<std::mutex> lk(g->mu);
+// group_search_large_locked: the caller holds g->mu and has checked the arguments (B > 0).
+rbk_status group_search_large_locked(rbk_group* g, const double* queries, int32_t B, int32_t k_fetch, double min_score,
+                                     int64_t* out_slots, double* out_scores, int32_t* out_counts, float* ms_out,
+                                     const int32_t* k_each = nullptr, const double* min_each = nullptr) {
+  rbk_status st;
   const bool sorted = k_fetch > RBK_MAX_K_FETCH_LARGE;
   const int k_eff = sorted ? static_cast<int>(std::min<int64_t>(k_fetch, rbk_group_count(g))) : k_fetch;
   if (k_eff == 0) {
@@ -404,6 +409,60 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
     if (st != RBK_OK) return st;
   }
   if (ms_out) cudaEventElapsedTime(ms_out, g->ev0, g->ev1);
+  return RBK_OK;
+}
+
+rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, int32_t query_dim, int32_t k_fetch,
+                              double min_score, int max_k, int64_t* out_slots, double* out_scores, int32_t* out_counts,
+                              float* ms_out, const int32_t* k_each = nullptr, const double* min_each = nullptr) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  rbk_status st = check_search_args(g->parts[0], B, queries != nullptr, query_dim, k_fetch, min_score, max_k);
+  if (st != RBK_OK) return st;
+  if (ms_out) *ms_out = 0.f;
+  if (B == 0) return RBK_OK;
+  std::lock_guard<std::mutex> lk(g->mu);
+  return group_search_large_locked(g, queries, B, k_fetch, min_score, out_slots, out_scores, out_counts, ms_out, k_each,
+                                   min_each);
+}
+
+// The stored values of global slots slots[0, B) (each < n_slots) as float64 queries into q [B][dim]: every member
+// gathers the rows it holds into its query scratch and copies them into the pinned staging g->h_sq, one wait per member,
+// which also brings back its count of tombstoned rows (RBK_EINVAL if any).  Caller holds g->mu.
+rbk_status group_gather(rbk_group* g, const int64_t* slots, int B, double* q) {
+  std::vector<std::vector<int64_t>> local, order;
+  split_slots(g, slots, B, &local, &order);
+  {
+    DeviceGuard dg(g->devices[0]);
+    CK(g->h_sq.ensure(static_cast<size_t>(B) * g->dim));
+  }
+  size_t first = 0;   // member d's rows land at h_sq rows [first, first + n) in member order
+  for (int d = 0; d < g->G; ++d) {
+    const int n = static_cast<int>(local[d].size());
+    if (n == 0) continue;
+    rbk_index* ix = g->parts[d];
+    std::lock_guard<std::mutex> il(ix->mu);
+    DeviceGuard dg(ix->device);
+    rbk_status st = gather_queries(ix, local[d].data(), n);
+    if (st != RBK_OK) return st;
+    CK(cudaMemcpyAsync(g->h_sq.p + first * g->dim, ix->q_raw.p, sizeof(double) * n * g->dim, cudaMemcpyDeviceToHost,
+                       ix->stream));
+    first += n;
+  }
+  first = 0;
+  for (int d = 0; d < g->G; ++d) {
+    const int n = static_cast<int>(local[d].size());
+    if (n == 0) continue;
+    rbk_index* ix = g->parts[d];
+    std::lock_guard<std::mutex> il(ix->mu);
+    DeviceGuard dg(ix->device);
+    CK(cudaStreamSynchronize(ix->stream));
+    rbk_status st = check_gathered(ix);
+    if (st != RBK_OK) return st;
+    for (int i = 0; i < n; ++i)
+      memcpy(q + static_cast<size_t>(order[d][i]) * g->dim, g->h_sq.p + (first + i) * g->dim, sizeof(double) * g->dim);
+    first += n;
+  }
   return RBK_OK;
 }
 
@@ -662,6 +721,7 @@ void rbk_group_destroy(rbk_group* g) {
     g->out.release();
     g->h_out.release();
     g->h_q.release();
+    g->h_sq.release();
     if (g->ev0) cudaEventDestroy(g->ev0);
     if (g->ev1) cudaEventDestroy(g->ev1);
   }
@@ -749,6 +809,7 @@ rbk_status rbk_group_trim(rbk_group* g) {
   g->out.release();
   g->h_out.release();
   g->h_q.release();
+  g->h_sq.release();
   return RBK_OK;
 }
 
@@ -840,6 +901,55 @@ rbk_status rbk_group_search_each_f64(rbk_group* g, const double* queries, int32_
                         k_fetch, min_score);
   return group_search_large(g, queries, B, query_dim, K, -INFINITY, INT32_MAX, out_slots, out_scores, out_counts,
                             device_ms_out, k_fetch, min_score);
+}
+
+rbk_status rbk_group_search_slots_f64(rbk_group* g, const int64_t* query_slots, int32_t B, const int32_t* k_fetch,
+                                      const double* min_score, int64_t* out_slots, double* out_scores,
+                                      int32_t* out_counts, float* device_ms_out) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  int K = 0;
+  rbk_status st = check_each_args(g->parts[0], B, query_slots != nullptr, g->dim, k_fetch, min_score, &K);
+  if (st != RBK_OK) return st;
+  if (device_ms_out) *device_ms_out = 0.f;
+  std::lock_guard<std::mutex> lk(g->mu);
+  for (int b = 0; b < B; ++b)
+    if (query_slots[b] < 0 || query_slots[b] >= g->n_slots)
+      return fail(RBK_EINVAL, "query_slots[" + std::to_string(b) + "] is not a slot of this group");
+  std::vector<double> q;
+  std::vector<int64_t> c_slots;
+  std::vector<double> c_scores;
+  for (int c0 = 0; c0 < B; c0 += kSlotChunk) {
+    const int Bc = std::min(kSlotChunk, B - c0);
+    const int Kc = *std::max_element(k_fetch + c0, k_fetch + c0 + Bc);
+    q.resize(static_cast<size_t>(Bc) * g->dim);
+    st = group_gather(g, query_slots + c0, Bc, q.data());
+    if (st != RBK_OK) return st;
+    // as in rbk_index_search_slots_f64: a chunk's rows are Kc entries long
+    const size_t o = static_cast<size_t>(c0) * K;
+    if (Kc < K) {
+      c_slots.resize(static_cast<size_t>(Bc) * Kc);
+      c_scores.resize(static_cast<size_t>(Bc) * Kc);
+    }
+    int64_t* cs = Kc < K ? c_slots.data() : out_slots + o;
+    double* cd = Kc < K ? c_scores.data() : out_scores + o;
+    float ms = 0.f;
+    st = Kc <= RBK_MAX_K_FETCH
+             ? group_search_locked(g, q.data(), 8, Bc, Kc, -INFINITY, cs, cd, out_counts + c0, &ms, k_fetch + c0,
+                                   min_score + c0)
+             : group_search_large_locked(g, q.data(), Bc, Kc, -INFINITY, cs, cd, out_counts + c0, &ms, k_fetch + c0,
+                                         min_score + c0);
+    if (st != RBK_OK) return st;
+    if (Kc < K) {
+      for (int b = 0; b < Bc; ++b) {
+        memcpy(out_slots + o + static_cast<size_t>(b) * K, cs + static_cast<size_t>(b) * Kc, sizeof(int64_t) * Kc);
+        memcpy(out_scores + o + static_cast<size_t>(b) * K, cd + static_cast<size_t>(b) * Kc, sizeof(double) * Kc);
+      }
+      fill_result_tail(out_slots + o, out_scores + o, Bc, K, Kc);
+    }
+    if (device_ms_out) *device_ms_out += ms;
+  }
+  return RBK_OK;
 }
 
 rbk_status rbk_group_search_unbounded_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,

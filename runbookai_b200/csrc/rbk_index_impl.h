@@ -208,6 +208,10 @@ struct rbk_index {
   // rbk_index_search_each_f64: each query's k_fetch (or k_eff) and min_score on the device
   rbk::impl::DevBuf<int> e_k;
   rbk::impl::DevBuf<double> e_min;
+  // rbk_index_search_slots_f64: one chunk's local query rows, and the count of tombstoned ones (device, pinned copy)
+  rbk::impl::DevBuf<int64_t> sq_rows;
+  rbk::impl::DevBuf<int> sq_dead;
+  rbk::impl::PinBuf<int> h_sq_dead;
   CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
@@ -252,6 +256,16 @@ rbk_status upload_cuts(rbk_index* ix, int B, const int32_t* k, const double* min
 // The argument checks of a search_each call, in check_search_args' order; *K = the largest k (0 when B == 0).
 rbk_status check_each_args(rbk_index* ix, int B, bool have_q, int query_dim, const int32_t* k, const double* min_score,
                            int* K);
+
+// A search_slots call works through its slots in chunks of this many queries, each one search, so that its device
+// scratch is that of one chunk however many slots it names.
+constexpr int kSlotChunk = 1024;
+// Enqueues the gather of the stored values of local rows rows[0, B) (host, each < n_rows) into ix->q_raw as float64
+// queries, and the copy of the number of tombstoned ones into ix->h_sq_dead[0], which the caller reads after its next
+// synchronisation of the stream (caller holds the lock, device current).
+rbk_status gather_queries(rbk_index* ix, const int64_t* rows, int B);
+// RBK_EINVAL when the last gather met a tombstoned row (after the synchronisation that follows it).
+rbk_status check_gathered(const rbk_index* ix);
 
 // caller holds ix->mu and has the index's device current.  The scan's query buffer keeps kBlockM zeroed rows beyond
 // the last whole query block, so that a scan launch may start at any query (a large-k search's query groups): such a

@@ -115,6 +115,13 @@ cudaError_t launch_row_norms(const uint16_t* rows_base, const void* rows_x_base,
                              const unsigned int* dead_bits = nullptr, bool f16 = false);
 cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows, float* inv_norm,
                              unsigned int* dead_bits, int* n_killed, cudaStream_t stream);
+// (rbk_gather.cu) Query b = the stored values of local row sel[b] (device [B], each < n_rows) as float64, into dst [B][d]: the exact
+// row widened (x_elem 8 / 4), the split's float32 rebuilt from both halves (x_elem 2), or the bf16 scan copy widened
+// (x_elem 0; never an RBK_INDEX_SCAN_F16 index, which keeps exact rows).  rows_x may be mapped host memory.  Adds the
+// number of tombstoned rows among them to *n_dead.
+cudaError_t launch_gather_rows(const uint16_t* rows, const void* rows_x, int x_elem, const unsigned int* dead_bits,
+                               const int64_t* sel, int B, int d, int dpad, double* dst, int* n_dead,
+                               cudaStream_t stream);
 // *found = 1 if any of the n doubles at src (device or mapped host memory) is one a float32 cannot hold (else *found is
 // left as it is): x is accepted iff it is NaN or (double)(float)x == x (so +-0, +-inf and float32 subnormals are, 0.1
 // and 1e-300 are not).
@@ -170,6 +177,12 @@ struct SlotLayout {
   __host__ __device__ int64_t global(int64_t row) const {
     if (block == 0) return base + row;
     return ((row / block) * G + g) * block + row % block;
+  }
+  // the inverse of global(): the local row of global slot s, or -1 when this shard does not deal it
+  __host__ __device__ int64_t local(int64_t s) const {
+    if (block == 0) return s >= base ? s - base : -1;
+    if (s < 0 || (s / block) % G != g) return -1;
+    return (s / block / G) * block + s % block;
   }
 };
 

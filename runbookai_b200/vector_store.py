@@ -677,6 +677,44 @@ class VectorStore:
         return [self._hydrate(ids[b], scores[b, :counts[b]], top_k, type_filter, service_filter)
                 for b in range(len(queries))]
 
+    def search_similar(self, chunk_id: str, options: dict | None = None, **kw) -> list[RetrievedChunk]:
+        """The chunks most like a stored chunk: search() whose query is the stored embedding of `vec_<chunk_id>`, read
+        where the index keeps it - no embedder call, so no API key.  Options as search(), plus excludeSelf (default
+        true): the chunk itself is left out, which gives search() on a store without it.  KeyError for a chunk id the
+        store does not hold (or has deleted); DimensionError on a ragged store, as search()."""
+        return self.search_similar_batch([chunk_id], options, **kw)[0]
+
+    def search_similar_batch(self, chunk_ids: Sequence[str], options: dict | None = None,
+                             **kw) -> list[list[RetrievedChunk]]:
+        """search_similar() for every chunk id, in one device call."""
+        o = dict(options or {})
+        o.update(kw)
+        top_k = js_or(o.get("topK"), o.get("top_k"), 10)
+        min_score = js_or(o.get("minScore"), o.get("min_score"), 0.5)
+        type_filter = o.get("typeFilter") or o.get("type_filter")
+        service_filter = o.get("serviceFilter") or o.get("service_filter")
+        exclude_self = o.get("excludeSelf", o.get("exclude_self", True))
+        vids = [f"vec_{c}" for c in chunk_ids]
+        with self._st.lock:   # the query slots and the slot table must be the ones the scan ran against
+            if self._ragged:
+                raise DimensionError(RBK_EDIM, "Vectors must have the same length")
+            for c, v in zip(chunk_ids, vids):
+                if v not in self._slot_of:
+                    raise KeyError(c)
+            if not vids:
+                return []
+            # one more hit than the cut, so that the cut still has 2*topK once the chunk itself is dropped
+            slots, scores, counts, _ = self._index.search_slots([self._slot_of[v] for v in vids],
+                                                                2 * top_k + (1 if exclude_self else 0), min_score)
+            hits = [[(self._ids[int(s)], float(sc)) for s, sc in zip(slots[b, :counts[b]], scores[b, :counts[b]])]
+                    for b in range(len(vids))]
+        out = []
+        for vid, h in zip(vids, hits):
+            if exclude_self:
+                h = [p for p in h if p[0] != vid][:int(2 * top_k)]
+            out.append(self._hydrate([i for i, _ in h], [sc for _, sc in h], top_k, type_filter, service_filter))
+        return out
+
     def _hydrate(self, top_ids, scores, top_k, type_filter, service_filter) -> list[RetrievedChunk]:
         """vector-store.ts:223-279 (a4): stays on the host."""
         pairs = [(i, float(sc)) for i, sc in zip(top_ids, scores) if i is not None]   # None: deleted meanwhile

@@ -251,6 +251,43 @@ export class GpuEmbeddingIndex {
     }
   }
 
+  /** Whether similarEach is available: the loaded addon's library has search by slot (rbk_*_search_slots_f64). */
+  get hasSimilarEach(): boolean {
+    return this.index !== null && this.index.hasSearchSlots === true;
+  }
+
+  /**
+   * bestEach whose queries are the stored embeddings of ids (the chunks most like a stored chunk), read where the index
+   * keeps them: no embedding call.  Result b is exactly what best(embedding of ids[b], limits[b], minScores[b]) returns,
+   * ids[b] itself included.  Throws for an id the Map does not hold, and against a library without search by slot
+   * (hasSimilarEach false).
+   */
+  async similarEach(ids: string[], limits: number[], minScores: number[]): Promise<ScoredId[][]> {
+    while (this.compacting) await this.compacting; // never search against a table that is being renumbered
+    if (this.badIds.size > 0) throw new Error('Vectors must have the same length');
+    const querySlots = ids.map((id) => {
+      const slot = this.slotOfId.get(id);
+      if (slot === undefined) throw new Error(`no embedding for id ${id}`);
+      return BigInt(slot);
+    });
+    if (!this.index || ids.length === 0) return [];
+    const K = Math.max(1, ...limits);
+    this.inFlight++;
+    try {
+      const { slots, scores, counts } = await this.index.searchSlots(
+        BigInt64Array.from(querySlots), ids.length, Int32Array.from(limits), Float64Array.from(minScores));
+      return ids.map((_, b) => {
+        const out: ScoredId[] = [];
+        for (let i = 0; i < counts[b]; i++) {
+          out.push({ id: this.idOfSlot[Number(slots[b * K + i])]!, score: scores[b * K + i] });
+        }
+        return out;
+      });
+    } finally {
+      if (--this.inFlight === 0) this.drained.splice(0).forEach((wake) => wake());
+    }
+  }
+
   /**
    * Give the slots of deleted ids back (the reference's Map.delete frees its entry; a tombstone alone does not): the
    * device index moves its live rows down in Map order and returns oldToNew, through which slotOfId and idOfSlot are
