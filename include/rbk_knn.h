@@ -359,6 +359,32 @@ rbk_status rbk_index_search_slots_f64(rbk_index* idx, const int64_t* query_slots
                                       const double* min_score, int64_t* out_slots, double* out_scores,
                                       int32_t* out_counts, float* kernel_ms_out);
 
+/* Every pair of stored rows at or above a cosine threshold ("which chunks are near-duplicates of each other"): each
+ * pair of live global slots a < b with first_slot <= a < *next_slot whose fp64 cosine of the stored values (those
+ * rbk_index_search_slots_f64 uses as a query) is >= min_score (inclusive; -INFINITY = every pair).  The score is bit for
+ * bit the reference's cosineSimilarity(row_a, row_b), which is symmetric in the bits - every product commutes exactly
+ * and sqrt(na) * sqrt(nb) == sqrt(nb) * sqrt(na) - so keeping only b > a loses nothing.  out_a[i], out_b[i],
+ * out_scores[i] for i < *n_out, ascending a, then score descending, ties by ascending b: the entries with first element a
+ * are exactly those of rbk_index_search_slots_f64({a}, count(), min_score) whose slot is > a, in the same order with
+ * the same score bits.  A tombstoned a contributes nothing (it is not refused); zero rows and rows containing NaN pair
+ * with nothing.
+ * Paging: the call returns the pairs of the longest run of query rows from first_slot that fits in max_pairs entries
+ * (never part of a row's pairs) and sets *next_slot to the first row not answered, slot_base + size() when the pass is
+ * complete; the next call continues there, and the pages concatenate to one call with a large enough buffer.  The rows
+ * go in chunks of 1024: when the buffer fills, the rest of that chunk's work is discarded and re-done by the next call.
+ * Argument checks, before any device work and in the order of the other searches: a null output, a NaN min_score, a
+ * first_slot outside [slot_base, slot_base + size()] or max_pairs < max(size(), 1) (so that every call makes progress)
+ * is RBK_EINVAL, and so is a call on a group member.  first_slot == slot_base + size() is RBK_OK with no pairs.  One call
+ * adds 1 to the searches counter and *next_slot - first_slot to the queries counter.
+ * How: per chunk [a0, a0 + Q), the gather of rbk_index_search_slots_f64, then the large-k pipeline over the rows from a0
+ * on only (the scans start at the tile holding a0), with theta_q from min_score and the query's error bound alone (no
+ * k), the exact re-score, the drop of b <= a, the global-memory sort with no cut, and the pairs packed query after query;
+ * one round trip brings back the counts, another the rows that fit.  Device memory stays within the large-k per-pass
+ * budget however many pairs there are.  kernel_ms_out (nullable): device time of the call.  Synchronous. */
+rbk_status rbk_index_similar_pairs_f64(rbk_index* idx, double min_score, int64_t first_slot, int64_t max_pairs,
+                                       int64_t* out_a, int64_t* out_b, double* out_scores, int64_t* n_out,
+                                       int64_t* next_slot, float* kernel_ms_out);
+
 /* Enqueue-only variant: nothing is synchronised, the call returns as soon as the kernels are queued on the index
  * stream, so batches pipeline back to back and an exchange step (all-gather + rbk_merge_topk_packed_device) can be
  * queued behind it without a host round trip in between.  dev_out_flags_i32[B]: 0 = the answer of query b is
@@ -473,6 +499,13 @@ rbk_status rbk_group_search_each_f64(rbk_group* grp, const double* queries, int3
 rbk_status rbk_group_search_slots_f64(rbk_group* grp, const int64_t* query_slots, int32_t B, const int32_t* k_fetch,
                                       const double* min_score, int64_t* out_slots, double* out_scores,
                                       int32_t* out_counts, float* device_ms_out);
+/* rbk_index_similar_pairs_f64 over the group's global slots [0, rbk_group_size()): the same arguments, checks, paging
+ * and answers as a single index holding the same rows.  Per chunk the owners gather its rows into the group's pinned
+ * query staging, every member pairs them with its own rows from the chunk's first slot on, and the host merges the
+ * members' sorted lists per query.  Every member's counters take the call.  Uses no NCCL. */
+rbk_status rbk_group_similar_pairs_f64(rbk_group* grp, double min_score, int64_t first_slot, int64_t max_pairs,
+                                       int64_t* out_a, int64_t* out_b, double* out_scores, int64_t* n_out,
+                                       int64_t* next_slot, float* device_ms_out);
 
 /* ---- introspection ---- */
 typedef struct {

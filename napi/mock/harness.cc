@@ -414,6 +414,68 @@ int main(int argc, char** argv) {
     }
   }
 
+  // similarPairs(): optional pairs.txt holds "minScore maxPairs" (minScore may be -inf).  has_similar_pairs.txt gets the
+  // hasSimilarPairs getter first; then the pages from slot 0 on, each of at most maxPairs entries, until nextSlot is
+  // n_rows, land concatenated in pairs_a / pairs_b / pairs_scores, and the page count in pairs_pages.txt.  Then one call
+  // with maxPairs 0 must reject with the library's message (err_pairs).
+  {
+    std::ifstream pf(g_dir + "/pairs.txt");
+    std::string ms_s, mp_s;
+    if (pf >> ms_s >> mp_s) {
+      napi_value has = nullptr;
+      if (!mock::get_accessor(env, ix, "hasSimilarPairs", &has, &err)) die("hasSimilarPairs threw: " + err);
+      write_text("has_similar_pairs.txt", mock::as_bool(has) ? "1" : "0");
+      const double ms = strtod(ms_s.c_str(), nullptr);
+      const double mp = strtod(mp_s.c_str(), nullptr);
+      std::vector<int64_t> all_a, all_b;
+      std::vector<double> all_s;
+      auto call_pairs = [&](double first, double max_pairs, double* next) {
+        napi_value promise = nullptr, settled = nullptr;
+        if (!mock::call_method(env, ix, "similarPairs",
+                               {mock::number(env, ms), mock::number(env, first), mock::number(env, max_pairs)},
+                               &promise, &err))
+          return false;
+        mock::run_event_loop(env);
+        const int state = mock::promise_state(promise, &settled);
+        if (state == 2) {
+          err = mock::error_message(settled);
+          return false;
+        }
+        if (state != 1) die("similarPairs() left its promise pending");
+        napi_typedarray_type t;
+        size_t na, nb, nv;
+        const void* pa = mock::typed_data(mock::get_property(env, settled, "a"), &t, &na);
+        if (!pa || t != napi_bigint64_array) die("similarPairs a is not a BigInt64Array");
+        const void* pb = mock::typed_data(mock::get_property(env, settled, "b"), &t, &nb);
+        if (!pb || t != napi_bigint64_array) die("similarPairs b is not a BigInt64Array");
+        const void* pv = mock::typed_data(mock::get_property(env, settled, "scores"), &t, &nv);
+        if (!pv || t != napi_float64_array) die("similarPairs scores is not a Float64Array");
+        if (na != nb || na != nv || na > static_cast<size_t>(max_pairs)) die("similarPairs arrays disagree");
+        all_a.insert(all_a.end(), static_cast<const int64_t*>(pa), static_cast<const int64_t*>(pa) + na);
+        all_b.insert(all_b.end(), static_cast<const int64_t*>(pb), static_cast<const int64_t*>(pb) + nb);
+        all_s.insert(all_s.end(), static_cast<const double*>(pv), static_cast<const double*>(pv) + nv);
+        *next = mock::as_number(mock::get_property(env, settled, "nextSlot"));
+        return true;
+      };
+      double next = 0;
+      int pages = 0;
+      while (next < n_rows) {
+        double after = 0;
+        if (!call_pairs(next, mp, &after)) die("similarPairs rejected: " + err);
+        if (!(after > next)) die("similarPairs made no progress");
+        next = after;
+        ++pages;
+      }
+      write_bin("pairs_a.i64", all_a.data(), all_a.size() * 8);
+      write_bin("pairs_b.i64", all_b.data(), all_b.size() * 8);
+      write_bin("pairs_scores.f64", all_s.data(), all_s.size() * 8);
+      write_text("pairs_pages.txt", std::to_string(pages));
+      double none = 0;
+      if (call_pairs(0, 0, &none)) die("similarPairs with maxPairs 0 did not reject");
+      log << "err_pairs " << err << "\n";
+    }
+  }
+
   // ---- error paths: each must surface as a JS exception / rejection with the reference's wording
   {
     std::vector<double> odd(static_cast<size_t>(dim) + 1, 1.0);

@@ -37,6 +37,10 @@
 //   await ix.searchSlots(BigInt64Array slots, B, Int32Array kFetch, Float64Array minScore)   // searchEach whose
 //        queries are the stored rows of those global slots, read where the index keeps them: the same result object
 //   ix.hasSearchSlots                          -> boolean: the library has searchSlots (else it throws)
+//   await ix.similarPairs(minScore, firstSlot, maxPairs)   // one page of every pair of live slots a < b with cosine
+//        >= minScore, rows a from firstSlot on, at most maxPairs (>= size()) entries, whole rows only
+//        -> { a: BigInt64Array, b: BigInt64Array, scores: Float64Array, nextSlot }   // nextSlot == size(): done
+//   ix.hasSimilarPairs                         -> boolean: the library has similarPairs (else it throws)
 //
 // Build (where Node headers exist):  node-gyp with  libraries: ["-lrbk_knn"], include_dirs: ["../include"].
 #include <node_api.h>
@@ -81,6 +85,9 @@
 // The same for stored rows as queries; `searchSlots` throws where it is missing.
 #pragma weak rbk_index_search_slots_f64
 #pragma weak rbk_group_search_slots_f64
+// The same for every pair above a threshold; `similarPairs` throws where it is missing.
+#pragma weak rbk_index_similar_pairs_f64
+#pragma weak rbk_group_similar_pairs_f64
 
 namespace {
 
@@ -170,6 +177,14 @@ struct Handle {
                           int32_t* c) {
     return grp ? rbk_group_search_slots_f64(grp, q, B, k, ms, s, v, c, nullptr)
                : rbk_index_search_slots_f64(ix, q, B, k, ms, s, v, c, nullptr);
+  }
+  bool has_similar_pairs() const {
+    return grp ? rbk_group_similar_pairs_f64 != nullptr : rbk_index_similar_pairs_f64 != nullptr;
+  }
+  rbk_status similar_pairs(double ms, int64_t first, int64_t max_pairs, int64_t* a, int64_t* b, double* v, int64_t* n,
+                           int64_t* next) {
+    return grp ? rbk_group_similar_pairs_f64(grp, ms, first, max_pairs, a, b, v, n, next, nullptr)
+               : rbk_index_similar_pairs_f64(ix, ms, first, max_pairs, a, b, v, n, next, nullptr);
   }
 };
 
@@ -657,6 +672,99 @@ napi_value HasSearchEach(napi_env env, napi_callback_info info) {
   return out;
 }
 
+// ---- similarPairs: one page of the pairs, on a libuv worker like search ----
+struct PairsJob {
+  Handle* ix;
+  double min_score;
+  int64_t first, max_pairs, n = 0, next = 0;
+  std::vector<int64_t> a, b;
+  std::vector<double> scores;
+  rbk_status st = RBK_OK;
+  std::string err;
+  napi_deferred deferred;
+  napi_async_work work;
+};
+
+void pairs_execute(napi_env, void* data) {
+  PairsJob* j = static_cast<PairsJob*>(data);
+  j->st = j->ix->similar_pairs(j->min_score, j->first, j->max_pairs, j->a.data(), j->b.data(), j->scores.data(), &j->n,
+                               &j->next);
+  if (j->st != RBK_OK) j->err = rbk_last_error();
+}
+
+void pairs_complete(napi_env env, napi_status, void* data) {
+  PairsJob* j = static_cast<PairsJob*>(data);
+  if (j->st != RBK_OK) {
+    napi_value msg, error;
+    napi_create_string_utf8(env, j->err.c_str(), NAPI_AUTO_LENGTH, &msg);
+    napi_create_error(env, nullptr, msg, &error);
+    napi_reject_deferred(env, j->deferred, error);
+  } else {
+    napi_value out, ab, ta, next;
+    void* p;
+    const size_t n = static_cast<size_t>(j->n);
+    napi_create_object(env, &out);
+    napi_create_arraybuffer(env, n * 8, &p, &ab);
+    memcpy(p, j->a.data(), n * 8);
+    napi_create_typedarray(env, napi_bigint64_array, n, ab, 0, &ta);
+    napi_set_named_property(env, out, "a", ta);
+    napi_create_arraybuffer(env, n * 8, &p, &ab);
+    memcpy(p, j->b.data(), n * 8);
+    napi_create_typedarray(env, napi_bigint64_array, n, ab, 0, &ta);
+    napi_set_named_property(env, out, "b", ta);
+    napi_create_arraybuffer(env, n * 8, &p, &ab);
+    memcpy(p, j->scores.data(), n * 8);
+    napi_create_typedarray(env, napi_float64_array, n, ab, 0, &ta);
+    napi_set_named_property(env, out, "scores", ta);
+    napi_create_int64(env, j->next, &next);
+    napi_set_named_property(env, out, "nextSlot", next);
+    napi_resolve_deferred(env, j->deferred, out);
+  }
+  napi_delete_async_work(env, j->work);
+  delete j;
+}
+
+napi_value SimilarPairs(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  Handle* ix = unwrap(env, info, &argc, argv);
+  if (!ix->has_similar_pairs()) {
+    napi_throw_error(env, nullptr, "similarPairs: this librbk_knn.so has no similar pairs (rbk_*_similar_pairs_f64)");
+    return nullptr;
+  }
+  PairsJob* j = new PairsJob();
+  j->ix = ix;
+  napi_get_value_double(env, argv[0], &j->min_score);   // -Infinity: every pair
+  napi_get_value_int64(env, argv[1], &j->first);
+  napi_get_value_int64(env, argv[2], &j->max_pairs);
+  // the library refuses a maxPairs below size() with its own message: the buffers are at least one entry (never null)
+  // and never larger than asked
+  const size_t cap = static_cast<size_t>(std::max<int64_t>(j->max_pairs, 1));
+  try {
+    j->a.resize(cap);
+    j->b.resize(cap);
+    j->scores.resize(cap);
+  } catch (const std::exception&) {
+    delete j;
+    napi_throw_error(env, nullptr, "similarPairs: no host memory for maxPairs entries");
+    return nullptr;
+  }
+  napi_value promise, name;
+  NAPI_OK(napi_create_promise(env, &j->deferred, &promise));
+  napi_create_string_utf8(env, "rbk_similar_pairs", NAPI_AUTO_LENGTH, &name);
+  NAPI_OK(napi_create_async_work(env, nullptr, name, pairs_execute, pairs_complete, j, &j->work));
+  NAPI_OK(napi_queue_async_work(env, j->work));
+  return promise;
+}
+
+napi_value HasSimilarPairs(napi_env env, napi_callback_info info) {
+  size_t argc = 0;
+  Handle* h = unwrap(env, info, &argc, nullptr);
+  napi_value out;
+  NAPI_OK(napi_get_boolean(env, h->has_similar_pairs(), &out));
+  return out;
+}
+
 napi_value HasSearchSlots(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
@@ -685,6 +793,8 @@ napi_value Init(napi_env env, napi_value exports) {
       {"hasSearchEach", nullptr, nullptr, HasSearchEach, nullptr, nullptr, napi_default, nullptr},
       {"searchSlots", nullptr, SearchSlots, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"hasSearchSlots", nullptr, nullptr, HasSearchSlots, nullptr, nullptr, napi_default, nullptr},
+      {"similarPairs", nullptr, SimilarPairs, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"hasSimilarPairs", nullptr, nullptr, HasSimilarPairs, nullptr, nullptr, napi_default, nullptr},
   };
   napi_value cls;
   NAPI_OK(napi_define_class(env, "RbkIndex", NAPI_AUTO_LENGTH, New, nullptr, sizeof props / sizeof props[0], props, &cls));

@@ -39,6 +39,7 @@ SYMBOLS = [
     "rbk_index_flags", "rbk_index_set_tier", "rbk_group_set_tier",
     "rbk_index_search_each_f64", "rbk_group_search_each_f64",
     "rbk_index_search_slots_f64", "rbk_group_search_slots_f64",
+    "rbk_index_similar_pairs_f64", "rbk_group_similar_pairs_f64",
 ]
 
 
@@ -136,6 +137,9 @@ def _load() -> C.CDLL:
         getattr(lib, n).argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp, C.POINTER(C.c_float)]
     for n in ("rbk_index_search_slots_f64", "rbk_group_search_slots_f64"):
         getattr(lib, n).argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, C.POINTER(C.c_float)]
+    for n in ("rbk_index_similar_pairs_f64", "rbk_group_similar_pairs_f64"):
+        getattr(lib, n).argtypes = [vp, f64, i64, i64, vp, vp, vp, C.POINTER(i64), C.POINTER(i64),
+                                    C.POINTER(C.c_float)]
     lib.rbk_index_debug_scores_f32.argtypes = [vp, vp, i32, vp]
     lib.rbk_index_flags.argtypes = [vp]
     lib.rbk_index_flags.restype = C.c_uint32
@@ -257,6 +261,23 @@ def _search_slots(fn, h, slots, k_fetch, min_score):
     return out_slots, scores, counts, ms.value
 
 
+def _similar_pairs(fn, h, first: int, size: int, min_score, first_slot, max_pairs):
+    """rbk_*_similar_pairs_f64: one page of the pairs (a, b) of live slots a < b with cosine >= min_score (None = -inf)
+    for the rows a from first_slot on (None: the first slot, `first`), at most max_pairs of them (None: max(size(),
+    2^20)), never part of a row's pairs.  Returns (a int64 [n], b int64 [n], scores float64 [n], next_slot): ascending
+    a, then score descending, ties by ascending b; next_slot == first + size() when the pass is complete."""
+    first_slot = first if first_slot is None else int(first_slot)
+    max_pairs = max(size, 1 << 20) if max_pairs is None else int(max_pairs)
+    cap = max(max_pairs, 0)
+    a = np.empty(cap, dtype=np.int64)
+    b = np.empty(cap, dtype=np.int64)
+    scores = np.empty(cap, dtype=np.float64)
+    n, nxt, ms = C.c_int64(0), C.c_int64(0), C.c_float(0)
+    ms_arg = -np.inf if min_score is None else float(min_score)
+    check(fn(h, ms_arg, first_slot, max_pairs, ptr(a), ptr(b), ptr(scores), C.byref(n), C.byref(nxt), C.byref(ms)))
+    return a[:n.value].copy(), b[:n.value].copy(), scores[:n.value].copy(), nxt.value
+
+
 def _search_any_k(ix, queries, k_fetch: int, min_score):
     """Shared by Index and Group: the scan path up to RBK_MAX_K_FETCH hits per query, the two-pass large-k search up
     to RBK_MAX_K_FETCH_LARGE, beyond it the exact scores of every row from the device and the reference's threshold /
@@ -313,6 +334,7 @@ class Index:
         self._h = h
         self.dim = dim
         self.device = device
+        self.slot_base = 0
 
     def close(self) -> None:
         if getattr(self, "_h", None):
@@ -333,6 +355,7 @@ class Index:
 
     def set_slot_base(self, base: int) -> None:
         check(lib.rbk_index_set_slot_base(self._h, base))
+        self.slot_base = int(base)
 
     @property
     def flags(self) -> int:
@@ -475,6 +498,15 @@ class Index:
         and min_score (None = -inf): one per query or one for all.  A query's own slot is among its hits; a slot this
         index does not hold, or a tombstoned one, raises RbkError (RBK_EINVAL)."""
         return _search_slots(lib.rbk_index_search_slots_f64, self._h, slots, k_fetch, min_score)
+
+    def similar_pairs(self, min_score, first_slot=None, max_pairs=None):
+        """One page of every pair of stored rows at or above min_score (None = -inf), exactly: (a [n], b [n],
+        scores [n], next_slot) numpy arrays, slots a < b, first_slot <= a < next_slot (first_slot None: slot_base), at
+        most max_pairs entries (None: max(size(), 2^20); at least size()).  Ascending a, then score descending, ties by
+        ascending b: a's entries are those of search_slots([a], count(), min_score) above a.  The pass is complete when
+        next_slot == slot_base + size(); otherwise call again from next_slot."""
+        return _similar_pairs(lib.rbk_index_similar_pairs_f64, self._h, self.slot_base, self.size(), min_score,
+                              first_slot, max_pairs)
 
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: the reference's cosine of every row, NaN for tombstoned / zero rows."""
@@ -641,6 +673,11 @@ class Group:
     def search_slots(self, slots, k_fetch, min_score):
         """Index.search_slots() over the group: each slot's member gathers its row, then one search_each."""
         return _search_slots(lib.rbk_group_search_slots_f64, self._h, slots, k_fetch, min_score)
+
+    def similar_pairs(self, min_score, first_slot=None, max_pairs=None):
+        """Index.similar_pairs() over the group's global slots [0, size()): the answers of a single index."""
+        return _similar_pairs(lib.rbk_group_similar_pairs_f64, self._h, 0, self.size(), min_score, first_slot,
+                              max_pairs)
 
     def exact_scores(self, queries) -> np.ndarray:
         """float64 [B, size()]: every device's exact scores, put back in global slot order (4096-row blocks dealt

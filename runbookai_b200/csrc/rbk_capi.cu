@@ -524,18 +524,20 @@ size_t scan_scratch_words(const rbk_index* ix, int Bs) {
   return static_cast<size_t>(Bs) * kHistBins + 2 * Bs + progress_slots(ix);
 }
 
-// The fields every scan mode shares, for the Bs queries from q0 on.
-void fill_scan_params(rbk_index* ix, int q0, int Bs, int kprime, ScanParams* sp) {
-  const int n_tiles = static_cast<int>((ix->n_rows + kBlockN - 1) / kBlockN);
+// The fields every scan mode shares, for the Bs queries from q0 on, against the rows from local row r0 on (a multiple
+// of kBlockN, with a corpus map that starts there: rbk_index_similar_pairs_f64).
+void fill_scan_params(rbk_index* ix, int q0, int Bs, int kprime, ScanParams* sp, int64_t r0 = 0) {
+  const int64_t n_rows = ix->n_rows - r0;
+  const int n_tiles = static_cast<int>((n_rows + kBlockN - 1) / kBlockN);
   const int QB = (Bs + kBlockM - 1) / kBlockM;
-  sp->inv_norm_c = ix->inv_norm;
+  sp->inv_norm_c = ix->inv_norm + r0;
   sp->thr_init = ix->thr_init.p + q0;
   sp->inv_norm_q = ix->q_inv_norm.p + q0;
   sp->hist = ix->hist.p;
   sp->maxbin = reinterpret_cast<int*>(ix->hist.p + static_cast<size_t>(Bs) * kHistBins);
   sp->gthr = reinterpret_cast<unsigned int*>(sp->maxbin + Bs);
   sp->progress = sp->maxbin + 2 * Bs;
-  sp->n_rows = static_cast<int>(ix->n_rows);
+  sp->n_rows = static_cast<int>(n_rows);
   sp->B = Bs;
   sp->kprime = kprime;
   sp->dpad = ix->dpad;
@@ -545,9 +547,9 @@ void fill_scan_params(rbk_index* ix, int q0, int Bs, int kprime, ScanParams* sp)
   sp->n_tiles = n_tiles;
 }
 
-LargeScanParams large_scan_params(rbk_index* ix, int q0, int Bs, int k_fetch) {
+LargeScanParams large_scan_params(rbk_index* ix, int q0, int Bs, int k_fetch, int64_t r0 = 0) {
   LargeScanParams sp{};
-  fill_scan_params(ix, q0, Bs, k_fetch, &sp);
+  fill_scan_params(ix, q0, Bs, k_fetch, &sp, r0);
   sp.q_eps = ix->q_eps.p + q0;
   return sp;
 }
@@ -570,8 +572,10 @@ rbk_status prep_queries(rbk_index* ix, const void* d_q, int src_type, int B, dou
 
 // Launches one filled sub-batch: its query map, then the scan kernel of kMode (0: the top-k' scan, P = ScanParams;
 // kScanCount / kScanEmit: a large-k pass, P = LargeScanParams) inside a timing pair unless the stream is being captured.
+// tmap_c (nullable): the corpus map, when it is not the index's own (rows from r0 on; see fill_scan_params).
 template <int kMode, typename P>
-rbk_status launch_sub_batch(rbk_index* ix, int q0, const P& sp) {
+rbk_status launch_sub_batch(rbk_index* ix, int q0, const P& sp, const CUtensorMap* tmap_c = nullptr) {
+  if (!tmap_c) tmap_c = &ix->tmap_c;
   CUtensorMap tmap_q;
   const int q_rows = static_cast<int>(round_up(sp.B, kBlockM));   // whole query blocks: no out-of-bounds box rows
   // every row the map covers must lie inside the query buffer: the scan's TMA loads whole boxes
@@ -583,9 +587,9 @@ rbk_status launch_sub_batch(rbk_index* ix, int q0, const P& sp) {
   cudaEvent_t* tev = ix->capturing ? nullptr : next_scan_events(ix);
   if (tev) CK(cudaEventRecord(tev[0], ix->stream));
   if constexpr (kMode == 0)
-    CK((ix->scan_f16 ? launch_scan_f16 : launch_scan)(tmap_q, ix->tmap_c, sp, ix->stream));
+    CK((ix->scan_f16 ? launch_scan_f16 : launch_scan)(tmap_q, *tmap_c, sp, ix->stream));
   else
-    CK((ix->scan_f16 ? launch_scan_large_f16 : launch_scan_large)(tmap_q, ix->tmap_c, sp,
+    CK((ix->scan_f16 ? launch_scan_large_f16 : launch_scan_large)(tmap_q, *tmap_c, sp,
                                                                   static_cast<LargeScanMode>(kMode), ix->stream));
   if (tev) CK(cudaEventRecord(tev[1], ix->stream));
   ix->stats.last_ring_stages = kStages;
@@ -978,6 +982,127 @@ rbk_status large_finish(rbk_index* ix) {
   return RBK_OK;
 }
 
+int64_t first_row_at(const SlotLayout& s, int64_t a) {
+  if (s.block == 0) return std::max<int64_t>(0, a - s.base);
+  const int64_t blk = a / s.block, cycle = blk / s.G, pos = blk % s.G;
+  if (pos == s.g) return cycle * s.block + a % s.block;
+  return (pos < s.g ? cycle : cycle + 1) * s.block;   // the first row of this member's next block
+}
+
+rbk_status pairs_count(rbk_index* ix, int Q, int64_t a0, double min_score) {
+  CK(ix->lg_theta.ensure(Q));
+  CK(ix->lg_cap.ensure(Q));
+  CK(ix->lg_cnt.ensure(Q));
+  CK(ix->lg_off.ensure(Q));
+  CK(ix->lg_err.ensure(1));
+  CK(ix->h_lcap.ensure(Q));
+  CK(ix->h_loff.ensure(Q));
+  CK(ix->h_lerr.ensure(1));
+  CK(ix->pr_cnt.ensure(Q));
+  CK(ix->pr_off.ensure(Q));
+  CK(ix->h_pcnt.ensure(Q));
+  rbk_status st = prep_queries(ix, ix->q_raw.p, 0, Q, min_score, /*with_norm2=*/true);
+  if (st != RBK_OK) return st;
+  const int64_t first = first_row_at(ix->slot, a0);
+  if (first >= ix->n_rows) {   // no row of this index can pair with the chunk
+    ix->pr_rows = 0;
+    memset(ix->h_lcap.p, 0, sizeof(int) * Q);
+    return RBK_OK;
+  }
+  // the triangle: the scans read the rows from the chunk's first slot on, from a map that starts at the tile holding it
+  ix->pr_r0 = first / kBlockN * kBlockN;
+  ix->pr_rows = ix->n_rows - ix->pr_r0;
+  st = encode_rows_tmap(&ix->pr_tmap, ix->rows + static_cast<size_t>(ix->pr_r0) * ix->dpad,
+                        round_up(ix->n_rows, kBlockN) - ix->pr_r0, ix->dpad, kBlockN, ix->scan_f16);
+  if (st != RBK_OK) return st;
+  // k = INT32_MAX: the count pass never raises its threshold above min_score's, and the select keeps it (theta_q from
+  // min_score and the query's bound alone, C_q every row counted at or above it)
+  const LargeScanParams sp = large_scan_params(ix, 0, Q, INT32_MAX, ix->pr_r0);
+  st = launch_sub_batch<kScanCount>(ix, 0, sp, &ix->pr_tmap);
+  if (st != RBK_OK) return st;
+  CK(launch_large_select(sp.hist, sp.thr_init, sp.inv_norm_q, sp.q_eps, Q, INT32_MAX, static_cast<int>(ix->pr_rows),
+                         ix->lg_theta.p, ix->lg_cap.p, ix->stream));
+  ix->stats.kernel_launches++;
+  CK(cudaMemcpyAsync(ix->h_lcap.p, ix->lg_cap.p, sizeof(int) * Q, cudaMemcpyDeviceToHost, ix->stream));
+  return RBK_OK;
+}
+
+rbk_status pairs_emit(rbk_index* ix, int q0, int q1, int64_t a0, double min_score) {
+  const int Bs = q1 - q0;
+  if (ix->pr_rows == 0) {
+    memset(ix->h_pcnt.p, 0, sizeof(int) * Bs);
+    ix->h_lerr.p[0] = 0;
+    return RBK_OK;
+  }
+  const int64_t r0 = ix->pr_r0;
+  int64_t cand = 0, group_tiles = 0;
+  for (int b = q0; b < q1; ++b) {
+    cand += ix->h_lcap.p[b];
+    group_tiles += sort_tiles(ix->h_lcap.p[b]);
+  }
+  CK(ix->pr_b.ensure(static_cast<size_t>(std::max<int64_t>(cand, 1))));
+  CK(ix->pr_s.ensure(static_cast<size_t>(std::max<int64_t>(cand, 1))));
+  LargeScanParams sp = large_scan_params(ix, q0, Bs, INT32_MAX, r0);
+  sp.thr_init = ix->lg_theta.p + q0;
+  sp.emit_off = ix->lg_off.p + q0;
+  sp.emit_cap = ix->lg_cap.p + q0;
+  sp.emit_cnt = ix->lg_cnt.p + q0;
+  sp.emit_rows = ix->lg_rows.p;
+  CK(cudaMemsetAsync(sp.progress, 0, sizeof(int) * progress_slots(ix), ix->stream));
+  rbk_status st = launch_sub_batch<kScanEmit>(ix, q0, sp, &ix->pr_tmap);
+  if (st != RBK_OK) return st;
+  if (std::find(ix->h_lcap.p + q0, ix->h_lcap.p + q1, static_cast<int>(ix->pr_rows)) != ix->h_lcap.p + q1) {
+    CK(launch_large_emit_all(ix->q_eps.p + q0, ix->dead_bits + r0 / 32, ix->pr_rows, Bs, sp.emit_off, sp.emit_cnt,
+                             ix->lg_rows.p, ix->stream));
+    ix->stats.kernel_launches++;
+  }
+  LargeRerankParams rp{};
+  rp.B = Bs;
+  rp.d = ix->dim;
+  rp.dpad = ix->dpad;
+  rp.min_score = min_score;
+  rp.rows = ix->rows + static_cast<size_t>(r0) * ix->dpad;
+  rp.rows_x = ix->rows_x ? static_cast<const char*>(ix->rows_x) + static_cast<size_t>(r0) * ix->x_row_bytes() : nullptr;
+  rp.row_norm2 = ix->norm2 + r0;
+  rp.slot = ix->slot;
+  rp.q_f64 = ix->q_f64.p + static_cast<size_t>(q0) * ix->dim;
+  rp.q_norm2 = ix->q_norm2.p + q0;
+  rp.emit_off = sp.emit_off;
+  rp.emit_cap = sp.emit_cap;
+  rp.emit_cnt = sp.emit_cnt;
+  rp.emit_rows = ix->lg_rows.p;
+  rp.cand_scores = ix->lg_scores.p;
+  rp.overflow = ix->lg_err.p;
+  const int max_cap = *std::max_element(ix->h_lcap.p + q0, ix->h_lcap.p + q1);
+  SegSortScratch ss;
+  ss.tile_off = ix->ub_toff.p + q0;
+  ss.scores = ix->ub_scores.p;
+  ss.rows = ix->ub_rows.p;
+  ss.len[0] = ix->ub_len.p;
+  ss.len[1] = ix->ub_len.p + group_tiles;
+  ss.max_tiles = static_cast<int>(sort_tiles(max_cap));
+  PairsParams pp;
+  pp.a0 = a0 + q0;
+  pp.r0 = r0;
+  pp.counts = ix->pr_cnt.p;
+  pp.offsets = ix->pr_off.p;
+  pp.out_b = ix->pr_b.p;
+  pp.out_scores = ix->pr_s.p;
+  int launches = 0;
+  CK(launch_pairs_rerank(rp, ss, max_cap, ix->rows_on_host, ix->x_elem, pp, ix->stream, &launches));
+  ix->stats.kernel_launches += launches;
+  CK(cudaMemcpyAsync(ix->h_pcnt.p, ix->pr_cnt.p, sizeof(int) * Bs, cudaMemcpyDeviceToHost, ix->stream));
+  return large_finish(ix);
+}
+
+rbk_status pairs_fetch(rbk_index* ix, int64_t n) {
+  if (n == 0) return RBK_OK;
+  CK(ix->h_block.ensure(static_cast<size_t>(n) * 16));
+  CK(cudaMemcpyAsync(ix->h_block.p, ix->pr_b.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, ix->stream));
+  CK(cudaMemcpyAsync(ix->h_block.p + n * 8, ix->pr_s.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ix->stream));
+  return RBK_OK;
+}
+
 }  // namespace impl
 }  // namespace rbk
 
@@ -1288,6 +1413,125 @@ rbk_status search_device_exact(rbk_index* ix, const void* d_q, int elem, int B, 
                                const double* min_each) {
   return search_core(ix, nullptr, d_q, elem, B, ix ? ix->dim : 0, k_fetch, min_score, d_slots, d_scores, d_counts,
                      nullptr, nullptr, nullptr, nullptr, k_each, min_each);
+}
+
+rbk_status check_pairs_args(int64_t slot_base, int64_t size, double min_score, int64_t first_slot, int64_t max_pairs,
+                            const void* out_a, const void* out_b, const void* out_scores, const void* n_out,
+                            const void* next_slot) {
+  if (!out_a || !out_b || !out_scores || !n_out || !next_slot) return fail(RBK_EINVAL, "null output");
+  if (min_score != min_score) return fail(RBK_EINVAL, "min_score is NaN");
+  if (first_slot < slot_base || first_slot > slot_base + size)
+    return fail(RBK_EINVAL, "first_slot must be in [" + std::to_string(slot_base) + ", " +
+                                std::to_string(slot_base + size) + "]");
+  if (max_pairs < std::max<int64_t>(size, 1))
+    return fail(RBK_EINVAL, "max_pairs must be >= max(size(), 1) = " + std::to_string(std::max<int64_t>(size, 1)));
+  return RBK_OK;
+}
+
+rbk_status similar_pairs_run(const std::vector<rbk_index*>& parts, int64_t end, double min_score, int64_t first_slot,
+                             int64_t max_pairs, const std::function<rbk_status(int64_t, int)>& load, int64_t* out_a,
+                             int64_t* out_b, double* out_scores, int64_t* n_out, int64_t* next_slot, float* ms_out) {
+  const int G = static_cast<int>(parts.size());
+  rbk_status st;
+  *n_out = 0;
+  *next_slot = first_slot;
+  if (ms_out) *ms_out = 0.f;
+  for (rbk_index* ix : parts) ix->stats.searches++;
+  if (first_slot >= end) return RBK_OK;
+  std::vector<TimedSearch> ts;
+  for (rbk_index* ix : parts) {
+    DeviceGuard dg(ix->device);
+    ts.push_back(TimedSearch{ix});
+    if ((st = ts.back().begin()) != RBK_OK) return st;
+  }
+  auto each = [&](const std::function<rbk_status(int, rbk_index*)>& f) -> rbk_status {
+    for (int d = 0; d < G; ++d) {
+      DeviceGuard dg(parts[d]->device);
+      rbk_status s2 = f(d, parts[d]);
+      if (s2 != RBK_OK) return s2;
+    }
+    return RBK_OK;
+  };
+  auto wait_all = [&]() { return each([&](int d, rbk_index*) { return ts[d].round_trip(); }); };
+  int64_t n = 0, a0 = first_slot;
+  bool full = false;
+  std::vector<int64_t> cost;
+  while (a0 < end && !full) {
+    const int Q = static_cast<int>(std::min<int64_t>(kSlotChunk, end - a0));
+    if ((st = each([&](int, rbk_index* ix) { return ensure_query_scratch(ix, Q, 8); })) != RBK_OK) return st;
+    if ((st = load(a0, Q)) != RBK_OK) return st;
+    if ((st = each([&](int, rbk_index* ix) { return pairs_count(ix, Q, a0, min_score); })) != RBK_OK) return st;
+    if ((st = wait_all()) != RBK_OK) return st;   // C_q sizes the candidate buffers and the query groups
+    // a query's cost: its candidates, their sort buffer and their packed pairs on every member
+    cost.assign(Q, 0);
+    for (int q = 0; q < Q; ++q)
+      for (rbk_index* ix : parts) cost[q] += ix->h_lcap.p[q] * (large_cand_bytes(true) + 16) + 16;
+    const std::vector<std::pair<int, int>> groups = split_by_budget(cost);
+    if ((st = each([&](int, rbk_index* ix) { return large_prepare(ix, Q, true, groups); })) != RBK_OK) return st;
+    for (const auto& gr : groups) {
+      st = each([&](int, rbk_index* ix) { return pairs_emit(ix, gr.first, gr.second, a0, min_score); });
+      if (st != RBK_OK || (st = wait_all()) != RBK_OK) return st;
+      for (rbk_index* ix : parts)
+        if ((st = large_check(ix)) != RBK_OK) return st;
+      // the whole query rows that still fit, and each member's share of their pairs (a prefix of its packed pairs)
+      int q1 = gr.first;
+      int64_t m = 0;
+      for (; q1 < gr.second; ++q1) {
+        int64_t c = 0;
+        for (rbk_index* ix : parts) c += ix->h_pcnt.p[q1 - gr.first];
+        if (n + m + c > max_pairs) break;
+        m += c;
+      }
+      std::vector<int64_t> share(G, 0);
+      for (int d = 0; d < G; ++d)
+        for (int q = gr.first; q < q1; ++q) share[d] += parts[d]->h_pcnt.p[q - gr.first];
+      if (m > 0) {
+        if ((st = each([&](int d, rbk_index* ix) { return pairs_fetch(ix, share[d]); })) != RBK_OK) return st;
+        if ((st = wait_all()) != RBK_OK) return st;
+      }
+      // every member's list of a query is sorted by (score desc, slot asc), and the members' slots are disjoint
+      std::vector<int64_t> at(G, 0);
+      for (int q = gr.first; q < q1; ++q) {
+        const int64_t o0 = n;
+        for (int d = 0; d < G; ++d) {
+          const int c = parts[d]->h_pcnt.p[q - gr.first];
+          const unsigned char* h = parts[d]->h_block.p;
+          memcpy(out_b + n, h + at[d] * 8, sizeof(int64_t) * c);
+          memcpy(out_scores + n, h + (share[d] + at[d]) * 8, sizeof(double) * c);
+          at[d] += c;
+          n += c;
+          if (d > 0 && c > 0) {
+            std::vector<std::pair<double, int64_t>> v;
+            for (int64_t i = o0; i < n; ++i) v.emplace_back(out_scores[i], out_b[i]);
+            std::inplace_merge(v.begin(), v.end() - c, v.end(), [](const auto& x, const auto& y) {
+              return x.first > y.first || (x.first == y.first && x.second < y.second);
+            });
+            for (int64_t i = o0; i < n; ++i) {
+              out_scores[i] = v[i - o0].first;
+              out_b[i] = v[i - o0].second;
+            }
+          }
+        }
+        std::fill(out_a + o0, out_a + n, a0 + q);
+      }
+      if (q1 < gr.second) {   // the buffer is full: the rest of the chunk is answered by the next call
+        full = true;
+        a0 += q1;
+        break;
+      }
+    }
+    if (!full) a0 += Q;
+  }
+  *n_out = n;
+  *next_slot = a0;
+  for (int d = 0; d < G; ++d) {
+    DeviceGuard dg(parts[d]->device);
+    parts[d]->stats.queries += a0 - first_slot;
+    float ms = 0.f;
+    ts[d].finish(&ms);
+    if (ms_out) *ms_out = std::max(*ms_out, ms);
+  }
+  return RBK_OK;
 }
 
 int64_t compact_row_bytes(const rbk_index* ix) {
@@ -2110,6 +2354,26 @@ rbk_status rbk_index_search_slots_f64(rbk_index* ix, const int64_t* query_slots,
   }
   ix->stats.searches = searches;
   return RBK_OK;
+}
+
+rbk_status rbk_index_similar_pairs_f64(rbk_index* ix, double min_score, int64_t first_slot, int64_t max_pairs,
+                                       int64_t* out_a, int64_t* out_b, double* out_scores, int64_t* n_out,
+                                       int64_t* next_slot, float* kernel_ms_out) {
+  if (!ix) return fail(RBK_EINVAL, "null index");
+  if (ix->slot.block != 0) return fail(RBK_EINVAL, "a group member answers through rbk_group_similar_pairs_f64");
+  std::lock_guard<std::mutex> lk(ix->mu);
+  rbk_status st = check_pairs_args(ix->slot.base, ix->n_rows, min_score, first_slot, max_pairs, out_a, out_b,
+                                   out_scores, n_out, next_slot);
+  if (st != RBK_OK) return st;
+  DeviceGuard dg(ix->device);
+  std::vector<int64_t> rows;
+  auto load = [&](int64_t a0, int Q) {
+    rows.resize(Q);
+    for (int q = 0; q < Q; ++q) rows[q] = a0 - ix->slot.base + q;
+    return gather_queries(ix, rows.data(), Q);   // a tombstoned row becomes a query of zeros: no pairs
+  };
+  return similar_pairs_run({ix}, ix->slot.base + ix->n_rows, min_score, first_slot, max_pairs, load, out_a, out_b,
+                           out_scores, n_out, next_slot, kernel_ms_out);
 }
 
 rbk_status rbk_index_exact_scores_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,

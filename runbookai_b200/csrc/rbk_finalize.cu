@@ -1349,6 +1349,60 @@ __global__ void __launch_bounds__(256) seg_write_kernel(LargeRerankParams p, Seg
   }
 }
 
+// --------------------------------------------------------------------------- similar pairs (DESIGN.md §6)
+// rbk_index_similar_pairs_f64 runs the unbounded search's re-rank with no cut, for queries that are the stored rows of
+// consecutive global slots pp.a0 + q and candidates that are rows pp.r0 + emit_rows[i] (p's row pointers start at row
+// r0).  (1) pairs_mask_kernel, between the re-score and the tile sort: a candidate whose global slot is not above its
+// query's gets the score NaN, which the tile sort drops together with the scores below min_score.  (2)
+// pairs_offsets_kernel: each query's exact pair count (the length of its sorted run) and their exclusive scan.  (3)
+// pairs_write_kernel: the sorted runs packed end to end as (global slot, score), query after query.
+__global__ void __launch_bounds__(256) pairs_mask_kernel(LargeRerankParams p, PairsParams pp) {
+  const int q = blockIdx.y;
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= min(p.emit_cnt[q], p.emit_cap[q])) return;
+  const size_t o = static_cast<size_t>(p.emit_off[q]) + i;
+  if (p.slot.global(pp.r0 + p.emit_rows[o]) <= pp.a0 + q) p.cand_scores[o] = __longlong_as_double(0x7FF8000000000000ll);
+}
+
+constexpr int kPairsScanThreads = 1024;   // one thread per query of a launch (B <= kMaxSubBatch)
+static_assert(kMaxSubBatch <= kPairsScanThreads, "one thread per query");
+
+__global__ void __launch_bounds__(kPairsScanThreads) pairs_offsets_kernel(LargeRerankParams p, SegSortScratch s,
+                                                                          int final_buf, PairsParams pp) {
+  __shared__ long long s_sum[kPairsScanThreads];
+  const int q = threadIdx.x;
+  int L = 0;
+  if (q < p.B) {
+    const int emitted = p.emit_cnt[q];
+    if (min(emitted, p.emit_cap[q]) > 0) L = (final_buf ? s.len[1] : s.len[0])[s.tile_off[q]];
+    pp.counts[q] = L;
+    if (emitted > p.emit_cap[q]) atomicAdd(p.overflow, 1);   // the count pass missed rows: the answer is not proven
+  }
+  s_sum[q] = L;
+  __syncthreads();
+  for (int o = 1; o < kPairsScanThreads; o <<= 1) {   // inclusive scan
+    const long long v = q >= o ? s_sum[q - o] : 0;
+    __syncthreads();
+    s_sum[q] += v;
+    __syncthreads();
+  }
+  if (q < p.B) pp.offsets[q] = s_sum[q] - L;
+}
+
+__global__ void __launch_bounds__(256) pairs_write_kernel(LargeRerankParams p, SegSortScratch s, int final_buf,
+                                                          PairsParams pp) {
+  const int q = blockIdx.y;
+  const int L = pp.counts[q];
+  const double* sc = final_buf ? s.scores : p.cand_scores;
+  const int* rw = final_buf ? s.rows : p.emit_rows;
+  const size_t seg = static_cast<size_t>(p.emit_off[q]);
+  const long long o = pp.offsets[q];
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < L; i += gridDim.x * 256) {
+    pp.out_b[o + i] = p.slot.global(pp.r0 + rw[seg + i]);
+    pp.out_scores[o + i] = sc[seg + i];
+  }
+}
+
 // --------------------------------------------------------------------------- all exact scores
 // One thread per (row, query): the reference's fp64 cosine of EVERY row, NaN for tombstoned / zero rows, for a host
 // that applies `>= minScore`, the stable sort and the cut itself (vector-store.ts:212-221).  Searches for any number of
@@ -1561,27 +1615,56 @@ cudaError_t launch_large_emit_all(const double* q_eps, const unsigned int* dead_
   return cudaGetLastError();
 }
 
-cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
-                                bool rows_on_host, int x_elem, cudaStream_t stream, int* launches) {
+namespace {
+// The exact re-score of every emitted candidate (launch_large_rerank, launch_pairs_rerank).
+cudaError_t launch_large_score(const LargeRerankParams& p, int max_cap, bool rows_on_host, int x_elem,
+                               cudaStream_t stream, int* launches) {
   using namespace entry;
-  *launches = 0;
-  if (p.B <= 0) return cudaSuccess;
-  cudaError_t e;
-  if (max_cap > 0) {
-    dim3 grid(static_cast<unsigned>((max_cap + 255) / 256), static_cast<unsigned>(p.B));
-    if (x_elem == 4) {
-      if (rows_on_host) large_score_f32_kernel<true><<<grid, 256, 0, stream>>>(p);
-      else large_score_f32_kernel<false><<<grid, 256, 0, stream>>>(p);
-    } else if (x_elem == 2) {
-      if (rows_on_host) large_score_split_kernel<true><<<grid, 256, 0, stream>>>(p);
-      else large_score_split_kernel<false><<<grid, 256, 0, stream>>>(p);
-    } else {
-      if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
-      else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);
-    }
+  if (max_cap <= 0) return cudaSuccess;
+  dim3 grid(static_cast<unsigned>((max_cap + 255) / 256), static_cast<unsigned>(p.B));
+  if (x_elem == 4) {
+    if (rows_on_host) large_score_f32_kernel<true><<<grid, 256, 0, stream>>>(p);
+    else large_score_f32_kernel<false><<<grid, 256, 0, stream>>>(p);
+  } else if (x_elem == 2) {
+    if (rows_on_host) large_score_split_kernel<true><<<grid, 256, 0, stream>>>(p);
+    else large_score_split_kernel<false><<<grid, 256, 0, stream>>>(p);
+  } else {
+    if (rows_on_host) large_score_kernel<true><<<grid, 256, 0, stream>>>(p);
+    else large_score_kernel<false><<<grid, 256, 0, stream>>>(p);
+  }
+  ++*launches;
+  return cudaGetLastError();
+}
+
+// The segmented sort's tile sort and merge passes; *passes: merge passes run (the sorted runs end in buffer
+// passes & 1).
+cudaError_t launch_seg_sort(const LargeRerankParams& p, const SegSortScratch& s, cudaStream_t stream, int* launches,
+                            int* passes) {
+  *passes = 0;
+  if (s.max_tiles <= 0) return cudaSuccess;
+  const size_t smem = static_cast<size_t>(kSortTile) * (sizeof(double) + sizeof(int));
+  cudaError_t e = cudaFuncSetAttribute(seg_tile_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  const dim3 grid(static_cast<unsigned>(s.max_tiles), static_cast<unsigned>(p.B));
+  seg_tile_sort_kernel<<<grid, kSortThreads, smem, stream>>>(p, s);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  ++*launches;
+  for (; (1 << *passes) < s.max_tiles; ++*passes) {
+    if (p.k_each != nullptr) seg_merge_kernel<true><<<grid, kMergeThreads, 0, stream>>>(p, s, *passes);
+    else seg_merge_kernel<<<grid, kMergeThreads, 0, stream>>>(p, s, *passes);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
   }
+  return cudaSuccess;
+}
+}  // namespace
+
+cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
+                                bool rows_on_host, int x_elem, cudaStream_t stream, int* launches) {
+  *launches = 0;
+  if (p.B <= 0) return cudaSuccess;
+  cudaError_t e = launch_large_score(p, max_cap, rows_on_host, x_elem, stream, launches);
+  if (e != cudaSuccess) return e;
   if (!sort) {   // the cut in shared memory, one block per query
     int S = 2048;
     while (S < p.k_fetch + kTopThreads) S <<= 1;
@@ -1594,26 +1677,41 @@ cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch
   }
   const SegSortScratch& s = *sort;
   int passes = 0;
-  if (s.max_tiles > 0) {
-    const size_t smem = static_cast<size_t>(kSortTile) * (sizeof(double) + sizeof(int));
-    e = cudaFuncSetAttribute(seg_tile_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const dim3 grid(static_cast<unsigned>(s.max_tiles), static_cast<unsigned>(p.B));
-    seg_tile_sort_kernel<<<grid, kSortThreads, smem, stream>>>(p, s);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    for (; (1 << passes) < s.max_tiles; ++passes) {
-      if (p.k_each != nullptr) seg_merge_kernel<true><<<grid, kMergeThreads, 0, stream>>>(p, s, passes);
-      else seg_merge_kernel<<<grid, kMergeThreads, 0, stream>>>(p, s, passes);
-      if ((e = cudaGetLastError()) != cudaSuccess) return e;
-      ++*launches;
-    }
-  }
+  if ((e = launch_seg_sort(p, s, stream, launches, &passes)) != cudaSuccess) return e;
   const long long need = (p.k_fetch + 255ll) / 256;
   const int wblocks = need < 1024 ? static_cast<int>(need) : 1024;
   seg_write_kernel<<<dim3(static_cast<unsigned>(wblocks), static_cast<unsigned>(p.B)), 256, 0, stream>>>(p, s,
                                                                                                        passes & 1);
   ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pairs_rerank(const LargeRerankParams& p_in, const SegSortScratch& s, int max_cap, bool rows_on_host,
+                                int x_elem, const PairsParams& pp, cudaStream_t stream, int* launches) {
+  *launches = 0;
+  if (p_in.B <= 0) return cudaSuccess;
+  if (p_in.B > kPairsScanThreads) return cudaErrorInvalidValue;
+  LargeRerankParams p = p_in;
+  p.k_fetch = INT_MAX;   // no cut: every pair is kept
+  p.k_each = nullptr;
+  cudaError_t e = launch_large_score(p, max_cap, rows_on_host, x_elem, stream, launches);
+  if (e != cudaSuccess) return e;
+  const int cap_blocks = (max_cap + 255) / 256;
+  const unsigned blocks = static_cast<unsigned>(cap_blocks < 1024 ? cap_blocks : 1024);
+  if (max_cap > 0) {
+    pairs_mask_kernel<<<dim3(static_cast<unsigned>(cap_blocks), static_cast<unsigned>(p.B)), 256, 0, stream>>>(p, pp);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+  }
+  int passes = 0;
+  if ((e = launch_seg_sort(p, s, stream, launches, &passes)) != cudaSuccess) return e;
+  pairs_offsets_kernel<<<1, kPairsScanThreads, 0, stream>>>(p, s, passes & 1, pp);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  ++*launches;
+  if (max_cap > 0) {
+    pairs_write_kernel<<<dim3(blocks, static_cast<unsigned>(p.B)), 256, 0, stream>>>(p, s, passes & 1, pp);
+    ++*launches;
+  }
   return cudaGetLastError();
 }
 

@@ -26,10 +26,14 @@ __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const XT* _
                                                                      const int64_t* __restrict__ sel, int d,
                                                                      double* __restrict__ dst, int* __restrict__ n_dead) {
   const int64_t r = sel[blockIdx.x];
-  if (threadIdx.x == 0 && ((dead_bits[r >> 5] >> (r & 31)) & 1u)) atomicAdd(n_dead, 1);
+  double* out = dst + static_cast<int64_t>(blockIdx.x) * d;
+  if ((dead_bits[r >> 5] >> (r & 31)) & 1u) {   // uniform over the block
+    if (threadIdx.x == 0) atomicAdd(n_dead, 1);
+    for (int j = threadIdx.x; j < d; j += kGatherThreads) out[j] = 0.0;
+    return;
+  }
   const XT* src = x + r * x_pitch;
   const uint16_t* hi = rows + r * dpad;
-  double* out = dst + static_cast<int64_t>(blockIdx.x) * d;
   constexpr int V = 16 / sizeof(XT);
   const int head = min(d, static_cast<int>(((16 - (reinterpret_cast<uintptr_t>(src) & 15)) & 15) / sizeof(XT)));
   const int nvec = (d - head) / V;

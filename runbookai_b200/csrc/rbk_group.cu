@@ -93,6 +93,7 @@ struct rbk_group {
   DevBuf<unsigned char> out;     // device 0: the merged block (dirty_word)
   PinBuf<unsigned char> h_out, h_q;
   PinBuf<double> h_sq;           // rbk_group_search_slots_f64: the members' gathered query rows
+  PinBuf<double> h_pq;           // rbk_group_similar_pairs_f64: one chunk's query rows in slot order
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int64_t redone_batches = 0;
 };
@@ -429,7 +430,16 @@ rbk_status group_search_large(rbk_group* g, const double* queries, int32_t B, in
 // The stored values of global slots slots[0, B) (each < n_slots) as float64 queries into q [B][dim]: every member
 // gathers the rows it holds into its query scratch and copies them into the pinned staging g->h_sq, one wait per member,
 // which also brings back its count of tombstoned rows (RBK_EINVAL if any).  Caller holds g->mu.
+rbk_status group_gather_locked(rbk_group* g, const int64_t* slots, int B, double* q, bool allow_dead);
 rbk_status group_gather(rbk_group* g, const int64_t* slots, int B, double* q) {
+  std::vector<std::unique_lock<std::mutex>> locks;
+  for (rbk_index* ix : g->parts) locks.emplace_back(ix->mu);
+  return group_gather_locked(g, slots, B, q, /*allow_dead=*/false);
+}
+
+// group_gather with every member's lock held by the caller.  allow_dead: a tombstoned slot is not refused; its query
+// is zeros (launch_gather_rows).
+rbk_status group_gather_locked(rbk_group* g, const int64_t* slots, int B, double* q, bool allow_dead) {
   std::vector<std::vector<int64_t>> local, order;
   split_slots(g, slots, B, &local, &order);
   {
@@ -441,7 +451,6 @@ rbk_status group_gather(rbk_group* g, const int64_t* slots, int B, double* q) {
     const int n = static_cast<int>(local[d].size());
     if (n == 0) continue;
     rbk_index* ix = g->parts[d];
-    std::lock_guard<std::mutex> il(ix->mu);
     DeviceGuard dg(ix->device);
     rbk_status st = gather_queries(ix, local[d].data(), n);
     if (st != RBK_OK) return st;
@@ -454,10 +463,9 @@ rbk_status group_gather(rbk_group* g, const int64_t* slots, int B, double* q) {
     const int n = static_cast<int>(local[d].size());
     if (n == 0) continue;
     rbk_index* ix = g->parts[d];
-    std::lock_guard<std::mutex> il(ix->mu);
     DeviceGuard dg(ix->device);
     CK(cudaStreamSynchronize(ix->stream));
-    rbk_status st = check_gathered(ix);
+    rbk_status st = allow_dead ? RBK_OK : check_gathered(ix);
     if (st != RBK_OK) return st;
     for (int i = 0; i < n; ++i)
       memcpy(q + static_cast<size_t>(order[d][i]) * g->dim, g->h_sq.p + (first + i) * g->dim, sizeof(double) * g->dim);
@@ -722,6 +730,7 @@ void rbk_group_destroy(rbk_group* g) {
     g->h_out.release();
     g->h_q.release();
     g->h_sq.release();
+    g->h_pq.release();
     if (g->ev0) cudaEventDestroy(g->ev0);
     if (g->ev1) cudaEventDestroy(g->ev1);
   }
@@ -810,6 +819,7 @@ rbk_status rbk_group_trim(rbk_group* g) {
   g->h_out.release();
   g->h_q.release();
   g->h_sq.release();
+  g->h_pq.release();
   return RBK_OK;
 }
 
@@ -950,6 +960,40 @@ rbk_status rbk_group_search_slots_f64(rbk_group* g, const int64_t* query_slots, 
     if (device_ms_out) *device_ms_out += ms;
   }
   return RBK_OK;
+}
+
+rbk_status rbk_group_similar_pairs_f64(rbk_group* g, double min_score, int64_t first_slot, int64_t max_pairs,
+                                       int64_t* out_a, int64_t* out_b, double* out_scores, int64_t* n_out,
+                                       int64_t* next_slot, float* device_ms_out) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  std::lock_guard<std::mutex> lk(g->mu);
+  rbk_status st = check_pairs_args(0, g->n_slots, min_score, first_slot, max_pairs, out_a, out_b, out_scores, n_out,
+                                   next_slot);
+  if (st != RBK_OK) return st;
+  std::vector<std::unique_lock<std::mutex>> locks;
+  for (rbk_index* ix : g->parts) locks.emplace_back(ix->mu);
+  std::vector<int64_t> slots;
+  // every member pairs the chunk's rows with its own: the owners gather them into pinned staging, from where one
+  // asynchronous copy per member feeds them all at once (the buffer is next written after the chunk's count pass, which
+  // every member's stream has finished by then)
+  auto load = [&](int64_t a0, int Q) -> rbk_status {
+    slots.resize(Q);
+    for (int i = 0; i < Q; ++i) slots[i] = a0 + i;
+    const size_t n = static_cast<size_t>(Q) * g->dim;
+    {
+      DeviceGuard dg(g->devices[0]);
+      CK(g->h_pq.ensure(n));
+    }
+    rbk_status s2 = group_gather_locked(g, slots.data(), Q, g->h_pq.p, /*allow_dead=*/true);
+    if (s2 != RBK_OK) return s2;
+    for (rbk_index* ix : g->parts) {
+      DeviceGuard dg(ix->device);
+      CK(cudaMemcpyAsync(ix->q_raw.p, g->h_pq.p, sizeof(double) * n, cudaMemcpyHostToDevice, ix->stream));
+    }
+    return RBK_OK;
+  };
+  return similar_pairs_run(g->parts, g->n_slots, min_score, first_slot, max_pairs, load, out_a, out_b, out_scores,
+                           n_out, next_slot, device_ms_out);
 }
 
 rbk_status rbk_group_search_unbounded_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,

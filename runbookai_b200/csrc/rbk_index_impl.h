@@ -4,6 +4,7 @@
 #pragma once
 #include <string.h>
 
+#include <functional>
 #include <mutex>
 #include <string>
 #include <utility>
@@ -212,6 +213,15 @@ struct rbk_index {
   rbk::impl::DevBuf<int64_t> sq_rows;
   rbk::impl::DevBuf<int> sq_dead;
   rbk::impl::PinBuf<int> h_sq_dead;
+  // rbk_index_similar_pairs_f64: the chunk's corpus map from row pr_r0 on (pr_rows rows; 0: no row can pair), one
+  // query group's exact pair counts (device, pinned copy), their offsets and the packed pairs (global slot, score);
+  // their copy-back goes to h_block
+  CUtensorMap pr_tmap;
+  int64_t pr_r0 = 0, pr_rows = 0;
+  rbk::impl::DevBuf<int> pr_cnt;
+  rbk::impl::DevBuf<long long> pr_off, pr_b;
+  rbk::impl::DevBuf<double> pr_s;
+  rbk::impl::PinBuf<int> h_pcnt;
   CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
@@ -314,6 +324,34 @@ rbk_status large_emit(rbk_index* ix, int q0, int q1, bool sorted, int k_eff, dou
                       double* d_scores, int* d_counts, const QueryCuts& each = QueryCuts());
 rbk_status large_finish(rbk_index* ix);
 rbk_status large_check(rbk_index* ix);
+
+// rbk_index_similar_pairs_f64 and rbk_group_similar_pairs_f64.  The argument checks, in the order of the other
+// searches, for an index or group answering for global slots [slot_base, slot_base + size).
+rbk_status check_pairs_args(int64_t slot_base, int64_t size, double min_score, int64_t first_slot, int64_t max_pairs,
+                            const void* out_a, const void* out_b, const void* out_scores, const void* n_out,
+                            const void* next_slot);
+// The first local row of a shard whose global slot is >= a (n_rows or more when there is none).
+int64_t first_row_at(const SlotLayout& s, int64_t a);
+// The steps of one chunk of Q <= kSlotChunk queries, the stored rows of global slots [a0, a0 + Q), already float64 in
+// ix->q_raw (caller holds the lock, device current, query scratch for Q queries allocated):
+//   pairs_count: prep, then the count scan and the threshold-only select over the rows from the tile that holds the
+//                first row with a global slot >= a0 on (the triangle), then the D2H of C_q (enqueue only);
+//   (after a synchronisation) split_by_budget, and large_prepare(sorted) as for the unbounded search;
+//   pairs_emit : emit scan, exact re-score, drop of every pair (a, b) with b <= a, sort and packing of the pairs of the
+//                queries [q0, q1), then the D2H of their counts into h_pcnt and of the overflow counter (enqueue only);
+//   pairs_fetch: (after a synchronisation) the D2H of the first n packed pairs into h_block: slots [n] | scores [n].
+rbk_status pairs_count(rbk_index* ix, int Q, int64_t a0, double min_score);
+rbk_status pairs_emit(rbk_index* ix, int q0, int q1, int64_t a0, double min_score);
+rbk_status pairs_fetch(rbk_index* ix, int64_t n);
+// The paged pass over members `parts` (one index, or a group's members, whose rows together are global slots
+// [0 or slot_base, end)), from first_slot on, checked arguments; the caller holds every member's lock.  load(a0, Q)
+// enqueues the stored rows of global slots [a0, a0 + Q) into every member's q_raw as float64 queries.  Chunk after
+// chunk and query group after query group, every member's packed pairs are counted (one round trip), the rows that
+// still fit in max_pairs are copied back (another) and merged per query on the host.  The first row that does not fit
+// ends the pass; the rest of its chunk is discarded.  Adds 1 search and *next_slot - first_slot queries to every member.
+rbk_status similar_pairs_run(const std::vector<rbk_index*>& parts, int64_t end, double min_score, int64_t first_slot,
+                             int64_t max_pairs, const std::function<rbk_status(int64_t, int)>& load, int64_t* out_a,
+                             int64_t* out_b, double* out_scores, int64_t* n_out, int64_t* next_slot, float* ms_out);
 
 // The steps of a compaction, shared by rbk_index_compact and rbk_group_compact (caller holds ix->mu and has the index's
 // device current).  Staging of C rows, packed: bf16 (or fp16) rows [C][dpad] | exact rows [C][dim] (x_elem bytes each,

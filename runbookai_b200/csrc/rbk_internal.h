@@ -118,7 +118,7 @@ cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows
 // (rbk_gather.cu) Query b = the stored values of local row sel[b] (device [B], each < n_rows) as float64, into dst [B][d]: the exact
 // row widened (x_elem 8 / 4), the split's float32 rebuilt from both halves (x_elem 2), or the bf16 scan copy widened
 // (x_elem 0; never an RBK_INDEX_SCAN_F16 index, which keeps exact rows).  rows_x may be mapped host memory.  Adds the
-// number of tombstoned rows among them to *n_dead.
+// number of tombstoned rows among them to *n_dead, and gives each of those the query of zeros, which matches nothing.
 cudaError_t launch_gather_rows(const uint16_t* rows, const void* rows_x, int x_elem, const unsigned int* dead_bits,
                                const int64_t* sel, int B, int d, int dpad, double* dst, int* n_dead,
                                cudaStream_t stream);
@@ -291,6 +291,22 @@ struct SegSortScratch {
 // *launches: kernels enqueued.
 cudaError_t launch_large_rerank(const LargeRerankParams& p, const SegSortScratch* sort, int max_cap,
                                 bool rows_on_host, int x_elem, cudaStream_t stream, int* launches);
+
+// rbk_index_similar_pairs_f64: B <= kMaxSubBatch queries that are the stored rows of global slots a0 + q, against the
+// rows from local row r0 on.  The LargeRerankParams row pointers (rows, rows_x, row_norm2) then start at row r0, and
+// so do the emitted rows; p.slot still maps local rows.  The re-score, then the drop of every candidate whose global slot
+// is not above its query's (and, as in the sort, of scores below min_score and NaN), the segmented sort with no cut,
+// counts [B] (each query's pairs), offsets [B] (their exclusive scan) and the pairs packed query after query into
+// out_b / out_scores from offsets[q] on.  p.k_fetch and p.k_each are ignored.
+struct PairsParams {
+  int64_t a0, r0;
+  int* counts;
+  long long* offsets;
+  long long* out_b;
+  double* out_scores;
+};
+cudaError_t launch_pairs_rerank(const LargeRerankParams& p, const SegSortScratch& sort, int max_cap, bool rows_on_host,
+                                int x_elem, const PairsParams& pp, cudaStream_t stream, int* launches);
 
 // Exact fp64 cosine of every row for B prepared queries: out [B][n_rows], NaN = tombstoned / zero row.
 cudaError_t launch_exact_scores(const uint16_t* rows, const void* rows_x, int x_elem, const double* row_norm2,

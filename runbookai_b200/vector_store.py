@@ -715,6 +715,27 @@ class VectorStore:
             out.append(self._hydrate([i for i, _ in h], [sc for _, sc in h], top_k, type_filter, service_filter))
         return out
 
+    def similar_pairs(self, min_score: float) -> list[tuple[str, str, float]]:
+        """Every pair of stored chunks whose embeddings' cosine is >= min_score ("which chunks are near-duplicates of
+        each other"), exactly: [(chunk_id_a, chunk_id_b, score), ...], each pair once, in the engine's order (a's slot
+        ascending, then score descending, ties by b's slot ascending).  The reference has no such call, so no default
+        applies.  ValueError for a NaN min_score; DimensionError on a ragged store, as search(); [] on an empty store."""
+        if min_score != min_score:
+            raise ValueError("min_score is NaN")
+        out: list[tuple[str, str, float]] = []
+        with self._st.lock:   # the slot table must be the one the pass ran against
+            if self._ragged:
+                raise DimensionError(RBK_EDIM, "Vectors must have the same length")
+            if self._index is None or not self._ids:
+                return out
+            nxt = None
+            while True:
+                a, b, scores, nxt = self._index.similar_pairs(min_score, nxt)
+                out += [(self._ids[int(x)].removeprefix("vec_"), self._ids[int(y)].removeprefix("vec_"), float(s))
+                        for x, y, s in zip(a, b, scores)]
+                if nxt >= self._index.size():
+                    return out
+
     def _hydrate(self, top_ids, scores, top_k, type_filter, service_filter) -> list[RetrievedChunk]:
         """vector-store.ts:223-279 (a4): stays on the host."""
         pairs = [(i, float(sc)) for i, sc in zip(top_ids, scores) if i is not None]   # None: deleted meanwhile

@@ -288,6 +288,39 @@ export class GpuEmbeddingIndex {
     }
   }
 
+  /** Whether similarPairs is available: the loaded addon's library has rbk_*_similar_pairs_f64. */
+  get hasSimilarPairs(): boolean {
+    return this.index !== null && this.index.hasSimilarPairs === true;
+  }
+
+  /**
+   * Every pair of stored embeddings whose cosine is >= minScore ("which chunks are near-duplicates of each other"),
+   * exactly, each pair once: [idA, idB, score] in the engine's order (idA's slot ascending, then score descending, ties
+   * by idB's slot ascending).  The addon answers in pages of whole rows; this loops them until the pass is complete.
+   * Throws on a ragged Map (as best does) and against a library without similar pairs (hasSimilarPairs false).
+   */
+  async similarPairs(minScore: number): Promise<Array<[string, string, number]>> {
+    while (this.compacting) await this.compacting; // never search against a table that is being renumbered
+    if (this.badIds.size > 0) throw new Error('Vectors must have the same length');
+    if (!this.index || this.slotOfId.size === 0) return [];
+    const end = this.idOfSlot.length;
+    const page = Math.max(end, 1 << 20);
+    const out: Array<[string, string, number]> = [];
+    this.inFlight++;
+    try {
+      for (let next = 0; next < end; ) {
+        const { a, b, scores, nextSlot } = await this.index.similarPairs(minScore, next, page);
+        for (let i = 0; i < scores.length; i++) {
+          out.push([this.idOfSlot[Number(a[i])]!, this.idOfSlot[Number(b[i])]!, scores[i]]);
+        }
+        next = Number(nextSlot);
+      }
+      return out;
+    } finally {
+      if (--this.inFlight === 0) this.drained.splice(0).forEach((wake) => wake());
+    }
+  }
+
   /**
    * Give the slots of deleted ids back (the reference's Map.delete frees its entry; a tombstone alone does not): the
    * device index moves its live rows down in Map order and returns oldToNew, through which slotOfId and idOfSlot are
