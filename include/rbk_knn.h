@@ -385,6 +385,41 @@ rbk_status rbk_index_similar_pairs_f64(rbk_index* idx, double min_score, int64_t
                                        int64_t* out_a, int64_t* out_b, double* out_scores, int64_t* n_out,
                                        int64_t* next_slot, float* kernel_ms_out);
 
+/* fetch_k[b] * dim must not exceed this: at most 256 MiB of float64 candidate rows staged per query. */
+#define RBK_MMR_MAX_FETCH_ELEMS (1 << 25)
+/* Diverse hits by maximal marginal relevance (MMR): k[b] of query b's fetch_k[b] best candidates, picked greedily so that
+ * each pick is relevant to the query and unlike the picks before it.  lambda_mult[b] in [0, 1] weighs the two (1: the
+ * plain ranking).  For query b the result is defined exactly as follows.
+ *  1. Candidates: c_0 .. c_{m-1} with relevance r_0 .. r_{m-1} are exactly row b of rbk_index_search_each_f64 at
+ *     k_fetch = fetch_k[b], min_score = min_score[b]: the same slots and fp64 score bits in the same order (score
+ *     descending, ties by ascending slot).  Candidate index i is the rank in that list.
+ *  2. Pair similarity: s(i, j) is the reference's cosineSimilarity of the stored values of the two rows - the values
+ *     rbk_index_search_slots_f64 uses as a query: the float64 row, the float32 row widened, the split float32 rebuilt
+ *     from its two halves, or the bf16 row widened.  Its bits are symmetric in i and j.
+ *  3. Greedy: the first pick is c_0.  For each later pick, every unpicked i has red_i, the largest non-NaN s(i, j) over
+ *     the picks j so far, or NaN if all of them are NaN (a new s replaces red_i only if it is strictly greater, or if
+ *     red_i is NaN), and mmr_i = lambda * r_i - (1 - lambda) * red_i, one correctly rounded fp64 operation per step in
+ *     this order: t = 1.0 - lambda, a = lambda * r_i, c = t * red_i, mmr = a - c.  The pick is the i that ranks first
+ *     under a total order: a NaN mmr ranks below every number, then the larger value wins, then the smaller i.
+ *  4. Output: out_counts[b] = min(k[b], m); row b of out_slots / out_scores ([B][K], K = max_b k[b]) holds the picks in
+ *     selection order, each pick's global slot and its relevance r; the tail is slot -1 and the quiet NaN
+ *     0x7FF8000000000000, as in rbk_index_search_each_f64.  No mmr value is returned.
+ * Invariants: at lambda = 1 the result is the first min(k, m) entries of the search_each row whenever no s is +-inf;
+ * k = 1 gives c_0; a group gives the answers of a single index holding the same rows.
+ * Argument checks, before any device work and in the order of rbk_index_search_each_f64: a null array with B > 0, a
+ * k[b] < 1, a fetch_k[b] < k[b], a fetch_k[b] > RBK_MAX_K_FETCH_LARGE or a fetch_k[b] * dim > RBK_MMR_MAX_FETCH_ELEMS is
+ * RBK_EINVAL; then the wrong query_dim is RBK_EDIM; then a NaN min_score[b] or a lambda_mult[b] outside [0, 1] (NaN
+ * included) is RBK_EINVAL.  B = 0 is RBK_OK.  One call adds 1 to the searches counter and B to the queries counter.
+ * How: queries go in chunks of 1024.  Each chunk runs the search_each pipeline at its largest fetch_k, then the
+ * candidates' rows are gathered as float64 into device scratch, for contiguous query groups whose rows fit the large-k
+ * per-pass budget (256 MiB), and one block per query runs the greedy selection on the device (rbk_mmr.cu).  The lock is
+ * held throughout, so the candidates and their rows come from the same state.  rbk_index_trim releases the scratch.
+ * kernel_ms_out (nullable): device time of the whole call.  Synchronous. */
+rbk_status rbk_index_search_mmr_f64(rbk_index* idx, const double* queries, int32_t B, int32_t query_dim,
+                                    const int32_t* k, const int32_t* fetch_k, const double* lambda_mult,
+                                    const double* min_score, int64_t* out_slots, double* out_scores,
+                                    int32_t* out_counts, float* kernel_ms_out);
+
 /* Enqueue-only variant: nothing is synchronised, the call returns as soon as the kernels are queued on the index
  * stream, so batches pipeline back to back and an exchange step (all-gather + rbk_merge_topk_packed_device) can be
  * queued behind it without a host round trip in between.  dev_out_flags_i32[B]: 0 = the answer of query b is
@@ -506,6 +541,14 @@ rbk_status rbk_group_search_slots_f64(rbk_group* grp, const int64_t* query_slots
 rbk_status rbk_group_similar_pairs_f64(rbk_group* grp, double min_score, int64_t first_slot, int64_t max_pairs,
                                        int64_t* out_a, int64_t* out_b, double* out_scores, int64_t* n_out,
                                        int64_t* next_slot, float* device_ms_out);
+/* rbk_index_search_mmr_f64 over the group: the candidates come from rbk_group_search_each_f64 (global slots); per query
+ * group the members that hold them gather their rows into pinned staging, and the selection runs on device_ids[0].
+ * Uses no NCCL beyond that of rbk_group_search_each_f64.  Same arguments, checks, layout and answers as the index call
+ * on a single index holding the same rows; rbk_group_trim releases the staging. */
+rbk_status rbk_group_search_mmr_f64(rbk_group* grp, const double* queries, int32_t B, int32_t query_dim,
+                                    const int32_t* k, const int32_t* fetch_k, const double* lambda_mult,
+                                    const double* min_score, int64_t* out_slots, double* out_scores,
+                                    int32_t* out_counts, float* device_ms_out);
 
 /* ---- introspection ---- */
 typedef struct {

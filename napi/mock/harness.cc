@@ -476,6 +476,75 @@ int main(int argc, char** argv) {
     }
   }
 
+  // searchMmr(): optional mmr.txt holds one "k fetchK lambdaMult minScore" line per query (minScore may be -inf);
+  // results land in mmr_* with rows of K = max k entries.  has_search_mmr.txt gets the hasSearchMmr getter first.  Then
+  // one call with a k of 0 (err_mmr) and one with a lambdaMult of 2 (err_mmr_lambda) must reject with the library's
+  // message.
+  {
+    std::ifstream mf(g_dir + "/mmr.txt");
+    std::vector<int32_t> kv, fv;
+    std::vector<double> lv, mv;
+    std::string ks, fs, ls, ms;
+    while (mf >> ks >> fs >> ls >> ms) {
+      kv.push_back(static_cast<int32_t>(strtol(ks.c_str(), nullptr, 10)));
+      fv.push_back(static_cast<int32_t>(strtol(fs.c_str(), nullptr, 10)));
+      lv.push_back(strtod(ls.c_str(), nullptr));
+      mv.push_back(strtod(ms.c_str(), nullptr));
+    }
+    if (!kv.empty()) {
+      if (kv.size() != static_cast<size_t>(n_q)) die("mmr.txt needs one line per query");
+      napi_value has = nullptr;
+      if (!mock::get_accessor(env, ix, "hasSearchMmr", &has, &err)) die("hasSearchMmr threw: " + err);
+      write_text("has_search_mmr.txt", mock::as_bool(has) ? "1" : "0");
+      int K = 0;
+      for (int32_t v : kv) K = v > K ? v : K;
+      auto call_mmr = [&](const std::vector<int32_t>& k, const std::vector<double>& lam, Result* out) {
+        napi_value promise = nullptr, settled = nullptr;
+        if (!mock::call_method(env, ix, "searchMmr",
+                               {mock::typed_array(env, napi_float64_array, queries.data(), queries.size()),
+                                mock::number(env, n_q), mock::typed_array(env, napi_int32_array, k.data(), k.size()),
+                                mock::typed_array(env, napi_int32_array, fv.data(), fv.size()),
+                                mock::typed_array(env, napi_float64_array, lam.data(), lam.size()),
+                                mock::typed_array(env, napi_float64_array, mv.data(), mv.size())},
+                               &promise, &err))
+          return false;
+        mock::run_event_loop(env);
+        const int state = mock::promise_state(promise, &settled);
+        if (state == 2) {
+          err = mock::error_message(settled);
+          return false;
+        }
+        if (state != 1) die("searchMmr() left its promise pending");
+        napi_typedarray_type t;
+        size_t n;
+        const void* p = mock::typed_data(mock::get_property(env, settled, "slots"), &t, &n);
+        if (!p || t != napi_bigint64_array || n != static_cast<size_t>(n_q) * K) die("searchMmr slots are not [B*K]");
+        out->slots.assign(static_cast<const int64_t*>(p), static_cast<const int64_t*>(p) + n);
+        p = mock::typed_data(mock::get_property(env, settled, "scores"), &t, &n);
+        if (!p || t != napi_float64_array || n != static_cast<size_t>(n_q) * K) die("searchMmr scores are not [B*K]");
+        out->scores.assign(static_cast<const double*>(p), static_cast<const double*>(p) + n);
+        p = mock::typed_data(mock::get_property(env, settled, "counts"), &t, &n);
+        if (!p || t != napi_int32_array || n != static_cast<size_t>(n_q)) die("searchMmr counts are not [B]");
+        out->counts.assign(static_cast<const int32_t*>(p), static_cast<const int32_t*>(p) + n);
+        return true;
+      };
+      Result mr;
+      if (!call_mmr(kv, lv, &mr)) die("searchMmr rejected: " + err);
+      write_bin("mmr_slots.i64", mr.slots.data(), mr.slots.size() * 8);
+      write_bin("mmr_scores.f64", mr.scores.data(), mr.scores.size() * 8);
+      write_bin("mmr_counts.i32", mr.counts.data(), mr.counts.size() * 4);
+      Result none;
+      std::vector<int32_t> bad_k = kv;
+      bad_k[0] = 0;
+      if (call_mmr(bad_k, lv, &none)) die("searchMmr with a k of 0 did not reject");
+      log << "err_mmr " << err << "\n";
+      std::vector<double> bad_l = lv;
+      bad_l[0] = 2.0;
+      if (call_mmr(kv, bad_l, &none)) die("searchMmr with a lambdaMult of 2 did not reject");
+      log << "err_mmr_lambda " << err << "\n";
+    }
+  }
+
   // ---- error paths: each must surface as a JS exception / rejection with the reference's wording
   {
     std::vector<double> odd(static_cast<size_t>(dim) + 1, 1.0);

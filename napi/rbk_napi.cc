@@ -37,6 +37,10 @@
 //   await ix.searchSlots(BigInt64Array slots, B, Int32Array kFetch, Float64Array minScore)   // searchEach whose
 //        queries are the stored rows of those global slots, read where the index keeps them: the same result object
 //   ix.hasSearchSlots                          -> boolean: the library has searchSlots (else it throws)
+//   await ix.searchMmr(Float64Array queries, B, Int32Array k, Int32Array fetchK, Float64Array lambdaMult,
+//                      Float64Array minScore)   // diverse hits by maximal marginal relevance: query b's k[b] picks
+//        from its fetchK[b] best, in selection order with their relevance: the result object with rows of max(k)
+//   ix.hasSearchMmr                            -> boolean: the library has searchMmr (else it throws)
 //   await ix.similarPairs(minScore, firstSlot, maxPairs)   // one page of every pair of live slots a < b with cosine
 //        >= minScore, rows a from firstSlot on, at most maxPairs (>= size()) entries, whole rows only
 //        -> { a: BigInt64Array, b: BigInt64Array, scores: Float64Array, nextSlot }   // nextSlot == size(): done
@@ -85,6 +89,9 @@
 // The same for stored rows as queries; `searchSlots` throws where it is missing.
 #pragma weak rbk_index_search_slots_f64
 #pragma weak rbk_group_search_slots_f64
+// The same for diverse hits by maximal marginal relevance; `searchMmr` throws where it is missing.
+#pragma weak rbk_index_search_mmr_f64
+#pragma weak rbk_group_search_mmr_f64
 // The same for every pair above a threshold; `similarPairs` throws where it is missing.
 #pragma weak rbk_index_similar_pairs_f64
 #pragma weak rbk_group_similar_pairs_f64
@@ -177,6 +184,14 @@ struct Handle {
                           int32_t* c) {
     return grp ? rbk_group_search_slots_f64(grp, q, B, k, ms, s, v, c, nullptr)
                : rbk_index_search_slots_f64(ix, q, B, k, ms, s, v, c, nullptr);
+  }
+  bool has_search_mmr() const {
+    return grp ? rbk_group_search_mmr_f64 != nullptr : rbk_index_search_mmr_f64 != nullptr;
+  }
+  rbk_status search_mmr(const double* q, int32_t B, int32_t qdim, const int32_t* k, const int32_t* f, const double* l,
+                        const double* ms, int64_t* s, double* v, int32_t* c) {
+    return grp ? rbk_group_search_mmr_f64(grp, q, B, qdim, k, f, l, ms, s, v, c, nullptr)
+               : rbk_index_search_mmr_f64(ix, q, B, qdim, k, f, l, ms, s, v, c, nullptr);
   }
   bool has_similar_pairs() const {
     return grp ? rbk_group_similar_pairs_f64 != nullptr : rbk_index_similar_pairs_f64 != nullptr;
@@ -498,8 +513,8 @@ napi_value Count(napi_env env, napi_callback_info info) {
 }
 
 // ---- search: runs on a libuv worker so the JS thread never blocks on the GPU ----
-// search / searchLarge / searchUnbounded / searchEach / searchSlots
-enum class SearchKind { kScan, kLarge, kUnbounded, kEach, kSlots };
+// search / searchLarge / searchUnbounded / searchEach / searchSlots / searchMmr
+enum class SearchKind { kScan, kLarge, kUnbounded, kEach, kSlots, kMmr };
 
 struct SearchJob {
   Handle* ix;
@@ -510,6 +525,8 @@ struct SearchJob {
   std::vector<int64_t> query_slots;  // searchSlots: the queries' global slots [B]
   std::vector<int32_t> k_each;      // searchEach, searchSlots: kFetch[B] and minScore[B]; k is then their largest k
   std::vector<double> min_each;
+  std::vector<int32_t> fetch_each;   // searchMmr: fetchK[B] and lambdaMult[B]; k_each is then k[B], min_each minScore[B]
+  std::vector<double> lambda_each;
   std::vector<int64_t> slots;
   std::vector<double> scores;
   std::vector<int32_t> counts;
@@ -524,6 +541,13 @@ void search_execute(napi_env, void* data) {
   if (j->kind == SearchKind::kSlots) {
     j->st = j->ix->search_slots(j->query_slots.data(), j->B, j->k_each.data(), j->min_each.data(), j->slots.data(),
                                 j->scores.data(), j->counts.data());
+    if (j->st != RBK_OK) j->err = rbk_last_error();
+    return;
+  }
+  if (j->kind == SearchKind::kMmr) {
+    j->st = j->ix->search_mmr(j->queries.data(), j->B, j->dim, j->k_each.data(), j->fetch_each.data(),
+                              j->lambda_each.data(), j->min_each.data(), j->slots.data(), j->scores.data(),
+                              j->counts.data());
     if (j->st != RBK_OK) j->err = rbk_last_error();
     return;
   }
@@ -664,6 +688,68 @@ napi_value SearchEach(napi_env env, napi_callback_info info) { return QueueSearc
 
 napi_value SearchSlots(napi_env env, napi_callback_info info) { return QueueSearch(env, info, SearchKind::kSlots); }
 
+// searchMmr(queries, B, k, fetchK, lambdaMult, minScore): one Int32Array or Float64Array entry per query each; the
+// library checks the values, so a k[b] < 1 or a lambdaMult[b] outside [0, 1] rejects with its message.
+napi_value SearchMmr(napi_env env, napi_callback_info info) {
+  size_t argc = 6;
+  napi_value argv[6];
+  Handle* ix = unwrap(env, info, &argc, argv);
+  if (!ix->has_search_mmr()) {
+    napi_throw_error(env, nullptr, "searchMmr: this librbk_knn.so has no MMR search (rbk_*_search_mmr_f64)");
+    return nullptr;
+  }
+  napi_typedarray_type t[6];
+  size_t len[6] = {};
+  void* data[6] = {};
+  for (int i : {0, 2, 3, 4, 5}) {
+    if (argc <= static_cast<size_t>(i) ||
+        napi_get_typedarray_info(env, argv[i], &t[i], &len[i], &data[i], nullptr, nullptr) != napi_ok)
+      t[i] = napi_uint8_array;   // not a typed array: refused below
+  }
+  if (t[0] != napi_float64_array || t[2] != napi_int32_array || t[3] != napi_int32_array ||
+      t[4] != napi_float64_array || t[5] != napi_float64_array) {
+    napi_throw_type_error(env, nullptr, "searchMmr: queries, lambdaMult and minScore must be Float64Arrays, k and "
+                                        "fetchK Int32Arrays");
+    return nullptr;
+  }
+  int32_t B = 0;
+  napi_get_value_int32(env, argv[1], &B);
+  if (B < 0 || len[2] != static_cast<size_t>(B) || len[3] != static_cast<size_t>(B) ||
+      len[4] != static_cast<size_t>(B) || len[5] != static_cast<size_t>(B)) {
+    napi_throw_error(env, nullptr, "searchMmr: k, fetchK, lambdaMult and minScore need one entry per query");
+    return nullptr;
+  }
+  auto* j = new SearchJob();
+  j->ix = ix;
+  j->kind = SearchKind::kMmr;
+  j->B = B;
+  j->dim = B > 0 ? (int32_t)(len[0] / (size_t)B) : 0;   // a wrong length surfaces as RBK_EDIM
+  j->queries.assign(static_cast<double*>(data[0]), static_cast<double*>(data[0]) + len[0]);
+  j->k_each.assign(static_cast<int32_t*>(data[2]), static_cast<int32_t*>(data[2]) + B);
+  j->fetch_each.assign(static_cast<int32_t*>(data[3]), static_cast<int32_t*>(data[3]) + B);
+  j->lambda_each.assign(static_cast<double*>(data[4]), static_cast<double*>(data[4]) + B);
+  j->min_each.assign(static_cast<double*>(data[5]), static_cast<double*>(data[5]) + B);
+  j->k = 0;   // the row stride: the largest k (a k[b] < 1 is refused by the library)
+  for (int32_t v : j->k_each) j->k = std::max(j->k, v);
+  j->slots.resize((size_t)B * j->k);
+  j->scores.resize((size_t)B * j->k);
+  j->counts.resize((size_t)B);
+  napi_value promise, name;
+  NAPI_OK(napi_create_promise(env, &j->deferred, &promise));
+  napi_create_string_utf8(env, "rbk_search_mmr", NAPI_AUTO_LENGTH, &name);
+  NAPI_OK(napi_create_async_work(env, nullptr, name, search_execute, search_complete, j, &j->work));
+  NAPI_OK(napi_queue_async_work(env, j->work));
+  return promise;
+}
+
+napi_value HasSearchMmr(napi_env env, napi_callback_info info) {
+  size_t argc = 0;
+  Handle* h = unwrap(env, info, &argc, nullptr);
+  napi_value out;
+  NAPI_OK(napi_get_boolean(env, h->has_search_mmr(), &out));
+  return out;
+}
+
 napi_value HasSearchEach(napi_env env, napi_callback_info info) {
   size_t argc = 0;
   Handle* h = unwrap(env, info, &argc, nullptr);
@@ -793,6 +879,8 @@ napi_value Init(napi_env env, napi_value exports) {
       {"hasSearchEach", nullptr, nullptr, HasSearchEach, nullptr, nullptr, napi_default, nullptr},
       {"searchSlots", nullptr, SearchSlots, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"hasSearchSlots", nullptr, nullptr, HasSearchSlots, nullptr, nullptr, napi_default, nullptr},
+      {"searchMmr", nullptr, SearchMmr, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"hasSearchMmr", nullptr, nullptr, HasSearchMmr, nullptr, nullptr, napi_default, nullptr},
       {"similarPairs", nullptr, SimilarPairs, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"hasSimilarPairs", nullptr, nullptr, HasSimilarPairs, nullptr, nullptr, napi_default, nullptr},
   };

@@ -40,6 +40,7 @@ SYMBOLS = [
     "rbk_index_search_each_f64", "rbk_group_search_each_f64",
     "rbk_index_search_slots_f64", "rbk_group_search_slots_f64",
     "rbk_index_similar_pairs_f64", "rbk_group_similar_pairs_f64",
+    "rbk_index_search_mmr_f64", "rbk_group_search_mmr_f64",
 ]
 
 
@@ -140,6 +141,8 @@ def _load() -> C.CDLL:
     for n in ("rbk_index_similar_pairs_f64", "rbk_group_similar_pairs_f64"):
         getattr(lib, n).argtypes = [vp, f64, i64, i64, vp, vp, vp, C.POINTER(i64), C.POINTER(i64),
                                     C.POINTER(C.c_float)]
+    for n in ("rbk_index_search_mmr_f64", "rbk_group_search_mmr_f64"):
+        getattr(lib, n).argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_float)]
     lib.rbk_index_debug_scores_f32.argtypes = [vp, vp, i32, vp]
     lib.rbk_index_flags.argtypes = [vp]
     lib.rbk_index_flags.restype = C.c_uint32
@@ -259,6 +262,39 @@ def _search_slots(fn, h, slots, k_fetch, min_score):
     ms = C.c_float(0)
     check(fn(h, ptr(sl), B, ptr(k32), ptr(m), ptr(out_slots), ptr(scores), ptr(counts), C.byref(ms)))
     return out_slots, scores, counts, ms.value
+
+
+def _per_query(B: int, v, name: str, dtype):
+    """A scalar or one value per query as a contiguous array [B] of dtype (None = -inf, for min_score)."""
+    vals = list(v) if np.ndim(v) else [v] * B
+    if len(vals) != B:
+        raise ValueError(f"{name} needs one entry per query ({B}), not {len(vals)}")
+    if dtype == np.int32:
+        a = np.asarray(vals, dtype=np.int64).reshape(-1)
+        if (np.abs(a) > np.iinfo(np.int32).max).any():
+            raise RbkError(RBK_EINVAL, f"every {name} must fit an int32")
+        return np.ascontiguousarray(a, dtype=np.int32)
+    return np.ascontiguousarray([-np.inf if x is None else float(x) for x in vals], dtype=np.float64)
+
+
+def _search_mmr(fn, h, queries, k, fetch_k, lambda_mult, min_score):
+    """rbk_*_search_mmr_f64: k, fetch_k, lambda_mult and min_score (None = -inf) one per query or one for all; the
+    library checks them.  Returns (slots int64 [B, K], scores float64 [B, K], counts int32 [B], device_ms) with
+    K = max(k): row b holds query b's picks in selection order with their relevance, then -1 / NaN."""
+    q = np.ascontiguousarray(np.atleast_2d(np.asarray(queries, dtype=np.float64)))
+    B = q.shape[0]
+    k32 = _per_query(B, k, "k", np.int32)
+    f32 = _per_query(B, fetch_k, "fetch_k", np.int32)
+    lam = _per_query(B, lambda_mult, "lambda_mult", np.float64)
+    m = _per_query(B, min_score, "min_score", np.float64)
+    K = int(max(k32.max(), 0)) if B else 0
+    slots = np.empty((B, K), dtype=np.int64)
+    scores = np.empty((B, K), dtype=np.float64)
+    counts = np.empty((B,), dtype=np.int32)
+    ms = C.c_float(0)
+    check(fn(h, ptr(q), B, q.shape[1], ptr(k32), ptr(f32), ptr(lam), ptr(m), ptr(slots), ptr(scores), ptr(counts),
+             C.byref(ms)))
+    return slots, scores, counts, ms.value
 
 
 def _similar_pairs(fn, h, first: int, size: int, min_score, first_slot, max_pairs):
@@ -499,6 +535,13 @@ class Index:
         index does not hold, or a tombstoned one, raises RbkError (RBK_EINVAL)."""
         return _search_slots(lib.rbk_index_search_slots_f64, self._h, slots, k_fetch, min_score)
 
+    def search_mmr(self, queries, k, fetch_k, lambda_mult=0.5, min_score=0.5):
+        """Diverse hits by maximal marginal relevance (include/rbk_knn.h): per query, k of the fetch_k hits search_each()
+        returns at min_score, picked greedily by lambda_mult * relevance - (1 - lambda_mult) * (largest cosine to a
+        pick so far).  Arguments one per query or one for all (min_score None = -inf).  Returns (slots [B, K], scores
+        [B, K], counts [B], device_ms), K = max(k): the picks in selection order with their relevance, then -1 / NaN."""
+        return _search_mmr(lib.rbk_index_search_mmr_f64, self._h, queries, k, fetch_k, lambda_mult, min_score)
+
     def similar_pairs(self, min_score, first_slot=None, max_pairs=None):
         """One page of every pair of stored rows at or above min_score (None = -inf), exactly: (a [n], b [n],
         scores [n], next_slot) numpy arrays, slots a < b, first_slot <= a < next_slot (first_slot None: slot_base), at
@@ -673,6 +716,10 @@ class Group:
     def search_slots(self, slots, k_fetch, min_score):
         """Index.search_slots() over the group: each slot's member gathers its row, then one search_each."""
         return _search_slots(lib.rbk_group_search_slots_f64, self._h, slots, k_fetch, min_score)
+
+    def search_mmr(self, queries, k, fetch_k, lambda_mult=0.5, min_score=0.5):
+        """Index.search_mmr() over the group: the candidates' owners gather their rows, device_ids[0] selects."""
+        return _search_mmr(lib.rbk_group_search_mmr_f64, self._h, queries, k, fetch_k, lambda_mult, min_score)
 
     def similar_pairs(self, min_score, first_slot=None, max_pairs=None):
         """Index.similar_pairs() over the group's global slots [0, size()): the answers of a single index."""

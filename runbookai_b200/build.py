@@ -13,7 +13,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "lib" / "librbk_knn.so"
-SOURCES = ["rbk_capi.cu", "rbk_group.cu", "rbk_scan.cu", "rbk_scan_f16.cu", "rbk_ingest.cu", "rbk_finalize.cu", "rbk_compact.cu", "rbk_gather.cu"]
+SOURCES = ["rbk_capi.cu", "rbk_group.cu", "rbk_scan.cu", "rbk_scan_f16.cu", "rbk_ingest.cu", "rbk_finalize.cu", "rbk_compact.cu", "rbk_gather.cu", "rbk_mmr.cu"]
 HEADERS = ["rbk_internal.h", "rbk_index_impl.h", "rbk_group_plan.h", "rbk_ptx.cuh", "rbk_epilogue.cuh", "rbk_scan_kernel.cuh", "rbk_f16.cuh", "../../include/rbk_knn.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

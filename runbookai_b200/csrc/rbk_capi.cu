@@ -699,6 +699,97 @@ rbk_status check_gathered(const rbk_index* ix) {
   return fail(RBK_EINVAL, "query slot is tombstoned (" + std::to_string(ix->h_sq_dead.p[0]) + " of the batch)");
 }
 
+rbk_status check_mmr_args(rbk_index* ix, int B, bool have_q, int query_dim, const int32_t* k, const int32_t* fetch_k,
+                          const double* lambda_mult, const double* min_score, const void* out_slots,
+                          const void* out_scores, const void* out_counts, int* K) {
+  *K = 0;
+  if (!ix) return fail(RBK_EINVAL, "null index");
+  if (B < 0 || (B > 0 && !have_q)) return fail(RBK_EINVAL, "bad queries argument");
+  if (B > 0 && (!k || !fetch_k || !lambda_mult || !min_score))
+    return fail(RBK_EINVAL, "null k, fetch_k, lambda_mult or min_score array");
+  if (B > 0 && (!out_slots || !out_scores || !out_counts)) return fail(RBK_EINVAL, "null output");
+  for (int b = 0; b < B; ++b) {
+    const std::string at = "[" + std::to_string(b) + "]";
+    if (k[b] < 1) return fail(RBK_EINVAL, "k" + at + " must be >= 1");
+    if (fetch_k[b] < k[b]) return fail(RBK_EINVAL, "fetch_k" + at + " must be >= k" + at);
+    if (fetch_k[b] > RBK_MAX_K_FETCH_LARGE)
+      return fail(RBK_EINVAL, "fetch_k" + at + " must be <= " + std::to_string(RBK_MAX_K_FETCH_LARGE));
+    if (static_cast<int64_t>(fetch_k[b]) * ix->dim > RBK_MMR_MAX_FETCH_ELEMS)
+      return fail(RBK_EINVAL, "fetch_k" + at + " * dim must be <= RBK_MMR_MAX_FETCH_ELEMS");
+    *K = std::max(*K, static_cast<int>(k[b]));
+  }
+  if (query_dim != ix->dim) return fail(RBK_EDIM, "Vectors must have the same length");  // embedder.ts:170
+  for (int b = 0; b < B; ++b) {
+    if (min_score[b] != min_score[b]) return fail(RBK_EINVAL, "min_score[" + std::to_string(b) + "] is NaN");
+    if (!(lambda_mult[b] >= 0.0 && lambda_mult[b] <= 1.0))
+      return fail(RBK_EINVAL, "lambda_mult[" + std::to_string(b) + "] must be in [0, 1]");
+  }
+  return RBK_OK;
+}
+
+rbk_status mmr_select_locked(rbk_index* ix, int Bc, int F, const int64_t* c_slots, const double* c_scores,
+                             const int32_t* c_counts, const int32_t* k, const double* lambda_mult, int K,
+                             const MmrStage& stage, bool check_dead, int64_t* out_slots, double* out_scores,
+                             int32_t* out_counts, float* ms_out) {
+  std::vector<int64_t> cost(Bc);
+  for (int b = 0; b < Bc; ++b) {
+    cost[b] = static_cast<int64_t>(c_counts[b]) * ix->dim * 8;
+    out_counts[b] = std::min(k[b], c_counts[b]);
+  }
+  // RBK_MMR_MAX_FETCH_ELEMS keeps every query's rows within the budget, so a group of one always fits
+  for (const auto& gr : split_by_budget(cost)) {
+    const int q0 = gr.first, Bg = gr.second - gr.first;
+    // packed inputs: off i64 [Bg + 1] | slots i64 [M] | rel f64 [M] | lambda f64 [Bg] | k i32 [Bg]
+    std::vector<int64_t> off(Bg + 1, 0);
+    int max_m = 0;
+    for (int b = 0; b < Bg; ++b) {
+      off[b + 1] = off[b] + c_counts[q0 + b];
+      max_m = std::max(max_m, static_cast<int>(c_counts[q0 + b]));
+    }
+    const int64_t M = off[Bg];
+    const size_t o_slots = 8 * static_cast<size_t>(Bg + 1), o_rel = o_slots + 8 * M, o_lam = o_rel + 8 * M,
+                 o_k = o_lam + 8 * static_cast<size_t>(Bg), bytes = o_k + 4 * static_cast<size_t>(Bg);
+    std::vector<unsigned char> h(bytes);
+    memcpy(h.data(), off.data(), o_slots);
+    int64_t* h_slots = reinterpret_cast<int64_t*>(h.data() + o_slots);
+    double* h_rel = reinterpret_cast<double*>(h.data() + o_rel);
+    for (int b = 0; b < Bg; ++b) {
+      memcpy(h_slots + off[b], c_slots + static_cast<size_t>(q0 + b) * F, 8 * static_cast<size_t>(c_counts[q0 + b]));
+      memcpy(h_rel + off[b], c_scores + static_cast<size_t>(q0 + b) * F, 8 * static_cast<size_t>(c_counts[q0 + b]));
+    }
+    memcpy(h.data() + o_lam, lambda_mult + q0, 8 * static_cast<size_t>(Bg));
+    memcpy(h.data() + o_k, k + q0, 4 * static_cast<size_t>(Bg));
+    const size_t nk = static_cast<size_t>(Bg) * K;
+    CK(ix->mm_in.ensure(bytes));
+    CK(ix->mm_out.ensure(16 * nk));
+    rbk_status st = stage.host(h_slots, static_cast<int>(M));
+    if (st != RBK_OK) return st;
+    CK(cudaEventRecord(ix->ev_start, ix->stream));
+    if ((st = stage.device(static_cast<int>(M))) != RBK_OK) return st;
+    // pageable source: the copy has read h when it returns
+    CK(cudaMemcpyAsync(ix->mm_in.p, h.data(), bytes, cudaMemcpyHostToDevice, ix->stream));
+    unsigned char* in = ix->mm_in.p;
+    int64_t* d_slots = reinterpret_cast<int64_t*>(ix->mm_out.p);
+    double* d_scores = reinterpret_cast<double*>(ix->mm_out.p + 8 * nk);
+    CK(launch_mmr_select(reinterpret_cast<const double*>(ix->q_raw.p), ix->dim, reinterpret_cast<const int64_t*>(in),
+                         reinterpret_cast<const int64_t*>(in + o_slots), reinterpret_cast<const double*>(in + o_rel),
+                         reinterpret_cast<const int*>(in + o_k), reinterpret_cast<const double*>(in + o_lam), Bg,
+                         max_m, K, d_slots, d_scores, ix->stream));
+    ix->stats.kernel_launches++;
+    CK(cudaEventRecord(ix->ev_stop, ix->stream));
+    CK(cudaMemcpyAsync(out_slots + static_cast<size_t>(q0) * K, d_slots, 8 * nk, cudaMemcpyDeviceToHost, ix->stream));
+    CK(cudaMemcpyAsync(out_scores + static_cast<size_t>(q0) * K, d_scores, 8 * nk, cudaMemcpyDeviceToHost,
+                       ix->stream));
+    CK(cudaStreamSynchronize(ix->stream));
+    if (check_dead && M > 0 && ix->h_sq_dead.p[0] != 0)
+      return fail(RBK_ECUDA, "MMR: " + std::to_string(ix->h_sq_dead.p[0]) + " candidate rows were tombstoned");
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, ix->ev_start, ix->ev_stop));
+    *ms_out += ms;
+  }
+  return RBK_OK;
+}
+
 }  // namespace impl
 }  // namespace rbk
 
@@ -1161,6 +1252,8 @@ void release_scratch(rbk_index* ix) {
   ix->sq_rows.release();
   ix->sq_dead.release();
   ix->h_sq_dead.release();
+  ix->mm_in.release();
+  ix->mm_out.release();
   ix->h_q.release();
 }
 
@@ -2350,6 +2443,57 @@ rbk_status rbk_index_search_slots_f64(rbk_index* ix, const int64_t* query_slots,
       }
       fill_result_tail(out_slots + o, out_scores + o, Bc, K, Kc);
     }
+    if (kernel_ms_out) *kernel_ms_out += ms;
+  }
+  ix->stats.searches = searches;
+  return RBK_OK;
+}
+
+rbk_status rbk_index_search_mmr_f64(rbk_index* ix, const double* queries, int32_t B, int32_t query_dim,
+                                    const int32_t* k, const int32_t* fetch_k, const double* lambda_mult,
+                                    const double* min_score, int64_t* out_slots, double* out_scores,
+                                    int32_t* out_counts, float* kernel_ms_out) {
+  int K = 0;
+  rbk_status st = check_mmr_args(ix, B, queries != nullptr, query_dim, k, fetch_k, lambda_mult, min_score, out_slots,
+                                 out_scores, out_counts, &K);
+  if (st != RBK_OK) return st;
+  std::lock_guard<std::mutex> lk(ix->mu);
+  DeviceGuard dg(ix->device);
+  if (kernel_ms_out) *kernel_ms_out = 0.f;
+  // one call is one search, however many chunks it takes
+  const int64_t searches = ix->stats.searches + 1;
+  // the candidates' rows, gathered where the index keeps them (a candidate is live, so the gather must count no dead row)
+  std::vector<int64_t> rows;
+  MmrStage stage;
+  stage.host = [&](const int64_t* slots, int n) -> rbk_status {
+    rows.resize(n);
+    for (int i = 0; i < n; ++i) rows[i] = ix->slot.local(slots[i]);
+    return RBK_OK;
+  };
+  stage.device = [&](int n) -> rbk_status { return gather_queries(ix, rows.data(), n); };
+  std::vector<int64_t> c_slots;
+  std::vector<double> c_scores;
+  std::vector<int32_t> c_counts;
+  for (int c0 = 0; c0 < B; c0 += kSlotChunk) {
+    const int Bc = std::min(kSlotChunk, B - c0);
+    const int F = *std::max_element(fetch_k + c0, fetch_k + c0 + Bc);
+    c_slots.resize(static_cast<size_t>(Bc) * F);
+    c_scores.resize(static_cast<size_t>(Bc) * F);
+    c_counts.resize(Bc);
+    QuerySource q;
+    q.host = queries + static_cast<size_t>(c0) * ix->dim;
+    float ms = 0.f;
+    // the candidates: rbk_index_search_each_f64 on the route of the chunk's largest fetch_k
+    st = F <= RBK_MAX_K_FETCH
+             ? search_locked(ix, q, 8, Bc, F, -INFINITY, nullptr, nullptr, nullptr, c_slots.data(), c_scores.data(),
+                             c_counts.data(), &ms, fetch_k + c0, min_score + c0)
+             : large_locked(ix, q, Bc, F, -INFINITY, c_slots.data(), c_scores.data(), c_counts.data(), &ms,
+                            fetch_k + c0, min_score + c0);
+    if (st != RBK_OK) return st;
+    const size_t o = static_cast<size_t>(c0) * K;
+    st = mmr_select_locked(ix, Bc, F, c_slots.data(), c_scores.data(), c_counts.data(), k + c0, lambda_mult + c0, K,
+                           stage, /*check_dead=*/true, out_slots + o, out_scores + o, out_counts + c0, &ms);
+    if (st != RBK_OK) return st;
     if (kernel_ms_out) *kernel_ms_out += ms;
   }
   ix->stats.searches = searches;

@@ -94,6 +94,7 @@ struct rbk_group {
   PinBuf<unsigned char> h_out, h_q;
   PinBuf<double> h_sq;           // rbk_group_search_slots_f64: the members' gathered query rows
   PinBuf<double> h_pq;           // rbk_group_similar_pairs_f64: one chunk's query rows in slot order
+  PinBuf<double> h_mm;           // rbk_group_search_mmr_f64: one query group's candidate rows in candidate order
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int64_t redone_batches = 0;
 };
@@ -731,6 +732,7 @@ void rbk_group_destroy(rbk_group* g) {
     g->h_q.release();
     g->h_sq.release();
     g->h_pq.release();
+    g->h_mm.release();
     if (g->ev0) cudaEventDestroy(g->ev0);
     if (g->ev1) cudaEventDestroy(g->ev1);
   }
@@ -820,6 +822,7 @@ rbk_status rbk_group_trim(rbk_group* g) {
   g->h_q.release();
   g->h_sq.release();
   g->h_pq.release();
+  g->h_mm.release();
   return RBK_OK;
 }
 
@@ -957,6 +960,68 @@ rbk_status rbk_group_search_slots_f64(rbk_group* g, const int64_t* query_slots, 
       }
       fill_result_tail(out_slots + o, out_scores + o, Bc, K, Kc);
     }
+    if (device_ms_out) *device_ms_out += ms;
+  }
+  return RBK_OK;
+}
+
+rbk_status rbk_group_search_mmr_f64(rbk_group* g, const double* queries, int32_t B, int32_t query_dim,
+                                    const int32_t* k, const int32_t* fetch_k, const double* lambda_mult,
+                                    const double* min_score, int64_t* out_slots, double* out_scores,
+                                    int32_t* out_counts, float* device_ms_out) {
+  if (!g) return fail(RBK_EINVAL, "null group");
+  int K = 0;
+  rbk_status st = check_mmr_args(g->parts[0], B, queries != nullptr, query_dim, k, fetch_k, lambda_mult, min_score,
+                                 out_slots, out_scores, out_counts, &K);
+  if (st != RBK_OK) return st;
+  if (device_ms_out) *device_ms_out = 0.f;
+  std::lock_guard<std::mutex> lk(g->mu);
+  rbk_index* ix0 = g->parts[0];
+  // the owners gather the candidates' rows (a candidate is live: a refusal there is a bug) into the pinned g->h_mm in
+  // candidate order, from where one asynchronous copy takes them to device_ids[0], which runs the selection; the copy
+  // is done before the next query group writes h_mm, since each group ends in a synchronisation of ix0's stream
+  MmrStage stage;
+  stage.host = [&](const int64_t* slots, int n) -> rbk_status {
+    {
+      DeviceGuard dg(g->devices[0]);
+      CK(g->h_mm.ensure(static_cast<size_t>(n) * g->dim));
+    }
+    rbk_status s2 = group_gather_locked(g, slots, n, g->h_mm.p, /*allow_dead=*/false);
+    if (s2 == RBK_EINVAL) return fail(RBK_ECUDA, std::string("MMR: a candidate row was tombstoned: ") + last_error());
+    return s2;
+  };
+  stage.device = [&](int n) -> rbk_status {
+    const size_t bytes = static_cast<size_t>(n) * g->dim * 8;
+    CK(ix0->q_raw.ensure(bytes));
+    CK(cudaMemcpyAsync(ix0->q_raw.p, g->h_mm.p, bytes, cudaMemcpyHostToDevice, ix0->stream));
+    return RBK_OK;
+  };
+  std::vector<int64_t> c_slots;
+  std::vector<double> c_scores;
+  std::vector<int32_t> c_counts;
+  for (int c0 = 0; c0 < B; c0 += kSlotChunk) {
+    const int Bc = std::min(kSlotChunk, B - c0);
+    const int F = *std::max_element(fetch_k + c0, fetch_k + c0 + Bc);
+    c_slots.resize(static_cast<size_t>(Bc) * F);
+    c_scores.resize(static_cast<size_t>(Bc) * F);
+    c_counts.resize(Bc);
+    const double* q = queries + static_cast<size_t>(c0) * g->dim;
+    float ms = 0.f;
+    st = F <= RBK_MAX_K_FETCH
+             ? group_search_locked(g, q, 8, Bc, F, -INFINITY, c_slots.data(), c_scores.data(), c_counts.data(), &ms,
+                                   fetch_k + c0, min_score + c0)
+             : group_search_large_locked(g, q, Bc, F, -INFINITY, c_slots.data(), c_scores.data(), c_counts.data(), &ms,
+                                         fetch_k + c0, min_score + c0);
+    if (st != RBK_OK) return st;
+    {
+      std::vector<std::unique_lock<std::mutex>> locks;
+      for (rbk_index* ix : g->parts) locks.emplace_back(ix->mu);
+      DeviceGuard dg(ix0->device);
+      const size_t o = static_cast<size_t>(c0) * K;
+      st = mmr_select_locked(ix0, Bc, F, c_slots.data(), c_scores.data(), c_counts.data(), k + c0, lambda_mult + c0, K,
+                             stage, /*check_dead=*/false, out_slots + o, out_scores + o, out_counts + c0, &ms);
+    }
+    if (st != RBK_OK) return st;
     if (device_ms_out) *device_ms_out += ms;
   }
   return RBK_OK;

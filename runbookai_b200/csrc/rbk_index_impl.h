@@ -222,6 +222,9 @@ struct rbk_index {
   rbk::impl::DevBuf<long long> pr_off, pr_b;
   rbk::impl::DevBuf<double> pr_s;
   rbk::impl::PinBuf<int> h_pcnt;
+  // rbk_index_search_mmr_f64: one query group's packed selection inputs, and its picks (slots | scores); the candidate
+  // rows are staged in q_raw
+  rbk::impl::DevBuf<unsigned char> mm_in, mm_out;
   CUtensorMap tmap_c;
   int max_lead_tiles = rbk::kMaxLeadTiles;
   int kprime_override = 0;   // > 0 while a batch is re-scanned with the widest candidate margin
@@ -276,6 +279,30 @@ constexpr int kSlotChunk = 1024;
 rbk_status gather_queries(rbk_index* ix, const int64_t* rows, int B);
 // RBK_EINVAL when the last gather met a tombstoned row (after the synchronisation that follows it).
 rbk_status check_gathered(const rbk_index* ix);
+
+// rbk_index_search_mmr_f64 and rbk_group_search_mmr_f64.  The argument checks, in the order of check_each_args; *K = the
+// largest k (0 when B == 0).
+rbk_status check_mmr_args(rbk_index* ix, int B, bool have_q, int query_dim, const int32_t* k, const int32_t* fetch_k,
+                          const double* lambda_mult, const double* min_score, const void* out_slots,
+                          const void* out_scores, const void* out_counts, int* K);
+// The candidate rows of one query group of an MMR call, the stored values of global slots slots[0, n), in two steps:
+// host(slots, n) does the host work they need first (outside the timed region), then device(n) enqueues on ix->stream
+// what puts them in ix->q_raw as float64 rows [n][dim].
+struct MmrStage {
+  std::function<rbk_status(const int64_t* slots, int n)> host;
+  std::function<rbk_status(int n)> device;
+};
+// The greedy selection of one chunk of Bc queries of an MMR call (caller holds ix->mu, device current): query b's
+// candidates are the first c_counts[b] entries of row b of c_slots / c_scores ([Bc][F], global slots, the search_each
+// answer at its fetch_k).  Per contiguous query group whose candidate rows fit kLargeBudget, stage.host, then stage.device put the rows
+// in ix->q_raw and launch_mmr_select writes row b of out_slots / out_scores ([Bc][K], host); out_counts[b] = min(k[b],
+// c_counts[b]).  check_dead: RBK_ECUDA when the stage's gather (gather_queries) met a tombstoned row, which a candidate
+// never is.  *ms_out += the device time from stage.device on (the staging copy or gather, the selection, the copy
+// back), which leaves out stage.host's host work.
+rbk_status mmr_select_locked(rbk_index* ix, int Bc, int F, const int64_t* c_slots, const double* c_scores,
+                             const int32_t* c_counts, const int32_t* k, const double* lambda_mult, int K,
+                             const MmrStage& stage, bool check_dead, int64_t* out_slots, double* out_scores,
+                             int32_t* out_counts, float* ms_out);
 
 // caller holds ix->mu and has the index's device current.  The scan's query buffer keeps kBlockM zeroed rows beyond
 // the last whole query block, so that a scan launch may start at any query (a large-k search's query groups): such a

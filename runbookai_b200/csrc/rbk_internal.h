@@ -122,6 +122,14 @@ cudaError_t launch_tombstone(const int64_t* dev_slots, int64_t n, int64_t n_rows
 cudaError_t launch_gather_rows(const uint16_t* rows, const void* rows_x, int x_elem, const unsigned int* dead_bits,
                                const int64_t* sel, int B, int d, int dpad, double* dst, int* n_dead,
                                cudaStream_t stream);
+// (rbk_mmr.cu) The greedy MMR selection (rbk_index_search_mmr_f64), one block per query b: its candidates are rows
+// [off[b], off[b + 1]) of x ([.][d] float64, device), at most max_m of them, with global slots slot[] and relevances
+// rel[] at the same positions; k[b] picks at lambda_mult[b] go to row b of out_slots / out_scores ([B][K]), then
+// -1 / quiet NaN.  Needs mmr_smem_bytes(max_m) of dynamic shared memory per block.
+size_t mmr_smem_bytes(int max_m);
+cudaError_t launch_mmr_select(const double* x, int d, const int64_t* off, const int64_t* slot, const double* rel,
+                              const int* k, const double* lambda_mult, int B, int max_m, int K, int64_t* out_slots,
+                              double* out_scores, cudaStream_t stream);
 // *found = 1 if any of the n doubles at src (device or mapped host memory) is one a float32 cannot hold (else *found is
 // left as it is): x is accepted iff it is NaN or (double)(float)x == x (so +-0, +-inf and float32 subnormals are, 0.1
 // and 1e-300 are not).

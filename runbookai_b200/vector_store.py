@@ -43,7 +43,7 @@ import numpy as np
 
 from . import embedder as _emb
 from ._native import (RBK_EDIM, RBK_ENOTF32, RBK_INDEX_F64_ON_HOST, RBK_INDEX_SCAN_F16, RBK_MAX_K_FETCH, DimensionError,
-                      Index, RbkError, exact_rows_of)
+                      RBK_MAX_K_FETCH_LARGE, Index, RbkError, exact_rows_of)
 
 SCHEMA = """
       CREATE TABLE IF NOT EXISTS vector_embeddings (
@@ -677,6 +677,45 @@ class VectorStore:
         return [self._hydrate(ids[b], scores[b, :counts[b]], top_k, type_filter, service_filter)
                 for b in range(len(queries))]
 
+    def search_mmr(self, query: str, options: dict | None = None, **kw) -> list[RetrievedChunk]:
+        """Diverse hits by maximal marginal relevance: search() whose top results are picked one at a time from the
+        fetchK best, each the chunk whose relevance minus its largest similarity to the picks so far, weighed by
+        lambdaMult, is largest (Index.search_mmr), so that near-copies of one chunk do not fill the result.  Options as
+        search() (topK 10, minScore 0.5, typeFilter, serviceFilter), plus lambdaMult (0.5; 1 is the plain ranking) and
+        fetchK (min(4096, 10 * topK)).  It selects min(2 * topK, fetchK) chunks, applies the filters to them, and keeps
+        selection order (no re-sort by score) up to topK.  ValueError for a lambdaMult outside [0, 1]; RuntimeError
+        without an embedder and DimensionError on a ragged store, as search()."""
+        return self.search_mmr_batch([query], options, **kw)[0]
+
+    def search_mmr_batch(self, queries: Sequence[str], options: dict | None = None,
+                         **kw) -> list[list[RetrievedChunk]]:
+        """search_mmr() for every query, in one device call."""
+        o = dict(options or {})
+        o.update(kw)
+        if not _emb.is_embedder_configured():
+            raise RuntimeError(NOT_CONFIGURED)
+        top_k = js_or(o.get("topK"), o.get("top_k"), 10)
+        min_score = js_or(o.get("minScore"), o.get("min_score"), 0.5)
+        lam = o.get("lambdaMult", o.get("lambda_mult"))
+        lam = 0.5 if lam is None else float(lam)
+        if not 0.0 <= lam <= 1.0:
+            raise ValueError(f"lambdaMult must be in [0, 1], not {lam}")
+        fetch_k = int(o.get("fetchK") or o.get("fetch_k") or min(RBK_MAX_K_FETCH_LARGE, 10 * top_k))
+        select = min(int(2 * top_k), fetch_k)   # the reference's extra for the filters, as search() cuts at 2*topK
+        type_filter = o.get("typeFilter") or o.get("type_filter")
+        service_filter = o.get("serviceFilter") or o.get("service_filter")
+        q = np.asarray(_emb.embed_texts(list(queries)) if len(queries) > 1 else [_emb.embed_text(queries[0])],
+                       dtype=np.float64)
+        with self._st.lock:   # the slot table must be the one the selection ran against
+            if self._index is None or not self._ids:
+                return [[] for _ in queries]
+            if self._ragged or q.shape[1] != self._index.dim:
+                raise DimensionError(RBK_EDIM, "Vectors must have the same length")
+            slots, scores, counts, _ = self._index.search_mmr(q, select, fetch_k, lam, min_score)
+            ids = [[self._ids[int(s)] for s in slots[b, :counts[b]]] for b in range(len(queries))]
+        return [self._hydrate(ids[b], scores[b, :counts[b]], top_k, type_filter, service_filter, keep_order=True)
+                for b in range(len(queries))]
+
     def search_similar(self, chunk_id: str, options: dict | None = None, **kw) -> list[RetrievedChunk]:
         """The chunks most like a stored chunk: search() whose query is the stored embedding of `vec_<chunk_id>`, read
         where the index keeps it - no embedder call, so no API key.  Options as search(), plus excludeSelf (default
@@ -736,8 +775,10 @@ class VectorStore:
                 if nxt >= self._index.size():
                     return out
 
-    def _hydrate(self, top_ids, scores, top_k, type_filter, service_filter) -> list[RetrievedChunk]:
-        """vector-store.ts:223-279 (a4): stays on the host."""
+    def _hydrate(self, top_ids, scores, top_k, type_filter, service_filter,
+                 keep_order: bool = False) -> list[RetrievedChunk]:
+        """vector-store.ts:223-279 (a4): stays on the host.  keep_order: the results stay in top_ids' order (an MMR
+        selection) instead of the reference's sort by score."""
         pairs = [(i, float(sc)) for i, sc in zip(top_ids, scores) if i is not None]   # None: deleted meanwhile
         top_ids = [i for i, _ in pairs]
         if not top_ids:
@@ -751,7 +792,9 @@ class VectorStore:
         with self._db_lock:
             rows = self.db.execute(sql, params).fetchall()
         score_map = dict(pairs)
+        rank = {i: n for n, i in enumerate(top_ids)}
         results: list[RetrievedChunk] = []
+        ranks: list[int] = []
         for row in rows:
             services = json.loads(row["services"] or "[]")
             if service_filter and not any(s in services for s in service_filter):   # :261-264
@@ -759,7 +802,11 @@ class VectorStore:
             results.append(RetrievedChunk(id=row["chunk_id"], documentId=row["document_id"], title=row["title"] or "",
                                           content=row["content"], type=row["type"], services=services,
                                           score=score_map.get(row["id"]) or 0))
-        results.sort(key=lambda r: -r.score)                          # :278 (stable, like V8)
+            ranks.append(rank[row["id"]])
+        if keep_order:
+            results = [r for _, r in sorted(zip(ranks, results), key=lambda p: p[0])]
+        else:
+            results.sort(key=lambda r: -r.score)                      # :278 (stable, like V8)
         return results[:top_k]                                        # :279
 
     # reference spellings

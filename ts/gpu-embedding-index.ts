@@ -251,6 +251,45 @@ export class GpuEmbeddingIndex {
     }
   }
 
+  /** Whether mmrEach is available: the loaded addon's library has the MMR search (rbk_*_search_mmr_f64). */
+  get hasMmrEach(): boolean {
+    return this.index !== null && this.index.hasSearchMmr === true;
+  }
+
+  /**
+   * Diverse hits by maximal marginal relevance, in ONE native call (rbk_*_search_mmr_f64): query b's limits[b] picks
+   * from the fetchKs[b] hits bestEach would return at minScores[b], each the candidate whose lambdas[b] * score -
+   * (1 - lambdas[b]) * (largest cosine to a pick so far) is largest, in selection order with their scores.  Throws for a
+   * limit < 1, a fetchK below its limit or above 4096, or a lambda outside [0, 1] (the library's checks), and against a
+   * library without the MMR search (hasMmrEach false).
+   */
+  async mmrEach(queries: number[][], limits: number[], fetchKs: number[], lambdas: number[],
+                minScores: number[]): Promise<ScoredId[][]> {
+    while (this.compacting) await this.compacting; // never search against a table that is being renumbered
+    if (!this.index || this.slotOfId.size === 0) return queries.map(() => []);
+    if (this.badIds.size > 0 || queries.some((q) => q.length !== this.dim)) {
+      throw new Error('Vectors must have the same length');
+    }
+    const B = queries.length;
+    const packed = new Float64Array(B * this.dim);
+    queries.forEach((q, b) => packed.set(q, b * this.dim));
+    const K = Math.max(0, ...limits);
+    this.inFlight++;
+    try {
+      const { slots, scores, counts } = await this.index.searchMmr(packed, B, Int32Array.from(limits),
+        Int32Array.from(fetchKs), Float64Array.from(lambdas), Float64Array.from(minScores));
+      return queries.map((_, b) => {
+        const out: ScoredId[] = [];
+        for (let i = 0; i < counts[b]; i++) {
+          out.push({ id: this.idOfSlot[Number(slots[b * K + i])]!, score: scores[b * K + i] });
+        }
+        return out;
+      });
+    } finally {
+      if (--this.inFlight === 0) this.drained.splice(0).forEach((wake) => wake());
+    }
+  }
+
   /** Whether similarEach is available: the loaded addon's library has search by slot (rbk_*_search_slots_f64). */
   get hasSimilarEach(): boolean {
     return this.index !== null && this.index.hasSearchSlots === true;
